@@ -6,8 +6,11 @@ Reddit-shaped synthetic graph (BASELINE.json configs[1]); one process per GPU.
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --steps 5 --warmup 1      # the reference op sequence on host cores
+    python bench.py --steps 50 --warmup 10 --dump-outputs DIR  # also write the last timed step's results as DIR/*.npy
 
-A step = one 512-seed batch through the whole hot path.  Prints ONE JSON line (rank 0).
+A step = one 512-seed batch through the whole hot path.  Each timed region is exactly --steps steps (times
+--repeats, default 1).  Inputs (graph, weights, seeds) are seeded: the same arguments give the same inputs on every
+run, so two builds can be compared output for output with --dump-outputs.  Prints ONE JSON line (rank 0).
 """
 import argparse
 import json
@@ -33,7 +36,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
@@ -104,7 +107,7 @@ def bench_config(workload, kind="mean"):
     """The same dict in both arms (the driver compares them): what is computed, not how."""
     return {"workload": workload, "batch": BATCH, "fanout": "25x10 (hop-1 draws 10, hop-2 draws 25)",
             "rows_gathered_per_step": ROWS_PER_BATCH, "feature_dtype": "bf16" if kind == "maxpool" else "f32",
-            "l2": "inputs larger than L2 (567 MB feature table vs 126 MB L2; fresh random seeds every step)"}
+            "l2": "inputs larger than L2 (567 MB feature table vs 50 MB L2; fresh random seeds every step)"}
 
 
 def make_weights(kind, rs):
@@ -169,26 +172,30 @@ def main():
     ap.add_argument("--aggregator", default="mean", choices=["mean", "gcn", "maxpool"],
                     help="mean = BASELINE configs[1] (default); maxpool (+ bf16 features, --math bf16) = configs[2]")
     ap.add_argument("--math", default=os.environ.get("GS_MATH", "tf32x3"),
-                    help="tf32x3 (tcgen05, fp32-grade: meets the 1e-4 parity bar) | fp32 (CUDA cores) | tf32 | bf16")
+                    help="tf32x3 (tensor cores, fp32-grade: meets the 1e-4 parity bar) | fp32 (CUDA cores) | tf32 | bf16")
     ap.add_argument("--cpu-batches", type=int, default=12)
     ap.add_argument("--depth", type=int, default=int(os.environ.get("GS_PIPE_DEPTH", "4")),
                     help="graph runners / compute streams alternating in the pipelined front end")
     ap.add_argument("--no-partitioned", action="store_true", help="skip the node-partitioned measurement at N > 1")
-    ap.add_argument("--repeats", type=int, default=0,
-                    help="how many times each K-step timed region is repeated (median reported); 0 = auto (~0.3 s per leg)")
+    ap.add_argument("--repeats", type=int, default=1,
+                    help="how many times each K-step timed region is repeated back to back (median reported)")
     ap.add_argument("--no-config3", action="store_true", help="skip the short max-pool/bf16 pass behind roofline_tensor")
     ap.add_argument("--workload", default="reddit", choices=["reddit", "unsup", "rmat", "train"],
                     help="reddit = BASELINE configs[1] (default; the contract line); unsup = configs[3]: unsupervised training "
                          "step, node-partitioned, data parallel; rmat = configs[4]: R-MAT graph, CSR sampler, partitioned")
     ap.add_argument("--rmat-scale", type=int, default=20, help="log2 of the R-MAT id space (27 = BASELINE configs[4])")
     ap.add_argument("--rmat-nodes", type=int, default=0, help="nodes after trimming (0 = 2^scale; 100000000 for configs[4])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1 or args.repeats < 1:
+        ap.error("--steps and --repeats must be >= 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     kind = args.aggregator
     if kind == "maxpool":
-        args.math = "bf16"            # config 3: bf16 features / weights, fp32 accumulate, K4 on tcgen05
+        args.math = "bf16"            # config 3: bf16 features / weights, fp32 accumulate, K4 on the tensor cores
     workload = "reddit-shape synthetic N=%d F=%d max_degree=%d graphsage_%s 2-hop fanout 25x10 batch=%d dims=[%d,%d,%d]" % (
         N_NODES, F, MAX_DEG, kind, BATCH, F, DIM, DIM)
 
@@ -214,7 +221,7 @@ def main():
             "gpu_launches": 0}))
         return
 
-    # ------------------------------------------------------------------ our arm (B200)
+    # ------------------------------------------------------------------ our arm (CUDA)
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback)"
     torch.cuda.set_device(local_rank)
     dist = None
@@ -266,8 +273,7 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    R = args.repeats if args.repeats > 0 else int(min(200, max(5, np.ceil(4000.0 / max(args.steps, 1)))))
-    total = args.warmup + args.steps * R
+    R = args.repeats
 
     def stats(ms_list):
         a = np.sort(np.asarray(ms_list, dtype=np.float64))
@@ -277,7 +283,7 @@ def main():
     def measure(mdl, lo, hi, tag, probe_name, do_e2e=True, reps=R):
         """value (ids resident in HBM) and e2e (pinned-host ids in, result to pinned host) for one model.  Each timed
         region is EXACTLY args.steps steps; it is repeated `reps` times back to back (fresh seeds every step) and the
-        median region is reported, so a 20-step / 1.6 ms region no longer rides on one PCIe or scheduling hiccup."""
+        median region is reported.  res["last_out"] is the embedding batch of the last step of the value region."""
         rs = np.random.RandomState(1000 + rank)
         n_total = args.warmup + args.steps * reps
         seeds_host = torch.from_numpy(rs.randint(lo, hi, size=(n_total, BATCH)).astype(np.int32)).pin_memory()
@@ -312,13 +318,14 @@ def main():
             for c in pipe.computes:
                 c.wait_event(e0)
             for i in range(args.steps):
-                pipe.submit_device(seeds_dev[base + i])
+                last_out = pipe.submit_device(seeds_dev[base + i])
             for c in pipe.computes:
                 cur.wait_stream(c)
             e1.record(cur)
             pipe.synchronize()
             barrier()
             ms_value.append(max_over_ranks(e0.elapsed_time(e1)))
+        last_out = last_out.clone()                      # the runner's buffer is overwritten by later passes
         clk = clocks.summary()
         launches_per_step = pipe.runners[0].launches_per_replay
         pipe.close()
@@ -340,7 +347,7 @@ def main():
         kernel_ms = float(np.mean([a.elapsed_time(b) for a, b in pev]))
         res = dict(ms_value=stats(ms_value), clocks=clk, launches=launches_per_step * args.steps,
                    launches_per_step=launches_per_step, ms_probe_step=ms_probe_total / n_probe,
-                   gather_kernel_ms=max_over_ranks(kernel_ms), reps=reps)
+                   gather_kernel_ms=max_over_ranks(kernel_ms), reps=reps, last_out=last_out)
         res["ms_total"] = res["ms_value"]["median"]
         res["value"] = world * BATCH * args.steps / (res["ms_total"] * 1e-3)
         if not do_e2e:
@@ -387,21 +394,7 @@ def main():
         peak, peak_src = peaks()
         avg_ms = res["gather_kernel_ms"]
         achieved = GATHER_BYTES / (avg_ms * 1e-3) / 1e9
-        traffic, src = None, None           # dram__bytes_read + dram__bytes_write of this kernel, committed ncu capture
-        for name in ("ncu_gather_r02_summary.txt", "ncu_gather_r01_final_summary.txt"):
-            prof = os.path.join(ROOT, "profiles", name)
-            if not os.path.exists(prof):
-                continue
-            vals = {}
-            for line in open(prof):
-                if line.strip() == "" and vals:
-                    break                                    # first kernel record = the layer-0 launch
-                if line.startswith("dram__bytes_") and "=" in line:
-                    k_, v_ = line.split("=")
-                    vals[k_.strip()] = float(v_.split()[0]) * 1e6
-            if len(vals) == 2:
-                traffic, src = sum(vals.values()), "profiles/%s (ncu --set full, one launch; bytes)" % name
-                break
+        traffic, src = None, None           # DRAM bytes of this kernel: not measured (no hardware counters here)
         step_ms = res["ms_total"] / args.steps
         return {"bound": "hbm", "kernel": "gather_mean (layer 0, hops 0+1: fused 2-hop feature gather + fanout mean)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
@@ -417,26 +410,18 @@ def main():
     def tensor_roofline(res):
         avg_ms = res["gather_kernel_ms"]
         flops = 2.0 * BATCH * 250 * F * 512                       # hop-2 MLP: [128000, 602] x [602, 512]
-        tpeak, tburst = 1444.6, 1725.0
+        tpeak, tburst, peak_src = 989.0, 989.0, "H100 SXM data sheet, dense bf16 (not measured)"
         pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(pk):
             d_ = json.load(open(pk))
             tpeak, tburst = float(d_.get("bf16_tflops_sustained", tpeak)), float(d_.get("bf16_tflops", tburst))
+            peak_src = "measured sustained bf16 GEMM (MEASURED_PEAKS.json); burst %.0f" % tburst
         ach = flops / (avg_ms * 1e-3) / 1e12
-        traffic, src = None, None
-        prof = os.path.join(ROOT, "profiles", "ncu_maxpool_r02_summary.txt")
-        if os.path.exists(prof):
-            vals = {}
-            for line in open(prof):
-                if line.startswith("dram__bytes_") and "=" in line and len(vals) < 2:
-                    k_, v_ = line.split("=")
-                    vals[k_.strip()] = float(v_.split()[0]) * 1e6
-            if len(vals) == 2:
-                traffic, src = sum(vals.values()), "profiles/ncu_maxpool_r02_summary.txt"
-        return {"bound": "tensor", "kernel": "maxpool_mlp (layer 0, hop 2: gather + MLP 602->512 + ReLU + max over 25), tcgen05 bf16",
+        traffic, src = None, None           # DRAM bytes of this kernel: not measured (no hardware counters here)
+        return {"bound": "tensor", "kernel": "maxpool_mlp (layer 0, hop 2: gather + MLP 602->512 + ReLU + max over 25), wgmma bf16",
                 "achieved": ach, "peak": tpeak, "unit": "TFLOP/s", "frac": ach / tpeak, "frac_of_burst_peak": ach / tburst,
                 "traffic": traffic, "traffic_source": src,
-                "peak_source": "measured sustained cuBLAS bf16 (MEASURED_PEAKS.json); burst %.0f" % tburst,
+                "peak_source": peak_src,
                 "avg_kernel_ms": avg_ms, "algorithmic_flops_per_launch": flops,
                 "kernel_share_of_step": avg_ms / (res["ms_total"] / args.steps),
                 "kernel_share_of_probed_step": avg_ms / res["ms_probe_step"]}
@@ -447,6 +432,7 @@ def main():
 
     # node-partitioned table with the halo exchange fused into the gather (peer loads over NVLink); owner-computes seeds
     part = None
+    dumps = {"embeddings": rep["last_out"]}
     if world > 1 and not args.no_partitioned and kind != "maxpool":
         from graphsage_b200 import parallel
         bounds = parallel.community_bounds(g["comm"], world)      # cuts moved to community starts: no community straddles
@@ -467,7 +453,9 @@ def main():
                    "replica_rows_per_gpu": int(len(hot)), "replica_fraction_of_table": float(len(hot)) / N_NODES,
                    "gather_kernel_ms": pr["gather_kernel_ms"],
                    "nvlink_GBps_per_gpu": rho * GATHER_BYTES / (pr["gather_kernel_ms"] * 1e-3) / 1e9,
-                   "nvlink_peak_GBps": 770.0, "halo_staging": bool(shard.stage_halo)}
+                   "nvlink_peak_GBps": 450.0, "halo_staging": bool(shard.stage_halo)}
+            if full:
+                dumps["partitioned_embeddings"] = pr["last_out"]
             if shard.stage_halo:
                 # with staging the gather kernel reads local memory only; the NVLink transfer is the fetch pass, which
                 # overlaps the neighbouring steps - its rate is bounded below by (unique remote bytes / step time)
@@ -495,15 +483,20 @@ def main():
         if sweep:
             part["replica_sweep"] = [run_partitioned(int(float(f) * N_NODES), False) for f in sweep.split(",") if f.strip()]
 
-    # config 3 (BASELINE configs[2]) in the same run: max-pool aggregator over a bf16 table, K4 on tcgen05
+    # config 3 (BASELINE configs[2]) in the same run: max-pool aggregator over a bf16 table, K4 on the tensor cores
     c3 = None
     if kind == "mean" and world == 1 and not args.no_config3:
         table3 = torch.zeros((N_NODES + 1, ops.pad_cols(F)), dtype=torch.bfloat16, device=dev)
         table3[:, :F] = table[:, :F].to(torch.bfloat16)
         model3, _ = build_model("maxpool", table3[:, :F], "bf16")
         c3 = measure(model3, 0, N_NODES, "config3", probe_of("maxpool"), do_e2e=False, reps=max(1, min(R, 5)))
+        dumps["config3_embeddings"] = c3["last_out"]
         gs.set_default_math(args.math)
 
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in dumps.items():                 # [BATCH, 2 * DIM] float32 each
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.float().cpu().numpy())
     if rank != 0:
         return
     head = part if part is not None else None

@@ -94,7 +94,7 @@ def run_unsup(args, g, rank, world, local_rank, dist, dev):
         "allreduce_bytes_per_step": model.last_allreduce_bytes, "weights_identical_across_ranks": same,
         "loss_first": loss_first, "loss_last": loss_last, "mrr_last": mrr, "gpu_launches": launches, "clocks": clk,
         "replica_rows_per_gpu": int(len(hot)),
-        "note": "forward through the library's kernels (fused gather+mean over the partitioned table, tcgen05 GEMMs), backward "
+        "note": "forward through the library's kernels (fused gather+mean over the partitioned table, wgmma GEMMs), backward "
                 "= autograd with library GEMMs, eager launches (no CUDA graph): the step is launch-bound, not HBM-bound"}))
 
 

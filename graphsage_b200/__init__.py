@@ -1,4 +1,4 @@
-"""graphsage_b200 - a B200-native (sm_100a) sample-and-aggregate engine behind the
+"""graphsage_b200 - an H100-native (sm_90a) sample-and-aggregate engine behind the
 graphsage.neigh_samplers / graphsage.aggregators / graphsage.models.SampleAndAggregate surface of
 williamleif/GraphSAGE.  `import graphsage_b200 as graphsage` is the intended drop-in for that path.
 

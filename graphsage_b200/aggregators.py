@@ -1,5 +1,5 @@
 """MeanAggregator / GCNAggregator / MaxPoolingAggregator - the surface of reference
-graphsage/aggregators.py:6-195 over the B200 kernels.
+graphsage/aggregators.py:6-195 over the library's CUDA kernels.
 
 Two entry points per aggregator:
   agg((self_vecs[n, in], neigh_vecs[n, k, neigh_in])) -> [n, out * (2 if concat else 1)]
@@ -21,7 +21,7 @@ _MATH_NAMES = {"fp32": ops.MATH_FP32_SIMT, "simt": ops.MATH_FP32_SIMT, "tf32x3":
 
 def set_default_math(mode):
     """Arithmetic of the dense contraction for aggregators created afterwards: 'fp32' (CUDA cores),
-    'tf32x3' (tcgen05, fp32-accurate), 'tf32', 'bf16'."""
+    'tf32x3' (tensor cores, fp32-accurate), 'tf32', 'bf16'."""
     _DEFAULT_MATH[0] = _MATH_NAMES[mode] if isinstance(mode, str) else int(mode)
 
 
@@ -42,7 +42,7 @@ USE_GEMM_IMAGES = [False]     # opt-in: tf32x3 layers hand the gathered rows to 
 
 class _SageAggregator(Layer):
     def _image_layer(self, src, segments, parts, combine, include_self, want_self):
-        """gather + mean -> tile images -> tcgen05 GEMM (tf32x3); None when the image form does not apply."""
+        """gather + mean -> tile images -> wgmma GEMM (tf32x3); None when the image form does not apply."""
         code, post = act_code(self.act)
         if not USE_GEMM_IMAGES[0] or self.math != ops.MATH_TF32X3 or post is not None or self.dropout \
                 or any(K != src.shape[1] for (_, K, _) in parts):
@@ -261,7 +261,7 @@ class MaxPoolingAggregator(_SageAggregator):
         rows = max(s.out_row0 + s.n for s in segments)
         dev = src.device
         if self._fused_ok(src, segments):
-            # K4: gather -> MLP -> ReLU -> max over the fanout in one tcgen05 kernel per hop (bf16 operands).
+            # K4: gather -> MLP -> ReLU -> max over the fanout in one wgmma kernel per hop (bf16 operands).
             # Every launch of this branch is one of the library's kernels (no torch copy / convert kernels in the step).
             table = self._bf16_table(src, src_persistent)
             if getattr(self, "_packed_mlp", None) is None:

@@ -40,10 +40,10 @@ int32_t tuning(const char* key, int32_t dflt) {
 int sm_count() {
   static int n[64] = {0};                        // per device ordinal
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (n[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     n[dev] = v;
   }
   return n[dev];

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libgraphsage_b200 (sm_100a only).
+// Shared host/device helpers for libgraphsage_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

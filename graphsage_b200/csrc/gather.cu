@@ -249,8 +249,8 @@ struct ShardRows {
 // ------------------------------------------------------------------------------------------
 constexpr int kGroupRows = 13;
 
-// A-operand images for the tcgen05 GEMM that follows (gs_sage_gemm_img, tf32x3): instead of (or besides) the fp32 rows,
-// the kernel writes each result row already SPLIT into tf32 hi / lo and laid out as the UMMA K-major SWIZZLE_128B tile
+// A-operand images for the wgmma GEMM that follows (gs_sage_gemm_img, tf32x3): instead of (or besides) the fp32 rows,
+// the kernel writes each result row already SPLIT into tf32 hi / lo and laid out as the K-major SWIZZLE_128B tile
 // images the GEMM multiplies - part p (0 = self rows, 1 = mean rows), 128-row tile mt, 32-column K-block kb:
 //   img + ((((p * n_mtiles + mt) * kblocks + kb) * 2 + hl) * 16 KB) + sw128_off(row % 128, chunk),  hl = 0 hi / 1 lo,
 // so the GEMM's A operand is one 32 KB bulk copy per K-block (no producer warps, no register round trip, no proxy fence).

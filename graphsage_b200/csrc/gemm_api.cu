@@ -10,7 +10,6 @@ int32_t sage_gemm_tc_img(int64_t M, const gs_gemm_part* parts, int32_t n_parts, 
 int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias,
                      int32_t act, int32_t math, float* out, int64_t ldo, const void* workspace, cudaStream_t st);
 int32_t sage_gemm_tc_pack(const gs_gemm_part* parts, int32_t n_parts, int32_t math, void* workspace, cudaStream_t st);
-int32_t tc_debug_read(unsigned long long* out_host, int n);
 }  // namespace gs
 
 static int32_t check_parts(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, bool need_a = true) {
@@ -79,9 +78,6 @@ int32_t gs_sage_gemm_img(int64_t M, const gs_gemm_part* parts_host, int32_t n_pa
   return gs::sage_gemm_tc_img(M, parts_host, n_parts, combine, bias, act, out, ldo, workspace, a_images, a_part0,
                               (cudaStream_t)stream);
 }
-
-/* developer probe (not part of the public header): timeline stamps of CTA (0,0) of the last tcgen05 GEMM */
-int32_t gs_debug_read_gemm_timeline(unsigned long long* out_host, int32_t n) { return gs::tc_debug_read(out_host, n); }
 
 int32_t gs_sage_gemm(int64_t M, const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
                      int32_t act, int32_t math, float* out, int64_t ldo, void* workspace, void* stream) {

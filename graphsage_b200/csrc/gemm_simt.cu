@@ -1,5 +1,5 @@
 // fp32 CUDA-core GEMM for the aggregator contraction (GS_MATH_FP32_SIMT): the bring-up and
-// cross-check path for the tcgen05 kernels in gemm_tc.cu.  Same math as
+// cross-check path for the wgmma kernels in gemm_tc.cu.  Same math as
 //   tf.matmul(neigh_means, neigh_weights), tf.matmul(self_vecs, self_weights),
 //   tf.add_n / tf.concat, (+bias), act             reference graphsage/aggregators.py:51-64
 //   Dense: matmul + bias + relu                      reference graphsage/layers.py:104-116

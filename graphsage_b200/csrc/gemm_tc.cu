@@ -1,27 +1,26 @@
-// tcgen05 path of gs_sage_gemm: the neigh_weights / self_weights contraction of the aggregators
+// Tensor-core path of gs_sage_gemm: the neigh_weights / self_weights contraction of the aggregators
 // (reference graphsage/aggregators.py:51-64, 110-116, 184-195; Dense graphsage/layers.py:104-116)
-// on the 5th-generation tensor cores, fp32 in / fp32 out.
+// on the Hopper tensor cores (wgmma), fp32 in / fp32 out.
 //
 //   GS_MATH_TF32X3 : A = A_hi + A_lo, B = B_hi + B_lo (each exactly representable in tf32);
-//                    D += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi, fp32 accumulate in TMEM  -> fp32-grade result
-//   GS_MATH_TF32   : one kind::tf32 pass (operands masked to tf32)
-//   GS_MATH_BF16   : one kind::f16 pass, operands rounded to bf16
+//                    D += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi, fp32 accumulate in registers  -> fp32-grade result
+//   GS_MATH_TF32   : one tf32 pass (operands masked to tf32)
+//   GS_MATH_BF16   : one bf16 pass, operands rounded to bf16
 //
-// Structure (one CTA = one 128 x 128 output tile, 320 threads):
-//   warps 0-7  A producers: ld.global (coalesced 128-bit, next K-block prefetched in registers) -> split /
-//              convert -> st.shared in the UMMA K-major SWIZZLE_128B layout -> fence.proxy.async -> mbarrier.
-//              The same warps run the epilogue (tcgen05.ld from TMEM, bias / ReLU, st.global).
-//   warp 8     MMA issuer: one elected thread issues tcgen05.mma (SS operands), tcgen05.commit frees stages.
-//   warp 9     B loader: cp.async.bulk of pre-swizzled weight tile images (built per call by
-//              pack_b_kernel into the caller's workspace) with mbarrier complete_tx.
-// A goes through registers on purpose: the hi/lo split (and the bf16 rounding) is arithmetic on the
-// operand, and the same producer slot later takes a row-id indirection (gather-A) for the max-pool MLP.
+// Structure (one CTA = one 128 x 128 output tile, two warpgroups of 128 threads, each owning 64 output rows):
+//   B (weights): pre-swizzled tile images of W^T (built per weight update by pack_b_kernel into the caller's
+//                workspace), one cp.async.bulk per K-block into a ring of stages, completion on an mbarrier.
+//   A          : register form - every thread loads its 16-byte chunks of the next K-block from global memory while
+//                the current K-block's wgmmas run, then splits / converts them and stores the SW128 tile image;
+//                image form (tf32x3 only) - the fused gather already wrote the tf32 hi / lo tile images
+//                (gs_gather_mean_img), so A arrives by bulk copy like B.  Both forms run the same MMAs in the same
+//                order, so their results are bit-identical.
+// A goes through registers on purpose: the hi/lo split (and the bf16 rounding) is arithmetic on the operand.
 #include "tc_common.cuh"
 
 namespace gs {
 
-constexpr int TC_PRODUCER_WARPS = 8;
-constexpr int TC_THREADS = (TC_PRODUCER_WARPS + 2) * 32;
+constexpr int TC_THREADS = 256;
 
 struct TcPart {
   const float* A;
@@ -45,15 +44,14 @@ struct TcParams {
   float* out;
   int64_t ldo;
   int32_t tiles_n0;    // number of N tiles of part 0 (CONCAT tile -> part mapping)
-  int32_t issue_elect; // 1: warp-uniform elect.sync issue (default), 0: one thread inside `if (lane == 0)`
-  const unsigned char* a_img;   // image form (sage_gemm_tc_img_kernel): A operands as tf32 hi/lo tile images (gs_gather_mean_img)
+  const unsigned char* a_img;   // image form: A operands as tf32 hi/lo tile images (gs_gather_mean_img)
   int32_t a_mtiles;             // 128-row tiles in the A images
   int32_t a_part0;              // A-image part that feeds GEMM part 0 (GEMM part p reads A part a_part0 + p)
 };
 
 // ---------------------------------------------------------------------------------------------
 // B packing: weights [K, N] row-major fp32 -> per (n tile, k block) tile images of W^T
-// (N rows x BK k-elements, K-major, SW128), hi (+ lo) or bf16.  Tiny (<= a few MB), runs per call.
+// (N rows x BK k-elements, K-major, SW128), hi (+ lo) or bf16.  Tiny (<= a few MB), runs per weight update.
 // MODE: 0 = tf32x3 (hi, lo images), 1 = tf32 (hi only), 2 = bf16
 // ---------------------------------------------------------------------------------------------
 template <int MODE>
@@ -100,34 +98,16 @@ __global__ void __launch_bounds__(256) pack_b_kernel(TcParams prm, unsigned char
 // ---------------------------------------------------------------------------------------------
 // main kernel
 // ---------------------------------------------------------------------------------------------
-// timeline probe (CTA (0,0) only): globaltimer stamps at pipeline milestones, read back by gs_debug_read
-__device__ unsigned long long g_tc_dbg[32];
-__device__ __forceinline__ void dbg_stamp(int slot) {
-  if (blockIdx.x == 0 && blockIdx.y == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    g_tc_dbg[slot] = t;
-  }
-}
-
-template <int MODE, bool ASYNC = false>
+template <int MODE>
 struct TcCfg {
   static constexpr int BK = MODE == 2 ? 64 : 32;             // K elements per block (128 B of operand row)
-  static constexpr int UK = MODE == 2 ? 16 : 8;              // UMMA K per instruction (32 B)
   static constexpr int NIMG = MODE == 0 ? 2 : 1;             // hi (+ lo)
   static constexpr int IMG_BYTES = NIMG * TC_TILE_BYTES;     // one operand's images for one K-block
-  // A and B have SEPARATE rings.  A is refilled by the producer warps (their prefetch lives in registers / the
-  // raw ring, so few stages suffice).  B tiles come straight from L2 by bulk copy, and a copy can only be posted
-  // once its slot is free - so the B ring is deep enough to cover the L2 -> shared latency (NB copies in flight).
-  static constexpr int SA = MODE == 0 ? 2 : 3;
-  static constexpr int NB = ASYNC ? (MODE == 0 ? 2 : 4) : (MODE == 0 ? 4 : 8);
-  static constexpr int RAW_BYTES = TC_BM * BK * 4;
-  static constexpr int RAW_SLOTS = ASYNC ? (MODE == 2 ? 3 : 4) : 0;
-  static constexpr int B_OFF = SA * IMG_BYTES;
-  static constexpr int RAW_OFF = B_OFF + NB * IMG_BYTES;
-  static constexpr int SMEM_BYTES = RAW_OFF + RAW_SLOTS * RAW_BYTES + 1024;  // + slack for 1024-B alignment
+  static constexpr int STAGES = MODE == 0 ? 3 : 4;           // A + B per stage: 64 KB (tf32x3) / 32 KB
+  static constexpr int STAGE_BYTES = 2 * IMG_BYTES;          // A images, then B images
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // + slack for 1024-B alignment
+  static constexpr int CPT = 4;                              // A chunks per thread per K-block (1024 / 256)
 };
-
 
 template <int MODE>
 __device__ __forceinline__ void load_a_chunk(const TcPart& P, int64_t M, int64_t grow, int gcol, bool vec, float (&v)[8]) {
@@ -171,17 +151,17 @@ __device__ __forceinline__ void store_a_chunk(unsigned char* a_img, int row, int
   }
 }
 
-template <int MODE, bool ASYNC>
+// kImg: A from the gather's tile images (MODE 0 only) instead of the fp32 rows
+template <int MODE, bool kImg>
 __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __grid_constant__ TcParams prm,
                                                                      const unsigned char* __restrict__ ws) {
-  using C = TcCfg<MODE, ASYNC>;
+  using C = TcCfg<MODE>;
+  static_assert(!kImg || MODE == 0, "the image form carries tf32 hi / lo images");
   extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_a[C::SA], empty_a[C::SA], full_b[C::NB], empty_b[C::NB], accum_bar;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t full[C::STAGES];
 
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) dbg_stamp(0);
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31, wq = (tid >> 5) & 3;
 
   // ---- which output tile, which parts feed it
   const int64_t m0 = (int64_t)blockIdx.x * TC_BM;
@@ -193,402 +173,110 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
   const int N = prm.p[part_lo].N;
   int total_it = 0;
   for (int pi = part_lo; pi < part_hi; ++pi) total_it += prm.p[pi].kblocks;
+  auto locate = [&](int it, int& pi, int& kb) {
+    pi = part_lo; kb = it;
+    while (kb >= prm.p[pi].kblocks) { kb -= prm.p[pi].kblocks; ++pi; }
+  };
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::SA; ++s) {
-      mbar_init(&full_a[s], ASYNC ? TC_PRODUCER_WARPS : TC_PRODUCER_WARPS / 2);   // one arrive per producing warp
-      mbar_init(&empty_a[s], 1);
-    }
-    for (int s = 0; s < C::NB; ++s) {
-      mbar_init(&full_b[s], 1);
-      mbar_init(&empty_b[s], 1);
-    }
-    mbar_init(&accum_bar, 1);
+  if (tid == 0) {
+    for (int s = 0; s < C::STAGES; ++s) mbar_init(&full[s], 1);
     fence_mbar_init();
   }
-  if (warp == TC_PRODUCER_WARPS) {   // MMA warp owns the TMEM allocation
-    tmem_alloc(&tmem_base_smem, TC_BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_base_smem;
-  if (threadIdx.x == 0) dbg_stamp(1);
 
-  if (warp < TC_PRODUCER_WARPS) {
-    // =============================== A producers ===============================
-    if constexpr (ASYNC) {
-      // All 8 warps share every K-block.  Each thread cp.async's ITS OWN 16-byte chunks of the raw fp32 tile
-      // into a private position of the staging ring (completion is tracked per thread by cp.async groups, so no
-      // cross-thread synchronisation is needed), RAW_SLOTS-1 K-blocks ahead; it then reads them back, splits /
-      // converts, and stores the UMMA tile.
-      constexpr int EPC = MODE == 2 ? 8 : 4;                 // fp32 elements per UMMA 16-byte chunk
-      constexpr int CPT = 4;                                 // UMMA chunks per thread per K-block (1024 / 256)
-      constexpr int RAW_PER_CHUNK = EPC / 4;                 // raw 16-byte pieces per UMMA chunk
-      unsigned char* raw = smem + C::RAW_OFF;
-      const int tid = threadIdx.x;                           // 0..255
-      auto locate = [&](int it, int& pi, int& kb) {
-        pi = part_lo; kb = it;
-        while (kb >= prm.p[pi].kblocks) { kb -= prm.p[pi].kblocks; ++pi; }
-      };
-      auto issue = [&](int it) {
-        if (it < total_it) {
-          int pi, kb;
-          locate(it, pi, kb);
-          const TcPart& P = prm.p[pi];
-          unsigned char* slot = raw + (size_t)(it % C::RAW_SLOTS) * C::RAW_BYTES;
+  // one thread posts the bulk copies of K-block `it` (B, and A in the image form) into its stage
+  auto post = [&](int it) {
+    if (tid != 0 || it >= total_it) return;
+    int pi, kb;
+    locate(it, pi, kb);
+    const TcPart& P = prm.p[pi];
+    const int s = it % C::STAGES;
+    unsigned char* st = smem + (size_t)s * C::STAGE_BYTES;
+    mbar_expect_tx(&full[s], kImg ? 2 * C::IMG_BYTES : C::IMG_BYTES);
+    bulk_g2s(st + C::IMG_BYTES, ws + P.img_off + ((int64_t)ntile * P.kblocks + kb) * C::IMG_BYTES, C::IMG_BYTES, &full[s]);
+    if constexpr (kImg)
+      bulk_g2s(st, prm.a_img + (((int64_t)(prm.a_part0 + pi) * prm.a_mtiles + blockIdx.x) * P.kblocks + kb) * C::IMG_BYTES,
+               C::IMG_BYTES, &full[s]);
+  };
+  float cur[C::CPT][8];
+  auto fetch = [&](int it) {
+    int pi, kb;
+    locate(it, pi, kb);
+    const TcPart& P = prm.p[pi];
+    const bool vec = ((P.lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.A) & 15u) == 0);
 #pragma unroll
-          for (int i = 0; i < CPT; ++i) {
-            const int q = tid + 256 * i;
-            const int row = q >> 3, c = q & 7;
-            const int64_t grow = m0 + row;
-#pragma unroll
-            for (int h = 0; h < RAW_PER_CHUNK; ++h) {
-              const int gcol = kb * C::BK + c * EPC + h * 4;
-              int nbytes = 0;
-              if (grow < prm.M && gcol < P.K) nbytes = min(4, P.K - gcol) * 4;
-              const float* src = nbytes ? (P.A + grow * P.lda + gcol) : P.A;   // always a valid, 16-B aligned address
-              cp_async16(slot + (size_t)(q * RAW_PER_CHUNK + h) * 16, src, nbytes);
-            }
-          }
-        }
-        cp_async_commit();                                   // empty groups keep the group count uniform
-      };
-#pragma unroll
-      for (int j = 0; j < C::RAW_SLOTS - 1; ++j) issue(j);
-      for (int it = 0; it < total_it; ++it) {
-        issue(it + C::RAW_SLOTS - 1);
-        cp_async_wait<C::RAW_SLOTS - 1>();                   // this thread's pieces of K-block `it` have landed
-        const unsigned char* slot = raw + (size_t)(it % C::RAW_SLOTS) * C::RAW_BYTES;
-        float v[CPT][8];
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) {
-          const int q = tid + 256 * i;
-#pragma unroll
-          for (int h = 0; h < RAW_PER_CHUNK; ++h) {
-            const float4 f = *reinterpret_cast<const float4*>(slot + (size_t)(q * RAW_PER_CHUNK + h) * 16);
-            v[i][h * 4 + 0] = f.x; v[i][h * 4 + 1] = f.y; v[i][h * 4 + 2] = f.z; v[i][h * 4 + 3] = f.w;
-          }
-        }
-        const int s = it % C::SA;
-        const uint32_t ph = (uint32_t)(it / C::SA) & 1u;
-        mbar_wait(&empty_a[s], ph ^ 1u);
-        unsigned char* a_img = smem + (size_t)s * C::IMG_BYTES;
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) {
-          const int q = tid + 256 * i;
-          store_a_chunk<MODE>(a_img, q >> 3, q & 7, v[i]);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&full_a[s]);
-      }
-    } else {
-    // two groups of 4 warps alternate K-blocks; each thread owns 8 chunks (rows tg>>3 + 16 i, chunk tg & 7)
-    const int group = warp >> 2;
-    const int tg = threadIdx.x & 127;
-    const int c = tg & 7, r0 = tg >> 3;
-    float cur[8][8];
-    auto locate = [&](int it, int& pi, int& kb) {
-      pi = part_lo; kb = it;
-      while (kb >= prm.p[pi].kblocks) { kb -= prm.p[pi].kblocks; ++pi; }
-    };
-    auto fetch = [&](int it, float (&dst)[8][8]) {
-      int pi, kb;
-      locate(it, pi, kb);
-      const TcPart& P = prm.p[pi];
-      const bool vec = ((P.lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(P.A) & 15u) == 0);
-      const int gcol = kb * C::BK + c * (MODE == 2 ? 8 : 4);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) load_a_chunk<MODE>(P, prm.M, m0 + r0 + 16 * i, gcol, vec, dst[i]);
-    };
-    int it = group;
-    if (it < total_it) fetch(it, cur);
-    for (; it < total_it; it += 2) {
-      const int s = it % C::SA;
-      const uint32_t ph = (uint32_t)(it / C::SA) & 1u;
-      float nxt[8][8];
-      const bool more = it + 2 < total_it;
-      if (more) fetch(it + 2, nxt);                    // prefetch this group's next K-block
-      mbar_wait(&empty_a[s], ph ^ 1u);
-      unsigned char* a_img = smem + (size_t)s * C::IMG_BYTES;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) store_a_chunk<MODE>(a_img, r0 + 16 * i, c, cur[i]);
-      fence_proxy_async();                             // generic-proxy stores -> visible to the MMA (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_a[s]);
-      if (threadIdx.x == 0 && it == 0) dbg_stamp(2);
-      if (threadIdx.x == 0 && it + 2 >= total_it) dbg_stamp(3);
-      if (more) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) cur[i][e] = nxt[i][e];
-      }
+    for (int i = 0; i < C::CPT; ++i) {
+      const int q = tid + TC_THREADS * i;
+      load_a_chunk<MODE>(P, prm.M, m0 + (q >> 3), kb * C::BK + (q & 7) * (MODE == 2 ? 8 : 4), vec, cur[i]);
     }
-    }
-    // =============================== epilogue ===============================
-    if (threadIdx.x == 0) dbg_stamp(4);
-    mbar_wait(&accum_bar, 0);
-    tc_fence_after();
-    if (threadIdx.x == 0) dbg_stamp(5);
-    const int q = warp & 3;                           // TMEM lane quarter this warp may touch
-    const int half = warp >> 2;                       // columns [64*half, 64*half + 64)
-    const int64_t grow = m0 + q * 32 + lane;
-#pragma unroll
-    for (int cb = 0; cb < 2; ++cb) {
-      const int col0 = half * 64 + cb * 32;
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)col0, r);
-      tmem_ld_wait();
-      if (grow < prm.M) {
-        const int gn0 = ntile * TC_BN + col0;
-        float* dst = prm.out + grow * prm.ldo + col_off + gn0;
-        const bool vec = ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) && gn0 + 32 <= N;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float v[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            v[e] = __uint_as_float(r[j + e]);
-            if (prm.bias && gn0 + j + e < N) v[e] += prm.bias[col_off + gn0 + j + e];
-            if (prm.act == GS_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
-          }
-          if (vec) {
-            *reinterpret_cast<float4*>(dst + j) = make_float4(v[0], v[1], v[2], v[3]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              if (gn0 + j + e < N) dst[j + e] = v[e];
-          }
-        }
-      }
-    }
-    tc_fence_before();
-    if (threadIdx.x == 0) dbg_stamp(6);
-  } else if (warp == TC_PRODUCER_WARPS) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(MODE == 2 ? 1u : 2u, TC_BM, TC_BN);
-    for (int it = 0; it < total_it; ++it) {
-      const int s = it % C::SA, sb = it % C::NB;
-      mbar_wait(&full_a[s], (uint32_t)(it / C::SA) & 1u);
-      if (lane == 0 && it == 0) dbg_stamp(8);
-      mbar_wait(&full_b[sb], (uint32_t)(it / C::NB) & 1u);
-      tc_fence_after();
-      if (lane == 0 && it == 0) dbg_stamp(9);
-      if (lane == 0 && it == 1) dbg_stamp(10);
-      if (lane == 0 && it == 8) dbg_stamp(11);
-      if (lane == 0 && it == total_it - 1) dbg_stamp(12);
-      const uint32_t a_base = smem_u32(smem + (size_t)s * C::IMG_BYTES);
-      const uint32_t b_base = smem_u32(smem + C::B_OFF + (size_t)sb * C::IMG_BYTES);
-      const uint64_t a_hi = make_smem_desc(a_base), b_hi = make_smem_desc(b_base);
-      if (prm.issue_elect) {
-        // whole warp, uniform operands, elect.sync on the instruction (tc_common.cuh: umma_ss_elect)
-#pragma unroll
-        for (int k = 0; k < C::BK / C::UK; ++k) {
-          const uint64_t koff = (uint64_t)((k * 32) >> 4);          // 32 B per UMMA K step inside the swizzle atom
-          const uint32_t acc = (it > 0 || k > 0) ? 1u : 0u;
-          umma_ss_elect<MODE == 2>(tmem_acc, a_hi + koff, b_hi + koff, idesc, acc);
-          if constexpr (MODE == 0) {
-            const uint64_t a_lo = make_smem_desc(a_base + TC_TILE_BYTES), b_lo = make_smem_desc(b_base + TC_TILE_BYTES);
-            umma_ss_elect<false>(tmem_acc, a_hi + koff, b_lo + koff, idesc, 1u);
-            umma_ss_elect<false>(tmem_acc, a_lo + koff, b_hi + koff, idesc, 1u);
-          }
-        }
-        umma_commit_elect(&empty_a[s]);                                // A stage and B slot reusable once these MMAs retire
-        umma_commit_elect(&empty_b[sb]);
-        if (it == total_it - 1) umma_commit_elect(&accum_bar);         // accumulator complete
-        if (lane == 0 && it == total_it - 1) dbg_stamp(13);
-      } else if (lane == 0) {
-#pragma unroll
-        for (int k = 0; k < C::BK / C::UK; ++k) {
-          const uint64_t koff = (uint64_t)((k * 32) >> 4);
-          const uint32_t acc = (it > 0 || k > 0) ? 1u : 0u;
-          umma_ss<MODE == 2>(tmem_acc, a_hi + koff, b_hi + koff, idesc, acc);
-          if constexpr (MODE == 0) {
-            const uint64_t a_lo = make_smem_desc(a_base + TC_TILE_BYTES), b_lo = make_smem_desc(b_base + TC_TILE_BYTES);
-            umma_ss<false>(tmem_acc, a_hi + koff, b_lo + koff, idesc, 1u);
-            umma_ss<false>(tmem_acc, a_lo + koff, b_hi + koff, idesc, 1u);
-          }
-        }
-        umma_commit(&empty_a[s]);
-        umma_commit(&empty_b[sb]);
-        if (it == total_it - 1) umma_commit(&accum_bar);
-        if (it == total_it - 1) dbg_stamp(13);
-      }
-      __syncwarp();
-    }
-  } else {
-    // =============================== B loader ===============================
-    if (lane == 0) {
-      int it = 0;
-      for (int pi = part_lo; pi < part_hi; ++pi) {
-        const TcPart& P = prm.p[pi];
-        const unsigned char* base = ws + P.img_off + (int64_t)ntile * P.kblocks * C::NIMG * TC_TILE_BYTES;
-        for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-          const int sb = it % C::NB;
-          const uint32_t ph = (uint32_t)(it / C::NB) & 1u;
-          mbar_wait(&empty_b[sb], ph ^ 1u);
-          mbar_expect_tx(&full_b[sb], C::IMG_BYTES);
-          bulk_g2s(smem + C::B_OFF + (size_t)sb * C::IMG_BYTES, base + (int64_t)kb * C::IMG_BYTES, C::IMG_BYTES,
-                   &full_b[sb]);
-        }
-      }
-    }
-    __syncwarp();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) dbg_stamp(7);
-  if (warp == TC_PRODUCER_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, TC_BN);
-  }
-}
+  };
 
-// ---------------------------------------------------------------------------------------------
-// Image form (tf32x3 only): the A operand arrives as the tf32 hi / lo UMMA tile images the fused gather wrote
-// (gs_gather_mean_img), so a K-block of A is ONE 32 KB bulk copy - no producer warps, no register round trip, no hi/lo
-// split here, no generic->async proxy fence.  Same arithmetic as sage_gemm_tc_kernel<0> (A_hi*B_hi + A_hi*B_lo +
-// A_lo*B_hi in that order, fp32 accumulate in TMEM): results are bit-identical to it.
-//   warp 0: A loader (bulk copies)   warp 1: B loader   warp 2: MMA issuer (+ TMEM alloc)   warps 4-7: epilogue
-// Three 32 KB stages per operand (192 KB): the ring covers the L2 -> shared latency, which the register-staged form could not.
-// ---------------------------------------------------------------------------------------------
-constexpr int TCI_THREADS = 256;
-constexpr int TCI_IMG = 2 * TC_TILE_BYTES;      // hi + lo image of one K-block
-constexpr int TCI_SA = 3, TCI_NB = 3;
-constexpr int TCI_SMEM = (TCI_SA + TCI_NB) * TCI_IMG + 1024;
+  for (int j = 0; j < C::STAGES - 1; ++j) post(j);
+  if constexpr (!kImg) fetch(0);
 
-__global__ void __launch_bounds__(TCI_THREADS, 1) sage_gemm_tc_img_kernel(const __grid_constant__ TcParams prm,
-                                                                          const unsigned char* __restrict__ ws) {
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_a[TCI_SA], empty_a[TCI_SA], full_b[TCI_NB], empty_b[TCI_NB], accum_bar;
-  __shared__ uint32_t tmem_base_smem;
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* a_ring = smem;
-  unsigned char* b_ring = smem + TCI_SA * TCI_IMG;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  const int64_t m0 = (int64_t)blockIdx.x * TC_BM;
-  int part_lo = 0, part_hi = prm.n_parts, ntile = blockIdx.y, col_off = 0;
-  if (prm.combine == GS_COMBINE_CONCAT && prm.n_parts == 2) {
-    if ((int)blockIdx.y < prm.tiles_n0) part_hi = 1;
-    else { part_lo = 1; ntile = blockIdx.y - prm.tiles_n0; col_off = prm.p[0].N; }
-  }
-  const int N = prm.p[part_lo].N;
-  int total_it = 0;
-  for (int pi = part_lo; pi < part_hi; ++pi) total_it += prm.p[pi].kblocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TCI_SA; ++s) { mbar_init(&full_a[s], 1); mbar_init(&empty_a[s], 1); }
-    for (int s = 0; s < TCI_NB; ++s) { mbar_init(&full_b[s], 1); mbar_init(&empty_b[s], 1); }
-    mbar_init(&accum_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(&tmem_base_smem, TC_BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_base_smem;
-
-  if (warp == 0) {
-    // =============================== A loader ===============================
-    if (lane == 0) {
-      int it = 0;
-      for (int pi = part_lo; pi < part_hi; ++pi) {
-        const TcPart& P = prm.p[pi];
-        const unsigned char* base = prm.a_img + (((int64_t)(prm.a_part0 + pi) * prm.a_mtiles + blockIdx.x) * P.kblocks) * TCI_IMG;
-        for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-          const int sa = it % TCI_SA;
-          mbar_wait(&empty_a[sa], ((uint32_t)(it / TCI_SA) & 1u) ^ 1u);
-          mbar_expect_tx(&full_a[sa], TCI_IMG);
-          bulk_g2s(a_ring + (size_t)sa * TCI_IMG, base + (int64_t)kb * TCI_IMG, TCI_IMG, &full_a[sa]);
-        }
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int it = 0; it < total_it; ++it) {
+    const int s = it % C::STAGES;
+    unsigned char* st = smem + (size_t)s * C::STAGE_BYTES;
+    if constexpr (!kImg) {
+#pragma unroll
+      for (int i = 0; i < C::CPT; ++i) {
+        const int q = tid + TC_THREADS * i;
+        store_a_chunk<MODE>(st, q >> 3, q & 7, cur[i]);
+      }
+      fence_proxy_async();                       // generic-proxy stores -> visible to wgmma (async proxy)
+    }
+    __syncthreads();                             // A stored; every warpgroup is done with K-block it - 1's stage
+    post(it + C::STAGES - 1);                    // ... which is the stage this refills
+    if constexpr (!kImg) {
+      if (it + 1 < total_it) fetch(it + 1);      // next K-block's loads fly under this one's MMAs
+    }
+    mbar_wait(&full[s], (uint32_t)(it / C::STAGES) & 1u);
+    const uint32_t a_base = smem_u32(st) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(st + C::IMG_BYTES);
+    const uint64_t a_hi = make_smem_desc(a_base), b_hi = make_smem_desc(b_base);
+    const uint64_t a_lo = make_smem_desc(a_base + TC_TILE_BYTES), b_lo = make_smem_desc(b_base + TC_TILE_BYTES);
+    acc_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {                // four K steps of 32 B inside the 128-B swizzle atom
+      const uint64_t koff = (uint64_t)((k * 32) >> 4);
+      wgmma_m64n128<MODE == 2>(acc, a_hi + koff, b_hi + koff, (it > 0 || k > 0) ? 1u : 0u);
+      if constexpr (MODE == 0) {
+        wgmma_m64n128<false>(acc, a_hi + koff, b_lo + koff, 1u);
+        wgmma_m64n128<false>(acc, a_lo + koff, b_hi + koff, 1u);
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // =============================== B loader ===============================
-    if (lane == 0) {
-      int it = 0;
-      for (int pi = part_lo; pi < part_hi; ++pi) {
-        const TcPart& P = prm.p[pi];
-        const unsigned char* base = ws + P.img_off + (int64_t)ntile * P.kblocks * TCI_IMG;
-        for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-          const int sb = it % TCI_NB;
-          mbar_wait(&empty_b[sb], ((uint32_t)(it / TCI_NB) & 1u) ^ 1u);
-          mbar_expect_tx(&full_b[sb], TCI_IMG);
-          bulk_g2s(b_ring + (size_t)sb * TCI_IMG, base + (int64_t)kb * TCI_IMG, TCI_IMG, &full_b[sb]);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 2) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(2u, TC_BM, TC_BN);            // tf32 x tf32 -> fp32
-    for (int it = 0; it < total_it; ++it) {
-      const int sa = it % TCI_SA, sb = it % TCI_NB;
-      mbar_wait_uniform(&full_a[sa], (uint32_t)(it / TCI_SA) & 1u);
-      mbar_wait_uniform(&full_b[sb], (uint32_t)(it / TCI_NB) & 1u);
-      tc_fence_after();
-      const uint32_t a_base = smem_u32(a_ring + (size_t)sa * TCI_IMG), b_base = smem_u32(b_ring + (size_t)sb * TCI_IMG);
-      const uint64_t a_hi = make_smem_desc(a_base), b_hi = make_smem_desc(b_base);
-      const uint64_t a_lo = make_smem_desc(a_base + TC_TILE_BYTES), b_lo = make_smem_desc(b_base + TC_TILE_BYTES);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {                                     // four K = 8 steps per 32-column K-block
-        const uint64_t koff = (uint64_t)((k * 32) >> 4);
-        umma_ss_elect<false>(tmem_acc, a_hi + koff, b_hi + koff, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        umma_ss_elect<false>(tmem_acc, a_hi + koff, b_lo + koff, idesc, 1u);
-        umma_ss_elect<false>(tmem_acc, a_lo + koff, b_hi + koff, idesc, 1u);
-      }
-      umma_commit_elect(&empty_a[sa]);
-      umma_commit_elect(&empty_b[sb]);
-      if (it == total_it - 1) umma_commit_elect(&accum_bar);
-    }
-  } else if (warp >= 4) {
-    // =============================== epilogue ===============================
-    mbar_wait(&accum_bar, 0);
-    tc_fence_after();
-    const int q = warp & 3;                           // TMEM lane quarter of this warp
-    const int64_t grow = m0 + q * 32 + lane;
-#pragma unroll 1
-    for (int cb = 0; cb < 4; ++cb) {
-      const int col0 = cb * 32;
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)col0, r);
-      tmem_ld_wait();
-      if (grow < prm.M) {
-        const int gn0 = ntile * TC_BN + col0;
-        float* dst = prm.out + grow * prm.ldo + col_off + gn0;
-        const bool vec = ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) && gn0 + 32 <= N;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float v[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            v[e] = __uint_as_float(r[j + e]);
-            if (prm.bias && gn0 + j + e < N) v[e] += prm.bias[col_off + gn0 + j + e];
-            if (prm.act == GS_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
-          }
-          if (vec) {
-            *reinterpret_cast<float4*>(dst + j) = make_float4(v[0], v[1], v[2], v[3]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              if (gn0 + j + e < N) dst[j + e] = v[e];
-          }
-        }
-      }
-    }
-    tc_fence_before();
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc);
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, TC_BN);
+
+  // =============================== epilogue: registers -> bias / ReLU -> global ===============================
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t grow = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+    if (grow >= prm.M) continue;
+    float* dst_row = prm.out + grow * prm.ldo + col_off;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int gn = ntile * TC_BN + 8 * j + 2 * (lane & 3);
+      float v[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        v[e] = acc[4 * j + 2 * h + e];
+        if (prm.bias && gn + e < N) v[e] += prm.bias[col_off + gn + e];
+        if (prm.act == GS_ACT_RELU) v[e] = fmaxf(v[e], 0.f);
+      }
+      float* dst = dst_row + gn;
+      if (gn + 2 <= N && (reinterpret_cast<uintptr_t>(dst) & 7u) == 0) {
+        *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+      } else {
+        if (gn < N) dst[0] = v[0];
+        if (gn + 1 < N) dst[1] = v[1];
+      }
+    }
   }
 }
 
@@ -614,7 +302,6 @@ static void fill_parts(TcParams& prm, int64_t M, const gs_gemm_part* parts, int3
     off += (int64_t)P.kblocks * P.ntiles * nimg * TC_TILE_BYTES;
   }
   prm.tiles_n0 = prm.p[0].ntiles;
-  prm.issue_elect = tuning("mma_issue", 1) != 0;
 }
 
 int64_t sage_gemm_tc_workspace(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t math) {
@@ -632,34 +319,16 @@ static int32_t launch_pack(const TcParams& prm, unsigned char* ws, cudaStream_t 
   return launch_check("pack_b_kernel");
 }
 
-template <int MODE, bool ASYNC>
-static int32_t launch_tc_impl(const TcParams& prm, const unsigned char* ws, cudaStream_t st) {
-  using C = TcCfg<MODE, ASYNC>;
-  {
-    const int32_t rc_attr = ensure_dyn_smem((const void*)sage_gemm_tc_kernel<MODE, ASYNC>, C::SMEM_BYTES);
-    if (rc_attr != GS_OK) return rc_attr;
-  }
+template <int MODE, bool kImg>
+static int32_t launch_tc(const TcParams& prm, const unsigned char* ws, cudaStream_t st) {
+  using C = TcCfg<MODE>;
+  const int32_t rc_attr = ensure_dyn_smem((const void*)sage_gemm_tc_kernel<MODE, kImg>, C::SMEM_BYTES);
+  if (rc_attr != GS_OK) return rc_attr;
   int tiles_n = prm.p[0].ntiles;
   if (prm.combine == GS_COMBINE_CONCAT && prm.n_parts == 2) tiles_n += prm.p[1].ntiles;
   dim3 grid((unsigned)((prm.M + TC_BM - 1) / TC_BM), (unsigned)tiles_n);
-  sage_gemm_tc_kernel<MODE, ASYNC><<<grid, TC_THREADS, C::SMEM_BYTES, st>>>(prm, ws);
+  sage_gemm_tc_kernel<MODE, kImg><<<grid, TC_THREADS, C::SMEM_BYTES, st>>>(prm, ws);
   return launch_check("sage_gemm_tc_kernel");
-}
-
-template <int MODE>
-static int32_t launch_tc(const TcParams& prm, const unsigned char* ws, cudaStream_t st) {
-  bool aligned = true;                         // cp.async needs 16-byte aligned rows
-  for (int i = 0; i < prm.n_parts; ++i)
-    aligned = aligned && (prm.p[i].lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(prm.p[i].A) & 15u) == 0);
-  if (aligned && tuning("gemm_async", 0)) return launch_tc_impl<MODE, true>(prm, ws, st);
-  return launch_tc_impl<MODE, false>(prm, ws, st);
-}
-
-int32_t tc_debug_read(unsigned long long* out_host, int n) {
-  if (n > 32) n = 32;
-  GS_CUDA(cudaDeviceSynchronize());
-  GS_CUDA(cudaMemcpyFromSymbol(out_host, g_tc_dbg, sizeof(unsigned long long) * n));
-  return GS_OK;
 }
 
 int32_t sage_gemm_tc_pack(const gs_gemm_part* parts, int32_t n_parts, int32_t math, void* workspace, cudaStream_t st) {
@@ -689,13 +358,7 @@ int32_t sage_gemm_tc_img(int64_t M, const gs_gemm_part* parts, int32_t n_parts, 
   prm.a_img = (const unsigned char*)a_images;
   prm.a_mtiles = (int32_t)((M + TC_BM - 1) / TC_BM);
   prm.a_part0 = a_part0;
-  const int32_t rc_attr = ensure_dyn_smem((const void*)sage_gemm_tc_img_kernel, TCI_SMEM);
-  if (rc_attr != GS_OK) return rc_attr;
-  int tiles_n = prm.p[0].ntiles;
-  if (combine == GS_COMBINE_CONCAT && n_parts == 2) tiles_n += prm.p[1].ntiles;
-  dim3 grid((unsigned)prm.a_mtiles, (unsigned)tiles_n);
-  sage_gemm_tc_img_kernel<<<grid, TCI_THREADS, TCI_SMEM, st>>>(prm, (const unsigned char*)workspace);
-  return launch_check("sage_gemm_tc_img_kernel");
+  return launch_tc<0, true>(prm, (const unsigned char*)workspace, st);
 }
 
 int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias,
@@ -711,9 +374,9 @@ int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int3
   prm.out = out;
   prm.ldo = ldo;
   const unsigned char* ws = (const unsigned char*)workspace;
-  if (mode == 0) return launch_tc<0>(prm, ws, st);
-  if (mode == 1) return launch_tc<1>(prm, ws, st);
-  return launch_tc<2>(prm, ws, st);
+  if (mode == 0) return launch_tc<0, false>(prm, ws, st);
+  if (mode == 1) return launch_tc<1, false>(prm, ws, st);
+  return launch_tc<2, false>(prm, ws, st);
 }
 
 }  // namespace gs

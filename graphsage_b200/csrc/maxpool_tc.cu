@@ -1,38 +1,39 @@
-// K4: the max-pool aggregator's neighbour branch as ONE kernel on tcgen05 (bf16 operands, fp32 accumulate):
+// K4: the max-pool aggregator's neighbour branch as ONE kernel on the Hopper tensor cores (wgmma, bf16 operands,
+// fp32 accumulate):
 //   out[g, h] = max_{j<k} relu( table[row(g, j), :] . Wm[:, h] + bm[h] )
 //   reference graphsage/aggregators.py:176-182 (reshape -> Dense(relu, bias) -> reshape -> reduce_max) with
 //   graphsage/layers.py:104-116 and the feature gather of graphsage/models.py:299 fused in front of it:
 //   neither the gathered [n*k, F] rows nor the [n*k, hidden] MLP activations ever touch HBM.
 //
-// Persistent CTAs.  A CTA owns one 128-wide slice of the hidden dimension for its whole life: that slice of
-// Wm^T (<= 10 K-blocks x 16 KB, pre-swizzled bf16 tile images) is bulk-copied into shared memory ONCE and stays
-// resident.  The CTA then walks M tiles (G = floor(128 / k) whole fanout groups per tile, zero rows after them):
-//   warps 0-3  gather-A producers: cp.async 16-byte pieces of the addressed table rows straight into the UMMA
-//              K-major SWIZZLE_128B tile (bf16 in the table = bf16 in the tile: no conversion), 2 K-blocks ahead.
-//              (Measured alternatives - 3-5 K-blocks of 128-bit register loads per thread, with 4 or 8 producer
-//              warps, and an L2 prefetch of the next tile - were slower; the limiter is shared-memory capacity:
-//              the 160 KB resident weight slice leaves 48 KB for A stages.  See DESIGN.md section 4.)
-//   warp  4    MMA issuer: tcgen05.mma.kind::f16 (M128 N128 K16), accumulators double-buffered in TMEM
-//   warp  5    loads the resident weight slice (cp.async.bulk + mbarrier)
-//   warps 6-9  epilogue: tcgen05.ld -> + bias -> ReLU -> staged transpose in shared memory -> max over the k rows
-//              of each group -> coalesced store; overlaps the next tile's MMAs (second TMEM buffer)
-#include <cuda.h>   // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint (no libcuda link)
-
+// One CTA = one tile of NT gathered rows (G = floor(NT / k) whole fanout groups, zero rows after them) x one 128-wide
+// slice of the hidden dimension; the n_slices CTAs of a tile are adjacent in the grid, so the rows the first of them
+// gathers are still in L2 for the others.  Two warpgroups.  K loop over 64-column K-blocks (128-byte operand rows,
+// SWIZZLE_128B), MP_STAGES stages: the gathered rows land straight in a K-major tile (bf16 in the table = bf16 in the
+// tile: no conversion), the slice's pre-swizzled Wm^T image comes by one cp.async.bulk on an mbarrier, then
+// wgmma.m64n128k16 x 4 per K-block with the accumulators in registers.  Epilogue: raw accumulators -> staging tile in
+// shared memory (reusing the operand ring, hidden-unit-major) -> max (or mean) over each group's k rows -> + bias ->
+// ReLU -> coalesced store.
+//
+// Variants (template parameters, chosen at run time by tuning keys; every one is parity-tested):
+//   kRowsA  (k4_operands = 1, the default): gathered rows = A operand (M = NT rows over the two warpgroups), Wm^T slice =
+//           B (N = 128); 0: the roles swapped - the weight slice is A (M = 64 hidden units per warpgroup) and the
+//           gathered rows are B (N = NT), so the weight image is read once per NT rows.
+//   NT      (k4_tile): 128 rows per tile (two CTAs per SM, fanout <= 128) or 256 (fanout <= 256, one CTA per SM).
+//   DEPTH   (k4_mma_depth): wgmma groups in flight; 2 lets the next K-block's MMAs queue behind the current ones at
+//           the price of one stage of prefetch.
+//   PROD    (k4_producer): 0 = cp.async 16-byte pieces; 1 = 128-bit register loads stored to the swizzled tile (the
+//           loads of K-block kb + 1 fly under K-block kb's MMAs).
+//   k4_cluster: launch the slices of a tile as a thread-block cluster (2 .. 8 CTAs; -1 = all slices of the tile) so
+//           they are co-scheduled on one GPC and the tile's rows are fetched from HBM once for the whole cluster.
 #include "tc_common.cuh"
 
 namespace gs {
 
-// K-blocks are 32 bf16 columns = 64-byte operand rows (UMMA K-major SWIZZLE_64B): an 8 KB stage instead of 16 KB, so
-// six A stages fit beside the resident weights (with 16 KB stages only three did, and the stage a producer needed
-// next was always the one whose MMA had just been published - a structural bubble), and K pads to 32, not 64.
-constexpr int MP_KCOLS = 32;                  // bf16 columns per K-block
-constexpr int MP_IMG = TC_BM * 64;            // one operand K-block image: 128 rows x 64 B
-constexpr int MP_MAX_KB = 20;                 // resident weight K-blocks (K <= 640)
-constexpr int MP_RING = 26;                   // 8 KB slots shared by the resident weights (kblocks) and the A stages
-constexpr int MP_PROD_WARPS = 4;               // gather-A producer warps
-constexpr int MP_THREADS = (MP_PROD_WARPS + 6) * 32;
-constexpr int MP_STAGE_LD = 129;              // padded row length of the epilogue staging [32][129]
-constexpr int MP_SMEM = MP_RING * MP_IMG + 32 * MP_STAGE_LD * 4 + 1024;
+constexpr int MP_KCOLS = 64;                   // bf16 columns per K-block (128 B of operand row)
+constexpr int MP_IMG = 128 * 128;              // one operand K-block image: 128 rows x 128 B
+constexpr int MP_MAX_KB = 10;                  // K <= 640
+constexpr int MP_STAGES = 3;
+constexpr int MP_THREADS = 256;
 
 struct MpParams {
   const __nv_bfloat16* table;   // [n_rows, pitch]
@@ -42,398 +43,22 @@ struct MpParams {
   int64_t row0;                 // used when row_ids == NULL: row(g, j) = row0 + g*k + j
   int64_t n_groups;
   int32_t k, G;                 // fanout, groups per tile
-  int64_t n_tiles;
-  int32_t hidden, n_slices;
+  int32_t n_slices;
   const unsigned char* wimg;    // packed Wm^T: [n_slices][kblocks][16 KB]
   const float* bias;            // [hidden] or NULL
   int32_t pool_mean;            // 0: max over the fanout (MaxPoolingAggregator), 1: mean (MeanPoolingAggregator)
   float* out;                   // [n_groups, hidden]
   int64_t ldo;
-  int32_t issue_elect;          // 1: warp-uniform elect.sync issue (default), 0: one thread inside `if (lane == 0)`
-  int32_t n_stages;             // wide kernel: X stages in the ring
-  int32_t kb_t;                 // tmem kernel: K-blocks of the weight slice held in tensor memory
-  const uint32_t* wrows;        // tmem kernel: Wm^T as rows of bf16 pairs [hidden][kblocks * 32]
-  int32_t dbg;                  // wide kernel timing probes (garbage results): 3 = no producers, MMA warp does not wait for stages;
-                                // 4 = producers run, MMA warp waits and commits but issues no MMA
 };
 
-// byte offset of 16-byte chunk c (0..3) of row r inside a K-major SWIZZLE_64B image (Swizzle<2,4,3>: address bits
-// [4,6) ^= bits [7,9); rows are 64 B apart, so bits [7,9) = (r >> 1) & 3)
-__host__ __device__ __forceinline__ uint32_t sw64_off(int r, int c) { return (uint32_t)(r * 64 + ((c ^ ((r >> 1) & 3)) << 4)); }
-
-// K-major SWIZZLE_64B shared-memory matrix descriptor: SBO = 8 rows x 64 B = 512 B, layout type 4
-__device__ __forceinline__ uint64_t make_smem_desc64(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
-  return d;
-}
-
-// Wm [K, hidden] row-major fp32 -> bf16 tile images of Wm^T (128 hidden rows x 32 k, K-major, SW64)
+// Wm [K, hidden] row-major fp32 -> bf16 tile images of Wm^T (128 hidden rows x 64 k, K-major, SW128)
 __global__ void __launch_bounds__(256) maxpool_pack_kernel(const float* __restrict__ W, int64_t ldw, int K, int hidden,
                                                            int kblocks, unsigned char* __restrict__ img) {
   const int slice = blockIdx.x / kblocks, kb = blockIdx.x % kblocks;
   unsigned char* dst = img + ((int64_t)slice * kblocks + kb) * MP_IMG;
-  for (int q = threadIdx.x; q < 128 * 4; q += blockDim.x) {
-    const int c = q >> 7, n = q & 127;
-    const int gn = slice * 128 + n, k0 = kb * MP_KCOLS + c * 8;
-    __nv_bfloat162 h[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      float a = (gn < hidden && k0 + 2 * e < K) ? W[(int64_t)(k0 + 2 * e) * ldw + gn] : 0.f;
-      float b = (gn < hidden && k0 + 2 * e + 1 < K) ? W[(int64_t)(k0 + 2 * e + 1) * ldw + gn] : 0.f;
-      h[e] = __floats2bfloat162_rn(a, b);
-    }
-    *reinterpret_cast<uint4*>(dst + sw64_off(n, c)) = *reinterpret_cast<uint4*>(h);
-  }
-}
-
-// timeline probe (CTA 0): globaltimer stamps, 8 slots per tile for the first 12 tiles
-__device__ unsigned long long g_mp_dbg[128];
-__device__ __forceinline__ void mp_stamp(uint32_t tcount, int slot) {
-  if (blockIdx.x == 0 && tcount < 12) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    g_mp_dbg[tcount * 8 + slot] = t;
-  }
-}
-
-// Optional epilogue cycle breakdown (build with GS_EXTRA_NVCC_FLAGS=-DGS_K4_EPI_PROBE; compiled out otherwise):
-// CTA 0, epilogue thread 0 accumulates clock64 deltas into g_mp_dbg[100..105] =
-// {tmem ld + wait, staging stores, barrier 1, pooling loop + global stores, barrier 2, column blocks counted}
-#ifdef GS_K4_EPI_PROBE
-#define MP_EPI_T(var) const long long var = clock64()
-#define MP_EPI_ACC(slot, a, b) \
-  do {                         \
-    if (blockIdx.x == 0 && et == 0) g_mp_dbg[100 + (slot)] += (unsigned long long)((b) - (a)); \
-  } while (0)
-#else
-#define MP_EPI_T(var) \
-  do {                \
-  } while (0)
-#define MP_EPI_ACC(slot, a, b) \
-  do {                         \
-  } while (0)
-#endif
-
-// ---- roles shared by the kernel variants (forced inline: one copy of the logic, no call overhead) ----
-
-// MMA issuer warp: waits for each A stage, issues the two K = 16 MMAs of the K-block against the resident weights,
-// commits the stage back to the producers and, after a tile's last K-block, the accumulator to the epilogue.
-template <int MP_SA, int CL = 1>
-__device__ __forceinline__ void mp_mma_role(const MpParams& prm, int lane, int kblocks, int64_t tile0, int64_t tile_step,
-                                            uint32_t tmem_base, uint64_t* full_a, uint64_t* empty_a, uint64_t* acc_full,
-                                            uint64_t* acc_empty, uint64_t& b_full, unsigned char* a_ring,
-                                            unsigned char* b_res) {
-  // =============================== MMA issuer ===============================
-  constexpr uint32_t idesc = make_idesc(1u, TC_BM, TC_BN);          // bf16 x bf16 -> fp32
-  mbar_wait(&b_full, 0);
-  uint32_t it = 0, tcount = 0;
-  for (int64_t t = tile0; t < prm.n_tiles; t += tile_step, ++tcount) {
-    const uint32_t buf = tcount & 1u;
-    if (lane == 0) mp_stamp(tcount, 2);
-    mbar_wait(&acc_empty[buf], ((tcount >> 1) & 1u) ^ 1u);          // epilogue has drained this accumulator
-    tc_fence_after();
-    if (lane == 0) mp_stamp(tcount, 3);
-    const uint32_t tmem_acc = tmem_base + buf * 128u;
-    for (int kb = 0; kb < kblocks; ++kb, ++it) {
-      const int s = it % MP_SA;
-      mbar_wait(&full_a[s], (it / MP_SA) & 1u);
-      tc_fence_after();
-      const uint64_t adesc = make_smem_desc64(smem_u32(a_ring + (size_t)s * MP_IMG));
-      const uint64_t bdesc = make_smem_desc64(smem_u32(b_res + (size_t)kb * MP_IMG));
-      if (prm.issue_elect) {
-        // whole warp, uniform operands, elect.sync on the instruction (tc_common.cuh: umma_ss_elect)
-#pragma unroll
-        for (int k2 = 0; k2 < 2; ++k2)            // two K = 16 steps per 32-column K-block (32 B apart inside the atom)
-          umma_ss_elect<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc,
-                              (kb > 0 || k2 > 0) ? 1u : 0u);
-        if constexpr (CL > 1)                       // frees the stage in every CTA of the cluster
-          umma_commit_elect_multicast(&empty_a[s], (uint16_t)((1u << CL) - 1u));
-        else
-          umma_commit_elect(&empty_a[s]);
-        if (kb == kblocks - 1) umma_commit_elect(&acc_full[buf]);
-        if (lane == 0 && kb == kblocks - 1) mp_stamp(tcount, 4);
-      } else if (lane == 0) {
-#pragma unroll
-        for (int k2 = 0; k2 < 2; ++k2)
-          umma_ss<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        umma_commit(&empty_a[s]);
-        if (kb == kblocks - 1) umma_commit(&acc_full[buf]);
-        if (kb == kblocks - 1) mp_stamp(tcount, 4);
-      }
-      __syncwarp();
-    }
-  }
-}
-
-// Weight loader warp: one bulk copy per K-block image of this CTA's slice, once.
-__device__ __forceinline__ void mp_weights_role(const MpParams& prm, int lane, int slice, int kblocks, uint64_t& b_full,
-                                                unsigned char* b_res) {
-  // =============================== resident weight slice ===============================
-  if (lane == 0) {
-    mbar_expect_tx(&b_full, (uint32_t)(kblocks * MP_IMG));
-    const unsigned char* src = prm.wimg + (int64_t)slice * kblocks * MP_IMG;
-    for (int kb = 0; kb < kblocks; ++kb)
-      bulk_g2s(b_res + (size_t)kb * MP_IMG, src + (int64_t)kb * MP_IMG, MP_IMG, &b_full);
-  }
-  __syncwarp();
-}
-
-// Epilogue (four consecutive warps; et = 0..127 is the thread's index among them).
-__device__ __forceinline__ void mp_epilogue_role(const MpParams& prm, int et, int warp, int lane, int slice, int64_t tile0,
-                                                 int64_t tile_step, uint32_t tmem_base, uint64_t* acc_full,
-                                                 uint64_t* acc_empty, float* stage, float* bias_s) {
-  // =============================== epilogue ===============================
-  const int q = warp & 3;                         // TMEM lane quarter of this warp (four consecutive warps cover 0..3)
-  const int row = q * 32 + lane;                  // tile row held by this thread
-  const int k = prm.k, G = prm.G;
-  bias_s[et] = prm.bias ? prm.bias[slice * 128 + et] : 0.f;     // this CTA's 128 bias values, once
-  named_bar_sync(1, 128);
-  uint32_t tcount = 0;
-  for (int64_t t = tile0; t < prm.n_tiles; t += tile_step, ++tcount) {
-    const uint32_t buf = tcount & 1u;
-    if (et == 0) mp_stamp(tcount, 5);
-    mbar_wait(&acc_full[buf], (tcount >> 1) & 1u);
-    tc_fence_after();
-    if (et == 0) mp_stamp(tcount, 6);
-    const uint32_t tmem_acc = tmem_base + buf * 128u + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int cb = 0; cb < 4; ++cb) {
-      uint32_t r[32];
-      MP_EPI_T(e0);
-      tmem_ld_32x32(tmem_acc + (uint32_t)(cb * 32), r);
-      tmem_ld_wait();
-      MP_EPI_T(e1);
-      const int hcol0 = slice * 128 + cb * 32;
-      // raw accumulators go to the staging tile; bias and ReLU are applied AFTER the max
-      // (max_j relu(x_j + b) == relu(max_j x_j + b): b is per column, relu is monotone)
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stage[j * MP_STAGE_LD + row] = __uint_as_float(r[j]);
-      MP_EPI_T(e2);
-      named_bar_sync(1, 128);
-      MP_EPI_T(e3);
-      // thread = (column cc, group residue): max over each group's k consecutive rows, 8 independent
-      // shared loads per batch
-      {
-        const int cc = et & 31;
-        for (int g = et >> 5; g < G; g += 4) {
-          const int64_t gg = t * G + g;
-          if (gg < prm.n_groups) {
-            const float* p = stage + cc * MP_STAGE_LD + g * k;
-            const float b = bias_s[cb * 32 + cc];
-            float res;
-            if (prm.pool_mean) {
-              // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU
-              // are applied per element, summed in j order, divided by k
-              float sacc = 0.f;
-              for (int j = 0; j < k; ++j) sacc += fmaxf(p[j] + b, 0.f);
-              res = sacc / (float)k;
-            } else {
-              float m = -3.0e38f;
-              int j = 0;
-              for (; j + 8 <= k; j += 8) {
-                float v[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) v[u] = p[j + u];
-                m = fmaxf(m, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
-              }
-              for (; j < k; ++j) m = fmaxf(m, p[j]);
-              res = fmaxf(m + b, 0.f);                                          // Dense bias + ReLU (commute with the max)
-            }
-            prm.out[gg * prm.ldo + hcol0 + cc] = res;
-          }
-        }
-      }
-      MP_EPI_T(e4);
-      named_bar_sync(1, 128);
-      MP_EPI_T(e5);
-      MP_EPI_ACC(0, e0, e1);
-      MP_EPI_ACC(1, e1, e2);
-      MP_EPI_ACC(2, e2, e3);
-      MP_EPI_ACC(3, e3, e4);
-      MP_EPI_ACC(4, e4, e5);
-      MP_EPI_ACC(5, 0, 1);
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    if (et == 0) mp_stamp(tcount, 7);
-  }
-}
-
-// MP_SA A stages of 8 KB, MP_INFLIGHT cp.async K-blocks in flight per producer thread: <7, 5> when the resident
-// weights need <= 19 slots (K <= 608), else <6, 4>
-// kAsyncArrive: the producers never wait for their own copies - each thread hands the stage's full barrier a
-// cp.async.mbarrier.arrive.noinc, which the hardware fires when that thread's copies have landed (no cp.async group
-// wait, no proxy fence, no elected arrive; the barrier counts one arrival per producer THREAD).
-template <int MP_SA, int MP_INFLIGHT, bool kAsyncArrive = false>
-__global__ void __launch_bounds__(MP_THREADS, 1) maxpool_mlp_kernel(const __grid_constant__ MpParams prm) {
-  static_assert(MP_INFLIGHT + 2 <= MP_SA, "a stage must be free while MP_INFLIGHT copies fly and one is consumed");
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_a[MP_SA], empty_a[MP_SA], acc_full[2], acc_empty[2], b_full;
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float bias_s[128];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* b_res = smem;                                        // resident weight slice
-  unsigned char* a_ring = smem + (MP_RING - MP_SA) * MP_IMG;
-  float* stage = reinterpret_cast<float*>(smem + MP_RING * MP_IMG);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int kblocks = prm.kblocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MP_SA; ++s) {
-      mbar_init(&full_a[s], kAsyncArrive ? MP_PROD_WARPS * 32 : MP_PROD_WARPS);   // one arrive per producer thread / warp
-      mbar_init(&empty_a[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);        // one arrive per epilogue warp
-    }
-    mbar_init(&b_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == MP_PROD_WARPS) {
-    tmem_alloc(&tmem_base_smem, 256);     // two 128-column fp32 accumulators
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp < MP_PROD_WARPS) {
-    // =============================== gather-A producers ===============================
-    const int tid = threadIdx.x;                    // 0..127
-    const int c = tid & 3, r0 = tid >> 2;           // 16-byte chunk of the 64-byte row; rows r0 + 32 i, i < 4
-    const int rows_valid = prm.G * prm.k;
-    uint32_t it = 0;                                // running K-block counter across tiles (stage / phase)
-    int pending = 0;                                // K-blocks issued but not yet published
-    auto publish = [&](uint32_t which) {
-      const int s = which % MP_SA;
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_a[s]);
-    };
-    uint32_t ptile = 0;
-    for (int64_t t = tile0; t < prm.n_tiles; t += tile_step, ++ptile) {
-      if (threadIdx.x == 0) mp_stamp(ptile, 0);
-      const __nv_bfloat16* rowp[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = r0 + 32 * i;
-        const int64_t flat = t * rows_valid + r;    // index into the (group, j) row list
-        rowp[i] = nullptr;
-        if (r < rows_valid && flat < prm.n_groups * prm.k) {
-          int64_t id = prm.row_ids ? (int64_t)prm.row_ids[flat] : prm.row0 + flat;
-          if (id < 0 || id >= prm.n_rows) id = prm.n_rows - 1;
-          rowp[i] = prm.table + id * prm.pitch;
-        }
-      }
-      for (int kb = 0; kb < kblocks; ++kb, ++it) {
-        const int s = it % MP_SA;
-        mbar_wait(&empty_a[s], ((it / MP_SA) & 1u) ^ 1u);
-        unsigned char* a_img = a_ring + (size_t)s * MP_IMG;
-        const int col = kb * MP_KCOLS + c * 8;      // first bf16 column of this 16-byte piece
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          int nbytes = 0;
-          if (rowp[i] != nullptr && col < prm.K) nbytes = min(8, prm.K - col) * 2;
-          const void* src = nbytes ? (const void*)(rowp[i] + col) : (const void*)prm.table;
-          cp_async16(a_img + sw64_off(r0 + 32 * i, c), src, nbytes);
-        }
-        if constexpr (kAsyncArrive) {
-          cp_async_mbar_arrive_noinc(&full_a[s]);
-          continue;
-        }
-        cp_async_commit();
-        ++pending;
-        if (pending == MP_INFLIGHT + 1) {           // MP_INFLIGHT K-blocks stay in flight; the oldest has landed
-          cp_async_wait<MP_INFLIGHT>();
-          publish(it - MP_INFLIGHT);
-          --pending;
-        }
-      }
-      if (threadIdx.x == 0) mp_stamp(ptile, 1);
-    }
-    // drain: publish the remaining K-blocks oldest first
-    while (pending > 0) {
-      if (pending >= 5) cp_async_wait<4>();
-      else if (pending == 4) cp_async_wait<3>();
-      else if (pending == 3) cp_async_wait<2>();
-      else if (pending == 2) cp_async_wait<1>();
-      else cp_async_wait<0>();
-      publish(it - pending);
-      --pending;
-    }
-  } else if (warp == MP_PROD_WARPS) {
-    mp_mma_role<MP_SA>(prm, lane, kblocks, tile0, tile_step, tmem_base, full_a, empty_a, acc_full, acc_empty, b_full, a_ring,
-                       b_res);
-  } else if (warp == MP_PROD_WARPS + 1) {
-    mp_weights_role(prm, lane, slice, kblocks, b_full, b_res);
-  } else {
-    mp_epilogue_role(prm, (int)threadIdx.x - (MP_PROD_WARPS + 2) * 32, warp, lane, slice, tile0, tile_step, tmem_base, acc_full,
-                     acc_empty, stage, bias_s);
-  }
-  __syncthreads();
-  if (warp == MP_PROD_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// K4, "wide" form (round 2; tuning k4_kernel = 0): the SAME contraction with the operand roles swapped -
-//   D^T[h, r] = sum_c Wm^T[h, c] * X[r, c]      (M = 128 hidden units of this CTA's slice, N = 256 gathered rows, K = 16)
-// i.e. the resident weight slice is the UMMA A operand and the gathered feature rows are the B operand.  Why:
-//   * a fanout group's k rows are now k consecutive accumulator COLUMNS of one TMEM lane, so a thread that reads its
-//     lane with tcgen05.ld (32x32b) holds a whole group in registers: the max (or mean) over the fanout is a register
-//     loop - no shared-memory transpose, no staging tile, no CTA-wide barriers in the epilogue - and lane = hidden
-//     unit makes the result stores coalesced (32 consecutive floats per warp);
-//   * N = 256 per instruction: a tile is 256 gathered rows (10 groups of 25), the weight image is read from shared
-//     memory once per 256 rows instead of once per 128 (96 B/clk of operand reads instead of 128 B/clk at the tensor
-//     pipe's floor), and TMEM holds two 128 x 256 fp32 accumulators (all 512 columns) so the epilogue of tile t
-//     overlaps the MMAs of tile t + 1;
-//   * the gather producers (8 warps, a thread = a 16-byte piece of 4 rows) never wait for their own copies: after
-//     the cp.asyncs of a K-block each thread posts cp.async.mbarrier.arrive.noinc on the stage's full barrier, which the
-//     hardware fires when that thread's copies have landed.  No cp.async group wait, no per-stage proxy fence in the
-//     producers (round 1's limiter: the fence drained every copy the thread still had in flight), no elected arrive.
-//     The generic->async proxy fence is executed once per stage by the MMA warp AFTER it has acquired the barrier.
-// Shared memory: 28 slots of 8 KB = kblocks resident weight images (128 x 64 B, SWIZZLE_64B) + n_stages X stages of two
-// slots (256 x 64 B); K = 608 gives 19 + 4 x 2.
-// ---------------------------------------------------------------------------------------------------------------------
-// Two operand geometries (template): <KC = 32, NT = 256>: 64-byte row pieces (SWIZZLE_64B), 256-row tiles as described
-// above; <KC = 64, NT = 128>: 128-byte row pieces (SWIZZLE_128B; one whole 128-byte line per row per K-block, half as
-// many gather requests per byte), 128-row tiles, K padded to a multiple of 64.
-constexpr int MPW_SMEM_BYTES = 28 * MP_IMG;      // operand ring: resident weight images + X stages
-constexpr int MPW_MAX_STAGES = 8;
-constexpr int MPW_SMEM = MPW_SMEM_BYTES + 1024;
-
-template <int KC>
-__host__ __device__ __forceinline__ uint32_t mpw_off(int r, int c) {
-  if constexpr (KC == 32) return sw64_off(r, c);
-  else return sw128_off(r, c);
-}
-template <int KC>
-__device__ __forceinline__ uint64_t mpw_desc(uint32_t saddr) {
-  if constexpr (KC == 32) return make_smem_desc64(saddr);
-  else return make_smem_desc(saddr);
-}
-
-// Wm [K, hidden] row-major fp32 -> bf16 tile images of Wm^T for the <KC = 64> geometry (128 hidden rows x 64 k, K-major, SW128)
-__global__ void __launch_bounds__(256) maxpool_pack128_kernel(const float* __restrict__ W, int64_t ldw, int K, int hidden,
-                                                              int kblocks, unsigned char* __restrict__ img) {
-  const int slice = blockIdx.x / kblocks, kb = blockIdx.x % kblocks;
-  unsigned char* dst = img + ((int64_t)slice * kblocks + kb) * (2 * MP_IMG);
   for (int q = threadIdx.x; q < 128 * 8; q += blockDim.x) {
     const int c = q >> 7, n = q & 127;
-    const int gn = slice * 128 + n, k0 = kb * 64 + c * 8;
+    const int gn = slice * 128 + n, k0 = kb * MP_KCOLS + c * 8;
     __nv_bfloat162 h[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
@@ -445,1495 +70,240 @@ __global__ void __launch_bounds__(256) maxpool_pack128_kernel(const float* __res
   }
 }
 
-__device__ __forceinline__ void tma_gather4(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int col, int r0, int r1,
-                                            int r2, int r3);
-__device__ __forceinline__ void tma_gather4_multicast(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, uint16_t mask,
-                                                      int col, int r0, int r1, int r2, int r3);
-__device__ __forceinline__ uint32_t cluster_ctarank();
-__device__ __forceinline__ void cluster_sync_all();
-
-// table row of tile row r of a CTA's local tile tl (padding rows of a tile read row 0: finite data the epilogue never
-// looks at)
-__device__ __forceinline__ int mpw_row_of(const MpParams& prm, int64_t tile0, int64_t tile_step, int64_t my_tiles,
-                                          int rows_valid, int64_t total_rows, int64_t tl, int r) {
-  const int64_t t = tile0 + tl * tile_step;
-  const int64_t flat = t * rows_valid + r;          // index into the (group, j) row list
-  int64_t id = 0;
-  if (tl < my_tiles && r < rows_valid && flat < total_rows) {
-    id = prm.row_ids ? (int64_t)prm.row_ids[flat] : prm.row0 + flat;
-    if (id < 0 || id >= prm.n_rows) id = prm.n_rows - 1;
-  }
-  return (int)id;
-}
-
-// cp.async gather producers: PW warps in two groups that alternate K-blocks (a group fills a whole stage, so two stages
-// are being filled at any time).  A thread owns one 16-byte chunk column of RPP-strided tile rows, keeps the row pointers
-// in registers and only adds the K-block step per copy.  Hand-off = cp.async groups + one elected arrive per warp, with
-// n_stages / 2 - 1 K-blocks in flight per thread; the generic->async proxy fence is on the consumer side.
-template <int KC, int NT, int PW>
-__device__ __forceinline__ void mpw_cpasync_producers(const MpParams& prm, int warp, int lane, int n_stages,
-                                                      unsigned char* x_ring, uint64_t* full_x, uint64_t* empty_x, int64_t tile0,
-                                                      int64_t tile_step, int64_t my_tiles, int rows_valid, int64_t total_rows) {
-  constexpr int ROWB = KC * 2;
-  constexpr int X_IMG = NT * ROWB;
-  const int kblocks = prm.kblocks;
-  auto row_of = [&](int64_t tl, int r) -> int { return mpw_row_of(prm, tile0, tile_step, my_tiles, rows_valid, total_rows, tl, r); };
-  {
-    constexpr int GT = PW * 32 / 2;               // threads per group
-    constexpr int TPR = ROWB / 16;                // threads per row piece (4 or 8)
-    constexpr int RPP = GT / TPR;                 // tile rows per pass of a group
-    constexpr int PASSES = NT / RPP;              // copies per thread per stage
-    static_assert(PASSES * RPP == NT && (PASSES == 8 || PASSES == 16), "a group fills a stage with 8 or 16 copies per thread");
-    const int grp = warp / (PW / 2);
-    const int tg = threadIdx.x - grp * GT;
-    const int c = tg % TPR, r0 = tg / TPR;
-    const uint32_t off0 = mpw_off<KC>(r0, c);     // + i * RPP * ROWB for pass i (the swizzle term only depends on r0)
-    const int64_t total_it = my_tiles * kblocks;
-    const int tail_bytes = (prm.K % KC) ? min(16, max(0, (prm.K - ((kblocks - 1) * KC + c * 8)) * 2)) : 16;
-    // Row ids are fetched a whole tile ahead in two steps: `request` only issues the loads (raw values, nothing depends on
-    // them), `finish` clamps them when the tile is reached.  (With load + clamp in one step ptxas consumed every id right
-    // after its load - eight serialised L2 round trips, ~4000 cycles, at every tile boundary.)
-    int raw[PASSES];
-    auto request = [&](int64_t tl) {
-      const int64_t t = tile0 + tl * tile_step;
-#pragma unroll
-      for (int i = 0; i < PASSES; ++i) {
-        const int r = r0 + RPP * i;
-        const int64_t flat = t * rows_valid + r;    // index into the (group, j) row list
-        const bool live = tl < my_tiles && r < rows_valid && flat < total_rows;
-        int v = 0;                                  // padding rows of a tile read row 0 (finite data, never looked at)
-        if (live) v = prm.row_ids ? __ldg(prm.row_ids + flat) : (int)(prm.row0 + flat);
-        raw[i] = v;
-      }
-    };
-    const unsigned char* rowp[PASSES];
-    auto finish = [&](int kb) {                     // clamp (as gs_gather_rows: out-of-range ids read the last row) -> row pointers
-#pragma unroll
-      for (int i = 0; i < PASSES; ++i) {
-        int id = raw[i];
-        if (id < 0 || (int64_t)id >= prm.n_rows) id = (int)(prm.n_rows - 1);
-        rowp[i] = reinterpret_cast<const unsigned char*>(prm.table + (int64_t)id * prm.pitch) + (size_t)kb * ROWB + c * 16;
-      }
-    };
-    int64_t tl = 0;
-    int kb = grp;
-    while (kb >= kblocks) { kb -= kblocks; ++tl; }
-    request(tl);
-    finish(kb);
-    request(tl + 1);
-    const int depth = min(6, max(1, n_stages / 2 - 1));   // K-blocks a group keeps in flight (its share of the ring minus one)
-    uint32_t s = grp % n_stages, ph = 0, s_old = s;
-    int pending = 0;
-    auto hand_over = [&]() {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_x[s_old]);
-      s_old += 2;
-      while (s_old >= (uint32_t)n_stages) s_old -= n_stages;
-      --pending;
-    };
-    for (int64_t it = grp; it < total_it; it += 2) {
-      mbar_wait(&empty_x[s], ph ^ 1u);
-      const uint32_t dst = smem_u32(x_ring + (size_t)s * X_IMG) + off0;
-      if (kb == kblocks - 1 && tail_bytes != 16) {
-#pragma unroll
-        for (int i = 0; i < PASSES; ++i)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + i * RPP * ROWB),
-                       "l"(tail_bytes ? (const void*)rowp[i] : (const void*)prm.table), "r"(tail_bytes) : "memory");
-      } else {
-#pragma unroll
-        for (int i = 0; i < PASSES; ++i)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + i * RPP * ROWB), "l"(rowp[i]) : "memory");
-      }
-      cp_async_commit();
-      if (++pending > depth) {
-        switch (depth) {                          // the oldest of this thread's K-blocks has landed
-          case 1: cp_async_wait<1>(); break;
-          case 2: cp_async_wait<2>(); break;
-          case 3: cp_async_wait<3>(); break;
-          case 4: cp_async_wait<4>(); break;
-          case 5: cp_async_wait<5>(); break;
-          default: cp_async_wait<6>(); break;
-        }
-        hand_over();
-      }
-      s += 2;
-      while (s >= (uint32_t)n_stages) { s -= n_stages; ph ^= 1u; }
-      kb += 2;
-      if (kb >= kblocks) {                        // next tile (two tiles on when a tile is a single K-block)
-        int adv = 0;
-        while (kb >= kblocks) { kb -= kblocks; ++adv; }
-        tl += adv;
-        if (adv != 1) request(tl);                // (single-K-block tiles: the prefetched tile is not the next one)
-        finish(kb);
-        request(tl + 1);                          // in flight while this tile's K-blocks are copied
-      } else {
-#pragma unroll
-        for (int i = 0; i < PASSES; ++i) rowp[i] += 2 * ROWB;
-      }
-    }
-    while (pending > 0) {                         // drain: hand the remaining K-blocks over, oldest first
-      switch (pending) {
-        case 1: cp_async_wait<0>(); break;
-        case 2: cp_async_wait<1>(); break;
-        case 3: cp_async_wait<2>(); break;
-        case 4: cp_async_wait<3>(); break;
-        case 5: cp_async_wait<4>(); break;
-        case 6: cp_async_wait<5>(); break;
-        default: cp_async_wait<6>(); break;
-      }
-      hand_over();
-    }
-  }
-}
-
-// PROD 0: cp.async gather producers - 8 warps in two groups that alternate K-blocks (a group fills a whole stage, so
-//         two stages are being filled at any time); a thread owns one 16-byte chunk column of RPP-strided tile rows,
-//         keeps the row pointers in registers and only adds the K-block step per copy (the first version recomputed
-//         addresses, tail predicates and swizzle offsets per copy: ~100 instructions per stage per warp, and with every
-//         warp taking part in every stage that instruction latency - not memory, not the barriers - set the stage rate:
-//         1070 cycles per stage against 256 cycles of MMA, identical with the copies removed);
-//         hand-off = cp.async groups + one elected arrive per warp; the generic->async proxy fence is consumer-side.
-// PROD 1: TMA producers - 4 warps, warp w owns ring slot w; per stage each lane issues ONE
-//         cp.async.bulk.tensor.2d.tile::gather4 (four table rows named by index, 128 bytes each, SWIZZLE_128B applied by
-//         the tensor map, columns >= K zero-filled) completing on the stage's mbarrier transaction count: no address
-//         arithmetic, no cp.async groups, no proxy fence, no arrives.  Needs NT == 128 (32 lanes x 4 rows) and 4 stages.
-template <int KC, int NT, int PROD>
-struct MpwCfg {
-  static constexpr int PW = PROD == 1 ? 4 : 8;             // producer warps
-  static constexpr int THREADS = (PW + 6) * 32;
-};
-
-template <int KC, int NT, int PROD>
-__global__ void __launch_bounds__(MpwCfg<KC, NT, PROD>::THREADS, 1)
-    maxpool_mlp_wide_kernel(const __grid_constant__ MpParams prm, const __grid_constant__ CUtensorMap tmap) {
-  constexpr int PW = MpwCfg<KC, NT, PROD>::PW;
-  constexpr int ROWB = KC * 2;                    // bytes of one operand row per K-block (64 or 128)
-  constexpr int W_IMG = 128 * ROWB;               // resident weight image of one K-block
-  constexpr int X_IMG = NT * ROWB;                // one X stage
-  static_assert(PROD == 0 || (NT == 128 && KC == 64), "the gather4 producers fill a 128-row SWIZZLE_128B stage per warp");
+template <bool kRowsA, int NT, int DEPTH, int PROD>
+__global__ void __launch_bounds__(MP_THREADS, NT == 128 ? 2 : 1) maxpool_mlp_kernel(const __grid_constant__ MpParams prm) {
+  constexpr int ROWS_IMG = NT * 128;                      // gathered rows of one K-block
+  constexpr int STAGE = ROWS_IMG + MP_IMG;                // rows image, then the weight image
+  constexpr int CPT = NT / 32;                            // 16-byte row pieces per thread per K-block
+  constexpr int LOOK = MP_STAGES - DEPTH;                 // K-blocks prefetched ahead of the one being multiplied
+  constexpr int MI = kRowsA ? NT / 128 : 1;               // m64 blocks per warpgroup
+  constexpr int NI = kRowsA ? 1 : NT / 128;               // n128 blocks
+  constexpr int LD = NT + 1;                              // staging: [128 hidden][NT + 1]
+  static_assert(128 * LD * 4 <= MP_STAGES * STAGE, "epilogue staging must fit in the operand ring");
+  static_assert(LOOK >= 1, "at least one K-block of prefetch");
   extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_x[MPW_MAX_STAGES], empty_x[MPW_MAX_STAGES], acc_full[2], acc_empty[2], w_full;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t full_b[MP_STAGES];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int kblocks = prm.kblocks;
-  const int n_stages = prm.n_stages;
-  unsigned char* w_res = smem;                                        // resident weight slice: kblocks images
-  unsigned char* x_ring = smem + MPW_SMEM_BYTES - (size_t)n_stages * X_IMG;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31, wq = (tid >> 5) & 3;
   const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int k = prm.k, G = prm.G;
-  const int rows_valid = G * k;
-  const int64_t total_rows = prm.n_groups * (int64_t)k;
-  const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
+  const int64_t t = blockIdx.x / prm.n_slices;
+  const int kblocks = prm.kblocks;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MPW_MAX_STAGES; ++s) {
-      mbar_init(&full_x[s], PROD == 1 ? 1 : PW / 2);  // gather4: the expect_tx arrive; cp.async: one arrive per warp of the group
-      mbar_init(&empty_x[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);                  // one arrive per epilogue warp
-    }
-    mbar_init(&w_full, 1);
+  if (tid == 0) {
+    for (int s = 0; s < MP_STAGES; ++s) mbar_init(&full_b[s], 1);
     fence_mbar_init();
   }
-  if (warp == PW + 1) {
-    tmem_alloc(&tmem_base_smem, 2 * NT);            // two 128-lane x NT-column fp32 accumulators
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  auto row_of = [&](int64_t tl, int r) -> int { return mpw_row_of(prm, tile0, tile_step, my_tiles, rows_valid, total_rows, tl, r); };
+  // this thread's 16-byte chunk column c of tile rows r0 + 32 i (padding rows and rows past the last group: zero-filled)
+  const int c = tid & 7, r0 = tid >> 3;
+  const int rows_valid = prm.G * prm.k;
+  const __nv_bfloat16* rowp[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) {
+    const int r = r0 + 32 * i;
+    const int64_t flat = t * rows_valid + r;        // index into the (group, j) row list
+    rowp[i] = nullptr;
+    if (r < rows_valid && flat < prm.n_groups * prm.k) {
+      int64_t id = prm.row_ids ? (int64_t)prm.row_ids[flat] : prm.row0 + flat;
+      if (id < 0 || id >= prm.n_rows) id = prm.n_rows - 1;
+      rowp[i] = prm.table + id * prm.pitch;
+    }
+  }
+  const unsigned char* wsrc = prm.wimg + (int64_t)slice * kblocks * MP_IMG;
+  auto stage_of = [&](int kb) { return smem + (size_t)(kb % MP_STAGES) * STAGE; };
+  // weight image by bulk copy (+ the row pieces by cp.async in the PROD 0 form) of K-block kb into its stage
+  auto issue = [&](int kb) {
+    if (kb < kblocks) {
+      unsigned char* st = stage_of(kb);
+      if (tid == 0) {
+        mbar_expect_tx(&full_b[kb % MP_STAGES], MP_IMG);
+        bulk_g2s(st + ROWS_IMG, wsrc + (int64_t)kb * MP_IMG, MP_IMG, &full_b[kb % MP_STAGES]);
+      }
+      if constexpr (PROD == 0) {
+        const int col = kb * MP_KCOLS + c * 8;      // first bf16 column of this 16-byte piece
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) {
+          int nbytes = 0;
+          if (rowp[i] != nullptr && col < prm.K) nbytes = min(8, prm.K - col) * 2;
+          const void* src = nbytes ? (const void*)(rowp[i] + col) : (const void*)prm.table;
+          cp_async16(st + sw128_off(r0 + 32 * i, c), src, nbytes);
+        }
+      }
+    }
+    if constexpr (PROD == 0) cp_async_commit();    // empty groups keep the group count uniform
+  };
+  uint4 regs[PROD == 1 ? CPT : 1];
+  auto load_regs = [&](int kb) {                    // PROD 1: K-block kb's pieces into registers
+    const int col = kb * MP_KCOLS + c * 8;
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) {
+      regs[i] = make_uint4(0, 0, 0, 0);
+      if (rowp[i] == nullptr || col >= prm.K) continue;
+      if (col + 8 <= prm.K) {
+        regs[i] = __ldg(reinterpret_cast<const uint4*>(rowp[i] + col));
+      } else {
+        unsigned short h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const unsigned short* src = reinterpret_cast<const unsigned short*>(rowp[i] + col);
+        for (int e = 0; e < prm.K - col; ++e) h[e] = __ldg(src + e);
+        regs[i] = *reinterpret_cast<const uint4*>(h);
+      }
+    }
+  };
 
-  if (warp < PW && prm.dbg != 3) {
+  for (int j = 0; j < LOOK; ++j) issue(j);
+  if constexpr (PROD == 1) load_regs(0);
+  float acc[MI * NI][64];
+#pragma unroll
+  for (int a = 0; a < MI * NI; ++a)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[a][i] = 0.f;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    unsigned char* st = stage_of(kb);
     if constexpr (PROD == 0) {
-      mpw_cpasync_producers<KC, NT, PW>(prm, warp, lane, n_stages, x_ring, full_x, empty_x, tile0, tile_step, my_tiles,
-                                        rows_valid, total_rows);
+      cp_async_wait<LOOK - 1>();                    // this thread's pieces of K-block kb have landed
     } else {
-      // =============================== gather producers (TMA tile::gather4) ===============================
-      const int64_t total_it = my_tiles * kblocks;
-      int cur[4], nxt[4];                           // table rows of this lane's tile rows 4 lane .. 4 lane + 3
-      auto load_ids = [&](int64_t tl, int (&ids)[4]) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) ids[i] = row_of(tl, 4 * lane + i);
-      };
-      int64_t tl = 0;
-      int kb = warp;
-      while (kb >= kblocks) { kb -= kblocks; ++tl; }
-      load_ids(tl, cur);
-      load_ids(tl + 1, nxt);
-      const int slot = warp;                        // this warp's ring slot (n_stages == PW)
-      uint32_t fill = 0;
-      for (int64_t it = warp; it < total_it; it += PW, ++fill) {
-        mbar_wait(&empty_x[slot], (fill & 1u) ^ 1u);
-        if (lane == 0) mbar_expect_tx(&full_x[slot], (uint32_t)X_IMG);
-        __syncwarp();
-        tma_gather4(x_ring + (size_t)slot * X_IMG + (size_t)lane * 4 * ROWB, &tmap, &full_x[slot], kb * KC, cur[0], cur[1],
-                    cur[2], cur[3]);
-        kb += PW;
-        if (kb >= kblocks) {
-          int adv = 0;
-          while (kb >= kblocks) { kb -= kblocks; ++adv; }
-          tl += adv;
-          if (adv == 1) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
-          } else {
-            load_ids(tl, cur);
-          }
-          load_ids(tl + 1, nxt);
-        }
-      }
+      for (int i = 0; i < CPT; ++i) *reinterpret_cast<uint4*>(st + sw128_off(r0 + 32 * i, c)) = regs[i];
     }
-  } else if (warp < PW) {
-    // timing probe: producers idle
-  } else if (warp == PW) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(1u, 128, NT);               // bf16 x bf16 -> fp32, M = 128, N = NT
-    mbar_wait(&w_full, 0);
-    uint32_t s = 0, ph = 0, tcount = 0;
-    for (int64_t t = tile0; t < prm.n_tiles; t += tile_step, ++tcount) {
-      const uint32_t buf = tcount & 1u;
-      mbar_wait(&acc_empty[buf], ((tcount >> 1) & 1u) ^ 1u);          // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        if (prm.dbg != 3) {
-          mbar_wait(&full_x[s], ph);
-          if constexpr (PROD == 0) fence_proxy_async();               // cp.async wrote the stage through the generic proxy
-          tc_fence_after();
-        }
-        const uint64_t adesc = mpw_desc<KC>(smem_u32(w_res + (size_t)kb * W_IMG));
-        const uint64_t bdesc = mpw_desc<KC>(smem_u32(x_ring + (size_t)s * X_IMG));
-        if (prm.dbg != 4) {
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)      // K = 16 per instruction, 32 B apart inside the swizzle atom
-            umma_ss_elect<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc,
-                                (kb > 0 || k2 > 0) ? 1u : 0u);
-        }
-        umma_commit_elect(&empty_x[s]);
-        if (kb == kblocks - 1) umma_commit_elect(&acc_full[buf]);
-        __syncwarp();
-        if (++s == (uint32_t)n_stages) { s = 0; ph ^= 1u; }
-      }
+    fence_proxy_async();                            // generic-proxy writes -> visible to wgmma (async proxy)
+    __syncthreads();                                // everyone's pieces are in; K-block kb - DEPTH's stage is free
+    issue(kb + LOOK);
+    if constexpr (PROD == 1) {
+      if (kb + 1 < kblocks) load_regs(kb + 1);
     }
-  } else if (warp == PW + 1) {
-    // =============================== resident weight slice ===============================
-    if (lane == 0) {
-      mbar_expect_tx(&w_full, (uint32_t)(kblocks * W_IMG));
-      const unsigned char* src = prm.wimg + (int64_t)slice * kblocks * W_IMG;
-      for (int kb = 0; kb < kblocks; ++kb) bulk_g2s(w_res + (size_t)kb * W_IMG, src + (int64_t)kb * W_IMG, W_IMG, &w_full);
-    }
-    __syncwarp();
-  } else {
-    // =============================== epilogue ===============================
-    const int q = warp & 3;                         // TMEM lane quarter of this warp (four consecutive warps cover 0..3)
-    const int h = slice * 128 + q * 32 + lane;      // this thread's hidden unit = its TMEM lane
-    const float b = prm.bias ? prm.bias[h] : 0.f;
-    const float inv_k = 1.0f / (float)k;
-    uint32_t tcount = 0;
-    for (int64_t t = tile0; t < prm.n_tiles; t += tile_step, ++tcount) {
-      const uint32_t buf = tcount & 1u;
-      const int64_t g_base = t * G;
-      const int groups_here = (int)min((int64_t)G, prm.n_groups - g_base);
-      mbar_wait(&acc_full[buf], (tcount >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT + ((uint32_t)(q * 32) << 16);
-      float* outp = prm.out + g_base * prm.ldo + h;
-      // One fanout group = k consecutive accumulator columns of this lane.  Each group is fetched from TMEM by itself, in
-      // pieces of 32 / 16 / 8 / 4 / 2 / 1 columns chosen by the bits of k (k = 25: x16 + x8 + x1), so every register is
-      // statically indexed and the pooling is straight-line FMNMX / FADD code; only the piece selection branches, and
-      // that is warp-uniform.  (Pooling fixed 32-column chunks with a running counter cost a compare + branch region per
-      // ELEMENT: the four epilogue warps were busy 85 % of the kernel and, not the producers, set the tile rate.)
-      const bool mean = prm.pool_mean != 0;
-      auto fold = [&](float m, uint32_t x) -> float {
-        const float v = __uint_as_float(x);
-        // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU are applied
-        // per element and summed in j order; max-pool: bias + ReLU after the max (they commute with it)
-        return mean ? m + fmaxf(v + b, 0.f) : fmaxf(m, v);
-      };
-      for (int g = 0; g < groups_here; ++g) {
-        uint32_t col = tmem_acc + (uint32_t)(g * k);
-        float m = mean ? 0.f : -3.0e38f;
-        int rem = k;
-        while (rem >= 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(col, r);
-          tmem_ld_wait();
+    mbar_wait(&full_b[kb % MP_STAGES], (uint32_t)(kb / MP_STAGES) & 1u);
+    const uint32_t rows_s = smem_u32(st), w_s = smem_u32(st + ROWS_IMG);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) m = fold(m, r[j]);
-          col += 32u;
-          rem -= 32;
-        }
-        uint32_t r16[16], r8[8], r4[4], r2[2], r1[1];
-        uint32_t cc = col;
-        if (rem & 16) { tmem_ld_32x16(cc, r16); cc += 16u; }
-        if (rem & 8) { tmem_ld_32x8(cc, r8); cc += 8u; }
-        if (rem & 4) { tmem_ld_32x4(cc, r4); cc += 4u; }
-        if (rem & 2) { tmem_ld_32x2(cc, r2); cc += 2u; }
-        if (rem & 1) { tmem_ld_32x1(cc, r1); }
-        tmem_ld_wait();
-        if (rem & 16) {
+    for (int a = 0; a < MI * NI; ++a) acc_fence(acc[a]);
+    wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) m = fold(m, r16[j]);
-        }
-        if (rem & 8) {
+    for (int k = 0; k < 4; ++k)                     // four K = 16 steps, 32 B apart inside the swizzle atom
 #pragma unroll
-          for (int j = 0; j < 8; ++j) m = fold(m, r8[j]);
-        }
-        if (rem & 4) {
+      for (int mi = 0; mi < MI; ++mi)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) m = fold(m, r4[j]);
+        for (int ni = 0; ni < NI; ++ni) {
+          const uint64_t adesc = kRowsA ? make_smem_desc(rows_s + (uint32_t)((wg * (NT / 2) + mi * 64) * 128))
+                                        : make_smem_desc(w_s + (uint32_t)(wg * 64 * 128));
+          const uint64_t bdesc = kRowsA ? make_smem_desc(w_s) : make_smem_desc(rows_s + (uint32_t)(ni * 128 * 128));
+          wgmma_m64n128<true>(acc[mi * NI + ni], adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2),
+                              (kb > 0 || k > 0) ? 1u : 0u);
         }
-        if (rem & 2) {
-          m = fold(m, r2[0]);
-          m = fold(m, r2[1]);
-        }
-        if (rem & 1) m = fold(m, r1[0]);
-        outp[(int64_t)g * prm.ldo] = mean ? m * inv_k : fmaxf(m + b, 0.f);
-      }
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
+    wgmma_commit();
+    wgmma_wait<DEPTH - 1>();
+#pragma unroll
+    for (int a = 0; a < MI * NI; ++a) acc_fence(acc[a]);
   }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int a = 0; a < MI * NI; ++a) acc_fence(acc[a]);
+  if constexpr (PROD == 0) cp_async_wait<0>();
+  __syncthreads();                                  // the operand ring becomes the staging tile
+
+  // =============================== epilogue ===============================
+  // raw accumulators go to the staging tile [hidden][row]; bias and ReLU are applied AFTER the max
+  // (max_j relu(x_j + b) == relu(max_j x_j + b): b is per column, relu is monotone)
+  float* stage = reinterpret_cast<float*>(smem);
+#pragma unroll
+  for (int mi = 0; mi < MI; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < NI; ++ni)
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int m = wq * 16 + (lane >> 2) + 8 * (e >> 1);       // accumulator row within the m64 block
+          const int n = 8 * j + 2 * (lane & 3) + (e & 1);           // accumulator column within the n128 block
+          const int row = kRowsA ? wg * (NT / 2) + mi * 64 + m : ni * 128 + n;
+          const int col = kRowsA ? n : wg * 64 + m;
+          stage[col * LD + row] = acc[mi * NI + ni][4 * j + e];
+        }
   __syncthreads();
-  if (warp == PW + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * NT);
-  }
-}
-
-// cp.async gather producers for the two-pipeline kernel: group g (PW / 2 warps) serves pipeline g alone - the CTA's local
-// tiles g, g + 2, ... - through its own ring of n_half stages (full / empty barriers and stage memory passed in already
-// offset).  Otherwise as mpw_cpasync_producers: a thread owns one 16-byte chunk column of RPP-strided tile rows, row
-// pointers stay in registers, ids are requested a tile ahead, hand-off by cp.async groups + one elected arrive per warp.
-template <int KC, int NT, int PW>
-__device__ __forceinline__ void mpw_cpasync_pipeline_producers(const MpParams& prm, int grp, int tg, int lane, int n_half,
-                                                               unsigned char* ring, uint64_t* full_x, uint64_t* empty_x,
-                                                               int64_t tile0, int64_t tile_step, int64_t my_tiles,
-                                                               int rows_valid, int64_t total_rows) {
-  constexpr int ROWB = KC * 2;
-  constexpr int X_IMG = NT * ROWB;
-  constexpr int GT = PW * 32 / 2;                 // threads per group
-  constexpr int TPR = ROWB / 16;                  // threads per row piece
-  constexpr int RPP = GT / TPR;                   // tile rows per pass of a group
-  constexpr int PASSES = NT / RPP;                // copies per thread per stage
-  static_assert(PASSES * RPP == NT && (PASSES == 8 || PASSES == 16), "a group fills a stage with 8 or 16 copies per thread");
-  const int kblocks = prm.kblocks;
-  const int c = tg % TPR, r0 = tg / TPR;
-  const uint32_t off0 = mpw_off<KC>(r0, c);
-  const int tail_bytes = (prm.K % KC) ? min(16, max(0, (prm.K - ((kblocks - 1) * KC + c * 8)) * 2)) : 16;
-  int raw[PASSES];
-  auto request = [&](int64_t tl) {
-    const int64_t t = tile0 + tl * tile_step;
-#pragma unroll
-    for (int i = 0; i < PASSES; ++i) {
-      const int r = r0 + RPP * i;
-      const int64_t flat = t * rows_valid + r;
-      const bool live = tl < my_tiles && r < rows_valid && flat < total_rows;
-      int v = 0;
-      if (live) v = prm.row_ids ? __ldg(prm.row_ids + flat) : (int)(prm.row0 + flat);
-      raw[i] = v;
-    }
-  };
-  const unsigned char* rowp[PASSES];
-  auto finish = [&]() {
-#pragma unroll
-    for (int i = 0; i < PASSES; ++i) {
-      int id = raw[i];
-      if (id < 0 || (int64_t)id >= prm.n_rows) id = (int)(prm.n_rows - 1);
-      rowp[i] = reinterpret_cast<const unsigned char*>(prm.table + (int64_t)id * prm.pitch) + c * 16;
-    }
-  };
-  const int depth = min(6, max(1, n_half - 1));   // K-blocks kept in flight per thread
-  uint32_t s = 0, ph = 0, s_old = 0;
-  int pending = 0;
-  auto hand_over = [&]() {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&full_x[s_old]);
-    if (++s_old == (uint32_t)n_half) s_old = 0;
-    --pending;
-  };
-  request(grp);
-  for (int64_t tl = grp; tl < my_tiles; tl += 2) {
-    finish();
-    request(tl + 2);                              // in flight while this tile's K-blocks are copied
-    for (int kb = 0; kb < kblocks; ++kb) {
-      mbar_wait(&empty_x[s], ph ^ 1u);
-      const uint32_t dst = smem_u32(ring + (size_t)s * X_IMG) + off0;
-      if (kb == kblocks - 1 && tail_bytes != 16) {
-#pragma unroll
-        for (int i = 0; i < PASSES; ++i)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + i * RPP * ROWB),
-                       "l"(tail_bytes ? (const void*)rowp[i] : (const void*)prm.table), "r"(tail_bytes) : "memory");
-      } else {
-#pragma unroll
-        for (int i = 0; i < PASSES; ++i)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + i * RPP * ROWB), "l"(rowp[i]) : "memory");
-      }
-      cp_async_commit();
-      if (++pending > depth) {
-        switch (depth) {
-          case 1: cp_async_wait<1>(); break;
-          case 2: cp_async_wait<2>(); break;
-          case 3: cp_async_wait<3>(); break;
-          case 4: cp_async_wait<4>(); break;
-          case 5: cp_async_wait<5>(); break;
-          default: cp_async_wait<6>(); break;
-        }
-        hand_over();
-      }
-      if (++s == (uint32_t)n_half) { s = 0; ph ^= 1u; }
-#pragma unroll
-      for (int i = 0; i < PASSES; ++i) rowp[i] += ROWB;
-    }
-  }
-  while (pending > 0) {
-    switch (pending) {
-      case 1: cp_async_wait<0>(); break;
-      case 2: cp_async_wait<1>(); break;
-      case 3: cp_async_wait<2>(); break;
-      case 4: cp_async_wait<3>(); break;
-      case 5: cp_async_wait<4>(); break;
-      case 6: cp_async_wait<5>(); break;
-      default: cp_async_wait<6>(); break;
-    }
-    hand_over();
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// K4, "tmem" form (k4_kernel = 0, the default): the wide form with the resident weight slice moved out of shared memory.
-// What the wide kernels showed (tools/k4_matrix.py probes): with the 160 KB weight slice resident in shared memory only
-// FOUR 16 KB operand stages fit, and one trip of a stage round the ring - issue the gather, the data lands, the MMA warp
-// wakes, the MMAs retire, the commit frees the slot, the producers wake - takes ~4000 cycles whatever the producer
-// mechanism (cp.async, hardware-fired arrives, TMA gather4) and even with the copies removed: ~1000 cycles per stage
-// against 256 cycles of MMA.  The cure is more stages in flight, and the place for the weights is tensor memory:
-//   * the A operand of tcgen05.mma may live in TMEM (TS form).  A = this CTA's slice of Wm^T (128 hidden units = 128
-//     lanes; bf16 pairs, K / 2 columns): the first kb_t <= 8 K-blocks (256 columns) sit in TMEM beside the two 128-column
-//     accumulators, written once per CTA by the epilogue warps with tcgen05.st; any further K-blocks stay in shared memory
-//     (SS form) - K = 602 -> 8 in TMEM + 2 in shared memory;
-//   * shared memory then holds 12 operand stages (192 KB in flight per SM) instead of 4;
-//   * the MMA warp's waits are warp votes (mbar_wait_uniform) so that descriptor arithmetic stays in uniform registers:
-//     with a divergent wait loop in front of them ptxas wrapped every tcgen05.mma in R2UR + ELECT + VOTEU sequences and
-//     the issue loop alone ran at 154 cycles per MMA (64 is the tensor pipe's floor).
-// Geometry: 128-row tiles, 64-column K-blocks (128-byte row pieces, SWIZZLE_128B); producers = mpw_cpasync_producers.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int MPT_MAX_STAGES = 14;
-constexpr int MPT_PW = 8;
-constexpr int MPT_THREADS = (MPT_PW + 6) * 32;
-constexpr int MPT_IMG = 128 * 128;                // one K-block image: 128 rows x 128 B
-constexpr int MPT_ACOL0 = 256;                    // TMEM columns [0, 256): two accumulators; [256, 256 + 32 kb_t): weights
-constexpr int MPT_MAX_KB_T = 8;
-
-// Wm [K, hidden] row-major fp32 -> wT[hidden_padded][kblocks * 32] uint32: word j of row h = bf16(W[2j, h]) | bf16(W[2j+1, h]) << 16
-__global__ void __launch_bounds__(256) maxpool_pack_rows_kernel(const float* __restrict__ W, int64_t ldw, int K, int hidden,
-                                                                int words, uint32_t* __restrict__ out) {
-  const int64_t total = (int64_t)gridDim.y * 128 * words;
-  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < (int64_t)128 * words; q += (int64_t)gridDim.x * blockDim.x) {
-    const int hl = (int)(q % 128), j = (int)(q / 128);          // hidden fastest: coalesced reads of W rows
-    const int h = blockIdx.y * 128 + hl;
-    const float a = (h < hidden && 2 * j < K) ? W[(int64_t)(2 * j) * ldw + h] : 0.f;
-    const float b = (h < hidden && 2 * j + 1 < K) ? W[(int64_t)(2 * j + 1) * ldw + h] : 0.f;
-    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    out[((int64_t)blockIdx.y * 128 + hl) * words + j] = *reinterpret_cast<const uint32_t*>(&v);
-  }
-  (void)total;
-}
-
-// NT = 128: two 128-column accumulators (the epilogue of tile t overlaps the MMAs of tile t + 1).
-// NT = 256 (default): ONE 256-column accumulator and 256-row tiles.  The MMA warp - a single warp - needs ~860 cycles of
-// waits, fences, descriptor moves and commits per four-MMA K-block whatever N is (measured: with NT = 128 it was never
-// waiting for operands any more, yet the tensor pipe idled 70 % of the time); N = 256 doubles the tensor work behind each
-// of those instructions (128 cycles per MMA instead of 64).  The price is that the epilogue of a tile is no longer
-// hidden behind the next tile's MMAs (TMEM has no room for a second 256-column accumulator beside the weights).
-template <int NT>
-__global__ void __launch_bounds__(MPT_THREADS, 1) maxpool_mlp_tmem_kernel(const __grid_constant__ MpParams prm) {
-  constexpr int KC = 64;
-  constexpr int NBUF = NT == 128 ? 2 : 1;
-  constexpr int X_IMG = NT * 128;
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_x[MPT_MAX_STAGES], empty_x[MPT_MAX_STAGES], acc_full[2], acc_empty[2], w_full, wt_full;
-  __shared__ uint32_t tmem_base_smem;
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int kblocks = prm.kblocks, kb_t = prm.kb_t, kb_s = kblocks - kb_t;
-  const int n_stages = prm.n_stages;
-  unsigned char* w_res = smem;                                        // K-blocks kb_t.. of the weight slice (SS operands)
-  unsigned char* x_ring = smem + (size_t)kb_s * MPT_IMG;     // n_stages stages of X_IMG bytes
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
+  // thread = (column cc, group): consecutive threads take consecutive columns (conflict-free staging reads,
+  // coalesced stores)
   const int k = prm.k, G = prm.G;
-  const int rows_valid = G * k;
-  const int64_t total_rows = prm.n_groups * (int64_t)k;
-  const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MPT_MAX_STAGES; ++s) {
-      mbar_init(&full_x[s], MPT_PW / 2);            // one arrive per warp of the filling group
-      mbar_init(&empty_x[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);                  // one arrive per epilogue warp
-    }
-    mbar_init(&w_full, 1);
-    mbar_init(&wt_full, 4);                         // one arrive per epilogue warp (each writes its 32 TMEM lanes)
-    fence_mbar_init();
-  }
-  if (warp == MPT_PW + 1) {
-    tmem_alloc(&tmem_base_smem, 512);               // 2 x 128 accumulator columns + up to 256 weight columns
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp < MPT_PW) {
-    mpw_cpasync_producers<KC, NT, MPT_PW>(prm, warp, lane, n_stages, x_ring, full_x, empty_x, tile0, tile_step, my_tiles,
-                                          rows_valid, total_rows);
-  } else if (warp == MPT_PW) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(1u, 128, NT);               // bf16 x bf16 -> fp32, M = 128, N = 128
-    if (kb_s > 0) mbar_wait_uniform(&w_full, 0);
-    if (kb_t > 0) mbar_wait_uniform(&wt_full, 0);
-    tc_fence_after();
-    const uint32_t x_base = smem_u32(x_ring), w_base = smem_u32(w_res);
-    uint32_t s = 0, ph = 0;
-    for (int64_t tl = 0; tl < my_tiles; ++tl) {
-      const uint32_t buf = NBUF == 2 ? ((uint32_t)tl & 1u) : 0u;
-      const uint32_t use = (uint32_t)(NBUF == 2 ? (tl >> 1) : tl);          // how often this accumulator has been used before
-      mbar_wait_uniform(&acc_empty[buf], (use & 1u) ^ 1u);                  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait_uniform(&full_x[s], ph);
-        fence_proxy_async();                        // cp.async wrote the stage through the generic proxy
-        tc_fence_after();
-        const uint64_t bdesc = make_smem_desc(x_base + s * (uint32_t)X_IMG);
-        if (kb < kb_t) {
-          const uint32_t a_t = tmem_base + (uint32_t)MPT_ACOL0 + (uint32_t)kb * 32u;
+  for (int u = tid; u < TC_BN * G; u += MP_THREADS) {
+    const int cc = u & (TC_BN - 1), g = u / TC_BN;
+    const int64_t gg = t * G + g;
+    if (gg >= prm.n_groups) break;
+    const float* p = stage + cc * LD + g * k;
+    const int hcol = slice * 128 + cc;
+    const float b = prm.bias ? prm.bias[hcol] : 0.f;
+    float res;
+    if (prm.pool_mean) {
+      // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU
+      // are applied per element, summed in j order, divided by k
+      float sacc = 0.f;
+      for (int j = 0; j < k; ++j) sacc += fmaxf(p[j] + b, 0.f);
+      res = sacc / (float)k;
+    } else {
+      float m = -3.0e38f;
+      int j = 0;
+      for (; j + 8 <= k; j += 8) {
+        float v[8];
 #pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)      // K = 16 per instruction: 8 TMEM columns of A, 32 B of B inside the atom
-            umma_ts_elect_bf16(tmem_acc, a_t + (uint32_t)(k2 * 8), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        } else {
-          const uint64_t adesc = make_smem_desc(w_base + (uint32_t)(kb - kb_t) * (uint32_t)MPT_IMG);
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)
-            umma_ss_elect<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        }
-        umma_commit_elect(&empty_x[s]);
-        if (kb == kblocks - 1) umma_commit_elect(&acc_full[buf]);
-        if (++s == (uint32_t)n_stages) { s = 0; ph ^= 1u; }
+        for (int w = 0; w < 8; ++w) v[w] = p[j + w];
+        m = fmaxf(m, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
       }
+      for (; j < k; ++j) m = fmaxf(m, p[j]);
+      res = fmaxf(m + b, 0.f);                      // Dense bias + ReLU (commute with the max)
     }
-  } else if (warp == MPT_PW + 1) {
-    // =============================== shared-memory part of the weight slice ===============================
-    if (lane == 0 && kb_s > 0) {
-      mbar_expect_tx(&w_full, (uint32_t)(kb_s * MPT_IMG));
-      const unsigned char* src = prm.wimg + ((int64_t)slice * kblocks + kb_t) * MPT_IMG;
-      for (int kb = 0; kb < kb_s; ++kb) bulk_g2s(w_res + (size_t)kb * MPT_IMG, src + (int64_t)kb * MPT_IMG, MPT_IMG, &w_full);
-    }
-    __syncwarp();
-  } else {
-    // =============================== epilogue warps ===============================
-    const int q = warp & 3;                         // TMEM lane quarter of this warp (four consecutive warps cover 0..3)
-    const int h = slice * 128 + q * 32 + lane;      // this thread's hidden unit = its TMEM lane
-    // once: this lane's row of Wm^T (bf16 pairs) for the first kb_t K-blocks -> tensor memory (A operand, TS form)
-    {
-      const uint32_t* wrow = prm.wrows + (int64_t)h * (kblocks * 32);
-      const uint32_t t_a = tmem_base + (uint32_t)MPT_ACOL0 + ((uint32_t)(q * 32) << 16);
-      for (int cb = 0; cb < kb_t; ++cb) {
-        uint32_t r[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 v = __ldg(reinterpret_cast<const uint4*>(wrow + cb * 32) + j);
-          r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
-        }
-        tmem_st_32x32(t_a + (uint32_t)(cb * 32), r);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&wt_full);
-    }
-    const float b = prm.bias ? prm.bias[h] : 0.f;
-    const float inv_k = 1.0f / (float)k;
-    const bool mean = prm.pool_mean != 0;
-    auto fold = [&](float m, uint32_t x) -> float {
-      const float v = __uint_as_float(x);
-      // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU are applied
-      // per element and summed in j order; max-pool: bias + ReLU after the max (they commute with it)
-      return mean ? m + fmaxf(v + b, 0.f) : fmaxf(m, v);
-    };
-    for (int64_t tl = 0; tl < my_tiles; ++tl) {
-      const int64_t t = tile0 + tl * tile_step;
-      const uint32_t buf = NBUF == 2 ? ((uint32_t)tl & 1u) : 0u;
-      const uint32_t use = (uint32_t)(NBUF == 2 ? (tl >> 1) : tl);
-      const int64_t g_base = t * G;
-      const int groups_here = (int)min((int64_t)G, prm.n_groups - g_base);
-      mbar_wait(&acc_full[buf], use & 1u);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT + ((uint32_t)(q * 32) << 16);
-      float* outp = prm.out + g_base * prm.ldo + h;
-      // one fanout group = k consecutive accumulator columns of this lane, fetched in pieces of 32 / 16 / 8 / 4 / 2 / 1
-      // columns chosen by the bits of k: statically indexed registers, straight-line pooling (see the wide kernel)
-      for (int g = 0; g < groups_here; ++g) {
-        uint32_t col = tmem_acc + (uint32_t)(g * k);
-        float m = mean ? 0.f : -3.0e38f;
-        int rem = k;
-        while (rem >= 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(col, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) m = fold(m, r[j]);
-          col += 32u;
-          rem -= 32;
-        }
-        uint32_t r16[16], r8[8], r4[4], r2[2], r1[1];
-        uint32_t cc = col;
-        if (rem & 16) { tmem_ld_32x16(cc, r16); cc += 16u; }
-        if (rem & 8) { tmem_ld_32x8(cc, r8); cc += 8u; }
-        if (rem & 4) { tmem_ld_32x4(cc, r4); cc += 4u; }
-        if (rem & 2) { tmem_ld_32x2(cc, r2); cc += 2u; }
-        if (rem & 1) { tmem_ld_32x1(cc, r1); }
-        tmem_ld_wait();
-        if (rem & 16) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) m = fold(m, r16[j]);
-        }
-        if (rem & 8) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) m = fold(m, r8[j]);
-        }
-        if (rem & 4) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) m = fold(m, r4[j]);
-        }
-        if (rem & 2) {
-          m = fold(m, r2[0]);
-          m = fold(m, r2[1]);
-        }
-        if (rem & 1) m = fold(m, r1[0]);
-        outp[(int64_t)g * prm.ldo] = mean ? m * inv_k : fmaxf(m + b, 0.f);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
-  }
-  __syncthreads();
-  if (warp == MPT_PW + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    prm.out[gg * prm.ldo + hcol] = res;
   }
 }
 
-// Cluster form (the default; k4_cluster = cluster size CL, 2 unless tuned): CL of the CTAs that hold the hidden slices of
-// ONE tile form a thread-block cluster.  Each CTA gathers only 128 / CL of the tile's rows - with the TMA row gather,
-// `cp.async.bulk.tensor.2d.tile::gather4` (four table rows named by index, 128 bytes each, SWIZZLE_128B applied by the
-// tensor map, columns >= K zero-filled) - and MULTICASTS them into the same stage of every CTA of the cluster, so a
-// gathered row crosses the L2 -> SM fabric once per cluster instead of once per slice (650 MB per launch without
-// clusters, 325 MB with pairs, 163 MB with clusters of four).  Measured (DESIGN 4a): the traffic cut alone did not move
-// the kernel - the MMA issue chain is what bounds it - but the producer side shrinks to one elected lane per warp with
-// no per-thread address arithmetic, no cp.async groups and no proxy fence, and pairs keep all 148 SMs busy (74 clusters)
-// where clusters of four fit only 33 (132 SMs): 111 us against 117 us at hop 2.  Hand-off: a CTA's full barrier = its own
-// expect_tx arrive + 16 KB of transactions from all CL issuers; its empty barrier counts CL arrivals - every CTA's MMA
-// warp commits with .multicast::cluster to all CL empty barriers -, so a stage is refilled only when the whole cluster
-// has consumed it.  Producer warp w owns the ring slots w, w + MPC_PW, ... (n_stages is a multiple of MPC_PW: a slot is
-// always filled by the same warp, so a wait is never more than one phase ahead - tools/pipeline_model.py).
-constexpr int MPC_PW = 4;                         // producer warps
-constexpr int MPC_THREADS = (MPC_PW + 6) * 32;
-
-template <int CL>
-__global__ void __launch_bounds__(MPC_THREADS, 1)
-    maxpool_mlp_tmemc_kernel(const __grid_constant__ MpParams prm, const __grid_constant__ CUtensorMap tmap) {
-  constexpr int KC = 64, NT = 128;
-  constexpr int NBUF = 2;
-  constexpr int X_IMG = NT * 128;
-  constexpr int ROWS_PER_CTA = NT / CL;             // this CTA's share of the tile's rows
-  constexpr int LANES = ROWS_PER_CTA / 4;           // one gather4 (4 rows) per active lane
-  constexpr uint16_t MASK = (uint16_t)((1u << CL) - 1u);
-  static_assert(CL == 2 || CL == 4 || CL == 8, "cluster = the 2, 4 or 8 hidden slices of one tile");
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_x[MPT_MAX_STAGES], empty_x[MPT_MAX_STAGES], acc_full[2], acc_empty[2], w_full, wt_full;
-  __shared__ uint32_t tmem_base_smem;
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int kblocks = prm.kblocks, kb_t = prm.kb_t, kb_s = kblocks - kb_t;
-  const int n_stages = prm.n_stages;
-  unsigned char* w_res = smem;                                        // K-blocks kb_t.. of the weight slice (SS operands)
-  unsigned char* x_ring = smem + (size_t)kb_s * MPT_IMG;     // n_stages stages of X_IMG bytes
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int k = prm.k, G = prm.G;
-  const int rows_valid = G * k;
-  const int64_t total_rows = prm.n_groups * (int64_t)k;
-  const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MPT_MAX_STAGES; ++s) {
-      mbar_init(&full_x[s], 1);                     // own expect_tx arrive; the 16 KB arrive from all CL issuers
-      mbar_init(&empty_x[s], CL);                   // one multicast commit per CTA of the cluster
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);                  // one arrive per epilogue warp
-    }
-    mbar_init(&w_full, 1);
-    mbar_init(&wt_full, 4);                         // one arrive per epilogue warp (each writes its 32 TMEM lanes)
-    fence_mbar_init();
+template <bool kRowsA, int NT, int DEPTH, int PROD>
+static int32_t launch_k4(const MpParams& prm, int64_t n_tiles, int cluster, cudaStream_t st) {
+  const void* fn = (const void*)maxpool_mlp_kernel<kRowsA, NT, DEPTH, PROD>;
+  const int smem = MP_STAGES * (NT * 128 + MP_IMG) + 1024;
+  const int32_t rc_attr = ensure_dyn_smem(fn, smem);
+  if (rc_attr != GS_OK) return rc_attr;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)(n_tiles * prm.n_slices));
+  cfg.blockDim = dim3((unsigned)MP_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr;
+  if (cluster > 1) {                               // the grid is a multiple of n_slices, which cluster divides
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = (unsigned)cluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
   }
-  if (warp == MPC_PW + 1) {
-    tmem_alloc(&tmem_base_smem, 512);               // 2 x 128 accumulator columns + up to 256 weight columns
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                               // every CTA's barriers exist before any remote arrive / multicast write
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp < MPC_PW) {
-    // =============================== gather producers (TMA gather4, multicast) ===============================
-    const int rank = (int)cluster_ctarank();        // == slice: the cluster spans the hidden slices of one tile
-    const int row_base = rank * ROWS_PER_CTA + 4 * lane;
-    const int64_t total_it = my_tiles * kblocks;
-    int raw[4], cur[4];
-    auto request = [&](int64_t tl) {                // ids of tile tl: loads only (nothing depends on them yet)
-      const int64_t t = tile0 + tl * tile_step;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = row_base + i;
-        const int64_t flat = t * rows_valid + r;
-        const bool live = lane < LANES && tl < my_tiles && r < rows_valid && flat < total_rows;
-        int v = 0;                                  // padding rows of a tile read row 0 (finite data, never looked at)
-        if (live) v = prm.row_ids ? __ldg(prm.row_ids + flat) : (int)(prm.row0 + flat);
-        raw[i] = v;
-      }
-    };
-    auto finish = [&]() {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        int id = raw[i];
-        if (id < 0 || (int64_t)id >= prm.n_rows) id = (int)(prm.n_rows - 1);
-        cur[i] = id;
-      }
-    };
-    int64_t tl = 0;
-    int kb = warp;
-    while (kb >= kblocks) { kb -= kblocks; ++tl; }
-    request(tl);
-    finish();
-    request(tl + 1);
-    for (int64_t it = warp; it < total_it; it += MPC_PW) {
-      const uint32_t s = (uint32_t)(it % n_stages);
-      const uint32_t fill = (uint32_t)(it / n_stages);
-      mbar_wait(&empty_x[s], (fill & 1u) ^ 1u);     // every CTA of the cluster has consumed the previous fill
-      if (lane == 0) mbar_expect_tx(&full_x[s], (uint32_t)X_IMG);
-      __syncwarp();
-      if (lane < LANES)
-        tma_gather4_multicast(x_ring + (size_t)s * X_IMG + (size_t)row_base * 128, &tmap, &full_x[s], MASK, kb * KC, cur[0],
-                              cur[1], cur[2], cur[3]);
-      kb += MPC_PW;
-      if (kb >= kblocks) {
-        int adv = 0;
-        while (kb >= kblocks) { kb -= kblocks; ++adv; }
-        tl += adv;
-        if (adv != 1) request(tl);
-        finish();
-        request(tl + 1);
-      }
-    }
-  } else if (warp == MPC_PW) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(1u, 128, NT);               // bf16 x bf16 -> fp32, M = 128, N = 128
-    if (kb_s > 0) mbar_wait_uniform(&w_full, 0);
-    if (kb_t > 0) mbar_wait_uniform(&wt_full, 0);
-    tc_fence_after();
-    const uint32_t x_base = smem_u32(x_ring), w_base = smem_u32(w_res);
-    uint32_t s = 0, ph = 0;
-    for (int64_t tl = 0; tl < my_tiles; ++tl) {
-      const uint32_t buf = NBUF == 2 ? ((uint32_t)tl & 1u) : 0u;
-      const uint32_t use = (uint32_t)(NBUF == 2 ? (tl >> 1) : tl);          // how often this accumulator has been used before
-      mbar_wait_uniform(&acc_empty[buf], (use & 1u) ^ 1u);                  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait_uniform(&full_x[s], ph);          // (TMA wrote the stage through the async proxy: no proxy fence)
-        tc_fence_after();
-        const uint64_t bdesc = make_smem_desc(x_base + s * (uint32_t)X_IMG);
-        if (kb < kb_t) {
-          const uint32_t a_t = tmem_base + (uint32_t)MPT_ACOL0 + (uint32_t)kb * 32u;
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)      // K = 16 per instruction: 8 TMEM columns of A, 32 B of B inside the atom
-            umma_ts_elect_bf16(tmem_acc, a_t + (uint32_t)(k2 * 8), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        } else {
-          const uint64_t adesc = make_smem_desc(w_base + (uint32_t)(kb - kb_t) * (uint32_t)MPT_IMG);
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)
-            umma_ss_elect<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        }
-        umma_commit_elect_multicast(&empty_x[s], MASK);     // frees the stage in every CTA of the cluster
-        if (kb == kblocks - 1) umma_commit_elect(&acc_full[buf]);
-        if (++s == (uint32_t)n_stages) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else if (warp == MPC_PW + 1) {
-    // =============================== shared-memory part of the weight slice ===============================
-    if (lane == 0 && kb_s > 0) {
-      mbar_expect_tx(&w_full, (uint32_t)(kb_s * MPT_IMG));
-      const unsigned char* src = prm.wimg + ((int64_t)slice * kblocks + kb_t) * MPT_IMG;
-      for (int kb = 0; kb < kb_s; ++kb) bulk_g2s(w_res + (size_t)kb * MPT_IMG, src + (int64_t)kb * MPT_IMG, MPT_IMG, &w_full);
-    }
-    __syncwarp();
-  } else {
-    // =============================== epilogue warps ===============================
-    const int q = warp & 3;                         // TMEM lane quarter of this warp (four consecutive warps cover 0..3)
-    const int h = slice * 128 + q * 32 + lane;      // this thread's hidden unit = its TMEM lane
-    // once: this lane's row of Wm^T (bf16 pairs) for the first kb_t K-blocks -> tensor memory (A operand, TS form)
-    {
-      const uint32_t* wrow = prm.wrows + (int64_t)h * (kblocks * 32);
-      const uint32_t t_a = tmem_base + (uint32_t)MPT_ACOL0 + ((uint32_t)(q * 32) << 16);
-      for (int cb = 0; cb < kb_t; ++cb) {
-        uint32_t r[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 v = __ldg(reinterpret_cast<const uint4*>(wrow + cb * 32) + j);
-          r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
-        }
-        tmem_st_32x32(t_a + (uint32_t)(cb * 32), r);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&wt_full);
-    }
-    const float b = prm.bias ? prm.bias[h] : 0.f;
-    const float inv_k = 1.0f / (float)k;
-    const bool mean = prm.pool_mean != 0;
-    auto fold = [&](float m, uint32_t x) -> float {
-      const float v = __uint_as_float(x);
-      // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU are applied
-      // per element and summed in j order; max-pool: bias + ReLU after the max (they commute with it)
-      return mean ? m + fmaxf(v + b, 0.f) : fmaxf(m, v);
-    };
-    for (int64_t tl = 0; tl < my_tiles; ++tl) {
-      const int64_t t = tile0 + tl * tile_step;
-      const uint32_t buf = NBUF == 2 ? ((uint32_t)tl & 1u) : 0u;
-      const uint32_t use = (uint32_t)(NBUF == 2 ? (tl >> 1) : tl);
-      const int64_t g_base = t * G;
-      const int groups_here = (int)min((int64_t)G, prm.n_groups - g_base);
-      mbar_wait(&acc_full[buf], use & 1u);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT + ((uint32_t)(q * 32) << 16);
-      float* outp = prm.out + g_base * prm.ldo + h;
-      // one fanout group = k consecutive accumulator columns of this lane, fetched in pieces of 32 / 16 / 8 / 4 / 2 / 1
-      // columns chosen by the bits of k: statically indexed registers, straight-line pooling (see the wide kernel)
-      for (int g = 0; g < groups_here; ++g) {
-        uint32_t col = tmem_acc + (uint32_t)(g * k);
-        float m = mean ? 0.f : -3.0e38f;
-        int rem = k;
-        while (rem >= 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(col, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) m = fold(m, r[j]);
-          col += 32u;
-          rem -= 32;
-        }
-        uint32_t r16[16], r8[8], r4[4], r2[2], r1[1];
-        uint32_t cc = col;
-        if (rem & 16) { tmem_ld_32x16(cc, r16); cc += 16u; }
-        if (rem & 8) { tmem_ld_32x8(cc, r8); cc += 8u; }
-        if (rem & 4) { tmem_ld_32x4(cc, r4); cc += 4u; }
-        if (rem & 2) { tmem_ld_32x2(cc, r2); cc += 2u; }
-        if (rem & 1) { tmem_ld_32x1(cc, r1); }
-        tmem_ld_wait();
-        if (rem & 16) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) m = fold(m, r16[j]);
-        }
-        if (rem & 8) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) m = fold(m, r8[j]);
-        }
-        if (rem & 4) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) m = fold(m, r4[j]);
-        }
-        if (rem & 2) {
-          m = fold(m, r2[0]);
-          m = fold(m, r2[1]);
-        }
-        if (rem & 1) m = fold(m, r1[0]);
-        outp[(int64_t)g * prm.ldo] = mean ? m * inv_k : fmaxf(m + b, 0.f);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
-  }
-  __syncthreads();
-  cluster_sync_all();                               // no CTA leaves while a peer may still write its stages or signal its barriers
-  if (warp == MPC_PW + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
+  MpParams p = prm;
+  void* args[1] = {(void*)&p};
+  GS_CUDA(cudaLaunchKernelExC(&cfg, fn, args));
+  return launch_check("maxpool_mlp_kernel");
 }
 
-
-// Two pipelines per CTA (k4_kernel = 0 with k4_tile = 128 and k4_pipes = 2, the default): the NT = 128 kernel showed the
-// single MMA warp saturated - ~860 cycles of instruction latency per four-MMA K-block, tensor pipe idle 70 % - and never
-// short of operands.  Here the CTA runs TWO independent producer -> MMA chains that share only the weights in TMEM, the
-// tensor pipe and the epilogue warps: chain p = producer group p (4 warps) -> its own half of the operand ring -> MMA warp
-// p -> accumulator p, working on the CTA's local tiles p, p + 2, ...  The tensor pipe interleaves the two accumulation
-// chains (they are independent), so two issuing warps double the MMA issue rate.
-__global__ void __launch_bounds__(MPT_THREADS, 1) maxpool_mlp_tmem2_kernel(const __grid_constant__ MpParams prm) {
-  constexpr int KC = 64, NT = 128;
-  constexpr int X_IMG = NT * 128;
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_x[MPT_MAX_STAGES], empty_x[MPT_MAX_STAGES], acc_full[2], acc_empty[2], w_full, wt_full;
-  __shared__ uint32_t tmem_base_smem;
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int kblocks = prm.kblocks, kb_t = prm.kb_t, kb_s = kblocks - kb_t;
-  const int n_stages = prm.n_stages;
-  unsigned char* w_res = smem;                                        // K-blocks kb_t.. of the weight slice (SS operands)
-  unsigned char* x_ring = smem + (size_t)kb_s * MPT_IMG;     // n_stages stages of X_IMG bytes
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int k = prm.k, G = prm.G;
-  const int rows_valid = G * k;
-  const int64_t total_rows = prm.n_groups * (int64_t)k;
-  const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MPT_MAX_STAGES; ++s) {
-      mbar_init(&full_x[s], MPT_PW / 2);            // one arrive per warp of the pipeline's producer group
-      mbar_init(&empty_x[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);                  // one arrive per epilogue warp
-    }
-    mbar_init(&w_full, 1);
-    mbar_init(&wt_full, 4);                         // one arrive per epilogue warp (each writes its 32 TMEM lanes)
-    fence_mbar_init();
-  }
-  if (warp == MPT_PW) {
-    tmem_alloc(&tmem_base_smem, 512);               // 2 x 128 accumulator columns + up to 256 weight columns
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  const int n_half = n_stages / 2;                  // stages per pipeline
-  if (warp < MPT_PW) {
-    const int grp = warp / (MPT_PW / 2);
-    mpw_cpasync_pipeline_producers<KC, NT, MPT_PW>(prm, grp, (int)threadIdx.x - grp * (MPT_PW * 16), lane, n_half,
-                                                   x_ring + (size_t)grp * n_half * X_IMG, full_x + grp * n_half,
-                                                   empty_x + grp * n_half, tile0, tile_step, my_tiles, rows_valid, total_rows);
-  } else if (warp == MPT_PW || warp == MPT_PW + 1) {
-    const int pipe = warp - MPT_PW;
-    if (pipe == 1 && lane == 0 && kb_s > 0) {       // shared-memory part of the weight slice (once)
-      mbar_expect_tx(&w_full, (uint32_t)(kb_s * MPT_IMG));
-      const unsigned char* src = prm.wimg + ((int64_t)slice * kblocks + kb_t) * MPT_IMG;
-      for (int kb = 0; kb < kb_s; ++kb) bulk_g2s(w_res + (size_t)kb * MPT_IMG, src + (int64_t)kb * MPT_IMG, MPT_IMG, &w_full);
-    }
-    __syncwarp();
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = make_idesc(1u, 128, NT);               // bf16 x bf16 -> fp32, M = 128, N = 128
-    if (kb_s > 0) mbar_wait_uniform(&w_full, 0);
-    if (kb_t > 0) mbar_wait_uniform(&wt_full, 0);
-    tc_fence_after();
-    const uint32_t x_base = smem_u32(x_ring + (size_t)pipe * n_half * X_IMG), w_base = smem_u32(w_res);
-    uint64_t* full_p = full_x + pipe * n_half;
-    uint64_t* empty_p = empty_x + pipe * n_half;
-    uint32_t s = 0, ph = 0;
-    for (int64_t tl = pipe; tl < my_tiles; tl += 2) {
-      const uint32_t buf = (uint32_t)pipe;
-      const uint32_t use = (uint32_t)(tl >> 1);                             // how often this accumulator has been used before
-      mbar_wait_uniform(&acc_empty[buf], (use & 1u) ^ 1u);                  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait_uniform(&full_p[s], ph);
-        fence_proxy_async();                        // cp.async wrote the stage through the generic proxy
-        tc_fence_after();
-        const uint64_t bdesc = make_smem_desc(x_base + s * (uint32_t)X_IMG);
-        if (kb < kb_t) {
-          const uint32_t a_t = tmem_base + (uint32_t)MPT_ACOL0 + (uint32_t)kb * 32u;
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)      // K = 16 per instruction: 8 TMEM columns of A, 32 B of B inside the atom
-            umma_ts_elect_bf16(tmem_acc, a_t + (uint32_t)(k2 * 8), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        } else {
-          const uint64_t adesc = make_smem_desc(w_base + (uint32_t)(kb - kb_t) * (uint32_t)MPT_IMG);
-#pragma unroll
-          for (int k2 = 0; k2 < KC / 16; ++k2)
-            umma_ss_elect<true>(tmem_acc, adesc + (uint64_t)(k2 * 2), bdesc + (uint64_t)(k2 * 2), idesc, (kb > 0 || k2 > 0) ? 1u : 0u);
-        }
-        umma_commit_elect(&empty_p[s]);
-        if (kb == kblocks - 1) umma_commit_elect(&acc_full[buf]);
-        if (++s == (uint32_t)n_half) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else {
-    // =============================== epilogue warps ===============================
-    const int q = warp & 3;                         // TMEM lane quarter of this warp (four consecutive warps cover 0..3)
-    const int h = slice * 128 + q * 32 + lane;      // this thread's hidden unit = its TMEM lane
-    // once: this lane's row of Wm^T (bf16 pairs) for the first kb_t K-blocks -> tensor memory (A operand, TS form)
-    {
-      const uint32_t* wrow = prm.wrows + (int64_t)h * (kblocks * 32);
-      const uint32_t t_a = tmem_base + (uint32_t)MPT_ACOL0 + ((uint32_t)(q * 32) << 16);
-      for (int cb = 0; cb < kb_t; ++cb) {
-        uint32_t r[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 v = __ldg(reinterpret_cast<const uint4*>(wrow + cb * 32) + j);
-          r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
-        }
-        tmem_st_32x32(t_a + (uint32_t)(cb * 32), r);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&wt_full);
-    }
-    const float b = prm.bias ? prm.bias[h] : 0.f;
-    const float inv_k = 1.0f / (float)k;
-    const bool mean = prm.pool_mean != 0;
-    auto fold = [&](float m, uint32_t x) -> float {
-      const float v = __uint_as_float(x);
-      // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU are applied
-      // per element and summed in j order; max-pool: bias + ReLU after the max (they commute with it)
-      return mean ? m + fmaxf(v + b, 0.f) : fmaxf(m, v);
-    };
-    for (int64_t tl = 0; tl < my_tiles; ++tl) {
-      const int64_t t = tile0 + tl * tile_step;
-      const uint32_t buf = (uint32_t)tl & 1u;
-      const uint32_t use = (uint32_t)(tl >> 1);
-      const int64_t g_base = t * G;
-      const int groups_here = (int)min((int64_t)G, prm.n_groups - g_base);
-      mbar_wait(&acc_full[buf], use & 1u);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + buf * (uint32_t)NT + ((uint32_t)(q * 32) << 16);
-      float* outp = prm.out + g_base * prm.ldo + h;
-      // one fanout group = k consecutive accumulator columns of this lane, fetched in pieces of 32 / 16 / 8 / 4 / 2 / 1
-      // columns chosen by the bits of k: statically indexed registers, straight-line pooling (see the wide kernel)
-      for (int g = 0; g < groups_here; ++g) {
-        uint32_t col = tmem_acc + (uint32_t)(g * k);
-        float m = mean ? 0.f : -3.0e38f;
-        int rem = k;
-        while (rem >= 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(col, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) m = fold(m, r[j]);
-          col += 32u;
-          rem -= 32;
-        }
-        uint32_t r16[16], r8[8], r4[4], r2[2], r1[1];
-        uint32_t cc = col;
-        if (rem & 16) { tmem_ld_32x16(cc, r16); cc += 16u; }
-        if (rem & 8) { tmem_ld_32x8(cc, r8); cc += 8u; }
-        if (rem & 4) { tmem_ld_32x4(cc, r4); cc += 4u; }
-        if (rem & 2) { tmem_ld_32x2(cc, r2); cc += 2u; }
-        if (rem & 1) { tmem_ld_32x1(cc, r1); }
-        tmem_ld_wait();
-        if (rem & 16) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) m = fold(m, r16[j]);
-        }
-        if (rem & 8) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) m = fold(m, r8[j]);
-        }
-        if (rem & 4) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) m = fold(m, r4[j]);
-        }
-        if (rem & 2) {
-          m = fold(m, r2[0]);
-          m = fold(m, r2[1]);
-        }
-        if (rem & 1) m = fold(m, r1[0]);
-        outp[(int64_t)g * prm.ldo] = mean ? m * inv_k : fmaxf(m + b, 0.f);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
-  }
-  __syncthreads();
-  if (warp == MPT_PW) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Variant (GS_TUNING=k4_producer=1, not the default until measured): the gather-A producers use the TMA's row gather,
-// `cp.async.bulk.tensor.2d.tile::gather4` - one instruction fetches a 64-byte K-block segment of FOUR table rows named
-// by index and writes them, SWIZZLE_64B applied by the tensor map, straight into the UMMA stage; completion is the
-// stage's mbarrier transaction count.  No per-thread cp.async group waits, no generic->async proxy fence, no per-warp
-// arrive: what remains per stage is one empty-barrier wait, one expect_tx and one gather4 per lane (32 lanes x 4 rows =
-// the 128-row stage).  ptxas serialises the 32 lanes of an instruction with per-lane operands (ELECT waterfall), so
-// there is one producer warp PER RING SLOT, each filling whole stages, to keep that latency off the critical path.
-// Producer warp w owns slot w and fills K-blocks w, w + MP_SA, ... in order: a warp that served several slots could get
-// two fills ahead of a slot it last touched long ago, and an mbarrier wait only carries ONE parity bit - it would pass on
-// the stale phase and overwrite a stage that has not been consumed (tools/pipeline_model.py reproduces exactly that for
-// 8 warps over 7 slots; with one warp per slot every wait is at most one phase ahead).
-// Columns >= K are out of bounds for the tensor map and zero-filled by the TMA; tile rows past the last fanout group
-// (never read by the epilogue) fetch row 0.
-// ---------------------------------------------------------------------------------------------------------------------
-
-__device__ __forceinline__ void tma_gather4(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int col, int r0, int r1,
-                                            int r2, int r3) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(tmap), "r"(smem_u32(bar)), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-      : "memory");
-}
-
-template <int MP_SA>
-__global__ void __launch_bounds__((MP_SA + 6) * 32, 1)
-    maxpool_mlp_g4_kernel(const __grid_constant__ MpParams prm, const __grid_constant__ CUtensorMap tmap) {
-  constexpr int MP_G4_WARPS = MP_SA;              // one producer warp per ring slot (see above)
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_a[MP_SA], empty_a[MP_SA], acc_full[2], acc_empty[2], b_full;
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float bias_s[128];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* b_res = smem;                                        // resident weight slice
-  unsigned char* a_ring = smem + (MP_RING - MP_SA) * MP_IMG;
-  float* stage = reinterpret_cast<float*>(smem + MP_RING * MP_IMG);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int kblocks = prm.kblocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MP_SA; ++s) {
-      mbar_init(&full_a[s], 1);           // the expect_tx arrive of the stage's producer warp (+ 8 KB of transactions)
-      mbar_init(&empty_a[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);        // one arrive per epilogue warp
-    }
-    mbar_init(&b_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == MP_G4_WARPS) {
-    tmem_alloc(&tmem_base_smem, 256);     // two 128-column fp32 accumulators
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp < MP_G4_WARPS) {
-    // =============================== gather-A producers (TMA gather4) ===============================
-    const int rows_valid = prm.G * prm.k;
-    const int64_t total_rows = prm.n_groups * prm.k;
-    const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
-    const int64_t total_it = my_tiles * kblocks;
-    const int pad_row = 0;                          // tile rows past the last group: never read by the epilogue, any valid row will do
-    int cur[4], nxt[4];                             // table rows of this lane's tile rows 4 lane .. 4 lane + 3
-    auto load_ids = [&](int64_t tl, int (&ids)[4]) {
-      const int64_t t = tile0 + tl * tile_step;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = 4 * lane + i;
-        const int64_t flat = t * rows_valid + r;    // index into the (group, j) row list
-        int64_t id = pad_row;
-        if (tl < my_tiles && r < rows_valid && flat < total_rows) {
-          id = prm.row_ids ? (int64_t)prm.row_ids[flat] : prm.row0 + flat;
-          if (id < 0 || id >= prm.n_rows) id = prm.n_rows - 1;
-        }
-        ids[i] = (int)id;
-      }
-    };
-    int64_t tl = 0;
-    int kb = warp;
-    while (kb >= kblocks) { kb -= kblocks; ++tl; }
-    load_ids(tl, cur);
-    load_ids(tl + 1, nxt);
-    const int s = warp;                             // this warp's slot
-    uint32_t fill = 0;                              // fills of the slot so far
-    for (int64_t it = warp; it < total_it; it += MP_G4_WARPS, ++fill) {
-      mbar_wait(&empty_a[s], (fill & 1u) ^ 1u);
-      if (lane == 0) mbar_expect_tx(&full_a[s], (uint32_t)MP_IMG);
-      __syncwarp();
-      tma_gather4(a_ring + (size_t)s * MP_IMG + lane * 256, &tmap, &full_a[s], kb * MP_KCOLS, cur[0], cur[1], cur[2], cur[3]);
-      // this warp's next K-block: MP_G4_WARPS further on, possibly in a later tile
-      kb += MP_G4_WARPS;
-      int adv = 0;
-      while (kb >= kblocks) { kb -= kblocks; ++adv; }
-      if (adv == 1) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
-        tl += 1;
-        load_ids(tl + 1, nxt);
-      } else if (adv > 1) {
-        tl += adv;
-        load_ids(tl, cur);
-        load_ids(tl + 1, nxt);
-      }
-    }
-  } else if (warp == MP_G4_WARPS) {
-    mp_mma_role<MP_SA>(prm, lane, kblocks, tile0, tile_step, tmem_base, full_a, empty_a, acc_full, acc_empty, b_full, a_ring,
-                       b_res);
-  } else if (warp == MP_G4_WARPS + 1) {
-    mp_weights_role(prm, lane, slice, kblocks, b_full, b_res);
-  } else {
-    mp_epilogue_role(prm, (int)threadIdx.x - (MP_G4_WARPS + 2) * 32, warp, lane, slice, tile0, tile_step, tmem_base, acc_full,
-                     acc_empty, stage, bias_s);
-  }
-  __syncthreads();
-  if (warp == MP_G4_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Variant 2 (k4_kernel=1 with k4_producer=2; run on a B200 in round 2 through tools/tc_check.py: bit-identical to the
-// cp.async producers, 259 us at hop 2 against 164 us for the gather4 variant without clusters - the round-1 geometry keeps
-// the gathered rows as the A operand, so a cluster of all slices serialises on one tile): as the gather4 variant, plus
-// thread-block clusters.
-// The n_slices CTAs that work on the SAME M tile (one per 128-wide slice of the hidden dimension) form a cluster of
-// CL = n_slices (2 or 4) CTAs; each gathers only 128 / CL of the tile's rows and MULTICASTS them into the A stage of
-// every CTA of the cluster, so an A row crosses the L2 -> SM fabric once per cluster instead of once per slice
-// (that fabric's chip-wide cap, not the tensor pipe, bounds the non-multicast kernels once the proxy fence is gone).
-// Hand-off: a CTA's full barrier collects its own expect_tx arrive + 8 KB of transactions from all CL issuers; its
-// empty barrier has CL arrivals - every CTA's MMA warp commits with .multicast::cluster to all CL empty barriers -,
-// so a producer re-fills a stage only when every CTA of the cluster has consumed it.
-// ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_gather4_multicast(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, uint16_t mask,
-                                                      int col, int r0, int r1, int r2, int r3) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5, %6, %7, %8}], [%2], %3;" ::"r"(smem_u32(smem_dst)),
-      "l"(tmap), "r"(smem_u32(bar)), "h"(mask), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-      : "memory");
-}
-
-template <int MP_SA, int CL>
-__global__ void __launch_bounds__((MP_SA + 6) * 32, 1)
-    maxpool_mlp_g4mc_kernel(const __grid_constant__ MpParams prm, const __grid_constant__ CUtensorMap tmap) {
-  static_assert(CL == 2 || CL == 4, "cluster = the 2 or 4 hidden slices of one M tile");
-  constexpr int MP_G4_WARPS = MP_SA;              // one producer warp per ring slot (see the gather4 variant)
-  extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t full_a[MP_SA], empty_a[MP_SA], acc_full[2], acc_empty[2], b_full;
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float bias_s[128];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* b_res = smem;                                        // resident weight slice
-  unsigned char* a_ring = smem + (MP_RING - MP_SA) * MP_IMG;
-  float* stage = reinterpret_cast<float*>(smem + MP_RING * MP_IMG);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int slice = blockIdx.x % prm.n_slices;                        // == rank in the cluster (n_slices == CL)
-  const int64_t tile0 = blockIdx.x / prm.n_slices, tile_step = gridDim.x / prm.n_slices;
-  const int kblocks = prm.kblocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MP_SA; ++s) {
-      mbar_init(&full_a[s], 1);           // own expect_tx arrive; the 8 KB arrive from all CL issuers
-      mbar_init(&empty_a[s], CL);         // one multicast commit per CTA of the cluster
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);        // one arrive per epilogue warp
-    }
-    mbar_init(&b_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == MP_G4_WARPS) {
-    tmem_alloc(&tmem_base_smem, 256);     // two 128-column fp32 accumulators
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                     // every CTA's barriers exist before any remote arrive / multicast write
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp < MP_G4_WARPS) {
-    // =============================== gather-A producers (TMA gather4, multicast) ===============================
-    constexpr int ROWS_PER_CTA = 128 / CL;          // this CTA's share of the tile's rows
-    constexpr int LANES = ROWS_PER_CTA / 4;         // one gather4 (4 rows) per active lane
-    const int rank = (int)cluster_ctarank();
-    const int rows_valid = prm.G * prm.k;
-    const int64_t total_rows = prm.n_groups * prm.k;
-    const int64_t my_tiles = tile0 < prm.n_tiles ? (prm.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
-    const int64_t total_it = my_tiles * kblocks;
-    const int pad_row = 0;                          // tile rows past the last group: never read by the epilogue, any valid row will do
-    const int row_base = rank * ROWS_PER_CTA + 4 * lane;
-    int cur[4], nxt[4];
-    auto load_ids = [&](int64_t tl, int (&ids)[4]) {
-      const int64_t t = tile0 + tl * tile_step;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = row_base + i;
-        const int64_t flat = t * rows_valid + r;
-        int64_t id = pad_row;
-        if (lane < LANES && tl < my_tiles && r < rows_valid && flat < total_rows) {
-          id = prm.row_ids ? (int64_t)prm.row_ids[flat] : prm.row0 + flat;
-          if (id < 0 || id >= prm.n_rows) id = prm.n_rows - 1;
-        }
-        ids[i] = (int)id;
-      }
-    };
-    int64_t tl = 0;
-    int kb = warp;
-    while (kb >= kblocks) { kb -= kblocks; ++tl; }
-    load_ids(tl, cur);
-    load_ids(tl + 1, nxt);
-    const int s = warp;                             // this warp's slot
-    uint32_t fill = 0;                              // fills of the slot so far
-    for (int64_t it = warp; it < total_it; it += MP_G4_WARPS, ++fill) {
-      mbar_wait(&empty_a[s], (fill & 1u) ^ 1u);     // every CTA of the cluster has consumed the previous fill
-      if (lane == 0) mbar_expect_tx(&full_a[s], (uint32_t)MP_IMG);
-      __syncwarp();
-      if (lane < LANES)
-        tma_gather4_multicast(a_ring + (size_t)s * MP_IMG + (size_t)(row_base / 4) * 256, &tmap, &full_a[s],
-                              (uint16_t)((1u << CL) - 1u), kb * MP_KCOLS, cur[0], cur[1], cur[2], cur[3]);
-      kb += MP_G4_WARPS;
-      int adv = 0;
-      while (kb >= kblocks) { kb -= kblocks; ++adv; }
-      if (adv == 1) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) cur[i] = nxt[i];
-        tl += 1;
-        load_ids(tl + 1, nxt);
-      } else if (adv > 1) {
-        tl += adv;
-        load_ids(tl, cur);
-        load_ids(tl + 1, nxt);
-      }
-    }
-  } else if (warp == MP_G4_WARPS) {
-    mp_mma_role<MP_SA, CL>(prm, lane, kblocks, tile0, tile_step, tmem_base, full_a, empty_a, acc_full, acc_empty, b_full,
-                           a_ring, b_res);
-  } else if (warp == MP_G4_WARPS + 1) {
-    mp_weights_role(prm, lane, slice, kblocks, b_full, b_res);
-  } else {
-    mp_epilogue_role(prm, (int)threadIdx.x - (MP_G4_WARPS + 2) * 32, warp, lane, slice, tile0, tile_step, tmem_base, acc_full,
-                     acc_empty, stage, bias_s);
-  }
-  __syncthreads();
-  cluster_sync_all();                     // no CTA leaves while a peer may still write its stages or signal its barriers
-  if (warp == MP_G4_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
+template <bool kRowsA, int NT>
+static int32_t launch_k4_by(const MpParams& prm, int64_t n_tiles, int cluster, int depth, int producer, cudaStream_t st) {
+  if (depth == 2)
+    return producer == 1 ? launch_k4<kRowsA, NT, 2, 1>(prm, n_tiles, cluster, st) : launch_k4<kRowsA, NT, 2, 0>(prm, n_tiles, cluster, st);
+  return producer == 1 ? launch_k4<kRowsA, NT, 1, 1>(prm, n_tiles, cluster, st) : launch_k4<kRowsA, NT, 1, 0>(prm, n_tiles, cluster, st);
 }
 
 }  // namespace gs
 
 extern "C" {
 
-/* developer probe (not in the public header) */
-int32_t gs_debug_read_maxpool_timeline(unsigned long long* out_host, int32_t n) {
-  if (n > 128) n = 128;
-  GS_CUDA(cudaDeviceSynchronize());
-  GS_CUDA(cudaMemcpyFromSymbol(out_host, gs::g_mp_dbg, sizeof(unsigned long long) * n));
-  return GS_OK;
-}
-
-// packed weights = region 0: [slices][ceil(K/32)] images of 128 x 64 B (SW64) | region 1: [slices][ceil(K/64)] images of
-// 128 x 128 B (SW128); every kernel geometry finds its own format (packing is per weight update, not per step)
-static int64_t mp_region0_bytes(int32_t K, int32_t hidden) {
-  const int kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS, slices = (hidden + 127) / 128;
-  return (int64_t)kblocks * slices * gs::MP_IMG;
-}
-
-static int64_t mp_region1_bytes(int32_t K, int32_t hidden) {
-  const int kb128 = (K + 63) / 64, slices = (hidden + 127) / 128;
-  return (int64_t)kb128 * slices * 2 * gs::MP_IMG;
-}
-
-// region 2: Wm^T as rows of bf16 pairs, [slices * 128][ceil(K/64) * 32] uint32 (what the tmem kernel stores into TMEM)
+// packed weights: [slices][ceil(K/64)] images of 128 x 128 B (SW128), re-packed per weight update, not per step
 int64_t gs_maxpool_mlp_workspace_bytes(int32_t K, int32_t hidden) {
   if (K < 1 || hidden < 1) return -1;
-  const int kb128 = (K + 63) / 64, slices = (hidden + 127) / 128;
-  return mp_region0_bytes(K, hidden) + mp_region1_bytes(K, hidden) + (int64_t)slices * 128 * kb128 * 32 * 4;
+  const int kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS, slices = (hidden + 127) / 128;
+  return (int64_t)kblocks * slices * gs::MP_IMG;
 }
 
 int32_t gs_maxpool_mlp_pack(const float* Wm, int64_t ldw, int32_t K, int32_t hidden, void* workspace, void* stream) {
   GS_REQUIRE(Wm && workspace && K >= 1 && hidden >= 1 && ldw >= hidden, "gs_maxpool_mlp_pack: bad arguments");
   GS_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 127u) == 0, "gs_maxpool_mlp_pack: workspace must be 128-byte aligned");
-  const int kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS, slices = (hidden + 127) / 128, kb128 = (K + 63) / 64;
-  unsigned char* ws = (unsigned char*)workspace;
-  gs::maxpool_pack_kernel<<<kblocks * slices, 256, 0, (cudaStream_t)stream>>>(Wm, ldw, K, hidden, kblocks, ws);
-  gs::maxpool_pack128_kernel<<<kb128 * slices, 256, 0, (cudaStream_t)stream>>>(Wm, ldw, K, hidden, kb128,
-                                                                               ws + mp_region0_bytes(K, hidden));
-  gs::maxpool_pack_rows_kernel<<<dim3(8, slices), 256, 0, (cudaStream_t)stream>>>(
-      Wm, ldw, K, hidden, kb128 * 32, (uint32_t*)(ws + mp_region0_bytes(K, hidden) + mp_region1_bytes(K, hidden)));
+  const int kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS, slices = (hidden + 127) / 128;
+  gs::maxpool_pack_kernel<<<kblocks * slices, 256, 0, (cudaStream_t)stream>>>(Wm, ldw, K, hidden, kblocks,
+                                                                             (unsigned char*)workspace);
   return gs::launch_check("maxpool_pack_kernel");
-}
-
-
-// bf16 table [n_rows, K] (row pitch in elements) as a 2-D tensor map for tile::gather4: box = one K-block segment
-// (32 columns = 64 bytes) of ONE row - the instruction names four rows -, SWIZZLE_64B to match the UMMA stage layout
-static int32_t make_table_tensor_map(CUtensorMap* out, const void* table, int64_t n_rows, int32_t K, int64_t pitch,
-                                     int box_cols = gs::MP_KCOLS) {
-  typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static encode_fn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    GS_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    GS_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled is not available from this driver");
-    encode = (encode_fn)fn;
-  }
-  const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)n_rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)pitch * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)box_cols, 1};   // one K-block segment of ONE row; the instruction names four rows
-  const cuuint32_t estride[2] = {1, 1};
-  const CUresult rc = encode(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(table), gdim, gstride, box, estride,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (rc != CUDA_SUCCESS) {
-    gs::set_error("cuTensorMapEncodeTiled failed (CUresult %d) for table [%lld, %d] pitch %lld", (int)rc, (long long)n_rows, K,
-                  (long long)pitch);
-    return GS_ERR_CUDA;
-  }
-  return GS_OK;
 }
 
 static int32_t pool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch, const int32_t* row_ids,
@@ -1946,13 +316,9 @@ static int32_t pool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
   GS_REQUIRE((pitch * 2) % 16 == 0 && (reinterpret_cast<uintptr_t>(table_bf16) & 15u) == 0,
              "gs_maxpool_mlp_fused: table rows must be 16-byte multiples and 16-byte aligned (pitch %% 8 == 0)");
   GS_REQUIRE((reinterpret_cast<uintptr_t>(packed_weights) & 127u) == 0, "gs_maxpool_mlp_fused: packed weights misaligned");
-  // k4_kernel: 0 = tmem form (weights in tensor memory, 12+ operand stages; default); 3 = wide form, weights resident in
-  //            shared memory, 128-row tiles (k4_wide_producer: 1 TMA gather4, 0 cp.async); 2 = wide form, 256-row tiles;
-  //            1 = round-1 form (gathered rows = A operand, shared-memory transpose in the epilogue)
-  const int kernel_sel = gs::tuning("k4_kernel", 0);
-  const int tile_rows = kernel_sel == 2 ? 256 : kernel_sel == 0 ? (gs::tuning("k4_tile", 128) == 256 ? 256 : 128) : 128;
-  if (k > tile_rows || (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS > gs::MP_MAX_KB || hidden % 128 != 0) {
-    gs::set_error("gs_maxpool_mlp_fused: needs k <= %d, K <= %d, hidden %% 128 == 0 (k=%d K=%d hidden=%d)", tile_rows,
+  const int nt = gs::tuning("k4_tile", 128) == 256 ? 256 : 128;
+  if (k > nt || (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS > gs::MP_MAX_KB || hidden % 128 != 0) {
+    gs::set_error("gs_maxpool_mlp_fused: needs k <= %d, K <= %d, hidden %% 128 == 0 (k=%d K=%d hidden=%d)", nt,
                   gs::MP_MAX_KB * gs::MP_KCOLS, k, K, hidden);
     return GS_ERR_UNSUPPORTED;
   }
@@ -1961,192 +327,24 @@ static int32_t pool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
   memset(&prm, 0, sizeof(prm));
   prm.table = (const __nv_bfloat16*)table_bf16;
   prm.n_rows = n_rows; prm.pitch = pitch; prm.K = K; prm.kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS;
-  prm.row_ids = row_ids; prm.row0 = row0; prm.n_groups = n_groups; prm.k = k; prm.G = tile_rows / k;
-  prm.n_tiles = (n_groups + prm.G - 1) / prm.G;
-  prm.hidden = hidden; prm.n_slices = hidden / 128;
+  prm.row_ids = row_ids; prm.row0 = row0; prm.n_groups = n_groups; prm.k = k; prm.G = nt / k;
+  prm.n_slices = hidden / 128;
   prm.wimg = (const unsigned char*)packed_weights; prm.bias = bias; prm.out = out; prm.ldo = ldo;
   prm.pool_mean = pool_mean;
-  prm.issue_elect = gs::tuning("mma_issue", 1) != 0;
-  if (kernel_sel == 0) {
-    const unsigned char* ws = (const unsigned char*)packed_weights;
-    const int nt = tile_rows;                         // 128 (default) or 256 (k4_tile = 256)
-    prm.kblocks = (K + 63) / 64;
-    prm.G = nt / k;
-    prm.n_tiles = (n_groups + prm.G - 1) / prm.G;
-    prm.kb_t = prm.kblocks < gs::MPT_MAX_KB_T ? prm.kblocks : gs::MPT_MAX_KB_T;
-    prm.n_stages = (gs::MPW_SMEM_BYTES - (prm.kblocks - prm.kb_t) * gs::MPT_IMG) / (nt * 128);
-    if (prm.n_stages > gs::MPT_MAX_STAGES) prm.n_stages = gs::MPT_MAX_STAGES;
-    const int lim = gs::tuning("k4_stages", 0);
-    if (lim >= 4 && lim < prm.n_stages) prm.n_stages = lim;
-    prm.wimg = ws + mp_region0_bytes(K, hidden);
-    prm.wrows = (const uint32_t*)(ws + mp_region0_bytes(K, hidden) + mp_region1_bytes(K, hidden));
-    const void* fn = nt == 256 ? (const void*)gs::maxpool_mlp_tmem_kernel<256> : (const void*)gs::maxpool_mlp_tmem_kernel<128>;
-    const int32_t rc_attr = gs::ensure_dyn_smem(fn, gs::MPW_SMEM);
-    if (rc_attr != GS_OK) return rc_attr;
-    int64_t ctas_t = (int64_t)(gs::sm_count() / prm.n_slices) * prm.n_slices;   // a whole number of slice groups
-    if (ctas_t < prm.n_slices) ctas_t = prm.n_slices;
-    if (ctas_t > prm.n_tiles * prm.n_slices) ctas_t = prm.n_tiles * prm.n_slices;
-    // k4_cluster: cluster size (2, 4 or 8 CTAs = that many hidden slices of one tile share their gathered rows); -1 = all
-    // hidden/128 slices of a tile; 0 = no clusters.  Default 2: pairs fill all 148 SMs (74 clusters), clusters of four only
-    // 132 (33 fit the GPCs): 111 us against 117 us at hop 2.
-    int cl = gs::tuning("k4_cluster", 2);
-    if (cl < 0 || cl > prm.n_slices) cl = prm.n_slices;
-    if (nt == 128 && (cl == 2 || cl == 4 || cl == 8) && prm.n_slices % cl == 0 && prm.n_stages >= gs::MPC_PW) {
-      prm.n_stages -= prm.n_stages % gs::MPC_PW;         // a ring slot is always filled by the same producer warp
-      CUtensorMap tmap;
-      const int32_t rcm = make_table_tensor_map(&tmap, table_bf16, n_rows, K, pitch, 64);
-      if (rcm != GS_OK) return rcm;
-      const void* fnc = cl == 2   ? (const void*)gs::maxpool_mlp_tmemc_kernel<2>
-                        : cl == 4 ? (const void*)gs::maxpool_mlp_tmemc_kernel<4>
-                                  : (const void*)gs::maxpool_mlp_tmemc_kernel<8>;
-      const int32_t rcc = gs::ensure_dyn_smem(fnc, gs::MPW_SMEM);
-      if (rcc != GS_OK) return rcc;
-
-      cudaLaunchConfig_t cfg;
-      memset(&cfg, 0, sizeof(cfg));
-      cfg.gridDim = dim3((unsigned)ctas_t);              // a multiple of n_slices: whole clusters
-      cfg.blockDim = dim3((unsigned)gs::MPC_THREADS);
-      cfg.dynamicSmemBytes = gs::MPW_SMEM;
-      cfg.stream = (cudaStream_t)stream;
-      cudaLaunchAttribute attr;
-      attr.id = cudaLaunchAttributeClusterDimension;
-      attr.val.clusterDim.x = (unsigned)cl;
-      attr.val.clusterDim.y = 1;
-      attr.val.clusterDim.z = 1;
-      cfg.attrs = &attr;
-      cfg.numAttrs = 1;
-      // persistent clusters: launch only as many as can be resident at once (a GPC whose SM count is not a multiple of the
-      // cluster size leaves SMs over, so 148 SMs do not always hold 148 / CL clusters)
-      static int max_clusters[3] = {0, 0, 0};
-      int& mc = max_clusters[cl == 2 ? 0 : cl == 4 ? 1 : 2];
-      if (mc == 0) {
-        int n = 0;
-        GS_CUDA(cudaOccupancyMaxActiveClusters(&n, fnc, &cfg));
-        mc = n > 0 ? n : 1;
-      }
-      // (the grid stays a multiple of n_slices: every tile needs all its slices)
-      if ((int64_t)mc * cl < ctas_t) cfg.gridDim = dim3((unsigned)(((int64_t)mc * cl / prm.n_slices) * prm.n_slices));
-      void* args[2] = {(void*)&prm, (void*)&tmap};
-      GS_CUDA(cudaLaunchKernelExC(&cfg, fnc, args));
-      return gs::launch_check("maxpool_mlp_tmemc_kernel");
-    }
-    if (nt == 128 && gs::tuning("k4_pipes", 1) == 2 && prm.n_stages >= 4) {
-      prm.n_stages &= ~1;                               // two half rings
-      const int32_t rc2 = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_tmem2_kernel, gs::MPW_SMEM);
-      if (rc2 != GS_OK) return rc2;
-      gs::maxpool_mlp_tmem2_kernel<<<(unsigned)ctas_t, gs::MPT_THREADS, gs::MPW_SMEM, (cudaStream_t)stream>>>(prm);
-      return gs::launch_check("maxpool_mlp_tmem2_kernel");
-    }
-    if (nt == 256)
-      gs::maxpool_mlp_tmem_kernel<256><<<(unsigned)ctas_t, gs::MPT_THREADS, gs::MPW_SMEM, (cudaStream_t)stream>>>(prm);
-    else
-      gs::maxpool_mlp_tmem_kernel<128><<<(unsigned)ctas_t, gs::MPT_THREADS, gs::MPW_SMEM, (cudaStream_t)stream>>>(prm);
-    return gs::launch_check("maxpool_mlp_tmem_kernel");
-  }
-  if (kernel_sel != 1) {
-    const int KC = kernel_sel == 3 ? 64 : 32;
-    const int prod = kernel_sel == 3 ? gs::tuning("k4_wide_producer", 1) : 0;     // 1: TMA gather4 (default), 0: cp.async
-    prm.kblocks = (K + KC - 1) / KC;
-    prm.G = tile_rows / k;
-    prm.n_tiles = (n_groups + prm.G - 1) / prm.G;
-    const int w_img = 128 * KC * 2, x_img = tile_rows * KC * 2;
-    prm.n_stages = (gs::MPW_SMEM_BYTES - prm.kblocks * w_img) / x_img;
-    if (prm.n_stages > gs::MPW_MAX_STAGES) prm.n_stages = gs::MPW_MAX_STAGES;
-    if (prod == 1) prm.n_stages = 4;                  // one producer warp per ring slot
-    if (prm.n_stages < 4) {
-      gs::set_error("gs_maxpool_mlp_fused: K=%d leaves %d operand stages (needs 4)", K, prm.n_stages);
-      return GS_ERR_UNSUPPORTED;
-    }
-    prm.dbg = gs::tuning("k4_dbg", 0);
-    if (kernel_sel == 3) prm.wimg += mp_region0_bytes(K, hidden);
-    CUtensorMap tmap;
-    memset(&tmap, 0, sizeof(tmap));
-    if (prod == 1) {
-      const int32_t rc = make_table_tensor_map(&tmap, table_bf16, n_rows, K, pitch, 64);
-      if (rc != GS_OK) return rc;
-    }
-    const void* fn = kernel_sel == 2 ? (const void*)gs::maxpool_mlp_wide_kernel<32, 256, 0>
-                     : prod == 1     ? (const void*)gs::maxpool_mlp_wide_kernel<64, 128, 1>
-                                     : (const void*)gs::maxpool_mlp_wide_kernel<64, 128, 0>;
-    const int32_t rc_attr = gs::ensure_dyn_smem(fn, gs::MPW_SMEM);
-    if (rc_attr != GS_OK) return rc_attr;
-    int64_t ctas_w = (int64_t)(gs::sm_count() / prm.n_slices) * prm.n_slices;   // a whole number of slice groups
-    if (ctas_w < prm.n_slices) ctas_w = prm.n_slices;
-    if (ctas_w > prm.n_tiles * prm.n_slices) ctas_w = prm.n_tiles * prm.n_slices;
-    const int threads = prod == 1 ? (4 + 6) * 32 : (8 + 6) * 32;
-    void* args[2] = {(void*)&prm, (void*)&tmap};
-    GS_CUDA(cudaLaunchKernel(fn, dim3((unsigned)ctas_w), dim3((unsigned)threads), args, gs::MPW_SMEM, (cudaStream_t)stream));
-    return gs::launch_check("maxpool_mlp_wide_kernel");
-  }
-  {
-    int32_t rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_kernel<7, 5>, gs::MP_SMEM);
-    if (rc_attr == GS_OK) rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_kernel<6, 4>, gs::MP_SMEM);
-    if (rc_attr != GS_OK) return rc_attr;
-  }
-  int64_t ctas = (int64_t)(gs::sm_count() / prm.n_slices) * prm.n_slices;   // a whole number of slice groups
-  if (ctas < prm.n_slices) ctas = prm.n_slices;
-  if (ctas > prm.n_tiles * prm.n_slices) ctas = prm.n_tiles * prm.n_slices;
-  const int producer = gs::tuning("k4_producer", 0);
-  if (producer == 2 && (prm.n_slices == 2 || prm.n_slices == 4) && prm.issue_elect) {
-    // clusters of n_slices CTAs, TMA gather4 multicast (see maxpool_mlp_g4mc_kernel)
-    CUtensorMap tmap;
-    const int32_t rc = make_table_tensor_map(&tmap, table_bf16, n_rows, K, pitch);
-    if (rc != GS_OK) return rc;
-    const bool sa7 = prm.kblocks <= gs::MP_RING - 7;
-    const void* fn = prm.n_slices == 4
-                         ? (sa7 ? (const void*)gs::maxpool_mlp_g4mc_kernel<7, 4> : (const void*)gs::maxpool_mlp_g4mc_kernel<6, 4>)
-                         : (sa7 ? (const void*)gs::maxpool_mlp_g4mc_kernel<7, 2> : (const void*)gs::maxpool_mlp_g4mc_kernel<6, 2>);
-    const int32_t rc_attr = gs::ensure_dyn_smem(fn, gs::MP_SMEM);
-    if (rc_attr != GS_OK) return rc_attr;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)ctas);                      // a multiple of n_slices: whole clusters
-    cfg.blockDim = dim3((unsigned)(((sa7 ? 7 : 6) + 6) * 32));
-    cfg.dynamicSmemBytes = gs::MP_SMEM;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = (unsigned)prm.n_slices;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    void* args[2] = {(void*)&prm, (void*)&tmap};
-    GS_CUDA(cudaLaunchKernelExC(&cfg, fn, args));
-    return gs::launch_check("maxpool_mlp_g4mc_kernel");
-  }
-  if (producer >= 1) {
-
-    // TMA gather4 producers (see maxpool_mlp_g4_kernel)
-    {
-      int32_t rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_g4_kernel<7>, gs::MP_SMEM);
-      if (rc_attr == GS_OK) rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_g4_kernel<6>, gs::MP_SMEM);
-      if (rc_attr != GS_OK) return rc_attr;
-    }
-    CUtensorMap tmap;
-    const int32_t rc = make_table_tensor_map(&tmap, table_bf16, n_rows, K, pitch);
-    if (rc != GS_OK) return rc;
-    if (prm.kblocks <= gs::MP_RING - 7)
-      gs::maxpool_mlp_g4_kernel<7><<<(unsigned)ctas, (7 + 6) * 32, gs::MP_SMEM, (cudaStream_t)stream>>>(prm, tmap);
-    else
-      gs::maxpool_mlp_g4_kernel<6><<<(unsigned)ctas, (6 + 6) * 32, gs::MP_SMEM, (cudaStream_t)stream>>>(prm, tmap);
-    return gs::launch_check("maxpool_mlp_g4_kernel");
-  }
-  if (producer == -1) {       // cp.async producers with hardware-fired arrives (no group wait / proxy fence)
-    int32_t rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_kernel<7, 5, true>, gs::MP_SMEM);
-    if (rc_attr == GS_OK) rc_attr = gs::ensure_dyn_smem((const void*)gs::maxpool_mlp_kernel<6, 4, true>, gs::MP_SMEM);
-    if (rc_attr != GS_OK) return rc_attr;
-    if (prm.kblocks <= gs::MP_RING - 7)
-      gs::maxpool_mlp_kernel<7, 5, true><<<(unsigned)ctas, gs::MP_THREADS, gs::MP_SMEM, (cudaStream_t)stream>>>(prm);
-    else
-      gs::maxpool_mlp_kernel<6, 4, true><<<(unsigned)ctas, gs::MP_THREADS, gs::MP_SMEM, (cudaStream_t)stream>>>(prm);
-    return gs::launch_check("maxpool_mlp_kernel<async arrive>");
-  }
-  if (prm.kblocks <= gs::MP_RING - 7)
-    gs::maxpool_mlp_kernel<7, 5><<<(unsigned)ctas, gs::MP_THREADS, gs::MP_SMEM, (cudaStream_t)stream>>>(prm);
-  else
-    gs::maxpool_mlp_kernel<6, 4><<<(unsigned)ctas, gs::MP_THREADS, gs::MP_SMEM, (cudaStream_t)stream>>>(prm);
-  return gs::launch_check("maxpool_mlp_kernel");
+  const int64_t n_tiles = (n_groups + prm.G - 1) / prm.G;
+  GS_REQUIRE(n_tiles * prm.n_slices < 0x7fffffffLL, "gs_maxpool_mlp_fused: too many groups (%lld)", (long long)n_groups);
+  int cluster = gs::tuning("k4_cluster", 0);       // -1 = all slices of a tile; clamped to a divisor of n_slices <= 8
+  if (cluster < 0 || cluster > prm.n_slices) cluster = prm.n_slices;
+  while (cluster > 1 && (cluster > 8 || prm.n_slices % cluster != 0)) --cluster;
+  const int depth = gs::tuning("k4_mma_depth", 1) == 2 ? 2 : 1;
+  const int producer = gs::tuning("k4_producer", 0) == 1 ? 1 : 0;
+  const bool rows_a = gs::tuning("k4_operands", 1) != 0;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (rows_a)
+    return nt == 256 ? gs::launch_k4_by<true, 256>(prm, n_tiles, cluster, depth, producer, st)
+                     : gs::launch_k4_by<true, 128>(prm, n_tiles, cluster, depth, producer, st);
+  return nt == 256 ? gs::launch_k4_by<false, 256>(prm, n_tiles, cluster, depth, producer, st)
+                   : gs::launch_k4_by<false, 128>(prm, n_tiles, cluster, depth, producer, st);
 }
 
 int32_t gs_maxpool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch, const int32_t* row_ids,

@@ -1,4 +1,8 @@
-// tcgen05 / TMEM / UMMA-descriptor helpers shared by the tensor-core kernels (gemm_tc.cu, maxpool_tc.cu).
+// wgmma / shared-memory-descriptor helpers shared by the Hopper tensor-core kernels (gemm_tc.cu, maxpool_tc.cu).
+//
+// Operand tiles in shared memory are K-major with the 128-byte swizzle: 128 rows of 128 bytes, 16-byte chunk c of row r
+// at r * 128 + ((c ^ (r & 7)) << 4), the image 1024-byte aligned.  A warpgroup's wgmma.m64n128 reads 64 rows of the A
+// image and all 128 rows of the B image.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -6,166 +10,68 @@
 
 namespace gs {
 
-constexpr int TC_BM = 128;       // UMMA M (cta_group::1)
-constexpr int TC_BN = 128;       // UMMA N
+constexpr int TC_BM = 128;       // output tile rows (two warpgroups of 64)
+constexpr int TC_BN = 128;       // output tile columns (wgmma N)
 constexpr int TC_TILE_BYTES = TC_BM * 128;   // one operand tile image: 128 rows x 128 B (one SW128 atom wide)
 
-// ---------------------------------------------------------------------------------------------
-// PTX wrappers (tcgen05 / TMEM)
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-template <bool kBf16>
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kBf16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-
-// Warp-uniform issue.  The WHOLE warp executes these with warp-uniform operands; only the instruction is predicated on
-// elect.sync.  ptxas then keeps the descriptors in uniform registers and emits UTCHMMA / UTCBAR back to back.  Issuing
-// from inside `if (lane == 0) { ... }` instead makes it wrap every tcgen05 instruction in an R2UR + ELECT/BRA.U.ANY
-// waterfall: measured 176 cycles per MMA (any N <= 256) against the tensor pipe's 64 (N = 128) / 128 (N = 256) floor,
-// which this form reaches (tools/mma_rate.py, csrc/probe_tc.cu).  elect.sync picks the same leader for the same
-// member mask, so a commit issued this way tracks the MMAs issued this way.
-template <bool kBf16>
-__device__ __forceinline__ void umma_ss_elect(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  if constexpr (kBf16) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\telect.sync _|q, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\telect.sync _|q, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void umma_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar))
-      : "memory");
-}
-
-// as umma_commit_elect, arriving on the barrier at the same shared-memory offset in every CTA of `cta_mask` (cluster)
-__device__ __forceinline__ void umma_commit_elect_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives row (lane base + t)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// narrower TMEM loads (same 32x32b shape: thread t receives lane base + t): N consecutive fp32 columns from `taddr`
-#define GS_TMEM_LD_N(NAME, XN, NREG, OUTS, INIDX)                                                            \
-  __device__ __forceinline__ void NAME(uint32_t taddr, uint32_t (&r)[NREG]) {                                 \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b." XN ".b32 " OUTS ", [%" INIDX "];" : GS_TMEM_OUT_##NREG(r) : "r"(taddr) : "memory"); \
-  }
-#define GS_TMEM_OUT_1(r) "=r"(r[0])
-#define GS_TMEM_OUT_2(r) "=r"(r[0]), "=r"(r[1])
-#define GS_TMEM_OUT_4(r) "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-#define GS_TMEM_OUT_8(r) GS_TMEM_OUT_4(r), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-#define GS_TMEM_OUT_16(r) GS_TMEM_OUT_8(r), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-GS_TMEM_LD_N(tmem_ld_32x1, "x1", 1, "{%0}", "1")
-GS_TMEM_LD_N(tmem_ld_32x2, "x2", 2, "{%0,%1}", "2")
-GS_TMEM_LD_N(tmem_ld_32x4, "x4", 4, "{%0,%1,%2,%3}", "4")
-GS_TMEM_LD_N(tmem_ld_32x8, "x8", 8, "{%0,%1,%2,%3,%4,%5,%6,%7}", "8")
-GS_TMEM_LD_N(tmem_ld_32x16, "x16", 16, "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}", "16")
-// A operand from tensor memory (TS form): D[tmem] (+)= A[tmem] * B[smem desc]; whole warp executes, elect.sync on the instruction
-__device__ __forceinline__ void umma_ts_elect_bf16(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                                   uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\telect.sync _|q, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// registers -> TMEM, 32x32b shape: thread t of the warp writes lane (lane base + t), 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// mbarrier wait whose loop condition is a warp vote: the compiler then knows control flow stays warp-uniform after the
-// wait and keeps descriptors / addresses of the following tcgen05 instructions in uniform registers
-__device__ __forceinline__ void mbar_wait_uniform(uint64_t* bar, uint32_t parity) {
-  while (!__all_sync(0xffffffffu, mbar_try_wait(bar, parity))) {
-  }
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm_100):
-//   [0,14) start address >> 4, [16,30) LBO >> 4 (= 1, unused for swizzled K-major),
-//   [32,46) SBO >> 4 (8 rows x 128 B = 1024 B -> 64), [46,48) version = 1, [61,64) layout = 2 (SWIZZLE_128B)
+// K-major, 128-byte-swizzled shared-memory matrix descriptor (sm_90 wgmma):
+//   [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1),
+//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B), [62,64) layout = 1 (SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// cute::UMMA::InstrDescriptor: [4,6) c_format (1 = F32), [7,10) a_format, [10,13) b_format
-// (F16 = 0, BF16 = 1, TF32 = 2), [15] a_major (0 = K), [16] b_major (0 = K), [17,23) N >> 3, [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define GS_WGMMA_D64                                                                                                       \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,"   \
+  "%61,%62,%63}"
+#define GS_WGMMA_OUT64(d)                                                                                                 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
+      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),             \
+      "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),             \
+      "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]),             \
+      "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]),             \
+      "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),             \
+      "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]),             \
+      "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// D[64 x 128] (+)= A[64 x K] * B[128 x K]^T, both operands K-major in shared memory, fp32 accumulate in registers.
+// kBf16: one K = 16 step of bf16 operands; else one K = 8 step of tf32 operands.  accumulate = 0 overwrites D.
+// Thread t of the warpgroup holds d[4j + e] = D[16 (t / 32) + (t % 32) / 4 + 8 (e / 2)][8 j + 2 (t % 4) + (e % 2)].
+template <bool kBf16>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (kBf16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " GS_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : GS_WGMMA_OUT64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " GS_WGMMA_D64 ", %64, %65, p, 1, 1;\n\t}"
+        : GS_WGMMA_OUT64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+  }
 }
 
 __device__ __forceinline__ uint32_t tf32_mask(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
@@ -175,22 +81,11 @@ __host__ __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
   return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4));
 }
 
-
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(src_bytes) : "memory");
 }
-// the mbarrier receives one arrival (counted against its expected count: .noinc) when all cp.async operations this
-// thread has issued so far have completed - an asynchronous hand-off, the thread itself does not wait
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
 }  // namespace gs

@@ -1,5 +1,5 @@
 """Layer base and Dense - the API shell of reference graphsage/layers.py:28-116 over the
-B200 kernels (Dense is only used as the max-pool aggregator's MLP)."""
+library's CUDA kernels (Dense is only used as the max-pool aggregator's MLP)."""
 import torch
 
 from . import ops

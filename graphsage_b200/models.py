@@ -1,5 +1,5 @@
 """SAGEInfo and SampleAndAggregate.sample / .aggregate - the surface of reference
-graphsage/models.py:178-330 over the B200 kernels.
+graphsage/models.py:178-330 over the library's CUDA kernels.
 
 The TF placeholders / FLAGS the reference threads through become explicit arguments:
 `placeholders` is a plain dict ({"batch_size": int, "dropout": float, ...}).

@@ -352,7 +352,7 @@ def _gather_mean_sharded(src, segments, include_self, want_self, out_pitch, out_
 
 
 def gather_mean_images(src, segments, include_self=False, want_self=True):
-    """gs_gather_mean_img: the fused gather + fanout mean whose result is written as tf32 hi/lo UMMA tile images (the A
+    """gs_gather_mean_img: the fused gather + fanout mean whose result is written as tf32 hi/lo tensor-core tile images (the A
     operand of sage_gemm_img).  Returns (images uint8 tensor, rows) or None when the image form does not apply."""
     sharded = hasattr(src, "c_table")
     if not sharded:
@@ -521,7 +521,7 @@ class PackedMlpWeights(object):
 
 
 def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0, K=None, out=None, pool="max"):
-    """out[g, :] = max_j relu(table[row(g, j), :K] @ W + bias) in one tcgen05 kernel (bf16 operands, fp32 accumulate).
+    """out[g, :] = max_j relu(table[row(g, j), :K] @ W + bias) in one wgmma kernel (bf16 operands, fp32 accumulate).
     table: bfloat16 [rows, >=K] row-major with pitch % 8 == 0; W: float32 [K, hidden] (hidden % 128 == 0)."""
     require_cuda(table, W, bias, row_ids)
     if table.dtype != torch.bfloat16 or table.stride(1) != 1:

@@ -1,7 +1,7 @@
 """SupervisedGraphsage - the training step around the hot path (SURVEY section 8f row 1; reference
 graphsage/supervised_models.py:10-126).
 
-Forward: the B200 kernels (sample -> fused gather+mean -> tcgen05 / fp32 GEMM), wrapped in
+Forward: the library's CUDA kernels (sample -> fused gather+mean -> wgmma / fp32 GEMM), wrapped in
 torch.autograd.Function so the step is differentiable.  Backward: the gradient formulas of the mean / GCN
 aggregators, with the weight-gradient GEMMs (X^T dZ) as plain library matmuls (torch / cuBLAS fp32) - features
 are not trainable (identity_dim = 0), so nothing is scattered into the table.  Head (l2_normalize -> Dense ->

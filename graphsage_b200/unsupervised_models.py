@@ -3,7 +3,7 @@ graphsage/models.py:332-405 `_build` / `_loss` / `_accuracy`, graphsage/predicti
 
 Three passes of the hot path share one set of aggregators (batch1, batch2, and neg_sample_size negatives drawn with
 probability ~ degree^0.75 and shared by the whole batch); skip-gram style cross-entropy on the l2-normalised
-outputs; MRR of the true pair among the negatives.  Forward through the B200 kernels, backward as in
+outputs; MRR of the true pair among the negatives.  Forward through the library's CUDA kernels, backward as in
 supervised_models.py.
 """
 import numpy as np

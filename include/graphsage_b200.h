@@ -1,5 +1,5 @@
 /*
- * graphsage_b200.h - C-ABI of libgraphsage_b200.so (sm_100a).
+ * graphsage_b200.h - C-ABI of libgraphsage_b200.so (sm_90a, H100).
  *
  * The reference (williamleif/GraphSAGE) has NO FFI boundary: its hot path is python
  * classes composing TensorFlow library ops.  Each entry point below therefore names the
@@ -45,9 +45,9 @@ typedef enum {
 /* arithmetic of the dense contraction */
 typedef enum {
   GS_MATH_FP32_SIMT = 0,  /* fp32 FFMA on CUDA cores (bring-up / cross-check path)          */
-  GS_MATH_TF32X3 = 1,     /* tcgen05 kind::tf32, 3-term hi/lo split, fp32 accumulate in TMEM */
-  GS_MATH_TF32 = 2,       /* tcgen05 kind::tf32 single pass                                  */
-  GS_MATH_BF16 = 3        /* tcgen05 kind::f16 (bf16 operands), fp32 accumulate              */
+  GS_MATH_TF32X3 = 1,     /* wgmma tf32, 3-term hi/lo split, fp32 accumulate                 */
+  GS_MATH_TF32 = 2,       /* wgmma tf32 single pass                                          */
+  GS_MATH_BF16 = 3        /* wgmma bf16 operands, fp32 accumulate                            */
 } gs_math;
 
 int32_t gs_version(void);
@@ -55,19 +55,15 @@ const char* gs_last_error_string(void);
 /* Tuning knobs for experiments; returns the previous value.  Keys (default):
  *   gather_variant (2)      gs_gather_mean / gs_gather_rows: 2 grouped double-buffered TMA, 1 whole-node TMA, 0 LDG
  *   gather_ctas_per_sm (8)  grid cap of the LDG / simple gather kernels
- *   gemm_async (0)          gs_sage_gemm tcgen05 producers: 1 = cp.async staging instead of register prefetch
- *   mma_issue (1)           tcgen05 issue form: 1 = whole warp + elect.sync (tensor-pipe floor), 0 = single thread
- *   k4_kernel (0)           gs_maxpool/meanpool_mlp_fused kernel family: 0 = weights in tensor memory, gathered rows = B
- *                           operand (default); 3 / 2 = weights resident in shared memory, 128- / 256-row tiles; 1 = the
- *                           round-1 form (gathered rows = A operand; k4_producer 0 cp.async, 1 gather4, 2 gather4 multicast)
- *   k4_cluster (2)          k4_kernel 0: thread-block cluster size (2, 4, 8; -1 = hidden / 128; 0 = no clusters) - the CTAs
- *                           of a cluster share one gathered tile through TMA gather4 multicast
- *   k4_tile (128)           k4_kernel 0: rows per tile (128; 256 = the wide tile, which runs without clusters)
- *   k4_pipes (1)            k4_kernel 0 without clusters: 2 = two half-ring pipelines / two accumulators
- *   k4_stages (0)           k4_kernel 0: cap on the operand ring depth (0 = as many as fit)
- *   k4_wide_producer (1)    k4_kernel 3: 1 = TMA gather4 producers, 0 = cp.async producers
  *   halo_fetch_ctas_per_sm (2)  grid of gs_halo_fetch
- * Every K4 variant is parity-tested (tests/test_gpu_parity.py: K4_VARIANTS); DESIGN.md section 4a has the measurements.
+ *   k4_operands (1)         gs_maxpool/meanpool_mlp_fused: 1 = gathered rows are the wgmma A operand, 0 = the weight slice is
+ *                           A and the gathered rows are B
+ *   k4_tile (128)           rows per K4 tile: 128 (fanout <= 128) or 256 (fanout <= 256)
+ *   k4_mma_depth (1)        wgmma groups in flight in the K4 K loop (1 or 2)
+ *   k4_producer (0)         K4 row gather: 0 = cp.async 16-byte pieces, 1 = register-staged 128-bit loads
+ *   k4_cluster (0)          launch a tile's hidden slices as a thread-block cluster of this size (-1 = all slices; clamped to
+ *                           a divisor of hidden / 128 that is <= 8; 0 = no clusters)
+ * Every K4 configuration the tests name is parity-tested (tests/test_gpu_parity.py: K4_VARIANTS).
  * The Python host also reads them from the environment: GS_TUNING="key=value,key=value". */
 int32_t gs_set_tuning(const char* key, int32_t value);
 
@@ -293,7 +289,7 @@ int32_t gs_sage_gemm_prepacked(int64_t M, const gs_gemm_part* parts_host, int32_
  *   gs_gather_mean_img : the fused gather + fanout mean of gs_gather_mean / gs_gather_mean_sharded (same segments, same
  *       table forms: pass `src` (dense fp32 [n_src_rows, pitch]) or `table_host` (node-partitioned; ids_are_locators /
  *       staging as in gs_gather_mean_sharded)), whose result rows are written ALREADY SPLIT into tf32 hi / lo and laid
- *       out as UMMA K-major SWIZZLE_128B tile images: part p (0 = self rows, 1 = mean rows when want_self; only the mean
+ *       out as K-major SWIZZLE_128B tensor-core tile images: part p (0 = self rows, 1 = mean rows when want_self; only the mean
  *       part when !want_self), 128-row tile mt, 32-column K-block kb at
  *       images + (((p * n_mtiles + mt) * kblocks + kb) * 2 + hl) * 16384, hl = 0 hi / 1 lo.  images: device buffer of
  *       gs_gather_mean_img_bytes(rows, F, want_self) bytes, 1024-byte aligned; rows = max(out_row0 + n).
@@ -331,7 +327,7 @@ int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int32_t F, int
                             void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * K4 - the max-pool aggregator's neighbour branch fused end to end on tcgen05 (bf16 operands, fp32
+ * K4 - the max-pool aggregator's neighbour branch fused end to end on the tensor cores (wgmma, bf16 operands, fp32
  * accumulate):   out[g, h] = max_{j<k} relu( table[row(g,j), 0:K] . Wm[0:K, h] + bm[h] )
  *   reference graphsage/aggregators.py:176-182 (reshape -> Dense(relu,bias) -> reshape -> reduce_max),
  *   graphsage/layers.py:104-116, with the gather of graphsage/models.py:299 fused in front.

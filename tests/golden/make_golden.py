@@ -351,6 +351,48 @@ def golden_heads():
     save("heads", **out)
 
 
+def golden_toy_ppi():
+    """A connected slice of the reference's example_data/toy-ppi (900 train, 200 val, 200 test nodes, breadth-first from
+    the first node of each kind, with the links among them) for the ingest / config-1 tests, which rebuild the
+    toy-ppi files from it.  The expected counts are taken from the raw JSON here, not from the loader under test."""
+    import json
+    prefix = "/root/reference/example_data/toy-ppi"
+    g = json.load(open(prefix + "-G.json"))
+    feats = np.load(prefix + "-feats.npy")
+    id_map = json.load(open(prefix + "-id_map.json"))
+    class_map = json.load(open(prefix + "-class_map.json"))
+    nodes = {n["id"]: n for n in g["nodes"]}
+    kind = {i: (bool(n["val"]), bool(n["test"])) for i, n in nodes.items()}
+    adj = {}
+    for l in g["links"]:
+        s, t = g["nodes"][l["source"]]["id"], g["nodes"][l["target"]]["id"]
+        adj.setdefault(s, []).append(t)
+        adj.setdefault(t, []).append(s)
+    keep = []
+    for want, quota in (((False, False), 900), ((True, False), 200), ((False, True), 200)):
+        start = next(i for i in sorted(nodes) if kind[i] == want)
+        seen, queue = {start}, [start]
+        while queue and len(seen) < quota:
+            u = queue.pop(0)
+            for v in adj.get(u, []):
+                if v not in seen and kind[v] == want and len(seen) < quota:
+                    seen.add(v)
+                    queue.append(v)
+        keep += sorted(seen)
+    keep = sorted(keep)
+    pos = {u: i for i, u in enumerate(keep)}
+    links = [(g["nodes"][l["source"]]["id"], g["nodes"][l["target"]]["id"], l["test_removed"], l["train_removed"])
+             for l in g["links"]]
+    links = [(pos[s], pos[t], a, b) for s, t, a, b in links if s in pos and t in pos]
+    kinds = [kind[u] for u in keep]
+    save("toy_ppi", ids=np.array(keep, np.int32), val=np.array([k[0] for k in kinds]), test=np.array([k[1] for k in kinds]),
+         feats=feats[[id_map[str(u)] for u in keep]], labels=np.packbits(np.array([class_map[str(u)] for u in keep], np.uint8), axis=1),
+         n_classes=np.int32(len(class_map[str(keep[0])])), src=np.array([l[0] for l in links], np.int16),
+         dst=np.array([l[1] for l in links], np.int16), test_removed=np.array([l[2] for l in links]),
+         train_removed=np.array([l[3] for l in links]),
+         n_kind=np.array([kinds.count((False, False)), kinds.count((True, False)), kinds.count((False, True))], np.int64))
+
+
 def _standalone(fn):
     """meanpool / iterators / heads were added after the first four fixtures: each starts from a fresh initialiser
     stream, so regenerating everything reproduces every committed file."""
@@ -359,7 +401,7 @@ def _standalone(fn):
 
 
 if __name__ == "__main__":
-    later = {"meanpool": golden_meanpool, "iterators": golden_iterators, "heads": golden_heads}
+    later = {"meanpool": golden_meanpool, "iterators": golden_iterators, "heads": golden_heads, "toy_ppi": golden_toy_ppi}
     if len(sys.argv) > 1:
         _standalone(later[sys.argv[1]])
         sys.exit(0)

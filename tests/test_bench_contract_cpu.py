@@ -1,6 +1,6 @@
 """bench.py's driver contract, checked without a GPU: the reference arm (`--impl reference`, the reference op sequence on
 the host cores) prints one JSON line carrying every key the contract names, and its `config` is the SAME dict as the one
-the CUDA arm printed on the B200 (profiles/bench_r02_final_1gpu.json) - the driver compares the two arms on it."""
+the CUDA arm printed on an H100 (tests/golden/bench_line_1gpu.json) - the two arms are compared on it."""
 import json
 import os
 import subprocess
@@ -28,7 +28,7 @@ def test_reference_arm_line_and_shared_config():
     assert d["e2e"] == {"value": d["value"], "unit": d["unit"], "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     cb = d["cpu_baseline"]
     assert cb["kind"] == "port" and cb["cores"] >= 1 and cb["value"] == d["value"] and "seeds" in cb["sample"]
-    gpu_line = json.load(open(os.path.join(ROOT, "profiles", "bench_r02_final_1gpu.json")))
+    gpu_line = json.load(open(os.path.join(ROOT, "tests", "golden", "bench_line_1gpu.json")))
     assert gpu_line["config"] == d["config"], "both arms must describe the workload with the same config dict"
     for k in ("metric", "unit", "higher_is_better", "scaling", "data"):
         assert gpu_line[k] == d[k], k

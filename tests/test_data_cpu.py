@@ -17,7 +17,7 @@ from graphsage_b200 import minibatch, utils  # noqa: E402
 from graphsage_b200.graph import Graph, node_link_graph, to_csr  # noqa: E402
 
 GOLD = os.path.join(HERE, "golden", "iterators.npz")
-TOY = "/root/reference/example_data/toy-ppi"
+TOY = os.path.join(HERE, "golden", "toy_ppi.npz")      # a connected slice of the reference's example_data/toy-ppi
 
 
 def fixture_graph():
@@ -258,13 +258,37 @@ def test_random_walk_pairs():
     assert all(H.degree(a) > 0 for a in per_start)
 
 
-@pytest.mark.skipif(not os.path.exists(TOY + "-G.json"), reason="reference example_data not present on this machine")
-def test_toy_ppi_ingest_and_tables():
-    G, feats, id_map, walks, class_map = utils.load_data(TOY, normalize=True, load_walks=False)
-    assert len(G) == 14755 and len(G.edges()) == 228431 and feats.shape == (14755, 50) and len(id_map) == 14755
+@pytest.fixture(scope="module")
+def toy(tmp_path_factory):
+    """The toy-ppi slice written back in the reference's file layout (<prefix>-G.json node-link graph, -feats.npy,
+    -id_map.json, -class_map.json); returns (prefix, the fixture arrays)."""
+    import json
+    d = np.load(TOY)
+    prefix = str(tmp_path_factory.mktemp("toy") / "toy-ppi")
+    ids = [int(u) for u in d["ids"]]
+    labels = np.unpackbits(d["labels"], axis=1)[:, :int(d["n_classes"])]
+    g = {"directed": False, "multigraph": False, "graph": {"name": "toy-ppi slice"},
+         "nodes": [{"id": u, "val": bool(v), "test": bool(t)} for u, v, t in zip(ids, d["val"], d["test"])],
+         "links": [{"source": int(a), "target": int(b), "test_removed": bool(x), "train_removed": bool(y)}
+                   for a, b, x, y in zip(d["src"], d["dst"], d["test_removed"], d["train_removed"])]}
+    with open(prefix + "-G.json", "w") as fp:
+        json.dump(g, fp)
+    np.save(prefix + "-feats.npy", d["feats"])
+    with open(prefix + "-id_map.json", "w") as fp:
+        json.dump({str(u): i for i, u in enumerate(ids)}, fp)
+    with open(prefix + "-class_map.json", "w") as fp:
+        json.dump({str(u): [int(x) for x in row] for u, row in zip(ids, labels)}, fp)
+    return prefix, d
+
+
+def test_toy_ppi_ingest_and_tables(toy):
+    prefix, d = toy
+    n_all, n_links = len(d["ids"]), len(d["src"])
+    G, feats, id_map, walks, class_map = utils.load_data(prefix, normalize=True, load_walks=False)
+    assert len(G) == n_all and len(G.edges()) == n_links and feats.shape == (n_all, 50) and len(id_map) == n_all
     assert len(next(iter(class_map.values()))) == 121 and isinstance(next(iter(id_map)), int)
     kinds = [(G.node[n]["val"], G.node[n]["test"]) for n in G.nodes()]
-    assert kinds.count((False, False)) == 9716 and kinds.count((True, False)) == 1825 and kinds.count((False, True)) == 3214
+    assert [kinds.count((False, False)), kinds.count((True, False)), kinds.count((False, True))] == list(d["n_kind"])
     tr = np.array([id_map[n] for n in G.nodes() if not G.node[n]["val"] and not G.node[n]["test"]])
     assert np.allclose(feats[tr].mean(axis=0), 0, atol=1e-9)
     np.random.seed(123)
@@ -286,14 +310,13 @@ def test_toy_ppi_ingest_and_tables():
     assert all(it.deg[id_map[u]] > 0 for u in it.train_nodes)
 
 
-@pytest.mark.skipif(not os.path.exists(TOY + "-G.json"), reason="reference example_data not present on this machine")
-def test_config1_toy_ppi_cpu_oracle_path_loss_decreases():
+def test_config1_toy_ppi_cpu_oracle_path_loss_decreases(toy):
     """SURVEY 8d config 1: toy-ppi, graphsage_mean, B = 512, max_degree 128, dims [50, 128, 128], 121 sigmoid classes,
     fanouts [25, 10], lr 0.01 (reference supervised_train.py:32-49) on the CPU oracle path (oracle/torch_ref.py):
     ingest -> iterator -> sample -> gather -> aggregate -> l2-normalise -> Dense head -> sigmoid xent -> clipped Adam."""
     import torch
     from oracle import torch_ref
-    G, feats, id_map, _, class_map = utils.load_data(TOY, normalize=True)
+    G, feats, id_map, _, class_map = utils.load_data(toy[0], normalize=True)
     np.random.seed(123)
     it = minibatch.NodeMinibatchIterator(G, id_map, None, class_map, 121, batch_size=512, max_degree=128)
     n, F, D, C = len(id_map), feats.shape[1], 128, 121
@@ -313,6 +336,8 @@ def test_config1_toy_ppi_cpu_oracle_path_loss_decreases():
     it.shuffle()
     losses = []
     for step in range(12):
+        if it.end():                                                  # next epoch (supervised_train.py:263-268)
+            it.shuffle()
         feed, labels = it.next_minibatch_feed_dict()
         seeds = torch.tensor(feed["batch"], dtype=torch.int32)
         out = torch_ref.forward(adj_t, feats_t, seeds, [25, 10], aggs, True, "mean", 123, 2 * step, normalize=True)

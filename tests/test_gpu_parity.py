@@ -309,7 +309,7 @@ BF16_TOL = 2e-2      # config 3 (bf16 operands, fp32 accumulate) vs the fp32 ora
 
 
 def test_full_size_maxpool_bf16_vs_oracle(gs, reddit):
-    """BASELINE configs[2] at its own size: bf16 feature table, K4 (tcgen05) for both layers' MLPs, against
+    """BASELINE configs[2] at its own size: bf16 feature table, K4 (wgmma) for both layers' MLPs, against
     oracle.forward_2hop (reference aggregators.py:168-195) - once on the fp32 operands (bf16 tolerance) and once on the
     bf16-rounded feature table + MLP weights (what K4 multiplies), where only layer 1's activation cast is left."""
     gs.set_default_math("bf16")
@@ -464,7 +464,7 @@ def test_graphed_forward_matches_eager_and_oracle(gs):
     runner.close()
 
 
-# ---------------------------------------------------------------- tcgen05 GEMM (all math modes) vs fp64
+# ---------------------------------------------------------------- tensor-core GEMM (all math modes) vs fp64
 GEMM_TOL = {"fp32": 2e-6, "tf32x3": 2e-5, "tf32": 3e-3, "bf16": 2e-2}
 
 
@@ -581,7 +581,7 @@ def test_packed_weights_follow_weight_updates(gs):
         gs.set_default_math("fp32")
 
 
-# ---------------------------------------------------------------- K4: fused max-pool MLP (bf16 tcgen05)
+# ---------------------------------------------------------------- K4: fused max-pool MLP (bf16 wgmma)
 @pytest.mark.parametrize("case", [
     # (n_groups, k, K, hidden, use_ids)
     (5120, 25, 602, 512, True),        # bench shape, hop 2 of layer 0 (one 10th of it)
@@ -594,53 +594,56 @@ def test_packed_weights_follow_weight_updates(gs):
 @pytest.mark.parametrize("variant", ["tmem128c", "tmem128c2", "tmem128", "tmem128x2", "tmem256", "wide128_tma", "wide128_cpasync", "wide256_cpasync", "round1"])
 def test_maxpool_mlp_fused_vs_reference(gs, case, variant):
     n_groups, k, K, hidden, use_ids = case
-    if k > K4_VARIANTS[variant][2]:
-        pytest.skip("fanout %d needs a wider tile than %d" % (k, K4_VARIANTS[variant][2]))
+    if k > K4_VARIANTS[variant][1]:
+        pytest.skip("fanout %d needs a wider tile than %d" % (k, K4_VARIANTS[variant][1]))
     _k4_select(gs, variant)
     try:
         _maxpool_mlp_case(gs, n_groups, k, K, hidden, use_ids)
     finally:
-        _k4_select(gs, "tmem128c2")
+        _k4_select(gs, K4_DEFAULT)
 
 
-# name -> (k4_kernel, k4_wide_producer, tile rows, k4_pipes, k4_cluster)
-K4_VARIANTS = {"tmem128c2": (0, 1, 128, 1, 2),        # default: weights in tensor memory, PAIRS of a tile's hidden slices form a
-                                                      # cluster, rows gathered once per cluster by TMA gather4 multicast
-               "tmem128c": (0, 1, 128, 1, -1),        # clusters of all hidden/128 slices of a tile
-               "tmem128": (0, 1, 128, 1, 0),          # one CTA per slice gathers its own rows (cp.async)
-               "tmem128x2": (0, 1, 128, 2, 0),        # two producer->MMA chains per CTA
-               "tmem256": (0, 1, 256, 1, 0),          # one chain, one 256-column accumulator
-               "wide128_tma": (3, 1, 128, 1, 0),      # weights resident in shared memory, 128-row tiles, TMA gather4 producers
-               "wide128_cpasync": (3, 0, 128, 1, 0),  # same geometry, cp.async producers
-               "wide256_cpasync": (2, 0, 256, 1, 0),  # 256-row tiles, 64-byte row pieces
-               "round1": (1, 0, 128, 1, 0)}           # gathered rows = A operand, shared-memory transpose in the epilogue
+# name -> (k4_operands, k4_tile, k4_mma_depth, k4_producer, k4_cluster): the Hopper kernel configuration each named variant
+# runs (maxpool_tc.cu).  k4_operands 1 = gathered rows are the wgmma A operand, 0 = the weight slice is A and the rows are
+# B; k4_tile = rows per tile; k4_mma_depth = wgmma groups in flight; k4_producer 0 = cp.async row pieces, 1 = register-
+# staged 128-bit loads; k4_cluster = thread-block cluster of a tile's hidden slices (-1 = all of them, 0 = none).
+K4_VARIANTS = {"tmem128c2": (0, 128, 1, 0, 2),        # weights as A, PAIRS of a tile's hidden slices form a cluster
+               "tmem128c": (0, 128, 1, 0, -1),        # weights as A, clusters of all hidden/128 slices of a tile
+               "tmem128": (0, 128, 1, 0, 0),          # weights as A, no clusters
+               "tmem128x2": (0, 128, 2, 0, 0),        # weights as A, two wgmma groups in flight
+               "tmem256": (0, 256, 1, 0, 0),          # weights as A, 256-row tiles (N = 2 x 128 per K step)
+               "wide128_tma": (0, 128, 1, 1, 0),      # weights as A, register-staged row loads
+               "wide128_cpasync": (1, 128, 2, 0, 0),  # rows as A, two wgmma groups in flight
+               "wide256_cpasync": (1, 256, 1, 0, 0),  # rows as A, 256-row tiles (two m64 blocks per warpgroup)
+               "round1": (1, 128, 1, 0, 0)}           # rows as A, 128-row tiles: the default
+K4_DEFAULT = "round1"
 
 
 def _k4_select(gs, name):
-    kernel, producer, tile, pipes, cluster = K4_VARIANTS[name]
-    gs._lib.set_tuning("k4_kernel", kernel)
-    gs._lib.set_tuning("k4_wide_producer", producer)
+    operands, tile, depth, producer, cluster = K4_VARIANTS[name]
+    gs._lib.set_tuning("k4_operands", operands)
     gs._lib.set_tuning("k4_tile", tile)
-    gs._lib.set_tuning("k4_pipes", pipes)
+    gs._lib.set_tuning("k4_mma_depth", depth)
+    gs._lib.set_tuning("k4_producer", producer)
     gs._lib.set_tuning("k4_cluster", cluster)
 
 
 def test_maxpool_mlp_fused_wide_fanouts(gs):
-    """ragged last tiles, one group per tile, single-K-block tiles, odd tile counts per CTA, K with / without a
-    shared-memory weight part, fanouts above 128 (256-row tiles only)"""
+    """ragged last tiles, one group per tile, single-K-block tiles, odd tile counts, K with / without a partial last
+    K-block, fanouts above 128 (256-row tiles only); a fanout above the tile is refused"""
     cases = ((7, 128, 602, 128), (1, 25, 602, 512), (2049, 3, 96, 128), (11, 100, 300, 128), (3, 33, 640, 256),
              (900, 5, 64, 128), (333, 7, 33, 128), (260, 25, 512, 256), (260, 25, 513, 128), (1500, 25, 602, 128))
     wide = ((7, 200, 602, 128), (2, 256, 64, 256), (11, 129, 300, 128), (700, 9, 32, 128))
     try:
         for name in ("tmem128c", "tmem128c2", "tmem128", "tmem128x2", "tmem256", "wide128_tma", "wide128_cpasync", "wide256_cpasync"):
             _k4_select(gs, name)
-            tile = K4_VARIANTS[name][2]
+            tile = K4_VARIANTS[name][1]
             for case in cases + (wide if tile == 256 else ()):
                 _maxpool_mlp_case(gs, *case, True)
             with pytest.raises(RuntimeError, match="k <= %d" % tile):
                 _maxpool_mlp_case(gs, 2, tile + 1, 64, 128, True)
     finally:
-        _k4_select(gs, "tmem128c2")
+        _k4_select(gs, K4_DEFAULT)
 
 
 def _maxpool_mlp_case(gs, n_groups, k, K, hidden, use_ids):

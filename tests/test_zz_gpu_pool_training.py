@@ -1,7 +1,7 @@
 """GPU: training step with the pooling aggregators (SURVEY 8f row 1) - loss and gradients of SupervisedGraphsage
 (aggregator_type maxpool / meanpool, unfused fp32 kernels) against torch-CPU autograd on the oracle's op sequence.
 
-First run on a B200 in round 1 (passed); a regression now fails the suite."""
+A regression fails the suite."""
 import numpy as np
 import pytest
 import torch

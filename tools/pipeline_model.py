@@ -115,7 +115,7 @@ def simulate(kind, sa, total_it, n_prod, cl=1, seed=0, stage_bytes=8192, max_ste
             def retire(s=s):
                 c.retired[s] = True
                 for dst in (ctas if kind == "g4mc" else [c]):
-                    dst.empty[s].arrive()                        # tcgen05.commit (multicast in g4mc)
+                    dst.empty[s].arrive()                        # the MMA commit (multicast in the cluster form)
             later(retire)
             yield None
 
