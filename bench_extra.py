@@ -109,16 +109,43 @@ def run_train(args, g, rank, world, local_rank, dist, dev):
     table = torch.zeros((N_NODES + 1, gs.ops.pad_cols(F)), dtype=torch.float32, device=dev)
     table[:, :F] = torch.from_numpy(g["features"]).to(dev)
     adj_dev = torch.from_numpy(g["adj"]).to(dev)
-    sampler = gs.UniformNeighborSampler(adj_dev, seed=123)
-    infos = [gs.SAGEInfo("node", sampler, FANOUT[0], DIM), gs.SAGEInfo("node", sampler, FANOUT[1], DIM)]
-    model = gs.SupervisedGraphsage(n_classes, {"batch_size": BATCH, "dropout": 0.}, table[:, :F], adj_dev, None, infos, concat=True,
-                                   aggregator_type="mean", sigmoid_loss=False, learning_rate=0.01, device=dev,
-                                   distributed=world > 1)
+
+    def make_model(features, identity_dim=0):
+        sampler = gs.UniformNeighborSampler(adj_dev, seed=123)
+        infos = [gs.SAGEInfo("node", sampler, FANOUT[0], DIM), gs.SAGEInfo("node", sampler, FANOUT[1], DIM)]
+        return gs.SupervisedGraphsage(n_classes, {"batch_size": BATCH, "dropout": 0.}, features, adj_dev, None, infos,
+                                      concat=True, aggregator_type="mean", sigmoid_loss=False, learning_rate=0.01, device=dev,
+                                      distributed=world > 1, identity_dim=identity_dim)
+
+    model = make_model(table[:, :F])
     rs = np.random.RandomState(4000 + rank)
     total = args.warmup + args.steps
     seeds = torch.from_numpy(rs.randint(0, N_NODES, size=(total, BATCH)).astype(np.int32)).to(dev)
     labels = torch.nn.functional.one_hot(torch.from_numpy(g["comm"][seeds.cpu().numpy().reshape(-1)].astype(np.int64)),
                                          n_classes).float().reshape(total, BATCH, n_classes).to(dev)   # label = community
+    ms, losses, launches = _timed_train_steps(model, seeds, labels, args, dist, dev)
+    identity = None
+    if getattr(args, "identity_dim", 0) > 0:
+        del model
+        identity = _identity_train(args, make_model(None if args.featureless else table[:, :F], args.identity_dim), seeds,
+                                   labels, ms, dist, dev)
+    if rank != 0:
+        return
+    if identity is not None:
+        print(json.dumps(identity))
+        return
+    print(json.dumps({
+        "metric": "training_seed_nodes_per_sec", "workload": "supervised graphsage_mean training step (fwd + bwd + clipped Adam), "
+        "reddit-shape synthetic, 2-hop 25x10, batch %d, 41 classes (label = community)" % BATCH,
+        "value": world * BATCH * args.steps / (ms * 1e-3), "unit": "nodes/s", "n_gpus": world, "steps": args.steps,
+        "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "dtype": "f32", "data": "synthetic",
+        "loss_first": float(losses[0]), "loss_last": float(losses[-1]), "gpu_launches": launches,
+        "note": "forward = the library's kernels, backward = autograd formulas with library (cuBLAS) GEMMs; eager launches, no CUDA graph"}))
+
+
+def _timed_train_steps(model, seeds, labels, args, dist, dev):
+    """args.warmup untimed, then args.steps timed train_step calls; (ms per step summed over the region, losses, launches)."""
+    import graphsage_b200 as gs
     for i in range(args.warmup):
         model.train_step(seeds[i], labels[i])
     _sync(dist, dev)
@@ -130,17 +157,71 @@ def run_train(args, g, rank, world, local_rank, dist, dev):
         losses.append(model.train_step(seeds[args.warmup + i], labels[args.warmup + i]))
     e1.record()
     _sync(dist, dev)
-    ms = _max_over_ranks(dist, dev, e0.elapsed_time(e1))
-    launches = gs.ops.LAUNCHES - l0
-    if rank != 0:
-        return
-    print(json.dumps({
-        "metric": "training_seed_nodes_per_sec", "workload": "supervised graphsage_mean training step (fwd + bwd + clipped Adam), "
-        "reddit-shape synthetic, 2-hop 25x10, batch %d, 41 classes (label = community)" % BATCH,
-        "value": world * BATCH * args.steps / (ms * 1e-3), "unit": "nodes/s", "n_gpus": world, "steps": args.steps,
-        "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "dtype": "f32", "data": "synthetic",
+    return _max_over_ranks(dist, dev, e0.elapsed_time(e1)), losses, gs.ops.LAUNCHES - l0
+
+
+def _identity_train(args, model, seeds, labels, ms_base, dist, dev):
+    """The same supervised step with a trainable [N+1, D] node-embedding table (identity_dim = D; reference
+    supervised_models.py:51-62), plus the two costs the table adds on their own: the embedding-gradient kernel
+    (gs_embedding_grad, on the layer-0 lists of a real step) and the dense Adam update of the [N+1, D] table."""
+    from graphsage_b200 import ops, supervised_models as sm
+    ms, losses, launches = _timed_train_steps(model, seeds, labels, args, dist, dev)
+    D, n_rows = model.embeds.shape[1], model.embeds.shape[0]
+    # the layer-0 lists of one more step, replayed through the kernel alone
+    seen = {}
+    real = sm._embedding_grad
+
+    def keep(emb_shape, lists):
+        seen["lists"] = lists
+        return real(emb_shape, lists)
+
+    sm._embedding_grad = keep
+    try:
+        model.train_step(seeds[0], labels[0])
+    finally:
+        sm._embedding_grad = real
+    lists = seen["lists"]
+    contributions = sum(int(ids.numel()) for ids, _, _, _ in lists)
+    out = torch.empty((n_rows, D), dtype=torch.float32, device=dev)
+    reps = 20
+    for _ in range(3):
+        ops.embedding_grad(lists, n_rows, D, out=out)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        ops.embedding_grad(lists, n_rows, D, out=out)
+    e1.record()
+    torch.cuda.synchronize(dev)
+    kernel_us = e0.elapsed_time(e1) * 1e3 / reps
+    kernel_bytes = contributions * (4 + 4 * D) + n_rows * D * 4     # ids + one gradient row per contribution + dense output
+    # dense Adam over the table alone (reads param, grad, m, v; writes param, m, v)
+    emb = model.embeds
+    emb.grad = out.clone()
+    opt = torch.optim.Adam([emb], lr=0.01)
+    for _ in range(3):
+        opt.step()
+    e0.record()
+    for _ in range(reps):
+        opt.step()
+    e1.record()
+    torch.cuda.synchronize(dev)
+    adam_us = e0.elapsed_time(e1) * 1e3 / reps
+    F_in = model.features.shape[1] - D
+    return {
+        "metric": "training_seed_nodes_per_sec", "workload": "supervised graphsage_mean training step (fwd + bwd + clipped Adam) "
+        "with a trainable [N+1, %d] node-embedding table%s, reddit-shape synthetic, 2-hop 25x10, batch %d, 41 classes"
+        % (D, " and no features" if F_in == 0 else " before %d feature columns" % F_in, BATCH),
+        "value": BATCH * args.steps / (ms * 1e-3), "unit": "nodes/s", "n_gpus": 1, "steps": args.steps,
+        "warmup": args.warmup, "ms_per_step": ms / args.steps, "ms_per_step_without_embeddings": ms_base / args.steps,
+        "identity_dim": D, "features": F_in, "higher_is_better": True, "dtype": "f32", "data": "synthetic",
         "loss_first": float(losses[0]), "loss_last": float(losses[-1]), "gpu_launches": launches,
-        "note": "forward = the library's kernels, backward = autograd formulas with library (cuBLAS) GEMMs; eager launches, no CUDA graph"}))
+        "embedding_grad": {"us": kernel_us, "contributions": contributions, "lists": len(lists), "algorithmic_bytes": kernel_bytes,
+                           "GB_per_s": kernel_bytes / (kernel_us * 1e-6) / 1e9},
+        "adam_embeddings": {"us": adam_us, "bytes_per_tensor": n_rows * D * 4, "algorithmic_bytes": 7 * n_rows * D * 4,
+                            "GB_per_s": 7 * n_rows * D * 4 / (adam_us * 1e-6) / 1e9},
+        "note": "the without-embeddings step runs first in the same process on the same seeds; embedding_grad = one call of "
+                "the library's deterministic scatter kernel on the layer-0 lists of a real step; adam_embeddings = "
+                "torch.optim.Adam.step over the [N+1, D] table view alone"}
 
 
 def run_rmat(args, rank, world, local_rank, dist, dev):

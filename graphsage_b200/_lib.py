@@ -38,6 +38,13 @@ class GemmPart(ctypes.Structure):
     _fields_ = [("A", c_vp), ("lda", c_i64), ("K", c_i32), ("B", c_vp), ("ldb", c_i64), ("N", c_i32)]
 
 
+MAX_EMBED_LISTS = 8
+
+
+class EmbedGradList(ctypes.Structure):
+    _fields_ = [("ids", c_vp), ("grad", c_vp), ("ldg", c_i64), ("n", c_i64), ("group", c_i32), ("scale", ctypes.c_float)]
+
+
 _SIGNATURES = {
     "gs_version": (c_i32, []),
     "gs_last_error_string": (ctypes.c_char_p, []),
@@ -95,6 +102,8 @@ _SIGNATURES = {
                                  c_vp, c_vp]),
     "gs_l2_normalize_rows": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp]),
     "gs_bump_counter": (c_i32, [c_vp, c_u64, c_vp]),
+    "gs_embedding_grad_workspace_bytes": (c_i64, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32]),
+    "gs_embedding_grad": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, c_vp, c_i64, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

@@ -29,6 +29,8 @@ class SampleAndAggregate(object):
     features : float32 CUDA tensor [N+1, F] whose LAST row is the all-zero dummy row
                (reference supervised_train.py:133-135), or a numpy array (uploaded, dummy row NOT added).
     adj      : int32 CUDA tensor [N+1, max_degree] padded adjacency (reference minibatch.py:227-245).
+    identity_dim : d > 0 adds a trainable [N+1, d] embedding table (`self.embeds`) in front of the features, or replaces
+               them when features is None (see _init_identity_table).
     """
 
     def __init__(self, placeholders, features, adj, degrees, layer_infos, concat=True, aggregator_type="mean",
@@ -42,15 +44,19 @@ class SampleAndAggregate(object):
                                           % aggregator_type)
             raise ValueError("Unknown aggregator: %r" % (aggregator_type,))
         self.aggregator_cls = _AGGREGATORS[aggregator_type]
-        if identity_dim > 0:
-            raise NotImplementedError("identity_dim > 0 (trainable node embeddings) is out of scope (SURVEY appendix A)")
-        if features is None:
+        if features is None and not identity_dim > 0:
             raise ValueError("Must have a positive value for identity feature dimension if no input features given.")
         self.placeholders = placeholders if placeholders is not None else {}
         self.inputs1 = self.placeholders.get("batch1")
         self.inputs2 = self.placeholders.get("batch2")
         self.model_size = model_size
         self.adj_info = adj
+        self.identity_dim, self.embeds = int(identity_dim), None
+        if identity_dim > 0:
+            self._init_identity_table(features, adj, int(identity_dim), device)
+            # self.features already holds the d embedding columns: dims[0] = d + F (models.py:244)
+            self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, 0, device)
+            return
         if hasattr(features, "c_table"):                 # parallel.ShardedFeatures: node-partitioned table
             self.features = features
             self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
@@ -68,6 +74,35 @@ class SampleAndAggregate(object):
             features = table[:, :F_]
         self.features = features
         self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
+
+    def _init_identity_table(self, features, adj, d, device):
+        """The trainable node embeddings (reference models.py:229-240, supervised_models.py:51-62) and the features in ONE
+        fp32 table [N+1, pad_cols(d + F)]: columns [0, d) are the embeddings (glorot over [N+1, d], TF's default
+        initializer for tf.get_variable), columns [d, d + F) the features, copied in once.  `self.features` is the
+        [N+1, d + F] view every forward path reads - the reference's concat([embeds, features], axis=1), embeddings
+        first - and `self.embeds` the [N+1, d] view that is trained.  Every row is trained, the dummy row N included:
+        only the features' dummy row is zero.  Adam updates the view in place, so CUDA graphs and the version-keyed
+        bf16 cast cache see the new values."""
+        from .inits import glorot
+        if hasattr(features, "c_table"):
+            raise NotImplementedError("identity_dim > 0 with a node-partitioned feature table is not implemented")
+        if features is not None:
+            if torch.is_tensor(features) and features.dtype == torch.bfloat16:
+                raise NotImplementedError("identity_dim > 0 with a bfloat16 feature table is not implemented")
+            features = torch.as_tensor(features, dtype=torch.float32)
+            if features.dim() != 2:
+                raise ValueError("features must be a 2-D [N+1, F] table")
+        n_rows = int(adj.shape[0])
+        if features is not None and features.shape[0] != n_rows:
+            raise ValueError("features has %d rows, the adjacency table %d: both must be [N+1, .] (dummy row last)"
+                             % (features.shape[0], n_rows))
+        F_ = 0 if features is None else int(features.shape[1])
+        table = torch.zeros((n_rows, ops.pad_cols(d + F_)), dtype=torch.float32, device=device)
+        table[:, :d] = glorot([n_rows, d], name="node_embeddings", device=device)
+        if F_:
+            table[:, d:d + F_] = features.to(device=device)
+        self.features = table[:, :d + F_]
+        self.embeds = table[:, :d]
 
     def _finish_init(self, placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device):
         self.degrees = degrees

@@ -541,6 +541,46 @@ def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0,
     return out
 
 
+def embedding_grad(lists, n_rows, d, out=None):
+    """Dense gradient of the trainable embedding table (gs_embedding_grad; the densified IndexedSlices gradient of
+    tf.nn.embedding_lookup at reference graphsage/models.py:299): out[r] = sum of scale * grad[i // group] over every
+    (ids, grad, group, scale) list entry i with ids[i] == r.  grad: float32 CUDA [>= ceil(n / group), >= d] with unit
+    column stride (a strided view is fine).  Returns out, a contiguous float32 [n_rows, d]; deterministic."""
+    if len(lists) > _lib.MAX_EMBED_LISTS:
+        raise ValueError("embedding_grad takes at most %d lists" % _lib.MAX_EMBED_LISTS)
+    arr = (_lib.EmbedGradList * max(len(lists), 1))()
+    keep = []
+    dev = None
+    for i, (ids, grad, group, scale) in enumerate(lists):
+        require_cuda(ids, grad)
+        ids = _i32(ids.reshape(-1), "ids")
+        n, group = ids.numel(), int(group)
+        if group < 1:
+            raise ValueError("group must be >= 1")
+        if grad.dtype != torch.float32 or grad.dim() != 2 or (grad.stride(1) != 1 and grad.shape[1] > 1) \
+                or grad.shape[1] < d or grad.shape[0] < (n + group - 1) // group:
+            raise ValueError("list %d: grad must be a float32 [>= %d, >= %d] matrix with unit column stride"
+                             % (i, (n + group - 1) // group, d))
+        keep.append(ids)
+        dev = grad.device
+        arr[i] = _lib.EmbedGradList(ptr(ids), ptr(grad), max(grad.stride(0), d), n, group, float(scale))
+    if out is None:
+        out = torch.empty((n_rows, d), dtype=torch.float32, device=dev if dev is not None else "cuda")
+    require_cuda(out)
+    if out.dtype != torch.float32 or out.dim() != 2 or out.shape[0] != n_rows or out.shape[1] != d \
+            or (out.stride(1) != 1 and d > 1):
+        raise ValueError("out must be a float32 [%d, %d] matrix with unit column stride" % (n_rows, d))
+    nbytes = lib().gs_embedding_grad_workspace_bytes(arr, len(lists), int(n_rows), int(d))
+    if nbytes < 0:
+        check(-1)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=out.device) if nbytes > 0 else None
+    ev = _probe("embedding_grad/%d" % sum(k.numel() for k in keep))
+    check(lib().gs_embedding_grad(arr, len(lists), int(n_rows), int(d), ptr(out), max(out.stride(0), d), ptr(ws), nbytes,
+                                  stream_ptr()))
+    _launched(3 if nbytes > 0 and n_rows * d else 0, ev)           # keys, chunk sums, combine (+ CUB's sort passes)
+    return out
+
+
 def l2_normalize_rows_(x):
     """In-place tf.nn.l2_normalize(x, 1) - reference graphsage/models.py:368."""
     require_cuda(x)

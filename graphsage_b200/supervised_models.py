@@ -3,9 +3,10 @@ graphsage/supervised_models.py:10-126).
 
 Forward: the library's CUDA kernels (sample -> fused gather+mean -> wgmma / fp32 GEMM), wrapped in
 torch.autograd.Function so the step is differentiable.  Backward: the gradient formulas of the mean / GCN
-aggregators, with the weight-gradient GEMMs (X^T dZ) as plain library matmuls (torch / cuBLAS fp32) - features
-are not trainable (identity_dim = 0), so nothing is scattered into the table.  Head (l2_normalize -> Dense ->
-sigmoid / softmax cross-entropy + weight decay), gradient clipping to +-5 and Adam follow
+aggregators, with the weight-gradient GEMMs (X^T dZ) as plain library matmuls (torch / cuBLAS fp32).  Features are
+not trainable; with identity_dim > 0 the embedding columns of the layer-0 table are, and their gradient is scattered
+into a dense [N+1, d] table by the library's deterministic embedding-gradient kernel (ops.embedding_grad).  Head
+(l2_normalize -> Dense -> sigmoid / softmax cross-entropy + weight decay), gradient clipping to +-5 and Adam follow
 supervised_models.py:85-126.
 """
 import torch
@@ -15,12 +16,18 @@ from .layers import act_code, identity, relu  # noqa: F401
 from .models import SampleAndAggregate
 
 
+def _embedding_grad(emb_shape, lists):
+    """The layer-0 gradient w.r.t. the embedding columns [0, d) of the table: (ids, grad rows, group, scale) lists."""
+    return ops.embedding_grad(lists, emb_shape[0], emb_shape[1])
+
+
 class _AggregateRowsFn(torch.autograd.Function):
     """y = agg.aggregate_rows(src, segments) for MeanAggregator / GCNAggregator, differentiable w.r.t. the
-    aggregator weights and (for layers >= 1, where rows are addressed by ranges) w.r.t. src."""
+    aggregator weights, (for layers >= 1, where rows are addressed by ranges) w.r.t. src, and (layer 0, identity_dim > 0)
+    w.r.t. `emb`, the [N+1, d] embedding view of src's first d columns."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, *weights):
+    def forward(ctx, agg, src, segments, emb, *weights):
         kind = "gcn" if "weights" in agg.vars else "mean"
         code, post = act_code(agg.act)
         if post is not None:
@@ -40,6 +47,7 @@ class _AggregateRowsFn(torch.autograd.Function):
         ctx.kind, ctx.relu, ctx.concat = kind, code == ops.ACT_RELU, bool(agg.concat)
         ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
         ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
+        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
         ctx.has_bias = "bias" in agg.vars
         ctx.save_for_backward(xm if xs is None else xs, xm, y, *weights)
         return y
@@ -77,7 +85,24 @@ class _AggregateRowsFn(torch.autograd.Function):
                     dsrc[s.self_row0:s.self_row0 + n].add_(dxm[rows] / div)
                 else:
                     dsrc[s.self_row0:s.self_row0 + n].add_(dxs[rows])
-        return (None, dsrc, None) + tuple(grads_w)
+        demb = None
+        if ctx.emb_shape is not None:
+            d = ctx.emb_shape[1]
+            # the source gradient restricted to the embedding columns: dZ @ W[:d]^T (feature columns are not trainable)
+            if ctx.kind == "mean":
+                es, em = dz_s @ weights[0][:d].t(), dz_n @ weights[1][:d].t()
+            else:
+                es, em = None, dz @ weights[0][:d].t()
+            lists = []
+            for s in ctx.segments:
+                n, k = s.n, s.k
+                rows = slice(s.out_row0, s.out_row0 + n)
+                if ctx.kind == "gcn":                       # mean over [neighbours, self]: every id gets dxm / (k + 1)
+                    lists += [(s.self_ids[:n], em[rows], 1, 1.0 / (k + 1)), (s.neigh_ids[:n * k], em[rows], k, 1.0 / (k + 1))]
+                else:                                       # self id: dxs; neighbour ids: dxm / k
+                    lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], em[rows], k, 1.0 / k)]
+            demb = _embedding_grad(ctx.emb_shape, lists)
+        return (None, dsrc, None, demb) + tuple(grads_w)
 
 
 def pool_branch_backward(pool, xn, h, hp, dhp, Wm, k, need_dx):
@@ -102,10 +127,11 @@ def pool_branch_backward(pool, xn, h, hp, dhp, Wm, k, need_dx):
 class _PoolAggregateRowsFn(torch.autograd.Function):
     """y = agg.aggregate_rows(src, segments) for MaxPoolingAggregator / MeanPoolingAggregator on the unfused fp32 path
     (gather -> Dense(relu, bias) -> pool over the fanout -> both matmuls), differentiable w.r.t. the four weight tensors
-    and (layers >= 1) src.  The gathered neighbour rows and the MLP activations are kept for the backward pass."""
+    and (layers >= 1) src, and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of src's first d columns.
+    The gathered neighbour rows and the MLP activations are kept for the backward pass."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm):
+    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None):
         code, post = act_code(agg.act)
         if post is not None:
             raise NotImplementedError("training supports act=relu or identity")
@@ -137,6 +163,7 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
         ctx.pool, ctx.relu, ctx.concat = agg.pool, code == ops.ACT_RELU, bool(agg.concat)
         ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
         ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
+        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
         ctx.save_for_backward(xs, hp, y, Ws, Wn, Wm, *kept)
         return y
 
@@ -153,19 +180,29 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
         dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dy.dtype, device=dy.device)
         dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
         dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
+        emb = ctx.emb_shape is not None
+        d = ctx.emb_shape[1] if emb else 0
+        # the embedding columns only need dZ @ W[:d]^T (feature columns are not trainable)
+        es = dz_s @ Ws[:d].t() if emb else None
+        W_dx = Wm if ctx.src_needs_grad else Wm[:d]
+        lists = []
         for i, s in enumerate(ctx.segments):
             n, k = s.n, s.k
             rows = slice(s.out_row0, s.out_row0 + n)
             xn, h = kept[2 * i][:, :F_in], kept[2 * i + 1]
-            g_wm, g_bm, dxn = pool_branch_backward(ctx.pool, xn, h, hp[rows], dhp[rows], Wm, k, ctx.src_needs_grad)
+            g_wm, g_bm, dxn = pool_branch_backward(ctx.pool, xn, h, hp[rows], dhp[rows], W_dx, k,
+                                                   ctx.src_needs_grad or emb)
             dWm += g_wm
             dbm += g_bm
+            if emb:                                          # self id: dxs; neighbour id of gathered row r: dxn[r]
+                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dxn[:, :d], 1, 1.0)]
             if ctx.src_needs_grad:
                 if s.self_ids is not None or s.neigh_ids is not None:
                     raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
                 dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dxn
                 dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
-        return None, dsrc, None, dWs, dWn, dWm, dbm
+        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
+        return None, dsrc, None, dWs, dWn, dWm, dbm, demb
 
 
 def differentiable_outputs(model, batch, normalize=True):
@@ -192,13 +229,16 @@ def differentiable_outputs(model, batch, normalize=True):
                 segs.append(ops.Seg(counts[hop], k, self_row0=row0[hop], neigh_row0=row0[hop + 1],
                                     out_row0=row0[hop]))
         agg = model.aggregators[layer]
+        # layer 0 reads the embedding table (identity_dim > 0) through src; handing it over as an input lets autograd
+        # deliver the scattered gradient as embeds.grad
+        emb = getattr(model, "embeds", None) if layer == 0 else None
         if hasattr(agg, "mlp_layers"):                      # max-pool / mean-pool
             mlp = agg.mlp_layers[0].vars
             src = _PoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
-                                             mlp["weights"], mlp["bias"])
+                                             mlp["weights"], mlp["bias"], emb)
         else:
             ws = (agg.vars["weights"],) if "weights" in agg.vars else (agg.vars["self_weights"], agg.vars["neigh_weights"])
-            src = _AggregateRowsFn.apply(agg, src, segs, *ws)
+            src = _AggregateRowsFn.apply(agg, src, segs, emb, *ws)
     out = src[:counts[0]]
     if normalize:
         out = out / torch.sqrt(torch.clamp((out * out).sum(dim=1, keepdim=True), min=1e-12))   # tf.nn.l2_normalize
@@ -232,6 +272,18 @@ def aggregator_parameters(aggregators):
     return decayed + extra, decayed
 
 
+def embedding_parameters(model):
+    """[model.embeds] when the model trains node embeddings (identity_dim > 0), else [].  Trained and clipped with the
+    rest, never weight-decayed (the reference decays aggregator and head variables only)."""
+    return [model.embeds] if getattr(model, "embeds", None) is not None else []
+
+
+def refuse_distributed_embeddings(identity_dim, distributed):
+    if identity_dim > 0 and distributed:
+        raise NotImplementedError("identity_dim > 0 with distributed=True is not implemented (the [N+1, d] table would "
+                                  "have to be sharded or its dense gradient all-reduced)")
+
+
 def classification_loss(logits, labels, sigmoid_loss):
     """reference supervised_models.py:109-117: mean over ALL elements of the sigmoid cross-entropy (multi-label), or the
     mean over nodes of the softmax cross-entropy."""
@@ -257,6 +309,7 @@ class SupervisedGraphsage(SampleAndAggregate):
     def __init__(self, num_classes, placeholders, features, adj, degrees, layer_infos, concat=True,
                  aggregator_type="mean", model_size="small", sigmoid_loss=False, identity_dim=0, learning_rate=0.01,
                  weight_decay=0.0, device="cuda", distributed=False, group=None, **kwargs):
+        refuse_distributed_embeddings(identity_dim, distributed)
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
                                                   identity_dim=identity_dim, device=device, **kwargs)
@@ -282,7 +335,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         self.optimizer = torch.optim.Adam(self.parameters(), lr=self.learning_rate)      # TF AdamOptimizer defaults
 
     def parameters(self):
-        return aggregator_parameters(self.aggregators)[0] + list(self.node_pred_vars.values())
+        return aggregator_parameters(self.aggregators)[0] + list(self.node_pred_vars.values()) + embedding_parameters(self)
 
     def decayed_parameters(self):
         return aggregator_parameters(self.aggregators)[1] + list(self.node_pred_vars.values())

@@ -12,7 +12,8 @@ import torch
 from . import ops
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
-from .supervised_models import aggregator_parameters, build_aggregators, differentiable_outputs, weight_decay_term
+from .supervised_models import (aggregator_parameters, build_aggregators, differentiable_outputs, embedding_parameters,
+                                refuse_distributed_embeddings, weight_decay_term)
 
 
 class UnigramNegativeSampler(object):
@@ -36,6 +37,7 @@ class UnsupervisedGraphsage(SampleAndAggregate):
     def __init__(self, placeholders, features, adj, degrees, layer_infos, concat=True, aggregator_type="mean",
                  model_size="small", identity_dim=0, neg_sample_size=20, neg_sample_weights=1.0, learning_rate=0.00001,
                  weight_decay=0.0, seed=123, device="cuda", distributed=False, group=None, **kwargs):
+        refuse_distributed_embeddings(identity_dim, distributed)
         super(UnsupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                     aggregator_type=aggregator_type, model_size=model_size,
                                                     identity_dim=identity_dim, device=device, **kwargs)
@@ -58,7 +60,7 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         self.optimizer = torch.optim.Adam(self.parameters(), lr=self.learning_rate)
 
     def parameters(self):
-        return aggregator_parameters(self.aggregators)[0]
+        return aggregator_parameters(self.aggregators)[0] + embedding_parameters(self)
 
     def decayed_parameters(self):
         return aggregator_parameters(self.aggregators)[1]

@@ -370,6 +370,41 @@ int32_t gs_pipeline_step(const void* ids_host, void* ids_dev, int64_t ids_bytes,
  * CUDA-graph replay reads, see gs_sample_padded) when the step's last kernel is not gs_sage_layer_small. */
 int32_t gs_bump_counter(uint64_t* counter_dev, uint64_t inc, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Gradient of the trainable node-embedding table (identity_dim > 0): the IndexedSlices gradient of
+ * tf.nn.embedding_lookup(embeds, ids) at reference graphsage/models.py:299, densified - TF 1.8's clip_by_value
+ * (supervised_models.py:95-99, models.py:379-383) converts it to a dense tensor with duplicate ids summed.
+ *   out[r, 0:d] = sum over lists l, contributions i < l.n with l.ids[i] == r of  l.scale * l.grad[(i / l.group) * l.ldg + 0:d]
+ * for every r in [0, n_rows); rows nobody addresses are zero (the whole [n_rows, d] block at row stride ldo is written, also
+ * when there are no contributions).  ids outside [0, n_rows) contribute nothing.  The layer-0 backward passes, per hop
+ * segment: mean - (self ids, dxs, 1, 1) and (neighbour ids, dxm, k, 1/k); gcn - (self ids, dxm, 1, 1/(k+1)) and
+ * (neighbour ids, dxm, k, 1/(k+1)); max-/mean-pool - (self ids, dxs, 1, 1) and (neighbour ids, dxn, 1, 1).
+ * Deterministic (bit-identical on every call, no atomics).  Summation order for a row r:
+ *   number the contributions of all lists in call order (list 0 first, i ascending) and sort them by (r, number); cut
+ *   that sorted sequence into fixed chunks of 32.  Within a chunk the products scale * grad are added left to right
+ *   in fp32.  A row whose contributions span several chunks gets one such partial sum per chunk (pieces q = 0, 1, ...
+ *   in sorted order); piece q goes to accumulator (q / 8) % 4 of lane q % 8, each accumulator adds its pieces in
+ *   ascending q, a lane adds its accumulators 0..3 in order, and the row is lane 0 + lane 1 + ... + lane 7, in order.
+ *   So a long run of one id (the padding id, a hub) is split into chunks that are summed in parallel.
+ * workspace: device scratch of gs_embedding_grad_workspace_bytes(...) bytes (0 when there are no contributions); it
+ * depends on the lists' lengths, n_rows and d only.  Limits: n_lists <= GS_MAX_EMBED_LISTS, fewer than 2^31 contributions,
+ * n_rows < 2^31 - 1, ldg >= d, group >= 1.
+ * --------------------------------------------------------------------------------------------- */
+#define GS_MAX_EMBED_LISTS 8
+typedef struct {
+  const int32_t* ids;   /* device, n ids */
+  const float* grad;    /* device gradient rows, row stride ldg (elements); contribution i reads row i / group */
+  int64_t ldg;
+  int64_t n;            /* contributions */
+  int32_t group;
+  float scale;
+} gs_embed_grad_list;
+
+int64_t gs_embedding_grad_workspace_bytes(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows,
+                                          int32_t d);
+int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float* out,
+                          int64_t ldo, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
