@@ -45,6 +45,10 @@ class EmbedGradList(ctypes.Structure):
     _fields_ = [("ids", c_vp), ("grad", c_vp), ("ldg", c_i64), ("n", c_i64), ("group", c_i32), ("scale", ctypes.c_float)]
 
 
+class DropoutSite(ctypes.Structure):
+    _fields_ = [("seed", c_u64), ("call", ctypes.c_uint32), ("rate", ctypes.c_float)]
+
+
 _SIGNATURES = {
     "gs_version": (c_i32, []),
     "gs_last_error_string": (ctypes.c_char_p, []),
@@ -104,6 +108,11 @@ _SIGNATURES = {
     "gs_bump_counter": (c_i32, [c_vp, c_u64, c_vp]),
     "gs_embedding_grad_workspace_bytes": (c_i64, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32]),
     "gs_embedding_grad": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "gs_gather_mean_dropout": (c_i32, [c_vp, c_i64, c_i32, c_i64, ctypes.POINTER(Segment), c_i32, ctypes.POINTER(DropoutSite),
+                                       ctypes.POINTER(DropoutSite), c_i32, c_vp, c_vp, c_i64, c_vp]),
+    "gs_dropout_apply": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, ctypes.c_float, DropoutSite, c_i32, c_vp, c_i64, c_vp]),
+    "gs_embedding_grad_dropout": (c_i32, [ctypes.POINTER(EmbedGradList), ctypes.POINTER(DropoutSite), c_i32, c_i64, c_i32, c_vp,
+                                          c_i64, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

@@ -1,6 +1,7 @@
 // Shared host/device helpers for libgraphsage_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -71,6 +72,45 @@ __host__ __device__ inline uint32_t philox_draw(uint64_t seed, uint64_t counter,
   u32x4 c{(uint32_t)counter, (uint32_t)(counter >> 32), c2, tag + (uint32_t)(i >> 2)};
   u32x4 r = philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
   return pick(r, i & 3);
+}
+
+// ---- dropout masks (contract: oracle/dropout.py) --------------------------------------------
+// A site (seed, call, rate) drops element (pos, c) of a logical [rows, F] tensor unless word c % 4 of
+// philox4x32_10(ctr = (c / 4, pos_lo32, pos_hi32, call), key = split64(seed)) is >= T = floor(rate * 2^32) (float64).
+// A kept element becomes x / keep with keep = fp32(1 - rate) (IEEE division), a dropped one 0.  rate = 0 keeps every
+// element and divides by 1, so it is the identity.
+struct DropSite {
+  uint32_t k0, k1, call, threshold;
+  float keep;
+};
+
+__host__ inline DropSite make_drop_site(const gs_dropout_site& s) {
+  DropSite d;
+  d.k0 = (uint32_t)s.seed;
+  d.k1 = (uint32_t)(s.seed >> 32);
+  d.call = s.call;
+  d.threshold = (uint32_t)floor((double)s.rate * 4294967296.0);
+  d.keep = (float)(1.0 - (double)s.rate);
+  return d;
+}
+
+// the four keep words of columns 4 * c4 .. 4 * c4 + 3 at position pos
+__host__ __device__ inline u32x4 drop_words(const DropSite& s, int64_t pos, uint32_t c4) {
+  u32x4 c{c4, (uint32_t)pos, (uint32_t)((uint64_t)pos >> 32), s.call};
+  return philox4x32_10(c, s.k0, s.k1);
+}
+
+__host__ __device__ inline float drop_one(const DropSite& s, uint32_t word, float x) {
+  return word >= s.threshold ? x / s.keep : 0.f;
+}
+
+__host__ __device__ inline float4 drop4(const DropSite& s, int64_t pos, uint32_t c4, float4 v) {
+  const u32x4 w = drop_words(s, pos, c4);
+  return make_float4(drop_one(s, w.x, v.x), drop_one(s, w.y, v.y), drop_one(s, w.z, v.z), drop_one(s, w.w, v.w));
+}
+
+__host__ __device__ inline float drop_col(const DropSite& s, int64_t pos, int c, float x) {
+  return drop_one(s, pick(drop_words(s, pos, (uint32_t)c >> 2), c & 3), x);
 }
 
 constexpr uint32_t kStreamPadded = 0u;

@@ -31,6 +31,7 @@ struct ListDev {
   int64_t offset;       // first global contribution index of this list
   int32_t group;
   float scale;
+  DropSite site;        // gs_embedding_grad_dropout only
 };
 struct Lists {
   ListDev l[GS_MAX_EMBED_LISTS];
@@ -53,6 +54,8 @@ __global__ void embed_keys_kernel(Lists L, int64_t total, uint32_t n_rows, uint3
   }
 }
 
+// kDrop: every product scale * grad goes through its list's dropout mask at pos = index in the list (the masked entry)
+template <bool kDrop>
 __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_t* __restrict__ keys,
                                                           const int32_t* __restrict__ vals, int64_t total,
                                                           uint32_t n_rows, int32_t d, float* __restrict__ out,
@@ -68,12 +71,16 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
     uint32_t my_key = n_rows;
     const float* my_row = nullptr;
     float my_scale = 0.f;
+    int64_t my_pos = 0;
+    int my_list = 0;
     if (lane < cnt) {
       my_key = keys[s + lane];
       if (my_key < n_rows) {
         int64_t c = vals[s + lane];
-        const ListDev& l = L.l[find_list(L, c)];
-        my_row = l.grad + ((c - l.offset) / l.group) * l.ldg;
+        my_list = find_list(L, c);
+        const ListDev& l = L.l[my_list];
+        my_pos = c - l.offset;
+        my_row = l.grad + (my_pos / l.group) * l.ldg;
         my_scale = l.scale;
       }
     }
@@ -93,10 +100,17 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
           const int i = (b + u) & 31;
           const float* row = (const float*)__shfl_sync(FULL, (unsigned long long)my_row, i);
           const float sc = __shfl_sync(FULL, my_scale, i);
+          int64_t pos = 0;
+          int li = 0;
+          if constexpr (kDrop) {
+            pos = __shfl_sync(FULL, my_pos, i);
+            li = __shfl_sync(FULL, my_list, i);
+          }
 #pragma unroll
           for (int q = 0; q < kColsPerLane; ++q) {
             const int col = c0 + lane + 32 * q;
             v[u][q] = (b + u < cnt && row != nullptr && col < d) ? sc * __ldg(row + col) : 0.f;
+            if constexpr (kDrop) v[u][q] = drop_col(L.l[li].site, pos, col, v[u][q]);
           }
         }
 #pragma unroll
@@ -246,16 +260,17 @@ int64_t gs_embedding_grad_workspace_bytes(const gs_embed_grad_list* lists_host, 
   return (int64_t)P.bytes;
 }
 
-int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float* out,
-                          int64_t ldo, void* workspace, int64_t workspace_bytes, void* stream) {
+static int32_t embedding_grad(const gs_embed_grad_list* lists_host, const gs_dropout_site* sites_host, int32_t n_lists,
+                              int64_t n_rows, int32_t d, float* out, int64_t ldo, void* workspace, int64_t workspace_bytes,
+                              void* stream, const char* who) {
   gs::Plan P;
-  int32_t rc = gs::make_plan(lists_host, n_lists, n_rows, d, P, "gs_embedding_grad");
+  int32_t rc = gs::make_plan(lists_host, n_lists, n_rows, d, P, who);
   if (rc != GS_OK) return rc;
   if (n_rows == 0 || d == 0) return GS_OK;
-  GS_REQUIRE(out != nullptr, "gs_embedding_grad: out is NULL");
-  GS_REQUIRE(ldo >= d, "gs_embedding_grad: ldo < d");
+  GS_REQUIRE(out != nullptr, "%s: out is NULL", who);
+  GS_REQUIRE(ldo >= d, "%s: ldo < d", who);
   GS_REQUIRE(workspace_bytes >= (int64_t)P.bytes && (P.bytes == 0 || workspace != nullptr),
-             "gs_embedding_grad: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
+             "%s: workspace of %lld bytes, %lld needed", who, (long long)workspace_bytes,
              (long long)P.bytes);
   cudaStream_t st = (cudaStream_t)stream;
   GS_CUDA(cudaMemset2DAsync(out, (size_t)ldo * 4, 0, (size_t)d * 4, (size_t)n_rows, st));
@@ -266,7 +281,9 @@ int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists,
   for (int i = 0; i < n_lists; ++i) {
     const gs_embed_grad_list& l = lists_host[i];
     if (l.n == 0) continue;
-    L.l[L.count++] = gs::ListDev{l.ids, l.grad, l.ldg, off, l.group, l.scale};
+    L.l[L.count] = gs::ListDev{l.ids, l.grad, l.ldg, off, l.group, l.scale, gs::DropSite{}};
+    if (sites_host) L.l[L.count].site = gs::make_drop_site(sites_host[i]);
+    ++L.count;
     off += l.n;
   }
   char* ws = (char*)workspace;
@@ -290,8 +307,12 @@ int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists,
 
   blocks = (P.nchunks * 32 + 255) / 256;
   if (blocks > cap * 2) blocks = cap * 2;
-  gs::embed_chunk_kernel<<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d, out,
-                                                           ldo, partial);
+  if (sites_host)
+    gs::embed_chunk_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d, out,
+                                                                   ldo, partial);
+  else
+    gs::embed_chunk_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d, out,
+                                                                    ldo, partial);
   rc = gs::launch_check("embed_chunk_kernel");
   if (rc != GS_OK) return rc;
 
@@ -299,6 +320,22 @@ int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists,
   gs::embed_combine_kernel<<<(unsigned)blocks, gs::kLanes * 32, 0, st>>>(keys_out, P.total, (uint32_t)n_rows, d,
                                                                           partial, out, ldo);
   return gs::launch_check("embed_combine_kernel");
+}
+
+int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float* out,
+                          int64_t ldo, void* workspace, int64_t workspace_bytes, void* stream) {
+  return embedding_grad(lists_host, nullptr, n_lists, n_rows, d, out, ldo, workspace, workspace_bytes, stream,
+                        "gs_embedding_grad");
+}
+
+int32_t gs_embedding_grad_dropout(const gs_embed_grad_list* lists_host, const gs_dropout_site* sites_host, int32_t n_lists,
+                                  int64_t n_rows, int32_t d, float* out, int64_t ldo, void* workspace,
+                                  int64_t workspace_bytes, void* stream) {
+  for (int i = 0; sites_host && i < n_lists; ++i)
+    GS_REQUIRE(sites_host[i].rate >= 0.f && sites_host[i].rate < 1.f, "gs_embedding_grad_dropout: list %d has rate %g outside [0, 1)",
+               i, (double)sites_host[i].rate);
+  return embedding_grad(lists_host, sites_host, n_lists, n_rows, d, out, ldo, workspace, workspace_bytes, stream,
+                        "gs_embedding_grad_dropout");
 }
 
 }  // extern "C"

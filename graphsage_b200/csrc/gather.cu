@@ -96,14 +96,23 @@ __global__ void __launch_bounds__(256) gather_mean_ldg_kernel(const float* __res
   }
 }
 
-// scalar fallback for tables whose pitch / alignment rules out 128-bit access
+// dropout sites of a gs_gather_mean_dropout call: one neighbour and one self site per segment
+struct DropTab {
+  DropSite neigh[GS_MAX_SEGMENTS];
+  DropSite self[GS_MAX_SEGMENTS];
+};
+
+// scalar fallback for tables whose pitch / alignment rules out 128-bit access (kDrop: gs_gather_mean_dropout's masks)
+template <bool kDrop>
 __global__ void __launch_bounds__(256) gather_mean_scalar_kernel(const float* __restrict__ src, int64_t n_src_rows, int F,
                                                                  int64_t pitch, const __grid_constant__ SegTable tab, int include_self,
                                                                  float* __restrict__ out_self,
-                                                                 float* __restrict__ out_mean, int64_t out_pitch) {
+                                                                 float* __restrict__ out_mean, int64_t out_pitch,
+                                                                 const __grid_constant__ DropTab drop) {
   for (int64_t r = blockIdx.x; r < tab.total_rows; r += gridDim.x) {
     int64_t i;
-    const gs_segment& sg = tab.s[find_segment(tab, r, i)];
+    const int si = find_segment(tab, r, i);
+    const gs_segment& sg = tab.s[si];
     const int k = sg.k;
     const int64_t orow = sg.out_row0 + i;
     const int64_t srow = clamp_row(sg.self_ids ? (int64_t)sg.self_ids[i] : sg.self_row0 + i, n_src_rows);
@@ -112,9 +121,11 @@ __global__ void __launch_bounds__(256) gather_mean_scalar_kernel(const float* __
       if (c < F) {
         for (int j = 0; j < k; ++j) {
           int64_t nr = clamp_row(sg.neigh_ids ? (int64_t)sg.neigh_ids[i * k + j] : sg.neigh_row0 + i * k + j, n_src_rows);
-          acc += src[nr * pitch + c];
+          if constexpr (kDrop) acc += drop_col(drop.neigh[si], i * k + j, c, src[nr * pitch + c]);
+          else acc += src[nr * pitch + c];
         }
         sv = src[srow * pitch + c];
+        if constexpr (kDrop) sv = drop_col(drop.self[si], i, c, sv);
         if (include_self) acc += sv;
         acc /= (float)(k + (include_self ? 1 : 0));
       }
@@ -275,12 +286,15 @@ __device__ __forceinline__ void gather_img_store(const GatherImg& im, int part, 
   *reinterpret_cast<uint4*>(dst + 16384) = lo;
 }
 
-template <class Rows>
+// kDrop: every gathered row is dropped in registers before it is summed (gs_gather_mean_dropout); the kDrop = false
+// instantiation is the plain gather.
+template <class Rows, bool kDrop>
 __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_constant__ Rows rows_of, int F,
                                                                const __grid_constant__ SegTable tab,
                                                                int include_self, float* __restrict__ out_self,
                                                                float* __restrict__ out_mean, int64_t out_pitch,
-                                                               int row_bytes, const __grid_constant__ GatherImg img) {
+                                                               int row_bytes, const __grid_constant__ GatherImg img,
+                                                               const __grid_constant__ DropTab drop) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t bar[2];
   if (threadIdx.x == 0) {
@@ -329,7 +343,8 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
   while (have) {
     const bool have_next = issue(buf ^ 1);                // prefetch the next group into the other buffer
     int64_t i;
-    const gs_segment& sg = tab.s[find_segment(tab, r, i)];
+    const int si = find_segment(tab, r, i);
+    const gs_segment& sg = tab.s[si];
     const int k = sg.k;
     const int rows_total = k + 1;
     const int first = g * kGroupRows;
@@ -346,6 +361,7 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
         float4 a = acc[q];
         for (int j = 0; j < nn; ++j) {
           float4 v = rows[j * row_f4 + c];
+          if constexpr (kDrop) v = drop4(drop.neigh[si], i * k + first + j, (uint32_t)c, v);
           a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
         }
         acc[q] = a;
@@ -362,6 +378,7 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
           if (c < ncol4 && c * 4 < F) {
             a = acc[q];
             sv = rows[(cnt - 1) * row_f4 + c];
+            if constexpr (kDrop) sv = drop4(drop.self[si], i, (uint32_t)c, sv);
             const float div = (float)(k + (include_self ? 1 : 0));
             if (include_self) { a.x += sv.x; a.y += sv.y; a.z += sv.z; a.w += sv.w; }
             a.x /= div; a.y /= div; a.z /= div; a.w /= div;
@@ -651,6 +668,30 @@ __global__ void __launch_bounds__(256) cast_rows_bf16_scalar_kernel(const float*
   }
 }
 
+// out[r, c] (+)= keep(site, r, c) ? (x[r / group, c] * scale) / keep : 0 - one thread per 4 columns of a row (one Philox
+// block), so every element is read and written by one thread (out may alias x when group == 1)
+__global__ void __launch_bounds__(256) dropout_apply_kernel(const float* x, int64_t ldx, int64_t rows, int F, int group,
+                                                            float scale, DropSite site, int accumulate, float* out,
+                                                            int64_t ldo) {
+  const int nc4 = (F + 3) >> 2;
+  const int64_t total = rows * nc4;
+  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = q / nc4;
+    const int c4 = (int)(q - r * nc4);
+    const u32x4 w = drop_words(site, r, (uint32_t)c4);
+    const float* xr = x + (r / group) * ldx;
+    float* orow = out + r * ldo;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = c4 * 4 + e;
+      if (c < F) {
+        const float v = pick(w, e) >= site.threshold ? (xr[c] * scale) / site.keep : 0.f;
+        orow[c] = accumulate ? orow[c] + v : v;
+      }
+    }
+  }
+}
+
 // *counter += inc on the stream (the samplers' device-side call counter, advanced once per step)
 __global__ void bump_counter_kernel(unsigned long long* counter, unsigned long long inc) { *counter += inc; }
 
@@ -849,10 +890,10 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 
 namespace gs {
 // launch of the grouped double-buffered bulk-copy gather (dense or sharded resolver), with or without A-operand images
-template <class Rows>
+template <class Rows, bool kDrop = false>
 static int32_t launch_gather_tma2(const Rows& rows_of, int F, const SegTable& tab, int include_self, float* out_self, float* out_mean,
-                                  int64_t out_pitch, const GatherImg& img, cudaStream_t st) {
-  const int32_t rc_attr = ensure_dyn_smem((const void*)gather_mean_tma2_kernel<Rows>, 200 * 1024);
+                                  int64_t out_pitch, const GatherImg& img, cudaStream_t st, const DropTab* drop = nullptr) {
+  const int32_t rc_attr = ensure_dyn_smem((const void*)gather_mean_tma2_kernel<Rows, kDrop>, 200 * 1024);
   if (rc_attr != GS_OK) return rc_attr;
   const int ncol4 = (int)(out_pitch / 4);
   const int row_bytes = ((F + 3) / 4) * 16;
@@ -867,8 +908,11 @@ static int32_t launch_gather_tma2(const Rows& rows_of, int F, const SegTable& ta
   int64_t blocks = tab.total_rows;
   int64_t cap = (int64_t)sm_count() * per_sm;
   if (blocks > cap) blocks = cap;
-  gather_mean_tma2_kernel<Rows><<<(unsigned)blocks, threads, smem2, st>>>(rows_of, F, tab, include_self, out_self, out_mean,
-                                                                          out_pitch, row_bytes, img);
+  DropTab no_drop;
+  memset(&no_drop, 0, sizeof(no_drop));
+  gather_mean_tma2_kernel<Rows, kDrop><<<(unsigned)blocks, threads, smem2, st>>>(rows_of, F, tab, include_self, out_self,
+                                                                                 out_mean, out_pitch, row_bytes, img,
+                                                                                 drop ? *drop : no_drop);
   return launch_check("gather_mean_tma2_kernel");
 }
 }  // namespace gs
@@ -972,8 +1016,11 @@ int32_t gs_gather_mean(const void* src, int32_t dtype, int64_t n_src_rows, int32
     int64_t blocks = tab.total_rows;
     int64_t cap = (int64_t)gs::sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    gs::gather_mean_scalar_kernel<<<(unsigned)blocks, 256, 0, st>>>(fsrc, n_src_rows, F, pitch, tab, include_self,
-                                                                    (float*)out_self, (float*)out_mean, out_pitch);
+    gs::DropTab no_drop;
+    memset(&no_drop, 0, sizeof(no_drop));
+    gs::gather_mean_scalar_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(fsrc, n_src_rows, F, pitch, tab, include_self,
+                                                                           (float*)out_self, (float*)out_mean, out_pitch,
+                                                                           no_drop);
     return gs::launch_check("gather_mean_scalar_kernel");
   }
   const int ncol4 = (int)(out_pitch / 4);
@@ -1071,6 +1118,76 @@ int32_t gs_segment_max(const float* x, int64_t n, int32_t k, int32_t C, int64_t 
   if (blocks > cap) blocks = cap;
   gs::segment_max_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, n, k, C, ldx, out, ldo);
   return gs::launch_check("segment_max_kernel");
+}
+
+static int32_t check_site(const gs_dropout_site& s, const char* who) {
+  GS_REQUIRE(s.rate >= 0.f && s.rate < 1.f, "%s: dropout rate %g outside [0, 1)", who, (double)s.rate);
+  return GS_OK;
+}
+
+int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, int64_t pitch, const gs_segment* segments_host,
+                               int32_t n_segments, const gs_dropout_site* neigh_sites_host,
+                               const gs_dropout_site* self_sites_host, int32_t include_self, float* out_self,
+                               float* out_mean, int64_t out_pitch, void* stream) {
+  GS_REQUIRE(n_segments >= 0 && n_segments <= GS_MAX_SEGMENTS, "gs_gather_mean_dropout: n_segments=%d (max %d)", n_segments,
+             GS_MAX_SEGMENTS);
+  GS_REQUIRE((segments_host && neigh_sites_host && self_sites_host) || n_segments == 0,
+             "gs_gather_mean_dropout: segments / sites are NULL");
+  gs::SegTable tab;
+  memset(&tab, 0, sizeof(tab));
+  gs::DropTab drop;
+  memset(&drop, 0, sizeof(drop));
+  tab.n_segments = n_segments;
+  for (int s = 0; s < n_segments; ++s) {
+    tab.s[s] = segments_host[s];
+    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "gs_gather_mean_dropout: segment %d has n=%lld k=%d", s,
+               (long long)tab.s[s].n, tab.s[s].k);
+    int32_t rc = check_site(neigh_sites_host[s], "gs_gather_mean_dropout");
+    if (rc == GS_OK) rc = check_site(self_sites_host[s], "gs_gather_mean_dropout");
+    if (rc != GS_OK) return rc;
+    drop.neigh[s] = gs::make_drop_site(neigh_sites_host[s]);
+    drop.self[s] = gs::make_drop_site(self_sites_host[s]);
+    tab.total_rows += tab.s[s].n;
+  }
+  if (tab.total_rows == 0) return GS_OK;
+  GS_REQUIRE(src && out_mean, "gs_gather_mean_dropout: NULL pointer");
+  GS_REQUIRE(F > 0 && pitch >= F && out_pitch >= F && n_src_rows > 0, "gs_gather_mean_dropout: bad F/pitch");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ncol4 = (int)(out_pitch / 4);
+  const bool vec_ok = gs::aligned16(src) && gs::aligned16(out_mean) && (!out_self || gs::aligned16(out_self)) &&
+                      pitch % 4 == 0 && out_pitch % 4 == 0 && ((F + 3) / 4) * 4 <= pitch;
+  if (vec_ok && ncol4 <= 2 * 160) {
+    const gs::DenseRows rows_of{src, n_src_rows, pitch};
+    gs::GatherImg img;
+    memset(&img, 0, sizeof(img));
+    return gs::launch_gather_tma2<gs::DenseRows, true>(rows_of, F, tab, include_self, out_self, out_mean, out_pitch, img, st,
+                                                       &drop);
+  }
+  int64_t blocks = tab.total_rows;
+  int64_t cap = (int64_t)gs::sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  gs::gather_mean_scalar_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(src, n_src_rows, F, pitch, tab, include_self, out_self,
+                                                                        out_mean, out_pitch, drop);
+  return gs::launch_check("gather_mean_scalar_kernel<drop>");
+}
+
+int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, int32_t group, float scale,
+                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, void* stream) {
+  int32_t rc = check_site(site, "gs_dropout_apply");
+  if (rc != GS_OK) return rc;
+  GS_REQUIRE(rows >= 0 && F >= 0 && group >= 1, "gs_dropout_apply: bad sizes (rows=%lld F=%d group=%d)", (long long)rows, F,
+             group);
+  if (rows == 0 || F == 0) return GS_OK;
+  GS_REQUIRE(x && out, "gs_dropout_apply: NULL pointer");
+  GS_REQUIRE(ldx >= F && ldo >= F, "gs_dropout_apply: row stride < F");
+  GS_REQUIRE(x != out || (group == 1 && ldx == ldo), "gs_dropout_apply: in place needs group == 1 and ldo == ldx");
+  const int64_t total = rows * ((F + 3) / 4);
+  int64_t blocks = (total + 255) / 256;
+  int64_t cap = (int64_t)gs::sm_count() * 16;
+  if (blocks > cap) blocks = cap;
+  gs::dropout_apply_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, F, group, scale,
+                                                                                gs::make_drop_site(site), accumulate, out, ldo);
+  return gs::launch_check("dropout_apply_kernel");
 }
 
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream) {

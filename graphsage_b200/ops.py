@@ -541,13 +541,87 @@ def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0,
     return out
 
 
-def embedding_grad(lists, n_rows, d, out=None):
+def dropout_site(site):
+    """(seed, call, rate) -> the C descriptor; rate must lie in [0, 1) (the mask contract is in the header and
+    oracle/dropout.py)."""
+    seed, call, rate = site
+    rate = float(rate)
+    if not 0.0 <= rate < 1.0:
+        raise ValueError("dropout rate must be in [0, 1) (got %r)" % (rate,))
+    return _lib.DropoutSite(int(seed) & _U64, int(call) & 0xFFFFFFFF, rate)
+
+
+def gather_mean_dropout(src, segments, neigh_sites, self_sites, include_self=False, want_self=True, out_pitch=None):
+    """gather_mean with training dropout (gs_gather_mean_dropout; reference aggregators.py:46-47 / 104-105): every gathered
+    neighbour row and self row is dropped in registers with its segment's site before the fanout mean.  neigh_sites /
+    self_sites: one (seed, call, rate) per segment.  Returns (dropped self rows or None, out_mean), [rows, out_pitch]."""
+    require_cuda(src)
+    if hasattr(src, "c_table") or src.dtype != torch.float32 or src.dim() != 2 or src.stride(1) != 1:
+        raise ValueError("gather_mean_dropout needs a row-major float32 CUDA table")
+    if len(segments) > _lib.MAX_SEGMENTS or len(neigh_sites) != len(segments) or len(self_sites) != len(segments):
+        raise ValueError("gather_mean_dropout takes at most %d segments and one neighbour and one self site per segment"
+                         % _lib.MAX_SEGMENTS)
+    F = src.shape[1]
+    if out_pitch is None:
+        out_pitch = pad_cols(F)
+    rows = max([s.out_row0 + s.n for s in segments] + [0])
+    out_mean = torch.empty((rows, out_pitch), dtype=torch.float32, device=src.device)
+    out_self = torch.empty((rows, out_pitch), dtype=torch.float32, device=src.device) if want_self else None
+    nseg = max(len(segments), 1)
+    arr = (Segment * nseg)(*[s.c_struct() for s in segments])
+    ns = (_lib.DropoutSite * nseg)(*[dropout_site(x) for x in neigh_sites])
+    ss = (_lib.DropoutSite * nseg)(*[dropout_site(x) for x in self_sites])
+    ev = _probe("gather_mean_dropout/%d" % rows)
+    check(lib().gs_gather_mean_dropout(ptr(src), src.shape[0], F, src.stride(0), arr, len(segments), ns, ss,
+                                       int(bool(include_self)), ptr(out_self), ptr(out_mean), out_pitch, stream_ptr()))
+    _launched(1 if rows else 0, ev)
+    return out_self, out_mean
+
+
+def dropout_apply(x, site, rows=None, group=1, scale=1.0, out=None, accumulate=False):
+    """Masked scale (gs_dropout_apply): out[r, c] (+)= keep(site, r, c) ? (x[r // group, c] * scale) / keep : 0 for
+    r < rows (default x.shape[0] * group).  x, out: float32 CUDA matrices with unit column stride (strided rows are fine).
+    Forward dropout (x -> drop(x)) and every dropout backward (the same mask applied to the incoming gradient).
+    Returns out (a new [rows, F] tensor unless given)."""
+    require_cuda(x, out)
+    group = int(group)
+    if group < 1:
+        raise ValueError("group must be >= 1")
+    if x.dtype != torch.float32 or x.dim() != 2 or (x.stride(1) != 1 and x.shape[1] > 1):
+        raise ValueError("x must be a float32 matrix with unit column stride")
+    F = x.shape[1]
+    rows = x.shape[0] * group if rows is None else int(rows)
+    if x.shape[0] < (rows + group - 1) // group:
+        raise ValueError("x has %d rows, %d needed" % (x.shape[0], (rows + group - 1) // group))
+    c_site = dropout_site(site)
+    if out is None:
+        if accumulate:
+            raise ValueError("accumulate needs out")
+        out = torch.empty((rows, F), dtype=torch.float32, device=x.device)
+    if out.dtype != torch.float32 or out.dim() != 2 or out.shape[0] < rows or out.shape[1] != F \
+            or (out.stride(1) != 1 and F > 1):
+        raise ValueError("out must be a float32 [>= %d, %d] matrix with unit column stride" % (rows, F))
+    ldx, ldo = max(x.stride(0), F), max(out.stride(0), F)
+    if out.data_ptr() == x.data_ptr() and (group != 1 or ldx != ldo):
+        raise ValueError("in-place dropout_apply needs group == 1 and equal row strides")
+    ev = _probe("dropout_apply/%d" % rows)
+    check(lib().gs_dropout_apply(ptr(x), ldx, rows, F, group, float(scale), c_site, int(bool(accumulate)), ptr(out), ldo,
+                                 stream_ptr()))
+    _launched(1 if rows * F else 0, ev)
+    return out
+
+
+def embedding_grad(lists, n_rows, d, out=None, sites=None):
     """Dense gradient of the trainable embedding table (gs_embedding_grad; the densified IndexedSlices gradient of
     tf.nn.embedding_lookup at reference graphsage/models.py:299): out[r] = sum of scale * grad[i // group] over every
     (ids, grad, group, scale) list entry i with ids[i] == r.  grad: float32 CUDA [>= ceil(n / group), >= d] with unit
-    column stride (a strided view is fine).  Returns out, a contiguous float32 [n_rows, d]; deterministic."""
+    column stride (a strided view is fine).  Returns out, a contiguous float32 [n_rows, d]; deterministic.
+    sites: optional (seed, call, rate) per list (gs_embedding_grad_dropout): entry i of list l is masked with site l at
+    position i, (scale * grad) / keep where kept, 0 where dropped - the gradient through training dropout."""
     if len(lists) > _lib.MAX_EMBED_LISTS:
         raise ValueError("embedding_grad takes at most %d lists" % _lib.MAX_EMBED_LISTS)
+    if sites is not None and len(sites) != len(lists):
+        raise ValueError("embedding_grad: one site per list")
     arr = (_lib.EmbedGradList * max(len(lists), 1))()
     keep = []
     dev = None
@@ -575,8 +649,13 @@ def embedding_grad(lists, n_rows, d, out=None):
         check(-1)
     ws = torch.empty((nbytes,), dtype=torch.uint8, device=out.device) if nbytes > 0 else None
     ev = _probe("embedding_grad/%d" % sum(k.numel() for k in keep))
-    check(lib().gs_embedding_grad(arr, len(lists), int(n_rows), int(d), ptr(out), max(out.stride(0), d), ptr(ws), nbytes,
-                                  stream_ptr()))
+    if sites is None:
+        check(lib().gs_embedding_grad(arr, len(lists), int(n_rows), int(d), ptr(out), max(out.stride(0), d), ptr(ws), nbytes,
+                                      stream_ptr()))
+    else:
+        c_sites = (_lib.DropoutSite * max(len(sites), 1))(*[dropout_site(s) for s in sites])
+        check(lib().gs_embedding_grad_dropout(arr, c_sites, len(lists), int(n_rows), int(d), ptr(out), max(out.stride(0), d),
+                                              ptr(ws), nbytes, stream_ptr()))
     _launched(3 if nbytes > 0 and n_rows * d else 0, ev)           # keys, chunk sums, combine (+ CUB's sort passes)
     return out
 

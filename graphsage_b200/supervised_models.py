@@ -8,6 +8,12 @@ not trainable; with identity_dim > 0 the embedding columns of the layer-0 table 
 into a dense [N+1, d] table by the library's deterministic embedding-gradient kernel (ops.embedding_grad).  Head
 (l2_normalize -> Dense -> sigmoid / softmax cross-entropy + weight decay), gradient clipping to +-5 and Adam follow
 supervised_models.py:85-126.
+
+Training dropout (placeholders['dropout'] = p > 0; reference aggregators.py:46-47 / 104-105, layers.py:107,
+supervised_models.py:88-90) follows the Philox mask contract of include/graphsage_b200.h (gs_dropout_site): the forward
+drops the gathered rows inside the fused gather (mean / GCN) or the pools' MLP input and the head input, and the backward
+regenerates the same masks instead of storing them.  A pass numbers its sites in the reference's call order
+(dropout_site_plan); the model's host `dropout_counter` gives the first call number and advances past them.
 """
 import torch
 
@@ -16,9 +22,35 @@ from .layers import act_code, identity, relu  # noqa: F401
 from .models import SampleAndAggregate
 
 
-def _embedding_grad(emb_shape, lists):
-    """The layer-0 gradient w.r.t. the embedding columns [0, d) of the table: (ids, grad rows, group, scale) lists."""
-    return ops.embedding_grad(lists, emb_shape[0], emb_shape[1])
+def _embedding_grad(emb_shape, lists, sites=None):
+    """The layer-0 gradient w.r.t. the embedding columns [0, d) of the table: (ids, grad rows, group, scale) lists, and with
+    dropout one (seed, call, rate) site per list."""
+    return ops.embedding_grad(lists, emb_shape[0], emb_shape[1], sites=sites)
+
+
+def dropout_site_plan(kind, n_layers, head=False):
+    """The dropout sites of one forward pass in the reference's call order (models.py:303-328 calls each layer's
+    aggregator once per hop): [(layer, hop, role)], role "neigh" then "self" for mean / gcn (aggregators.py:46-47,
+    104-105), the one "mlp" input of the pools' Dense (layers.py:107), then (None, None, "head") for the supervised head
+    (supervised_models.py:88-90).  Site i of a pass draws with call = first call + i."""
+    plan = []
+    for layer in range(n_layers):
+        for hop in range(n_layers - layer):
+            plan += [(layer, hop, "mlp")] if kind in ("maxpool", "meanpool") else [(layer, hop, "neigh"), (layer, hop, "self")]
+    return plan + ([(None, None, "head")] if head else [])
+
+
+class _DropoutFn(torch.autograd.Function):
+    """y = drop(x) for one site (the supervised head's input, layers.py:107); the backward applies the same mask."""
+
+    @staticmethod
+    def forward(ctx, x, site):
+        ctx.site = site
+        return ops.dropout_apply(x.detach(), site)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return ops.dropout_apply(dy.contiguous(), ctx.site), None
 
 
 class _AggregateRowsFn(torch.autograd.Function):
@@ -27,13 +59,18 @@ class _AggregateRowsFn(torch.autograd.Function):
     w.r.t. `emb`, the [N+1, d] embedding view of src's first d columns."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, emb, *weights):
+    def forward(ctx, agg, src, segments, emb, sites, *weights):
+        """sites: None, or one (neighbour site, self site) pair of (seed, call, rate) per segment (training dropout);
+        xs / xm are then the dropped self rows and the mean of the dropped rows, which is what dW = X^T dZ needs."""
         kind = "gcn" if "weights" in agg.vars else "mean"
         code, post = act_code(agg.act)
         if post is not None:
             raise NotImplementedError("training supports act=relu or identity")
         with torch.no_grad():
-            if kind == "mean":
+            if sites is not None:
+                ns, ss = [p[0] for p in sites], [p[1] for p in sites]
+                xs, xm = ops.gather_mean_dropout(src, segments, ns, ss, include_self=kind == "gcn", want_self=kind == "mean")
+            elif kind == "mean":
                 xs, xm = ops.gather_mean(src, segments, want_self=True)
             else:
                 xs, xm = None, ops.gather_mean(src, segments, include_self=True, want_self=False)[1]
@@ -45,7 +82,7 @@ class _AggregateRowsFn(torch.autograd.Function):
                 parts, combine = [(xm, F_in, weights[0])], ops.COMBINE_ADD
             y = ops.sage_gemm(parts, combine=combine, bias=agg.vars.get("bias"), act=code, math=agg.math)
         ctx.kind, ctx.relu, ctx.concat = kind, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
+        ctx.segments, ctx.src_shape, ctx.F_in, ctx.sites = segments, tuple(src.shape), F_in, sites
         ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
         ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
         ctx.has_bias = "bias" in agg.vars
@@ -74,12 +111,21 @@ class _AggregateRowsFn(torch.autograd.Function):
                 dxs = None
         if ctx.src_needs_grad:
             dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device)
-            for s in ctx.segments:
+            for si, s in enumerate(ctx.segments):
                 if s.self_ids is not None or s.neigh_ids is not None:
                     raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
                 n, k = s.n, s.k
                 rows = slice(s.out_row0, s.out_row0 + n)
                 div = float(k + (1 if ctx.kind == "gcn" else 0))
+                if ctx.sites is not None:
+                    # the masks regenerated: neighbour row i*k + j gets mask * dxm[i] / div / keep, the self row mask * dxs[i]
+                    # (gcn: mask * dxm[i] / div); launched in this fixed order, so dsrc is reproducible
+                    nsite, ssite = ctx.sites[si]
+                    ops.dropout_apply(dxm[rows], nsite, rows=n * k, group=k, scale=1.0 / div, accumulate=True,
+                                      out=dsrc[s.neigh_row0:s.neigh_row0 + n * k])
+                    self_g, self_scale = (dxm[rows], 1.0 / div) if ctx.kind == "gcn" else (dxs[rows], 1.0)
+                    ops.dropout_apply(self_g, ssite, scale=self_scale, accumulate=True, out=dsrc[s.self_row0:s.self_row0 + n])
+                    continue
                 dsrc[s.neigh_row0:s.neigh_row0 + n * k].view(n, k, -1).add_((dxm[rows] / div).unsqueeze(1))
                 if ctx.kind == "gcn":
                     dsrc[s.self_row0:s.self_row0 + n].add_(dxm[rows] / div)
@@ -93,16 +139,18 @@ class _AggregateRowsFn(torch.autograd.Function):
                 es, em = dz_s @ weights[0][:d].t(), dz_n @ weights[1][:d].t()
             else:
                 es, em = None, dz @ weights[0][:d].t()
-            lists = []
-            for s in ctx.segments:
+            lists, sites = [], ([] if ctx.sites is not None else None)
+            for si, s in enumerate(ctx.segments):
                 n, k = s.n, s.k
                 rows = slice(s.out_row0, s.out_row0 + n)
                 if ctx.kind == "gcn":                       # mean over [neighbours, self]: every id gets dxm / (k + 1)
                     lists += [(s.self_ids[:n], em[rows], 1, 1.0 / (k + 1)), (s.neigh_ids[:n * k], em[rows], k, 1.0 / (k + 1))]
                 else:                                       # self id: dxs; neighbour ids: dxm / k
                     lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], em[rows], k, 1.0 / k)]
-            demb = _embedding_grad(ctx.emb_shape, lists)
-        return (None, dsrc, None, demb) + tuple(grads_w)
+                if sites is not None:                       # entry i of a list is position i of its site
+                    sites += [ctx.sites[si][1], ctx.sites[si][0]]
+            demb = _embedding_grad(ctx.emb_shape, lists, sites)
+        return (None, dsrc, None, demb, None) + tuple(grads_w)
 
 
 def pool_branch_backward(pool, xn, h, hp, dhp, Wm, k, need_dx):
@@ -131,7 +179,9 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
     The gathered neighbour rows and the MLP activations are kept for the backward pass."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None):
+    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None, sites=None):
+        """sites: None, or one (seed, call, rate) per segment for the MLP input (training dropout, layers.py:107; the self
+        rows are not dropped); the kept xn is the dropped input, which is what dWm = xn^T dpre needs."""
         code, post = act_code(agg.act)
         if post is not None:
             raise NotImplementedError("training supports act=relu or identity")
@@ -143,10 +193,12 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
             xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
             hp = torch.empty((rows, hid), dtype=torch.float32, device=src.device)
             kept = []
-            for s in segments:
+            for si, s in enumerate(segments):
                 n, k = s.n, s.k
                 xn = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
                     src[s.neigh_row0:s.neigh_row0 + n * k]
+                if sites is not None:                        # out of place: layer >= 1 rows belong to the previous layer
+                    xn = ops.dropout_apply(xn, sites[si])
                 mlp = agg.mlp_layers[0]
                 mlp.math = agg.math
                 h = mlp(xn)
@@ -161,7 +213,7 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
                 kept.extend([xn, h])
             y = agg._finish([(xs, agg.input_dim, Ws), (hp, hid, Wn)], agg._combine())
         ctx.pool, ctx.relu, ctx.concat = agg.pool, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
+        ctx.segments, ctx.src_shape, ctx.F_in, ctx.sites = segments, tuple(src.shape), F_in, sites
         ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
         ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
         ctx.save_for_backward(xs, hp, y, Ws, Wn, Wm, *kept)
@@ -194,6 +246,8 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
                                                    ctx.src_needs_grad or emb)
             dWm += g_wm
             dbm += g_bm
+            if dxn is not None and ctx.sites is not None:    # through the input mask, regenerated
+                dxn = ops.dropout_apply(dxn, ctx.sites[i])
             if emb:                                          # self id: dxs; neighbour id of gathered row r: dxn[r]
                 lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dxn[:, :d], 1, 1.0)]
             if ctx.src_needs_grad:
@@ -202,12 +256,17 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
                 dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dxn
                 dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
         demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
-        return None, dsrc, None, dWs, dWn, dWm, dbm, demb
+        return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
 
 
-def differentiable_outputs(model, batch, normalize=True):
+def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     """sample -> aggregate (-> l2_normalize) with an autograd graph over the aggregator weights; `model` is a
-    SampleAndAggregate whose .aggregators exist (reference models.py:347-350 / supervised_models.py:79-85)."""
+    SampleAndAggregate whose .aggregators exist (reference models.py:347-350 / supervised_models.py:79-85).
+    dropout = p > 0: training dropout, sites numbered by dropout_site_plan from model.dropout_counter, which advances
+    past them (p = 0 draws nothing and leaves the counter alone)."""
+    dropout = check_dropout_rate(dropout)
+    if dropout:
+        refuse_dropout_table(model.features)
     batch = batch.to(device=model.device, dtype=torch.int32).reshape(-1)
     n = batch.numel()
     with torch.no_grad():
@@ -216,6 +275,9 @@ def differentiable_outputs(model, batch, normalize=True):
     L = len(num_samples)
     counts = [n * support[h] for h in range(L + 1)]
     src = model.features
+    pool = hasattr(model.aggregators[0], "mlp_layers")
+    plan = dropout_site_plan("maxpool" if pool else "mean", L) if dropout else []
+    call = {site: model.dropout_counter + i for i, site in enumerate(plan)}
     for layer in range(L):
         hops = L - layer
         row0 = [sum(counts[:h]) for h in range(hops + 1)]
@@ -232,26 +294,61 @@ def differentiable_outputs(model, batch, normalize=True):
         # layer 0 reads the embedding table (identity_dim > 0) through src; handing it over as an input lets autograd
         # deliver the scattered gradient as embeds.grad
         emb = getattr(model, "embeds", None) if layer == 0 else None
-        if hasattr(agg, "mlp_layers"):                      # max-pool / mean-pool
+        sites = None
+        if dropout:                                          # per hop: the MLP-input site, or the (neighbour, self) pair
+            key = model.dropout_key
+            if pool:
+                sites = [(key, call[(layer, h, "mlp")], dropout) for h in range(hops)]
+            else:
+                sites = [((key, call[(layer, h, "neigh")], dropout), (key, call[(layer, h, "self")], dropout))
+                         for h in range(hops)]
+        if pool:                                             # max-pool / mean-pool
             mlp = agg.mlp_layers[0].vars
             src = _PoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
-                                             mlp["weights"], mlp["bias"], emb)
+                                             mlp["weights"], mlp["bias"], emb, sites)
         else:
             ws = (agg.vars["weights"],) if "weights" in agg.vars else (agg.vars["self_weights"], agg.vars["neigh_weights"])
-            src = _AggregateRowsFn.apply(agg, src, segs, emb, *ws)
+            src = _AggregateRowsFn.apply(agg, src, segs, emb, sites, *ws)
+    model.dropout_counter += len(plan)
     out = src[:counts[0]]
     if normalize:
         out = out / torch.sqrt(torch.clamp((out * out).sum(dim=1, keepdim=True), min=1e-12))   # tf.nn.l2_normalize
     return out
 
 
+def check_dropout_rate(rate):
+    rate = float(rate or 0.)
+    if not 0.0 <= rate < 1.0:
+        raise ValueError("dropout must be in [0, 1) (got %r)" % (rate,))
+    return rate
+
+
+def refuse_dropout_table(features):
+    """Training dropout needs the dense fp32 table of the masked gather kernel."""
+    if hasattr(features, "c_table"):
+        raise NotImplementedError("training dropout with a node-partitioned (ShardedFeatures) table is not implemented")
+    if features.dtype != torch.float32:
+        raise NotImplementedError("training dropout with a %s feature table is not implemented (float32 only)"
+                                  % features.dtype)
+
+
+def init_dropout(model, dropout_seed, distributed, group):
+    """The training rate placeholders['dropout'] (validated), the mask key and the site counter.  With distributed=True
+    the key is dropout_seed + rank, so the ranks draw independent masks for their different batches."""
+    rate = check_dropout_rate(model.placeholders.get("dropout", 0.))
+    if rate:
+        refuse_dropout_table(model.features)
+    key = int(dropout_seed)
+    if distributed:
+        import torch.distributed as dist
+        key += dist.get_rank(group)
+    model.dropout_rate, model.dropout_key, model.dropout_counter = rate, key, 0
+
+
 def build_aggregators(model):
-    """One aggregator per layer, as SampleAndAggregate.aggregate creates them (reference models.py:303-315)."""
-    if float(model.placeholders.get("dropout", 0.) or 0.) != 0.:
-        # the reference applies dropout inside the aggregators and in the prediction Dense (supervised_models.py:88-90);
-        # the differentiable path here has no dropout, so refuse rather than silently train a different model
-        raise NotImplementedError("training with placeholders['dropout'] > 0 is not implemented (forward-only "
-                                  "dropout runs through SampleAndAggregate.aggregate's materialised path)")
+    """One aggregator per layer, as SampleAndAggregate.aggregate creates them (reference models.py:303-315).  Their own
+    .dropout stays 0 - forward, graphed, pipelined and export paths keep the fused inference kernels; the training rate
+    placeholders['dropout'] is applied by the training pass (differentiable_outputs)."""
     L = len(model.layer_infos)
     aggs = []
     for layer in range(L):
@@ -308,13 +405,16 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def __init__(self, num_classes, placeholders, features, adj, degrees, layer_infos, concat=True,
                  aggregator_type="mean", model_size="small", sigmoid_loss=False, identity_dim=0, learning_rate=0.01,
-                 weight_decay=0.0, device="cuda", distributed=False, group=None, **kwargs):
+                 weight_decay=0.0, device="cuda", distributed=False, group=None, dropout_seed=12345, **kwargs):
+        """dropout_seed: key of the training dropout masks (placeholders['dropout'] > 0); with distributed=True each rank
+        uses dropout_seed + rank."""
         refuse_distributed_embeddings(identity_dim, distributed)
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
                                                   identity_dim=identity_dim, device=device, **kwargs)
         if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool"):
             raise NotImplementedError("training is implemented for the mean, gcn, maxpool and meanpool aggregators")
+        init_dropout(self, dropout_seed, distributed, group)
         self.num_classes = num_classes
         self.sigmoid_loss = sigmoid_loss
         self.learning_rate, self.weight_decay = learning_rate, weight_decay
@@ -340,17 +440,24 @@ class SupervisedGraphsage(SampleAndAggregate):
     def decayed_parameters(self):
         return aggregator_parameters(self.aggregators)[1] + list(self.node_pred_vars.values())
 
-    def outputs(self, batch):
-        """l2-normalised node representations, differentiable (supervised_models.py:79-85)."""
-        return differentiable_outputs(self, batch)
+    def outputs(self, batch, dropout=0.):
+        """l2-normalised node representations, differentiable (supervised_models.py:79-85).  dropout: the training
+        rate (0 = the reference's evaluation default, placeholder_with_default(0.))."""
+        return differentiable_outputs(self, batch, dropout=dropout)
 
-    def logits(self, batch):
-        return self.outputs(batch) @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
+    def logits(self, batch, dropout=0.):
+        """node_pred(outputs) (supervised_models.py:88-92); with dropout > 0 the head input is dropped too (one more
+        site, after the aggregators')."""
+        out = self.outputs(batch, dropout=dropout)
+        if check_dropout_rate(dropout):
+            out = _DropoutFn.apply(out, (self.dropout_key, self.dropout_counter, dropout))
+            self.dropout_counter += 1
+        return out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
 
-    def loss(self, batch, labels):
+    def loss(self, batch, labels, dropout=0.):
         """supervised_models.py:101-118: weight decay * l2_loss(var) over aggregator + head variables, then the
         mean of the per-element sigmoid xent (multi-label) or the mean of the per-node softmax xent."""
-        logits = self.logits(batch)
+        logits = self.logits(batch, dropout=dropout) if dropout else self.logits(batch)    # overrides take (batch)
         labels = labels.to(device=logits.device, dtype=torch.float32)
         loss = classification_loss(logits, labels, self.sigmoid_loss)
         if self.weight_decay:
@@ -358,8 +465,9 @@ class SupervisedGraphsage(SampleAndAggregate):
         return loss
 
     def train_step(self, batch, labels):
+        """One Adam step at the training dropout rate placeholders['dropout'] (supervised_train.py:271)."""
         self.optimizer.zero_grad(set_to_none=True)
-        loss = self.loss(batch, labels)
+        loss = self.loss(batch, labels, dropout=self.dropout_rate)
         loss.backward()
         if self.distributed:                                                     # data parallel: mean gradient over ranks
             from .parallel import allreduce_gradients

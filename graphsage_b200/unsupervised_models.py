@@ -13,7 +13,7 @@ from . import ops
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
 from .supervised_models import (aggregator_parameters, build_aggregators, differentiable_outputs, embedding_parameters,
-                                refuse_distributed_embeddings, weight_decay_term)
+                                init_dropout, refuse_distributed_embeddings, weight_decay_term)
 
 
 class UnigramNegativeSampler(object):
@@ -36,13 +36,16 @@ class UnsupervisedGraphsage(SampleAndAggregate):
 
     def __init__(self, placeholders, features, adj, degrees, layer_infos, concat=True, aggregator_type="mean",
                  model_size="small", identity_dim=0, neg_sample_size=20, neg_sample_weights=1.0, learning_rate=0.00001,
-                 weight_decay=0.0, seed=123, device="cuda", distributed=False, group=None, **kwargs):
+                 weight_decay=0.0, seed=123, device="cuda", distributed=False, group=None, dropout_seed=12345, **kwargs):
+        """dropout_seed: key of the training dropout masks (placeholders['dropout'] > 0); with distributed=True each rank
+        uses dropout_seed + rank."""
         refuse_distributed_embeddings(identity_dim, distributed)
         super(UnsupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                     aggregator_type=aggregator_type, model_size=model_size,
                                                     identity_dim=identity_dim, device=device, **kwargs)
         if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool"):
             raise NotImplementedError("training is implemented for the mean, gcn, maxpool and meanpool aggregators")
+        init_dropout(self, dropout_seed, distributed, group)
         self.neg_sample_size, self.neg_sample_weights = int(neg_sample_size), float(neg_sample_weights)
         self.learning_rate, self.weight_decay = learning_rate, weight_decay
         self.neg_sampler = UnigramNegativeSampler(degrees, 0.75, seed, device)      # models.py:336-343
@@ -65,19 +68,21 @@ class UnsupervisedGraphsage(SampleAndAggregate):
     def decayed_parameters(self):
         return aggregator_parameters(self.aggregators)[1]
 
-    def embed(self, batch):
-        return differentiable_outputs(self, batch)                                   # models.py:347-370
+    def embed(self, batch, dropout=0.):
+        """dropout: the training rate (0 = the reference's evaluation default); each call draws fresh sites."""
+        return differentiable_outputs(self, batch, dropout=dropout)                  # models.py:347-370
 
-    def _passes(self, batch1, batch2):
+    def _passes(self, batch1, batch2, dropout=0.):
         neg = self.neg_sampler(self.neg_sample_size)
-        o1, o2 = self.embed(batch1), self.embed(batch2)
-        on = self.embed(neg)                                                         # batch_size = neg_sample_size (:356-360)
+        o1, o2 = self.embed(batch1, dropout), self.embed(batch2, dropout)
+        on = self.embed(neg, dropout)                                                # batch_size = neg_sample_size (:356-360)
         return o1, o2, on, neg
 
-    def loss(self, batch1, batch2):
+    def loss(self, batch1, batch2, dropout=0.):
         """weight decay + BipartiteEdgePredLayer._xent_loss (prediction.py:102-110), divided by the batch size
-        (models.py:378)."""
-        o1, o2, on, _ = self._passes(batch1, batch2)
+        (models.py:378).  The edge-prediction layer has no dropout (models.py:363-366)."""
+        # at dropout 0 the two-argument form, which overrides of _passes implement
+        o1, o2, on, _ = self._passes(batch1, batch2, dropout) if dropout else self._passes(batch1, batch2)
         loss = self.link_pred_layer.loss(o1, o2, on)
         if self.weight_decay:
             loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)       # models.py:385-387
@@ -91,7 +96,7 @@ class UnsupervisedGraphsage(SampleAndAggregate):
 
     def train_step(self, batch1, batch2):
         self.optimizer.zero_grad(set_to_none=True)
-        loss = self.loss(batch1, batch2)
+        loss = self.loss(batch1, batch2, dropout=self.dropout_rate)                 # unsupervised_train.py:269
         loss.backward()
         if self.distributed:                                                         # data parallel: mean gradient over ranks
             from .parallel import allreduce_gradients

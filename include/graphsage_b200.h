@@ -405,6 +405,48 @@ int64_t gs_embedding_grad_workspace_bytes(const gs_embed_grad_list* lists_host, 
 int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float* out,
                           int64_t ldo, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Dropout for training (tf.nn.dropout at reference aggregators.py:46-47 / 104-105, layers.py:107).  TF's mask stream
+ * cannot be reproduced, so masks follow a counter-based contract (oracle/dropout.py), regenerated in the backward pass
+ * instead of being stored.  A SITE is one dropout application over a logical [rows, F] tensor:
+ *   element (pos, c) is kept iff word c % 4 of philox4x32_10(ctr = (c / 4, pos & 0xffffffff, pos >> 32, call),
+ *   key = (seed & 0xffffffff, seed >> 32)) is >= T = floor(rate * 2^32) (computed in float64 from the fp32 rate);
+ *   a kept element becomes x / keep, keep = fp32(1 - rate) (IEEE division), a dropped element 0.  0 <= rate < 1.
+ * Columns are logical (0 .. F-1, independent of any pitch).  Positions: neighbour j of output row i of a segment:
+ * pos = i * k + j (the row-major [n, k, F] flattening); self row of i: pos = i; any other [rows, F] tensor: pos = row.
+ * --------------------------------------------------------------------------------------------- */
+typedef struct {
+  uint64_t seed;
+  uint32_t call;
+  float rate;
+} gs_dropout_site;
+
+/* gs_gather_mean (GS_F32 tables only) with dropout applied to the gathered rows in registers:
+ *   out_self[r] = drop(self_sites[s], pos = i, self row)                                   (if out_self != NULL)
+ *   out_mean[r] = (sum_j drop(neigh_sites[s], pos = i*k + j, neigh row j) (+ drop(self row))) / (k (+1 if include_self))
+ * summed in j order, the self row last - the order of gs_gather_mean, which this equals bit for bit when every rate is 0.
+ * neigh_sites_host / self_sites_host hold one site per segment. */
+int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, int64_t pitch, const gs_segment* segments_host,
+                               int32_t n_segments, const gs_dropout_site* neigh_sites_host,
+                               const gs_dropout_site* self_sites_host, int32_t include_self, float* out_self,
+                               float* out_mean, int64_t out_pitch, void* stream);
+
+/* Masked scale, elementwise over a [rows, F] block:
+ *   v = keep(site, pos = r, c) ? (x[(r / group) * ldx + c] * scale) / keep : 0
+ *   out[r * ldo + c] = accumulate ? out[r * ldo + c] + v : v
+ * group >= 1 repeats each x row for `group` consecutive output rows (the fanout mean's backward).  out may alias x when
+ * group == 1 and ldo == ldx.  Each element is read and written by one thread: bit-identical on every call. */
+int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, int32_t group, float scale,
+                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, void* stream);
+
+/* gs_embedding_grad with a dropout site per list (sites_host[l]; NULL: no masks): contribution i of list l adds
+ *   keep(site_l, pos = i, c) ? (l.scale * l.grad[(i / l.group) * l.ldg + c]) / keep : 0
+ * to column c of its row - the gradient through drop(embedding_lookup(...)) with the masks regenerated, not stored.
+ * Workspace, limits and the summation order are those of gs_embedding_grad (the query above gives the size). */
+int32_t gs_embedding_grad_dropout(const gs_embed_grad_list* lists_host, const gs_dropout_site* sites_host, int32_t n_lists,
+                                  int64_t n_rows, int32_t d, float* out, int64_t ldo, void* workspace,
+                                  int64_t workspace_bytes, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
