@@ -39,6 +39,8 @@ class GemmPart(ctypes.Structure):
 
 
 MAX_EMBED_LISTS = 8
+MAX_UNIQUE_SAMPLED = 1024          # GS_MAX_UNIQUE_SAMPLED
+UNIQUE_DRAW_BUDGET = 1 << 20       # GS_UNIQUE_DRAW_BUDGET
 
 
 class EmbedGradList(ctypes.Structure):
@@ -58,6 +60,7 @@ _SIGNATURES = {
                                       ctypes.POINTER(c_vp), c_vp]),
     "gs_build_padded_adj": (c_i32, [c_vp, c_vp, c_i64, c_i32, c_vp, c_u64, c_u64, c_vp, c_vp, c_vp]),
     "gs_sample_unigram": (c_i32, [c_vp, c_i64, c_i32, c_u64, c_u64, c_vp, c_vp, c_vp]),
+    "gs_sample_unigram_unique": (c_i32, [c_vp, c_i64, c_i32, c_u64, c_u64, c_vp, c_vp, c_vp, c_vp]),
     "gs_sample_csr": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_vp, c_i32, c_vp, c_vp]),
     "gs_perm_prefix_host": (c_i32, [c_u64, c_u64, c_i32, c_i32, ctypes.POINTER(c_i32)]),
     "gs_gather_rows": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp]),
@@ -113,6 +116,11 @@ _SIGNATURES = {
     "gs_dropout_apply": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, ctypes.c_float, DropoutSite, c_i32, c_vp, c_i64, c_vp]),
     "gs_embedding_grad_dropout": (c_i32, [ctypes.POINTER(EmbedGradList), ctypes.POINTER(DropoutSite), c_i32, c_i64, c_i32, c_vp,
                                           c_i64, c_vp, c_i64, c_vp]),
+    "gs_embedding_sgd": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, ctypes.c_float, c_vp, c_i64, c_vp, c_i64,
+                                 c_vp]),
+    "gs_skipgram_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32]),
+    "gs_skipgram_grad": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,
+                                 c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

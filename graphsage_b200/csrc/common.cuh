@@ -117,6 +117,7 @@ constexpr uint32_t kStreamPadded = 0u;
 constexpr uint32_t kStreamCsr = 0x40000000u;
 constexpr uint32_t kStreamUnigram = 0x20000000u;
 constexpr uint32_t kStreamBuild = 0x10000000u;
+constexpr uint32_t kStreamUnigramUnique = 0x30000000u;
 
 // ---- PTX wrappers (mbarrier / bulk copy) ---------------------------------------------------
 #ifdef __CUDACC__

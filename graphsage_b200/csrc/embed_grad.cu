@@ -10,6 +10,8 @@
 //      that crosses a chunk edge leaves its piece in a partial slot (first piece of chunk j -> slot 2j, last -> 2j+1).
 //   4. combine pass: the chunk where a crossing run starts adds the run's pieces in a fixed lane / chunk order.
 // No atomics anywhere: the result depends on the inputs only.
+// gs_embedding_sgd is the same machinery with the stores turned into in-place updates of the touched rows,
+// table[id] += alpha * sum (kApply); it clears nothing, so untouched rows are neither read nor written.
 #define CUB_WRAPPED_NAMESPACE gs_cub
 #include <cub/device/device_radix_sort.cuh>
 
@@ -55,11 +57,12 @@ __global__ void embed_keys_kernel(Lists L, int64_t total, uint32_t n_rows, uint3
 }
 
 // kDrop: every product scale * grad goes through its list's dropout mask at pos = index in the list (the masked entry)
-template <bool kDrop>
+// kApply: out is a table updated in place, out[id] += alpha * (row sum), instead of a gradient written with out[id] = sum
+template <bool kDrop, bool kApply>
 __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_t* __restrict__ keys,
                                                           const int32_t* __restrict__ vals, int64_t total,
                                                           uint32_t n_rows, int32_t d, float* __restrict__ out,
-                                                          int64_t ldo, float* __restrict__ partial) {
+                                                          int64_t ldo, float* __restrict__ partial, float alpha) {
   const unsigned FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int64_t nchunks = (total + kChunk - 1) / kChunk;
@@ -124,12 +127,17 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
             if (key < n_rows) {
               const bool before = piece_start == 0 && key_before == key;
               const bool after = i == cnt - 1 && key_after == key;
-              float* dst = (!before && !after) ? out + (int64_t)key * ldo
-                                               : partial + (2 * j + (piece_start == 0 ? 0 : 1)) * (int64_t)d;
+              const bool whole = !before && !after;
+              float* dst = whole ? out + (int64_t)key * ldo
+                                 : partial + (2 * j + (piece_start == 0 ? 0 : 1)) * (int64_t)d;
 #pragma unroll
               for (int q = 0; q < kColsPerLane; ++q) {
                 const int col = c0 + lane + 32 * q;
-                if (col < d) dst[col] = acc[q];
+                if constexpr (kApply) {
+                  if (col < d) dst[col] = whole ? dst[col] + alpha * acc[q] : acc[q];
+                } else {
+                  if (col < d) dst[col] = acc[q];
+                }
               }
             }
 #pragma unroll
@@ -142,10 +150,11 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
   }
 }
 
+template <bool kApply>
 __global__ void __launch_bounds__(kLanes * 32) embed_combine_kernel(const uint32_t* __restrict__ keys, int64_t total,
                                                                     uint32_t n_rows, int32_t d,
                                                                     const float* __restrict__ partial,
-                                                                    float* __restrict__ out, int64_t ldo) {
+                                                                    float* __restrict__ out, int64_t ldo, float alpha) {
   __shared__ float red[kLanes][32];
   __shared__ int64_t run_end;
   const int cl = threadIdx.x & 31, p = threadIdx.x >> 5;
@@ -194,7 +203,10 @@ __global__ void __launch_bounds__(kLanes * 32) embed_combine_kernel(const uint32
         float r = red[0][cl];
 #pragma unroll
         for (int pp = 1; pp < kLanes; ++pp) r += red[pp][cl];
-        out[(int64_t)X * ldo + col] = r;
+        if constexpr (kApply)
+          out[(int64_t)X * ldo + col] = out[(int64_t)X * ldo + col] + alpha * r;
+        else
+          out[(int64_t)X * ldo + col] = r;
       }
       __syncthreads();
     }
@@ -262,7 +274,7 @@ int64_t gs_embedding_grad_workspace_bytes(const gs_embed_grad_list* lists_host, 
 
 static int32_t embedding_grad(const gs_embed_grad_list* lists_host, const gs_dropout_site* sites_host, int32_t n_lists,
                               int64_t n_rows, int32_t d, float* out, int64_t ldo, void* workspace, int64_t workspace_bytes,
-                              void* stream, const char* who) {
+                              void* stream, const char* who, bool apply = false, float alpha = 0.f) {
   gs::Plan P;
   int32_t rc = gs::make_plan(lists_host, n_lists, n_rows, d, P, who);
   if (rc != GS_OK) return rc;
@@ -273,7 +285,7 @@ static int32_t embedding_grad(const gs_embed_grad_list* lists_host, const gs_dro
              "%s: workspace of %lld bytes, %lld needed", who, (long long)workspace_bytes,
              (long long)P.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  GS_CUDA(cudaMemset2DAsync(out, (size_t)ldo * 4, 0, (size_t)d * 4, (size_t)n_rows, st));
+  if (!apply) GS_CUDA(cudaMemset2DAsync(out, (size_t)ldo * 4, 0, (size_t)d * 4, (size_t)n_rows, st));
   if (P.total == 0) return GS_OK;
 
   gs::Lists L{};
@@ -307,18 +319,25 @@ static int32_t embedding_grad(const gs_embed_grad_list* lists_host, const gs_dro
 
   blocks = (P.nchunks * 32 + 255) / 256;
   if (blocks > cap * 2) blocks = cap * 2;
-  if (sites_host)
-    gs::embed_chunk_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d, out,
-                                                                   ldo, partial);
+  if (apply)
+    gs::embed_chunk_kernel<false, true><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d,
+                                                                          out, ldo, partial, alpha);
+  else if (sites_host)
+    gs::embed_chunk_kernel<true, false><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d,
+                                                                          out, ldo, partial, 0.f);
   else
-    gs::embed_chunk_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d, out,
-                                                                    ldo, partial);
+    gs::embed_chunk_kernel<false, false><<<(unsigned)blocks, 256, 0, st>>>(L, keys_out, vals_out, P.total, (uint32_t)n_rows, d,
+                                                                           out, ldo, partial, 0.f);
   rc = gs::launch_check("embed_chunk_kernel");
   if (rc != GS_OK) return rc;
 
   blocks = P.nchunks < cap ? P.nchunks : cap;
-  gs::embed_combine_kernel<<<(unsigned)blocks, gs::kLanes * 32, 0, st>>>(keys_out, P.total, (uint32_t)n_rows, d,
-                                                                          partial, out, ldo);
+  if (apply)
+    gs::embed_combine_kernel<true><<<(unsigned)blocks, gs::kLanes * 32, 0, st>>>(keys_out, P.total, (uint32_t)n_rows, d,
+                                                                                partial, out, ldo, alpha);
+  else
+    gs::embed_combine_kernel<false><<<(unsigned)blocks, gs::kLanes * 32, 0, st>>>(keys_out, P.total, (uint32_t)n_rows, d,
+                                                                                 partial, out, ldo, 0.f);
   return gs::launch_check("embed_combine_kernel");
 }
 
@@ -336,6 +355,13 @@ int32_t gs_embedding_grad_dropout(const gs_embed_grad_list* lists_host, const gs
                i, (double)sites_host[i].rate);
   return embedding_grad(lists_host, sites_host, n_lists, n_rows, d, out, ldo, workspace, workspace_bytes, stream,
                         "gs_embedding_grad_dropout");
+}
+
+int32_t gs_embedding_sgd(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float alpha,
+                         float* table, int64_t ldt, void* workspace, int64_t workspace_bytes, void* stream) {
+  GS_REQUIRE(isfinite(alpha), "gs_embedding_sgd: alpha must be finite");
+  return embedding_grad(lists_host, nullptr, n_lists, n_rows, d, table, ldt, workspace, workspace_bytes, stream,
+                        "gs_embedding_sgd", true, alpha);
 }
 
 }  // extern "C"

@@ -179,6 +179,54 @@ __global__ void __launch_bounds__(128) sample_unigram_kernel(const double* __res
   out[j] = (int32_t)lo;
 }
 
+// the u -> id rule of sample_unigram_kernel: first index whose inclusive prefix sum exceeds u
+__device__ __forceinline__ int32_t unigram_lookup(const double* __restrict__ cdf, int64_t n, uint32_t r) {
+  const double u = ((double)r + 0.5) * (1.0 / 4294967296.0) * cdf[n - 1];
+  int64_t lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (cdf[mid] > u) hi = mid; else lo = mid + 1;
+  }
+  return (int32_t)lo;
+}
+
+// unique=True: ONE warp.  Round t draws candidates 32t .. 32t+31 (lane l owns draw 32t + l); a lane is accepted iff its id
+// is not in the accepted set and no lower lane of the round holds the same id (__match_any_sync); a ballot prefix keeps
+// draw order and the round is cut at num.  That is exactly "draw in sequence, reject ids already held".  The set is a
+// linear list in shared memory (num <= kMaxUniqueSampled), scanned by every lane with broadcast reads.
+__global__ void __launch_bounds__(32) sample_unigram_unique_kernel(const double* __restrict__ cdf, int64_t n, int32_t num,
+                                                                   int64_t max_draws, uint64_t seed, uint64_t counter,
+                                                                   const uint64_t* __restrict__ counter_dev,
+                                                                   int32_t* __restrict__ out, int32_t* __restrict__ status) {
+  __shared__ int32_t held[GS_MAX_UNIQUE_SAMPLED];
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x;
+  const unsigned lower = (1u << lane) - 1u;
+  const uint64_t ctr = counter + (counter_dev ? *counter_dev : 0ull);
+  int count = 0;
+  int64_t j0 = 0;
+  for (; count < num && j0 < max_draws; j0 += 32) {
+    const int64_t j = j0 + lane;
+    const bool live = j < max_draws;
+      const int32_t id = live ? unigram_lookup(cdf, n, philox_draw(seed, ctr, 0u, kStreamUnigramUnique, (int)j)) : -1 - lane;
+    bool fresh = live;
+    for (int q = 0; q < count; ++q) fresh &= held[q] != id;
+    const unsigned same = __match_any_sync(FULL, id);
+    fresh &= (same & lower) == 0u;
+    const unsigned acc = __ballot_sync(FULL, fresh);
+    const int pos = count + __popc(acc & lower);
+    if (fresh && pos < num) {
+      held[pos] = id;
+      out[pos] = id;
+    }
+    count = min(num, count + __popc(acc));
+    __syncwarp();
+  }
+  // draw budget exhausted: the unfilled positions get -1 and the (sticky) status word says so
+  for (int p = count + lane; p < num; p += 32) out[p] = -1;
+  if (lane == 0 && status != nullptr && count < num) *status = 1;
+}
+
 // padded adjacency from CSR, one warp per node (start-up time, not per batch)
 __global__ void __launch_bounds__(256) build_padded_adj_kernel(const int64_t* __restrict__ indptr,
                                                                const int32_t* __restrict__ indices, int64_t n_nodes,
@@ -298,6 +346,19 @@ int32_t gs_sample_unigram(const double* cdf, int64_t n, int32_t num_sampled, uin
   gs::sample_unigram_kernel<<<(num_sampled + 127) / 128, 128, 0, (cudaStream_t)stream>>>(cdf, n, num_sampled, seed, counter,
                                                                                        counter_dev, out);
   return gs::launch_check("sample_unigram_kernel");
+}
+
+int32_t gs_sample_unigram_unique(const double* cdf, int64_t n, int32_t num_sampled, uint64_t seed, uint64_t counter,
+                                 const uint64_t* counter_dev, int32_t* out, int32_t* status, void* stream) {
+  GS_REQUIRE(n >= 1 && n < 0x7fffffffLL, "gs_sample_unigram_unique: need 1 <= n < 2^31 - 1 (got %lld)", (long long)n);
+  GS_REQUIRE(num_sampled >= 0 && num_sampled <= GS_MAX_UNIQUE_SAMPLED && num_sampled <= n,
+             "gs_sample_unigram_unique: num_sampled=%d must be in [0, min(%d, n=%lld)]", num_sampled, GS_MAX_UNIQUE_SAMPLED,
+             (long long)n);
+  if (num_sampled == 0) return GS_OK;
+  GS_REQUIRE(cdf && out, "gs_sample_unigram_unique: NULL pointer");
+  gs::sample_unigram_unique_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(cdf, n, num_sampled, GS_UNIQUE_DRAW_BUDGET, seed,
+                                                                      counter, counter_dev, out, status);
+  return gs::launch_check("sample_unigram_unique_kernel");
 }
 
 int32_t gs_sample_csr(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, const int32_t* ids, int64_t n,

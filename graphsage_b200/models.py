@@ -441,3 +441,6 @@ class PipelinedForward(object):
         self.synchronize()
         for run in self.runners:
             run.close()
+
+
+from .node2vec import Node2VecModel  # noqa: E402,F401  (reference graphsage/models.py:408-501)

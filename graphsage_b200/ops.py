@@ -115,6 +115,27 @@ def sample_unigram(cdf, num_sampled, seed, counter, counter_dev=None):
     return out
 
 
+def sample_unigram_unique(cdf, num_sampled, seed, counter, counter_dev=None, status=None):
+    """tf.nn.fixed_unigram_candidate_sampler(unique=True) - reference graphsage/models.py:450-457 (Node2VecModel): the first
+    num_sampled DISTINCT ids of the unigram draw sequence, in draw order (contract: oracle/node2vec.py).  cdf: float64 CUDA
+    tensor, inclusive prefix sum of the weights.  The caller checks that at least num_sampled ids have positive weight
+    (UniqueUnigramSampler does); if the draw budget runs out anyway the missing ids are -1 and status (an int32 CUDA
+    tensor [1], optional) is set to 1."""
+    require_cuda(cdf, counter_dev, status)
+    if cdf.dtype != torch.float64:
+        raise TypeError("cdf must be float64")
+    if status is not None and (status.dtype != torch.int32 or status.numel() < 1):
+        raise TypeError("status must be an int32 tensor with >= 1 element")
+    if not 0 <= int(num_sampled) <= min(_lib.MAX_UNIQUE_SAMPLED, cdf.numel()):
+        raise ValueError("num_sampled must be in [0, min(%d, %d)] (got %d)" % (_lib.MAX_UNIQUE_SAMPLED, cdf.numel(), num_sampled))
+    out = torch.empty((num_sampled,), dtype=torch.int32, device=cdf.device)
+    ev = _probe("sample_unigram_unique")
+    check(lib().gs_sample_unigram_unique(ptr(cdf), cdf.numel(), int(num_sampled), seed & _U64, counter & _U64, ptr(counter_dev),
+                                         ptr(out), ptr(status), stream_ptr()))
+    _launched(1 if num_sampled else 0, ev)
+    return out
+
+
 def sample_csr(indptr, indices, ids, k, seed, counter, replace_if_short=True, pad_id=-1, counter_dev=None):
     require_cuda(indptr, indices, ids)
     if indptr.dtype != torch.int64:
@@ -611,17 +632,10 @@ def dropout_apply(x, site, rows=None, group=1, scale=1.0, out=None, accumulate=F
     return out
 
 
-def embedding_grad(lists, n_rows, d, out=None, sites=None):
-    """Dense gradient of the trainable embedding table (gs_embedding_grad; the densified IndexedSlices gradient of
-    tf.nn.embedding_lookup at reference graphsage/models.py:299): out[r] = sum of scale * grad[i // group] over every
-    (ids, grad, group, scale) list entry i with ids[i] == r.  grad: float32 CUDA [>= ceil(n / group), >= d] with unit
-    column stride (a strided view is fine).  Returns out, a contiguous float32 [n_rows, d]; deterministic.
-    sites: optional (seed, call, rate) per list (gs_embedding_grad_dropout): entry i of list l is masked with site l at
-    position i, (scale * grad) / keep where kept, 0 where dropped - the gradient through training dropout."""
+def _embed_lists(lists, d, who):
+    """(ids, grad, group, scale) tuples -> (gs_embed_grad_list array, the int32 id tensors kept alive, device)."""
     if len(lists) > _lib.MAX_EMBED_LISTS:
-        raise ValueError("embedding_grad takes at most %d lists" % _lib.MAX_EMBED_LISTS)
-    if sites is not None and len(sites) != len(lists):
-        raise ValueError("embedding_grad: one site per list")
+        raise ValueError("%s takes at most %d lists" % (who, _lib.MAX_EMBED_LISTS))
     arr = (_lib.EmbedGradList * max(len(lists), 1))()
     keep = []
     dev = None
@@ -638,6 +652,19 @@ def embedding_grad(lists, n_rows, d, out=None, sites=None):
         keep.append(ids)
         dev = grad.device
         arr[i] = _lib.EmbedGradList(ptr(ids), ptr(grad), max(grad.stride(0), d), n, group, float(scale))
+    return arr, keep, dev
+
+
+def embedding_grad(lists, n_rows, d, out=None, sites=None):
+    """Dense gradient of the trainable embedding table (gs_embedding_grad; the densified IndexedSlices gradient of
+    tf.nn.embedding_lookup at reference graphsage/models.py:299): out[r] = sum of scale * grad[i // group] over every
+    (ids, grad, group, scale) list entry i with ids[i] == r.  grad: float32 CUDA [>= ceil(n / group), >= d] with unit
+    column stride (a strided view is fine).  Returns out, a contiguous float32 [n_rows, d]; deterministic.
+    sites: optional (seed, call, rate) per list (gs_embedding_grad_dropout): entry i of list l is masked with site l at
+    position i, (scale * grad) / keep where kept, 0 where dropped - the gradient through training dropout."""
+    if sites is not None and len(sites) != len(lists):
+        raise ValueError("embedding_grad: one site per list")
+    arr, keep, dev = _embed_lists(lists, d, "embedding_grad")
     if out is None:
         out = torch.empty((n_rows, d), dtype=torch.float32, device=dev if dev is not None else "cuda")
     require_cuda(out)
@@ -657,6 +684,69 @@ def embedding_grad(lists, n_rows, d, out=None, sites=None):
         check(lib().gs_embedding_grad_dropout(arr, c_sites, len(lists), int(n_rows), int(d), ptr(out), max(out.stride(0), d),
                                               ptr(ws), nbytes, stream_ptr()))
     _launched(3 if nbytes > 0 and n_rows * d else 0, ev)           # keys, chunk sums, combine (+ CUB's sort passes)
+    return out
+
+
+def _fp32_table(t, name, min_cols):
+    require_cuda(t)
+    if t.dtype != torch.float32 or t.dim() != 2 or (t.stride(1) != 1 and t.shape[1] > 1) or t.shape[1] < min_cols:
+        raise ValueError("%s must be a float32 CUDA matrix with >= %d columns and unit column stride" % (name, min_cols))
+
+
+def embedding_sgd(table, lists, lr):
+    """Sparse gradient-descent update (gs_embedding_sgd; tf.train.GradientDescentOptimizer on the IndexedSlices gradient of
+    embedding_lookup, reference graphsage/models.py:476): table[r] += -lr * (sum of scale * grad[i // group] over every
+    (ids, grad, group, scale) entry i with ids[i] == r), in place, for the touched rows only; duplicate ids - also across
+    lists - are summed first, in the deterministic order of embedding_grad.  table: float32 CUDA [n_rows, d], unit column
+    stride (a strided view, e.g. the embedding columns of a wider table, is fine).  Returns table."""
+    _fp32_table(table, "table", 1)
+    n_rows, d = table.shape
+    arr, keep, _ = _embed_lists(lists, d, "embedding_sgd")
+    nbytes = lib().gs_embedding_grad_workspace_bytes(arr, len(lists), int(n_rows), int(d))
+    if nbytes < 0:
+        check(-1)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=table.device) if nbytes > 0 else None
+    ev = _probe("embedding_sgd/%d" % sum(k.numel() for k in keep))
+    check(lib().gs_embedding_sgd(arr, len(lists), int(n_rows), int(d), -float(lr), ptr(table), max(table.stride(0), d), ptr(ws),
+                                 nbytes, stream_ptr()))
+    _launched(3 if nbytes > 0 and n_rows * d else 0, ev)           # keys, chunk sums, combine (+ CUB's sort passes)
+    return table
+
+
+def skipgram_grad(target, context, batch1, batch2, neg):
+    """One skip-gram forward + backward of Node2VecModel (gs_skipgram_grad; reference graphsage/models.py:459-501).
+    target: float32 CUDA [V, d]; context: float32 CUDA [V, d + 1], its column d the context bias (unit column strides,
+    strided rows fine).  batch1 / batch2: the B pairs, neg: the S shared negatives (int32 ids).  Returns a dict of new
+    tensors: loss (0-d), aff [B] and neg_aff [B, S] (without the biases), gt [B, d] (gradient of target[batch1]),
+    gc_pos [B, d + 1] and gc_neg [S, d + 1] (gradients of the context rows, bias gradient in column d).  Deterministic."""
+    _fp32_table(target, "target", 1)
+    d = target.shape[1]
+    _fp32_table(context, "context", d + 1)
+    if context.shape[0] != target.shape[0]:
+        raise ValueError("target and context must have the same number of rows")
+    require_cuda(batch1, batch2, neg)
+    batch1, batch2, neg = _i32(batch1.reshape(-1), "batch1"), _i32(batch2.reshape(-1), "batch2"), _i32(neg.reshape(-1), "neg")
+    B, S = batch1.numel(), neg.numel()
+    if batch2.numel() != B or B < 1:
+        raise ValueError("batch1 and batch2 must hold the same number (>= 1) of ids")
+    if not 1 <= S <= _lib.MAX_UNIQUE_SAMPLED:
+        raise ValueError("the number of negatives must be in [1, %d] (got %d)" % (_lib.MAX_UNIQUE_SAMPLED, S))
+    dev = target.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    wd = pad_cols(d + 1)
+    out = dict(loss=torch.empty((), **f32), aff=torch.empty((B,), **f32), neg_aff=torch.empty((B, S), **f32),
+               gt=torch.empty((B, pad_cols(d)), **f32)[:, :d], gc_pos=torch.empty((B, wd), **f32)[:, :d + 1],
+               gc_neg=torch.empty((S, wd), **f32)[:, :d + 1])
+    nbytes = lib().gs_skipgram_workspace_bytes(B, S, d)
+    if nbytes < 0:
+        check(-1)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+    ev = _probe("skipgram_grad/%d" % B)
+    check(lib().gs_skipgram_grad(ptr(target), target.stride(0), ptr(context), context.stride(0), target.shape[0], d, ptr(batch1),
+                                 ptr(batch2), B, ptr(neg), S, ptr(out["loss"]), ptr(out["aff"]), ptr(out["neg_aff"]),
+                                 ptr(out["gt"]), out["gt"].stride(0), ptr(out["gc_pos"]), ptr(out["gc_neg"]), wd, ptr(ws), nbytes,
+                                 stream_ptr()))
+    _launched(2, ev)
     return out
 
 

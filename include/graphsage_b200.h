@@ -105,6 +105,19 @@ int32_t gs_sample_csr(const int64_t* indptr, const int32_t* indices, int64_t n_n
 int32_t gs_sample_unigram(const double* cdf, int64_t n, int32_t num_sampled, uint64_t seed, uint64_t counter,
                           const uint64_t* counter_dev, int32_t* out, void* stream);
 
+/* tf.nn.fixed_unigram_candidate_sampler(unique=True)   reference graphsage/models.py:450-457 (Node2VecModel)
+ *   num_sampled DISTINCT ids: the first num_sampled distinct ids of the draw sequence, in draw order - TF draws in sequence
+ *   and rejects ids it already holds.  Draw j (j = 0, 1, ...) maps to an id by the rule of gs_sample_unigram, with word j&3
+ *   of Philox4x32-10 block (counter + (counter_dev ? *counter_dev : 0), c2 = 0, GS unique-unigram stream tag + j>>2)
+ *   (oracle/node2vec.py:sample_unigram_unique).  The true classes do not change which ids are drawn.
+ *   Limits: num_sampled <= GS_MAX_UNIQUE_SAMPLED and <= n.  The caller must not ask for more ids than have positive weight
+ *   (the Python host refuses it); the kernel stops after GS_UNIQUE_DRAW_BUDGET draws in any case: positions it could not
+ *   fill are -1 and *status (device int32, may be NULL; never cleared by the kernel) is set to 1.  One warp, no host sync. */
+#define GS_MAX_UNIQUE_SAMPLED 1024
+#define GS_UNIQUE_DRAW_BUDGET (1 << 20)
+int32_t gs_sample_unigram_unique(const double* cdf, int64_t n, int32_t num_sampled, uint64_t seed, uint64_t counter,
+                                 const uint64_t* counter_dev, int32_t* out, int32_t* status, void* stream);
+
 /* Device-side construction of the padded adjacency table from CSR (the sampler's input contract, reference
  * graphsage/minibatch.py:227-259; SURVEY section 8f row 3).  adj is [n_nodes + 1, max_deg] int32:
  *   row n_nodes (dummy) and rows of skipped nodes (skip[u] != 0: val/test nodes, minibatch.py:232-233) or of
@@ -446,6 +459,42 @@ int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, i
 int32_t gs_embedding_grad_dropout(const gs_embed_grad_list* lists_host, const gs_dropout_site* sites_host, int32_t n_lists,
                                   int64_t n_rows, int32_t d, float* out, int64_t ldo, void* workspace,
                                   int64_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Node2Vec / DeepWalk baseline (reference graphsage/models.py:408-501, Node2VecModel).
+ *
+ * gs_embedding_sgd - the sparse GradientDescentOptimizer update of embedding tables (tf.train.GradientDescentOptimizer on the
+ *   IndexedSlices gradient of embedding_lookup: scatter_sub with duplicate ids summed):
+ *     table[r, 0:d] += alpha * (sum over list entries i with ids[i] == r of l.scale * l.grad[(i / l.group) * l.ldg + 0:d])
+ *   for every TOUCHED row r, in place (alpha = -learning rate).  Rows no id addresses are never read or written; ids outside
+ *   [0, n_rows) contribute nothing.  The row sum is formed in the summation order documented for gs_embedding_grad (same
+ *   sort, chunks and combine), then added once: table[r] = table[r] + alpha * sum, fp32.  Bit-identical on every call.
+ *   Lists, workspace (gs_embedding_grad_workspace_bytes) and limits as for gs_embedding_grad; ldt >= d.  Pass every list
+ *   that touches the table in ONE call so that an id appearing in several lists is summed before the update. */
+int32_t gs_embedding_sgd(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float alpha,
+                         float* table, int64_t ldt, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* gs_skipgram_grad - one skip-gram forward + backward over the two tables (Node2VecModel._loss / _accuracy,
+ * models.py:478-501), reading the tables only.  target row r = target[r * ldt + 0:d]; context row r = context[r * ldc + 0:d]
+ * with its bias in column d (context[r * ldc + d]; ldc >= d + 1).  With t_i = target[batch1[i]], c_i = context[batch2[i]],
+ * b_i its bias, n_j = context[neg[j]], nb_j its bias (i < B, j < S); ids outside [0, n_rows) read a zero row and bias:
+ *     aff[i]        = t_i . c_i                      (no bias: the MRR affinities, models.py:491)
+ *     neg_aff[i, j] = t_i . n_j                      ([B, S] row-major, no bias, models.py:493)
+ *     *loss         = (sum_i softplus(-(aff_i + b_i)) + sum_ij softplus(neg_aff_ij + nb_j)) / B     (models.py:479-486)
+ *   and the gradient of *loss, per lookup (duplicate ids are summed later, by gs_embedding_sgd):
+ *     g_i = (sigmoid(aff_i + b_i) - 1) / B,  h_ij = sigmoid(neg_aff_ij + nb_j) / B
+ *     gt[i, 0:d]     = g_i c_i + sum_j h_ij n_j      (j ascending)
+ *     gc_pos[i, 0:d] = g_i t_i,   gc_pos[i, d] = g_i                       (bias gradient in column d)
+ *     gc_neg[j, 0:d] = sum_i h_ij t_i,   gc_neg[j, d] = sum_i h_ij         (ldgc >= d + 1)
+ *   Dot products are per-lane strided partial sums (lane l owns columns l, l + 32, ...) combined by a fixed xor butterfly.
+ *   The batch reductions (loss, gc_neg) are per-CTA partial sums over the CTA's rows in ascending i, combined in CTA order
+ *   by a second kernel: no atomics, bit-identical on every call.  workspace: gs_skipgram_workspace_bytes(B, S, d).
+ *   Limits: 1 <= B < 2^31, 1 <= S <= GS_MAX_UNIQUE_SAMPLED, d >= 1, n_rows < 2^31. */
+int64_t gs_skipgram_workspace_bytes(int64_t B, int32_t S, int32_t d);
+int32_t gs_skipgram_grad(const float* target, int64_t ldt, const float* context, int64_t ldc, int64_t n_rows, int32_t d,
+                         const int32_t* batch1, const int32_t* batch2, int64_t B, const int32_t* neg, int32_t S, float* loss,
+                         float* aff, float* neg_aff, float* gt, int64_t ldgt, float* gc_pos, float* gc_neg, int64_t ldgc,
+                         void* workspace, int64_t workspace_bytes, void* stream);
 
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
