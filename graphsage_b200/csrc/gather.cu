@@ -18,14 +18,19 @@ struct SegTable {
   int64_t total_rows;
 };
 
+// segment of flattened row r: the last segment whose cumulative start is <= r.  The comparison is against the cumulative end
+// of segment q, which never decreases, so a later shorter (or empty) segment cannot claim a row an earlier one holds.
 __device__ __forceinline__ int find_segment(const SegTable& t, int64_t r, int64_t& local) {
   int si = 0;
-  int64_t base = 0;
+  int64_t base = 0, end = 0;
 #pragma unroll
   for (int q = 0; q < GS_MAX_SEGMENTS - 1; ++q) {
-    if (q < t.n_segments - 1 && r >= base + t.s[q].n) {
-      base += t.s[q].n;
-      si = q + 1;
+    if (q < t.n_segments - 1) {
+      end += t.s[q].n;
+      if (r >= end) {
+        base = end;
+        si = q + 1;
+      }
     }
   }
   local = r - base;

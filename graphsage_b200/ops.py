@@ -302,8 +302,8 @@ def _shard_prepare(src, segments):
         # reads local memory only.  All buffers are per call: under CUDA-graph capture they live in the graph's pool.
         lists, order = {}, []
         for s in segments:
-            if (s.self_ids is None) != (s.neigh_ids is None):
-                raise ValueError("a segment over a sharded table must address self and neighbours the same way")
+            if s.self_ids is None or s.neigh_ids is None:
+                raise ValueError("with halo staging every segment of a sharded gather must address its rows by ids")
             for t in (s.self_ids, s.neigh_ids):
                 key = (t.data_ptr(), t.numel())
                 if key not in lists:
@@ -336,16 +336,15 @@ def _shard_prepare(src, segments):
         done, segs = {}, []
 
         def tr(t):
-            if t is None:
-                return None
             key = (t.data_ptr(), t.numel())
             if key not in done:
                 done[key] = translate_ids(src, t)
             return done[key]
 
         for s in segments:
-            if (s.self_ids is None) != (s.neigh_ids is None):
-                raise ValueError("a segment over a replicated sharded table must address self and neighbours the same way")
+            # locators are row indices of this GPU's buffer: a row-range segment in the same call would be read as such
+            if s.self_ids is None or s.neigh_ids is None:
+                raise ValueError("with replicas every segment of a sharded gather must address its rows by ids")
             segs.append(Seg(s.n, s.k, tr(s.self_ids), tr(s.neigh_ids), s.self_row0, s.neigh_row0, s.out_row0))
         segments, locators = segs, 1
     return segments, locators, staging

@@ -155,6 +155,37 @@ def test_gather_mean_matches_numpy(gs, variant):
         gs._lib.set_tuning("gather_variant", 2)
 
 
+@pytest.mark.parametrize("form", ["tma2", "tma", "ldg", "scalar", "bf16"])
+def test_gather_mean_segments_of_any_size(gs, form):
+    """A call's segments may come in any size order, empty ones included: each output row must use its own segment's
+    fanout and ids (a row of a long segment followed by a shorter or empty one used to be placed in the later segment)."""
+    rs = np.random.RandomState(17)
+    n_src, F = 1000, 7 if form == "scalar" else 50
+    feats = rs.randn(n_src, F).astype(np.float32)
+    if form == "bf16":
+        feats = bf16_round(feats)
+    spec = [(40, 25), (0, 13), (9, 128), (17, 14)]
+    segs, ref, row = [], [], 0
+    for n, k in spec:
+        s = rs.randint(0, n_src, size=n).astype(np.int32)
+        nb = rs.randint(0, n_src, size=n * k).astype(np.int32)
+        segs.append(gs.ops.Seg(n, k, self_ids=dev(s), neigh_ids=dev(nb), out_row0=row))
+        ref.append(feats[nb].astype(np.float64).reshape(n, k, F).mean(1))
+        row += n
+    if form == "scalar":
+        src = dev(feats)                                      # pitch 7: no 16-byte rows -> scalar kernel
+    else:
+        table = torch.zeros((n_src, gs.ops.pad_cols(F)), dtype=torch.float32, device="cuda")
+        table[:, :F] = dev(feats)
+        src = (table.to(torch.bfloat16) if form == "bf16" else table)[:, :F]
+    gs._lib.set_tuning("gather_variant", {"tma2": 2, "tma": 1, "ldg": 0}.get(form, 2))
+    try:
+        _, xm = gs.ops.gather_mean(src, segs, want_self=False)
+    finally:
+        gs._lib.set_tuning("gather_variant", 2)
+    assert rel_err(xm[:, :F].cpu().numpy(), np.vstack(ref)) < 1e-6
+
+
 def test_gather_mean_odd_width_scalar_path(gs):
     rs = np.random.RandomState(2)
     x = rs.randn(500, 7).astype(np.float32)                  # pitch 7: no 16-B alignment -> scalar kernel

@@ -287,6 +287,39 @@ def test_sharded_table_single_rank_matches_dense():
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("stage_halo", [False, True])
+def test_sharded_table_emulated_shards_match_dense(stage_halo):
+    """The same checks with three shards emulated on one GPU (tests/shard_emu.py: one device allocation per shard, NaN
+    wherever nothing may read) and hot-row replicas: owner search, replica lookup and, with stage_halo, the halo passes.
+    tests/test_gpu_sharded_emulated.py covers the other layouts, widths and entry points."""
+    import graphsage_b200 as gs
+    from shard_emu import EmulatedShards
+    rs = np.random.RandomState(1)
+    n, f = 2000, 602
+    feats = rs.randn(n, f).astype(np.float32)
+    bounds = [0, 900, 901, n]                               # the middle shard owns a single row
+    full = torch.from_numpy(np.vstack([feats, np.zeros((1, f), np.float32)])).cuda()
+    ids = torch.from_numpy(np.concatenate([rs.randint(-3, n + 5, size=4000), bounds, np.subtract(bounds, 1)])
+                           .astype(np.int32)).cuda()
+    clamp = ids.clone().long()
+    clamp[(clamp < 0) | (clamp >= n)] = n
+    s0 = torch.from_numpy(rs.randint(0, n, size=40).astype(np.int32)).cuda()
+    s1 = torch.from_numpy(rs.randint(0, n + 1, size=400).astype(np.int32)).cuda()
+    seg = [gs.ops.Seg(40, 10, self_ids=s0, neigh_ids=s1)]
+    gs._lib.set_tuning("gather_variant", 0)
+    b = gs.ops.gather_mean(full, seg, include_self=True)
+    gs._lib.set_tuning("gather_variant", 2)
+    for rank in range(3):
+        lo, hi = bounds[rank], bounds[rank + 1]
+        hot = np.array([x for x in [0, 450, 899, 900, 901, 1500] + list(range(1700, 1760)) if not lo <= x < hi], np.int64)
+        shard = EmulatedShards(feats, bounds, rank, replica_ids=hot, stage_halo=stage_halo)
+        assert torch.equal(gs.ops.gather_rows(shard, ids), full[clamp])
+        a = gs.ops.gather_mean(shard, seg, include_self=True)
+        assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1])
+        shard.close()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("kind,concat,dim", [("mean", True, 128), ("gcn", False, 256)])
 def test_partitioned_forward_single_rank_vs_oracle(kind, concat, dim):
     """The node-partitioned path (ShardedFeatures + the sharded gather kernels) against the ORACLE, runnable on a
