@@ -48,7 +48,7 @@ class EmbedGradList(ctypes.Structure):
 
 
 class DropoutSite(ctypes.Structure):
-    _fields_ = [("seed", c_u64), ("call", ctypes.c_uint32), ("rate", ctypes.c_float)]
+    _fields_ = [("seed", c_u64), ("call", ctypes.c_uint32), ("rate", ctypes.c_float), ("call_dev", c_vp)]
 
 
 _SIGNATURES = {

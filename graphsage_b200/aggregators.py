@@ -245,9 +245,9 @@ class MaxPoolingAggregator(_SageAggregator):
             if src.stride(0) % 8 != 0 or src.data_ptr() % 16 != 0:
                 raise ValueError("bfloat16 source rows must be 16-byte aligned multiples (pitch % 8 == 0)")
             return src
-        if not persistent:
+        if not persistent or ops.REPACK_ALWAYS[0]:
             return ops.cast_rows_bf16(src)
-        key = (src.data_ptr(), src._version, tuple(src.shape))
+        key = (ops.CACHE_EPOCH[0], src.data_ptr(), src._version, tuple(src.shape))
         if getattr(self, "_bf16_ref", None) is not src or getattr(self, "_bf16_key", None) != key:
             self._bf16_src, self._bf16_ref, self._bf16_key = ops.cast_rows_bf16(src), src, key
         return self._bf16_src

@@ -79,9 +79,11 @@ __host__ __device__ inline uint32_t philox_draw(uint64_t seed, uint64_t counter,
 // philox4x32_10(ctr = (c / 4, pos_lo32, pos_hi32, call), key = split64(seed)) is >= T = floor(rate * 2^32) (float64).
 // A kept element becomes x / keep with keep = fp32(1 - rate) (IEEE division), a dropped one 0.  rate = 0 keeps every
 // element and divides by 1, so it is the identity.
+// call_dev (optional, device) is added to call by the kernel: see drop_call_offset.
 struct DropSite {
   uint32_t k0, k1, call, threshold;
   float keep;
+  const uint64_t* call_dev;
 };
 
 __host__ inline DropSite make_drop_site(const gs_dropout_site& s) {
@@ -91,7 +93,20 @@ __host__ inline DropSite make_drop_site(const gs_dropout_site& s) {
   d.call = s.call;
   d.threshold = (uint32_t)floor((double)s.rate * 4294967296.0);
   d.keep = (float)(1.0 - (double)s.rate);
+  d.call_dev = s.call_dev;
   return d;
+}
+
+#ifdef __CUDACC__
+// what the device word adds to a site's call number (0 without one); a kernel reads it once, not per element
+__device__ __forceinline__ uint32_t drop_call_offset(const DropSite& s) {
+  return s.call_dev ? (uint32_t)*s.call_dev : 0u;
+}
+#endif
+
+__host__ __device__ inline DropSite with_call_offset(DropSite s, uint32_t off) {
+  s.call += off;
+  return s;
 }
 
 // the four keep words of columns 4 * c4 .. 4 * c4 + 3 at position pos

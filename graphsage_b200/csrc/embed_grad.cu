@@ -64,6 +64,11 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
                                                           uint32_t n_rows, int32_t d, float* __restrict__ out,
                                                           int64_t ldo, float* __restrict__ partial, float alpha) {
   const unsigned FULL = 0xffffffffu;
+  __shared__ uint32_t call_off[GS_MAX_EMBED_LISTS];       // kDrop: each list's device-side call offset
+  if constexpr (kDrop) {
+    if (threadIdx.x < L.count) call_off[threadIdx.x] = drop_call_offset(L.l[threadIdx.x].site);
+    __syncthreads();
+  }
   const int lane = threadIdx.x & 31;
   const int64_t nchunks = (total + kChunk - 1) / kChunk;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -113,7 +118,7 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
           for (int q = 0; q < kColsPerLane; ++q) {
             const int col = c0 + lane + 32 * q;
             v[u][q] = (b + u < cnt && row != nullptr && col < d) ? sc * __ldg(row + col) : 0.f;
-            if constexpr (kDrop) v[u][q] = drop_col(L.l[li].site, pos, col, v[u][q]);
+            if constexpr (kDrop) v[u][q] = drop_col(with_call_offset(L.l[li].site, call_off[li]), pos, col, v[u][q]);
           }
         }
 #pragma unroll

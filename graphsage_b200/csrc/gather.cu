@@ -114,6 +114,14 @@ __global__ void __launch_bounds__(256) gather_mean_scalar_kernel(const float* __
                                                                  float* __restrict__ out_self,
                                                                  float* __restrict__ out_mean, int64_t out_pitch,
                                                                  const __grid_constant__ DropTab drop) {
+  __shared__ uint32_t drop_off[2 * GS_MAX_SEGMENTS];      // kDrop: the device-side call offsets, neighbour sites then self
+  if constexpr (kDrop) {
+    if (threadIdx.x < 2 * GS_MAX_SEGMENTS) {
+      const int s = threadIdx.x % GS_MAX_SEGMENTS;
+      drop_off[threadIdx.x] = drop_call_offset(threadIdx.x < GS_MAX_SEGMENTS ? drop.neigh[s] : drop.self[s]);
+    }
+    __syncthreads();
+  }
   for (int64_t r = blockIdx.x; r < tab.total_rows; r += gridDim.x) {
     int64_t i;
     const int si = find_segment(tab, r, i);
@@ -121,16 +129,21 @@ __global__ void __launch_bounds__(256) gather_mean_scalar_kernel(const float* __
     const int k = sg.k;
     const int64_t orow = sg.out_row0 + i;
     const int64_t srow = clamp_row(sg.self_ids ? (int64_t)sg.self_ids[i] : sg.self_row0 + i, n_src_rows);
+    DropSite nsite{}, ssite{};
+    if constexpr (kDrop) {
+      nsite = with_call_offset(drop.neigh[si], drop_off[si]);
+      ssite = with_call_offset(drop.self[si], drop_off[GS_MAX_SEGMENTS + si]);
+    }
     for (int c = threadIdx.x; c < (int)out_pitch; c += blockDim.x) {
       float acc = 0.f, sv = 0.f;
       if (c < F) {
         for (int j = 0; j < k; ++j) {
           int64_t nr = clamp_row(sg.neigh_ids ? (int64_t)sg.neigh_ids[i * k + j] : sg.neigh_row0 + i * k + j, n_src_rows);
-          if constexpr (kDrop) acc += drop_col(drop.neigh[si], i * k + j, c, src[nr * pitch + c]);
+          if constexpr (kDrop) acc += drop_col(nsite, i * k + j, c, src[nr * pitch + c]);
           else acc += src[nr * pitch + c];
         }
         sv = src[srow * pitch + c];
-        if constexpr (kDrop) sv = drop_col(drop.self[si], i, c, sv);
+        if constexpr (kDrop) sv = drop_col(ssite, i, c, sv);
         if (include_self) acc += sv;
         acc /= (float)(k + (include_self ? 1 : 0));
       }
@@ -302,10 +315,17 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
                                                                const __grid_constant__ DropTab drop) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t bar[2];
+  __shared__ uint32_t drop_off[2 * GS_MAX_SEGMENTS];      // kDrop: the device-side call offsets, neighbour sites then self
   if (threadIdx.x == 0) {
     mbar_init(&bar[0], 1);
     mbar_init(&bar[1], 1);
     fence_mbar_init();
+  }
+  if constexpr (kDrop) {
+    if (threadIdx.x < 2 * GS_MAX_SEGMENTS) {
+      const int s = threadIdx.x % GS_MAX_SEGMENTS;
+      drop_off[threadIdx.x] = drop_call_offset(threadIdx.x < GS_MAX_SEGMENTS ? drop.neigh[s] : drop.self[s]);
+    }
   }
   __syncthreads();
   const int ncol4 = (int)(out_pitch >> 2);
@@ -359,6 +379,8 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
     phase[buf] ^= 1u;
     const float4* rows = reinterpret_cast<const float4*>(smem + buf * buf_bytes);
     const int nn = last ? cnt - 1 : cnt;                  // neighbour rows in this group (the self row is the node's last row)
+    DropSite nsite{};
+    if constexpr (kDrop) nsite = with_call_offset(drop.neigh[si], drop_off[si]);
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       const int c = threadIdx.x + q * blockDim.x;
@@ -366,7 +388,7 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
         float4 a = acc[q];
         for (int j = 0; j < nn; ++j) {
           float4 v = rows[j * row_f4 + c];
-          if constexpr (kDrop) v = drop4(drop.neigh[si], i * k + first + j, (uint32_t)c, v);
+          if constexpr (kDrop) v = drop4(nsite, i * k + first + j, (uint32_t)c, v);
           a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
         }
         acc[q] = a;
@@ -383,7 +405,7 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
           if (c < ncol4 && c * 4 < F) {
             a = acc[q];
             sv = rows[(cnt - 1) * row_f4 + c];
-            if constexpr (kDrop) sv = drop4(drop.self[si], i, (uint32_t)c, sv);
+            if constexpr (kDrop) sv = drop4(with_call_offset(drop.self[si], drop_off[GS_MAX_SEGMENTS + si]), i, (uint32_t)c, sv);
             const float div = (float)(k + (include_self ? 1 : 0));
             if (include_self) { a.x += sv.x; a.y += sv.y; a.z += sv.z; a.w += sv.w; }
             a.x /= div; a.y /= div; a.z /= div; a.w /= div;
@@ -680,6 +702,7 @@ __global__ void __launch_bounds__(256) dropout_apply_kernel(const float* x, int6
                                                             int64_t ldo) {
   const int nc4 = (F + 3) >> 2;
   const int64_t total = rows * nc4;
+  site.call += drop_call_offset(site);
   for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = q / nc4;
     const int c4 = (int)(q - r * nc4);

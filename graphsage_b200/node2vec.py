@@ -18,6 +18,7 @@ import torch
 
 from . import ops
 from ._lib import MAX_UNIQUE_SAMPLED
+from .graphed_training import GraphedTrainStep
 from .prediction import mrr_from_affinities
 
 
@@ -121,6 +122,11 @@ class Node2VecModel(object):
         ops.embedding_sgd(self._context[:, :self.hidden_dim + 1], [(b2, out["gc_pos"], 1, 1.0), (neg, out["gc_neg"], 1, 1.0)],
                           self.lr)
         return out["loss"]
+
+    def graphed_train_step(self, batch_size):
+        """train_step for a fixed batch size captured in one CUDA graph: returns step(batch1, batch2) -> loss, a static 0-d
+        CUDA tensor (see graphed_training.GraphedTrainStep; a short last batch runs through the eager train_step)."""
+        return GraphedTrainStep(self, batch_size)
 
     def mrr(self):
         """models.py:489-501 on the bias-free affinities of the last loss() / train_step() call."""

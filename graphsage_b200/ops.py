@@ -13,6 +13,12 @@ PROBE = None
 LAUNCHES = 0          # kernels of ours launched through this module (bench.py reports it as gpu_launches)
 STAGE_HOOK = None     # callable(name, "pre"|"post") around probe-able launches (models.GraphedForward splits graphs here)
 
+# The host-keyed caches (PackedWeights, PackedMlpWeights, the max-pool bf16 cast) re-pack when data_ptr() / _version say a
+# tensor changed.  A replay of a captured training step (graphed_training) updates the weights without the host seeing it,
+# and a capture would freeze the decision, so:
+CACHE_EPOCH = [0]         # part of every cache key; advanced after each training replay
+REPACK_ALWAYS = [False]   # set while a training step is captured: every call packs / casts afresh, inside the graph
+
 
 def _probe(name):
     if STAGE_HOOK is not None:
@@ -459,17 +465,24 @@ class PackedWeights(object):
         self.key, self.ws = None, None
 
     def get(self, parts, arr, math, dev):
-        key = (math,) + tuple((p[2].data_ptr(), p[2]._version, tuple(p[2].shape)) for p in parts)
+        if REPACK_ALWAYS[0]:                     # captured: the pack is part of the graph, into a buffer of its pool
+            return self._pack(parts, arr, math, dev, None)
+        key = (CACHE_EPOCH[0], math) + tuple((p[2].data_ptr(), p[2]._version, tuple(p[2].shape)) for p in parts)
         if key != self.key:
-            nbytes = lib().gs_sage_gemm_workspace_bytes(1, arr, len(parts), math)
-            if nbytes < 0:
-                check(-1)
-            if self.ws is None or self.ws.numel() < nbytes:
-                self.ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev)
-            check(lib().gs_sage_gemm_pack(arr, len(parts), math, ptr(self.ws), stream_ptr()))
-            _launched(1)
+            self.ws = self._pack(parts, arr, math, dev, self.ws)
             self.key = key
         return self.ws
+
+    @staticmethod
+    def _pack(parts, arr, math, dev, ws):
+        nbytes = lib().gs_sage_gemm_workspace_bytes(1, arr, len(parts), math)
+        if nbytes < 0:
+            check(-1)
+        if ws is None or ws.numel() < nbytes:
+            ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev)
+        check(lib().gs_sage_gemm_pack(arr, len(parts), math, ptr(ws), stream_ptr()))
+        _launched(1)
+        return ws
 
 
 def sage_gemm(parts, combine=COMBINE_ADD, bias=None, act=ACT_NONE, math=MATH_FP32_SIMT, out=None, packed=None):
@@ -528,16 +541,23 @@ class PackedMlpWeights(object):
         self.key, self.ws = None, None
 
     def get(self, W):
-        key = (W.data_ptr(), W._version, tuple(W.shape))
+        if REPACK_ALWAYS[0]:
+            return self._pack(W)
+        key = (CACHE_EPOCH[0], W.data_ptr(), W._version, tuple(W.shape))
         if key != self.key:
-            K, hidden = W.shape
-            nbytes = lib().gs_maxpool_mlp_workspace_bytes(K, hidden)
-            self.ws = torch.empty((nbytes,), dtype=torch.uint8, device=W.device)
-            Wc = W.contiguous()
-            check(lib().gs_maxpool_mlp_pack(ptr(Wc), Wc.stride(0), K, hidden, ptr(self.ws), stream_ptr()))
-            _launched(1)
+            self.ws = self._pack(W)
             self.key = key
         return self.ws
+
+    @staticmethod
+    def _pack(W):
+        K, hidden = W.shape
+        nbytes = lib().gs_maxpool_mlp_workspace_bytes(K, hidden)
+        ws = torch.empty((nbytes,), dtype=torch.uint8, device=W.device)
+        Wc = W.contiguous()
+        check(lib().gs_maxpool_mlp_pack(ptr(Wc), Wc.stride(0), K, hidden, ptr(ws), stream_ptr()))
+        _launched(1)
+        return ws
 
 
 def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0, K=None, out=None, pool="max"):
@@ -562,13 +582,19 @@ def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0,
 
 
 def dropout_site(site):
-    """(seed, call, rate) -> the C descriptor; rate must lie in [0, 1) (the mask contract is in the header and
-    oracle/dropout.py)."""
-    seed, call, rate = site
+    """(seed, call, rate) or (seed, call, rate, call_dev) -> the C descriptor; rate must lie in [0, 1) (the mask contract
+    is in the header and oracle/dropout.py).  call_dev: None, or an int64 CUDA tensor whose first element the kernel adds to
+    `call` when it runs (a CUDA graph replays with whatever it holds then)."""
+    seed, call, rate = site[:3]
+    call_dev = site[3] if len(site) > 3 else None
     rate = float(rate)
     if not 0.0 <= rate < 1.0:
         raise ValueError("dropout rate must be in [0, 1) (got %r)" % (rate,))
-    return _lib.DropoutSite(int(seed) & _U64, int(call) & 0xFFFFFFFF, rate)
+    if call_dev is not None:
+        require_cuda(call_dev)
+        if call_dev.dtype != torch.int64 or call_dev.numel() < 1:
+            raise TypeError("call_dev must be an int64 CUDA tensor with >= 1 element")
+    return _lib.DropoutSite(int(seed) & _U64, int(call) & 0xFFFFFFFF, rate, ptr(call_dev))
 
 
 def gather_mean_dropout(src, segments, neigh_sites, self_sites, include_self=False, want_self=True, out_pitch=None):

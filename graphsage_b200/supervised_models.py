@@ -18,6 +18,7 @@ regenerates the same masks instead of storing them.  A pass numbers its sites in
 import torch
 
 from . import ops
+from .graphed_training import GraphedTrainStep
 from .layers import act_code, identity, relu  # noqa: F401
 from .models import SampleAndAggregate
 
@@ -263,7 +264,8 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     """sample -> aggregate (-> l2_normalize) with an autograd graph over the aggregator weights; `model` is a
     SampleAndAggregate whose .aggregators exist (reference models.py:347-350 / supervised_models.py:79-85).
     dropout = p > 0: training dropout, sites numbered by dropout_site_plan from model.dropout_counter, which advances
-    past them (p = 0 draws nothing and leaves the counter alone)."""
+    past them (p = 0 draws nothing and leaves the counter alone); model.dropout_call_dev, when set, is the device-side
+    offset every site adds to its call number (graphed_training)."""
     dropout = check_dropout_rate(dropout)
     if dropout:
         refuse_dropout_table(model.features)
@@ -296,11 +298,11 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
         emb = getattr(model, "embeds", None) if layer == 0 else None
         sites = None
         if dropout:                                          # per hop: the MLP-input site, or the (neighbour, self) pair
-            key = model.dropout_key
+            key, dev = model.dropout_key, model.dropout_call_dev
             if pool:
-                sites = [(key, call[(layer, h, "mlp")], dropout) for h in range(hops)]
+                sites = [(key, call[(layer, h, "mlp")], dropout, dev) for h in range(hops)]
             else:
-                sites = [((key, call[(layer, h, "neigh")], dropout), (key, call[(layer, h, "self")], dropout))
+                sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
                          for h in range(hops)]
         if pool:                                             # max-pool / mean-pool
             mlp = agg.mlp_layers[0].vars
@@ -343,6 +345,7 @@ def init_dropout(model, dropout_seed, distributed, group):
         import torch.distributed as dist
         key += dist.get_rank(group)
     model.dropout_rate, model.dropout_key, model.dropout_counter = rate, key, 0
+    model.dropout_call_dev = None       # device offset of every call number, set while a training step is captured
 
 
 def build_aggregators(model):
@@ -450,7 +453,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         site, after the aggregators')."""
         out = self.outputs(batch, dropout=dropout)
         if check_dropout_rate(dropout):
-            out = _DropoutFn.apply(out, (self.dropout_key, self.dropout_counter, dropout))
+            out = _DropoutFn.apply(out, (self.dropout_key, self.dropout_counter, dropout, self.dropout_call_dev))
             self.dropout_counter += 1
         return out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
 
@@ -477,6 +480,11 @@ class SupervisedGraphsage(SampleAndAggregate):
                 p.grad.clamp_(-5.0, 5.0)
         self.optimizer.step()
         return loss.detach()
+
+    def graphed_train_step(self, batch_size):
+        """train_step for a fixed batch size captured in one CUDA graph: returns step(batch, labels) -> loss, a static 0-d
+        CUDA tensor (see graphed_training.GraphedTrainStep; a short last batch runs through the eager train_step)."""
+        return GraphedTrainStep(self, batch_size)
 
     def predict(self, batch):
         with torch.no_grad():

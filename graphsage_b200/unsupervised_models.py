@@ -10,6 +10,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .graphed_training import GraphedTrainStep
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
 from .supervised_models import (aggregator_parameters, build_aggregators, differentiable_outputs, embedding_parameters,
@@ -106,3 +107,8 @@ class UnsupervisedGraphsage(SampleAndAggregate):
                 p.grad.clamp_(-5.0, 5.0)                                             # models.py:380-381
         self.optimizer.step()
         return loss.detach()
+
+    def graphed_train_step(self, batch_size):
+        """train_step for a fixed batch size captured in one CUDA graph: returns step(batch1, batch2) -> loss, a static 0-d
+        CUDA tensor (see graphed_training.GraphedTrainStep; a short last batch runs through the eager train_step)."""
+        return GraphedTrainStep(self, batch_size)

@@ -427,11 +427,16 @@ int32_t gs_embedding_grad(const gs_embed_grad_list* lists_host, int32_t n_lists,
  *   a kept element becomes x / keep, keep = fp32(1 - rate) (IEEE division), a dropped element 0.  0 <= rate < 1.
  * Columns are logical (0 .. F-1, independent of any pitch).  Positions: neighbour j of output row i of a segment:
  * pos = i * k + j (the row-major [n, k, F] flattening); self row of i: pos = i; any other [rows, F] tensor: pos = row.
+ * The call number a kernel uses is (uint32_t)(call + (call_dev ? *call_dev : 0)), read on the stream when the kernel runs -
+ * the convention of the samplers' counter_dev.  A CUDA graph bakes `call` into its launches; with call_dev pointing at a
+ * device word that is set (or advanced with gs_bump_counter) before each replay, every replay draws fresh masks.  With
+ * call_dev == NULL the site is exactly the host-numbered site.
  * --------------------------------------------------------------------------------------------- */
 typedef struct {
   uint64_t seed;
   uint32_t call;
   float rate;
+  const uint64_t* call_dev;   /* device, optional: added to call */
 } gs_dropout_site;
 
 /* gs_gather_mean (GS_F32 tables only) with dropout applied to the gathered rows in registers:
