@@ -105,6 +105,15 @@ _SIGNATURES = {
                                      c_vp]),
     "gs_meanpool_mlp_fused": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,
                                       c_vp]),
+    "gs_pool_mlp_dp_bytes": (c_i64, [c_i64, c_i32, c_i32]),
+    "gs_pool_mlp_backward_dp": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,
+                                        c_i32, c_vp, c_vp]),
+    "gs_pool_mlp_dw_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32, c_i32]),
+    "gs_pool_mlp_backward_dw": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp,
+                                        c_i64, c_vp, c_vp]),
+    "gs_pool_mlp_dx_pack_bytes": (c_i64, [c_i32, c_i32]),
+    "gs_pool_mlp_dx_pack": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
+    "gs_pool_mlp_backward_dx": (c_i32, [c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp]),
     "gs_pipeline_step": (c_i32, [c_vp, c_vp, c_i64, ctypes.POINTER(c_vp), c_i32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
                                  c_vp, c_vp]),
     "gs_l2_normalize_rows": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp]),

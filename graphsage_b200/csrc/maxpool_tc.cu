@@ -49,6 +49,11 @@ struct MpParams {
   int32_t pool_mean;            // 0: max over the fanout (MaxPoolingAggregator), 1: mean (MeanPoolingAggregator)
   float* out;                   // [n_groups, hidden]
   int64_t ldo;
+  // B1 (kGrad, gs_pool_mlp_backward_dp) only
+  const float* dhp;             // [n_groups, hidden] (row stride lddhp): gradient of the pooled output
+  int64_t lddhp;
+  unsigned char* dp;            // dP^T tile images: [n_tiles][n_slices][2 row halves][128 hidden x 64 rows, bf16, SW128]
+  float* dbm_part;              // [n_tiles][hidden]: per-tile column sums of dpre
 };
 
 // Wm [K, hidden] row-major fp32 -> bf16 tile images of Wm^T (128 hidden rows x 64 k, K-major, SW128)
@@ -70,7 +75,9 @@ __global__ void __launch_bounds__(256) maxpool_pack_kernel(const float* __restri
   }
 }
 
-template <bool kRowsA, int NT, int DEPTH, int PROD>
+// kGrad (B1 of the pooling branch's backward, only <true, 128, 1, 0>): the same main loop recomputes the tile's
+// pre-activations, and the epilogue turns them into dpre instead of the pooled output (see gs_pool_mlp_backward_dp)
+template <bool kRowsA, int NT, int DEPTH, int PROD, bool kGrad = false>
 __global__ void __launch_bounds__(MP_THREADS, NT == 128 ? 2 : 1) maxpool_mlp_kernel(const __grid_constant__ MpParams prm) {
   constexpr int ROWS_IMG = NT * 128;                      // gathered rows of one K-block
   constexpr int STAGE = ROWS_IMG + MP_IMG;                // rows image, then the weight image
@@ -219,36 +226,96 @@ __global__ void __launch_bounds__(MP_THREADS, NT == 128 ? 2 : 1) maxpool_mlp_ker
           stage[col * LD + row] = acc[mi * NI + ni][4 * j + e];
         }
   __syncthreads();
-  // thread = (column cc, group): consecutive threads take consecutive columns (conflict-free staging reads,
-  // coalesced stores)
   const int k = prm.k, G = prm.G;
-  for (int u = tid; u < TC_BN * G; u += MP_THREADS) {
-    const int cc = u & (TC_BN - 1), g = u / TC_BN;
-    const int64_t gg = t * G + g;
-    if (gg >= prm.n_groups) break;
-    const float* p = stage + cc * LD + g * k;
-    const int hcol = slice * 128 + cc;
+  if constexpr (kGrad) {
+    static_assert(kRowsA && NT == 128, "B1 reads the <rows as A, 128-row tile> staging layout");
+    // thread = (column cc, group parity): dpre of each of its groups overwrites that group's staging entries;
+    // the per-group sums (j order) are summed in g order per parity, then the two parities are added
+    const int cc = tid & (TC_BN - 1), hcol = slice * 128 + cc;
     const float b = prm.bias ? prm.bias[hcol] : 0.f;
-    float res;
-    if (prm.pool_mean) {
-      // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU
-      // are applied per element, summed in j order, divided by k
-      float sacc = 0.f;
-      for (int j = 0; j < k; ++j) sacc += fmaxf(p[j] + b, 0.f);
-      res = sacc / (float)k;
-    } else {
-      float m = -3.0e38f;
-      int j = 0;
-      for (; j + 8 <= k; j += 8) {
-        float v[8];
-#pragma unroll
-        for (int w = 0; w < 8; ++w) v[w] = p[j + w];
-        m = fmaxf(m, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
+    float part = 0.f;
+    for (int g = tid >> 7; g < G; g += 2) {
+      const int64_t gg = t * G + g;
+      if (gg >= prm.n_groups) break;
+      float* p = stage + cc * LD + g * k;
+      const float d = prm.dhp[gg * prm.lddhp + hcol];
+      float s = 0.f;
+      if (prm.pool_mean) {                          // dpre_j = (dhp / k) * [fl(pre_j + b) > 0]
+        const float q = d / (float)k;
+        for (int j = 0; j < k; ++j) {
+          const float v = (p[j] + b > 0.f) ? q : 0.f;
+          p[j] = v;
+          s += v;
+        }
+      } else {                                      // ties at hp > 0 share dhp evenly; hp == 0: ReLU blocks everything
+        float m = -3.0e38f;
+        for (int j = 0; j < k; ++j) m = fmaxf(m, p[j]);
+        const float hp = fmaxf(m + b, 0.f);
+        int cnt = 0;
+        if (hp > 0.f)
+          for (int j = 0; j < k; ++j) cnt += (p[j] + b == hp) ? 1 : 0;
+        const float q = cnt ? d / (float)cnt : 0.f;
+        for (int j = 0; j < k; ++j) {
+          const float v = (cnt && p[j] + b == hp) ? q : 0.f;
+          p[j] = v;
+          s += v;
+        }
       }
-      for (; j < k; ++j) m = fmaxf(m, p[j]);
-      res = fmaxf(m + b, 0.f);                      // Dense bias + ReLU (commute with the max)
+      part += s;
     }
-    prm.out[gg * prm.ldo + hcol] = res;
+    float* red = stage + TC_BN * LD;                // [2][128] behind the staging tile, inside the operand ring
+    red[(tid >> 7) * TC_BN + cc] = part;
+    __syncthreads();
+    if (tid < TC_BN) prm.dbm_part[t * (int64_t)prm.n_slices * 128 + hcol] = red[cc] + red[TC_BN + cc];
+    // dP^T images of this (tile, slice): half h holds rows 64h .. 64h + 63; 16-byte piece = 8 rows of one hidden unit.
+    // Padding rows and rows past the last group are zero.
+    const int nvalid = (int)min((int64_t)G * k, prm.n_groups * k - t * (int64_t)G * k);
+    unsigned char* img = prm.dp + (t * prm.n_slices + slice) * (int64_t)(2 * MP_IMG);
+#pragma unroll
+    for (int i = 0; i < (2 * 128 * 8) / MP_THREADS; ++i) {
+      const int q = tid + MP_THREADS * i;
+      const int h = q >> 10, n = (q >> 3) & 127, c = q & 7;
+      const int r0 = h * 64 + c * 8;
+      __nv_bfloat162 v[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float a0 = (r0 + 2 * e < nvalid) ? stage[n * LD + r0 + 2 * e] : 0.f;
+        const float a1 = (r0 + 2 * e + 1 < nvalid) ? stage[n * LD + r0 + 2 * e + 1] : 0.f;
+        v[e] = __floats2bfloat162_rn(a0, a1);
+      }
+      *reinterpret_cast<uint4*>(img + h * MP_IMG + sw128_off(n, c)) = *reinterpret_cast<uint4*>(v);
+    }
+  } else {
+    // thread = (column cc, group): consecutive threads take consecutive columns (conflict-free staging reads,
+    // coalesced stores)
+    for (int u = tid; u < TC_BN * G; u += MP_THREADS) {
+      const int cc = u & (TC_BN - 1), g = u / TC_BN;
+      const int64_t gg = t * G + g;
+      if (gg >= prm.n_groups) break;
+      const float* p = stage + cc * LD + g * k;
+      const int hcol = slice * 128 + cc;
+      const float b = prm.bias ? prm.bias[hcol] : 0.f;
+      float res;
+      if (prm.pool_mean) {
+        // mean-pool (reference aggregators.py:246-273): ReLU does not commute with the mean, so bias + ReLU
+        // are applied per element, summed in j order, divided by k
+        float sacc = 0.f;
+        for (int j = 0; j < k; ++j) sacc += fmaxf(p[j] + b, 0.f);
+        res = sacc / (float)k;
+      } else {
+        float m = -3.0e38f;
+        int j = 0;
+        for (; j + 8 <= k; j += 8) {
+          float v[8];
+#pragma unroll
+          for (int w = 0; w < 8; ++w) v[w] = p[j + w];
+          m = fmaxf(m, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
+        }
+        for (; j < k; ++j) m = fmaxf(m, p[j]);
+        res = fmaxf(m + b, 0.f);                      // Dense bias + ReLU (commute with the max)
+      }
+      prm.out[gg * prm.ldo + hcol] = res;
+    }
   }
 }
 
@@ -359,6 +426,51 @@ int32_t gs_meanpool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
                               int32_t hidden, float* out, int64_t ldo, void* stream) {
   return pool_mlp_fused(table_bf16, n_rows, K, pitch, row_ids, row0, n_groups, k, packed_weights, bias, hidden, out, ldo, 1,
                         stream);
+}
+
+// B1's output buffer: the dP^T tile images (n_tiles * hidden * 256 bytes), then the fp32 dbm partials [n_tiles][hidden]
+int64_t gs_pool_mlp_dp_bytes(int64_t n_groups, int32_t k, int32_t hidden) {
+  if (n_groups < 0 || k < 1 || k > 128 || hidden < 128 || hidden % 128 != 0) return -1;
+  const int64_t G = 128 / k, n_tiles = (n_groups + G - 1) / G;
+  return n_tiles * hidden * (256 + 4);
+}
+
+int32_t gs_pool_mlp_backward_dp(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch, const int32_t* row_ids,
+                                int64_t row0, int64_t n_groups, int32_t k, const void* packed_weights, const float* bias,
+                                int32_t hidden, const float* dhp, int64_t lddhp, int32_t pool_mean, void* dp, void* stream) {
+  GS_REQUIRE(n_groups >= 0 && k >= 1, "gs_pool_mlp_backward_dp: bad n_groups / k");
+  if (n_groups == 0) return GS_OK;
+  GS_REQUIRE(table_bf16 && packed_weights && dhp && dp, "gs_pool_mlp_backward_dp: NULL pointer");
+  GS_REQUIRE(n_rows > 0 && n_rows < 0x7fffffffLL && K >= 1 && pitch >= K, "gs_pool_mlp_backward_dp: bad table shape");
+  GS_REQUIRE((pitch * 2) % 16 == 0 && (reinterpret_cast<uintptr_t>(table_bf16) & 15u) == 0,
+             "gs_pool_mlp_backward_dp: table rows must be 16-byte multiples and 16-byte aligned (pitch %% 8 == 0)");
+  GS_REQUIRE((reinterpret_cast<uintptr_t>(packed_weights) & 127u) == 0 && (reinterpret_cast<uintptr_t>(dp) & 15u) == 0,
+             "gs_pool_mlp_backward_dp: packed weights / dp misaligned");
+  if (k > 128 || (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS > gs::MP_MAX_KB || hidden % 128 != 0 || hidden < 128) {
+    gs::set_error("gs_pool_mlp_backward_dp: needs k <= 128, K <= %d, hidden %% 128 == 0 (k=%d K=%d hidden=%d)",
+                  gs::MP_MAX_KB * gs::MP_KCOLS, k, K, hidden);
+    return GS_ERR_UNSUPPORTED;
+  }
+  GS_REQUIRE(lddhp >= hidden, "gs_pool_mlp_backward_dp: lddhp < hidden");
+  gs::MpParams prm;
+  memset(&prm, 0, sizeof(prm));
+  prm.table = (const __nv_bfloat16*)table_bf16;
+  prm.n_rows = n_rows; prm.pitch = pitch; prm.K = K; prm.kblocks = (K + gs::MP_KCOLS - 1) / gs::MP_KCOLS;
+  prm.row_ids = row_ids; prm.row0 = row0; prm.n_groups = n_groups; prm.k = k; prm.G = 128 / k;
+  prm.n_slices = hidden / 128;
+  prm.wimg = (const unsigned char*)packed_weights; prm.bias = bias; prm.pool_mean = pool_mean;
+  prm.dhp = dhp; prm.lddhp = lddhp;
+  const int64_t n_tiles = (n_groups + prm.G - 1) / prm.G;
+  prm.dp = (unsigned char*)dp;
+  prm.dbm_part = reinterpret_cast<float*>((unsigned char*)dp + n_tiles * hidden * 256);
+  GS_REQUIRE(n_tiles * prm.n_slices < 0x7fffffffLL, "gs_pool_mlp_backward_dp: too many groups (%lld)", (long long)n_groups);
+  const void* fn = (const void*)gs::maxpool_mlp_kernel<true, 128, 1, 0, true>;
+  const int smem = gs::MP_STAGES * (128 * 128 + gs::MP_IMG) + 1024;
+  const int32_t rc_attr = gs::ensure_dyn_smem(fn, smem);
+  if (rc_attr != GS_OK) return rc_attr;
+  gs::maxpool_mlp_kernel<true, 128, 1, 0, true>
+      <<<(unsigned)(n_tiles * prm.n_slices), gs::MP_THREADS, smem, (cudaStream_t)stream>>>(prm);
+  return gs::launch_check("maxpool_mlp_kernel<grad>");
 }
 
 }  // extern "C"

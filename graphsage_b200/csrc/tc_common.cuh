@@ -55,14 +55,18 @@ __device__ __forceinline__ void acc_fence(float (&d)[64]) {
 // D[64 x 128] (+)= A[64 x K] * B[128 x K]^T, both operands K-major in shared memory, fp32 accumulate in registers.
 // kBf16: one K = 16 step of bf16 operands; else one K = 8 step of tf32 operands.  accumulate = 0 overwrites D.
 // Thread t of the warpgroup holds d[4j + e] = D[16 (t / 32) + (t % 32) / 4 + 8 (e / 2)][8 j + 2 (t % 4) + (e % 2)].
-template <bool kBf16>
+// kTransA (bf16 only): A is MN-major instead - the 64 M values of one K index are one 128-byte row of the SW128 image
+// (K-rows at 128 B, 8-row groups at the descriptor's 1024-byte stride), i.e. the same bytes as a K-major 64-column
+// image read the other way round; the descriptor is unchanged (one 64-wide atom along M, so its leading offset is unused).
+template <bool kBf16, int kTransA = 0>
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  static_assert(kBf16 || kTransA == 0, "transposed operands are bf16 only");
   if constexpr (kBf16) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " GS_WGMMA_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " GS_WGMMA_D64 ", %64, %65, p, 1, 1, %67, 0;\n\t}"
         : GS_WGMMA_OUT64(d)
-        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransA)
         : "memory");
   } else {
     asm volatile(

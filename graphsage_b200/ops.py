@@ -581,6 +581,101 @@ def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0,
     return out
 
 
+class PackedMlpDxWeights(PackedMlpWeights):
+    """bf16 images of Wm[:cols] (K-major over hidden) for pool_mlp_backward_dx, re-packed when the weight changes."""
+
+    def __init__(self, cols):
+        PackedMlpWeights.__init__(self)
+        self.cols = int(cols)
+
+    def get(self, W):
+        if REPACK_ALWAYS[0]:
+            return self._pack_dx(W, self.cols)
+        key = (CACHE_EPOCH[0], W.data_ptr(), W._version, tuple(W.shape), self.cols)
+        if key != self.key:
+            self.ws = self._pack_dx(W, self.cols)
+            self.key = key
+        return self.ws
+
+    @staticmethod
+    def _pack_dx(W, cols):
+        if not 1 <= cols <= W.shape[0]:
+            raise ValueError("pool_mlp_backward_dx: cols must be in [1, %d] (the rows of Wm), got %d" % (W.shape[0], cols))
+        nbytes = lib().gs_pool_mlp_dx_pack_bytes(cols, W.shape[1])
+        if nbytes < 0:
+            raise ValueError("pool_mlp_backward_dx: needs 1 <= cols and hidden % 128 == 0 (cols=%d hidden=%d)"
+                             % (cols, W.shape[1]))
+        ws = torch.empty((nbytes,), dtype=torch.uint8, device=W.device)
+        Wc = W.contiguous()
+        check(lib().gs_pool_mlp_dx_pack(ptr(Wc), Wc.stride(0), cols, Wc.shape[1], ptr(ws), stream_ptr()))
+        _launched(1)
+        return ws
+
+
+def pool_mlp_backward_dp(table, n_groups, k, W, bias, packed, dhp, row_ids=None, row0=0, K=None, pool="max"):
+    """B1 of the pooling branch's backward (gs_pool_mlp_backward_dp): recomputes pre = X W of maxpool_mlp_fused's rows
+    and returns a uint8 buffer with dP = bf16(dpre) as dP^T tile images, then the fp32 per-tile column sums of dpre
+    (contract: include/graphsage_b200.h, oracle/pool_grad.py).  dhp: float32 [n_groups, hidden], unit column stride."""
+    require_cuda(table, W, bias, row_ids, dhp)
+    if table.dtype != torch.bfloat16 or table.stride(1) != 1:
+        raise TypeError("table must be row-major bfloat16")
+    K = W.shape[0] if K is None else K
+    hidden = W.shape[1]
+    if dhp.dtype != torch.float32 or dhp.dim() != 2 or dhp.stride(1) != 1 or tuple(dhp.shape) != (n_groups, hidden):
+        raise ValueError("dhp must be a float32 [%d, %d] matrix with unit column stride" % (n_groups, hidden))
+    nbytes = lib().gs_pool_mlp_dp_bytes(n_groups, k, hidden)
+    if nbytes < 0:
+        raise ValueError("pool_mlp_backward_dp: needs k <= 128 and hidden % 128 == 0 (k=%d hidden=%d)" % (k, hidden))
+    grad = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=table.device)
+    if row_ids is not None:
+        row_ids = _i32(row_ids.reshape(-1), "row_ids")
+    ws = packed.get(W)
+    ev = _probe("pool_mlp_backward_dp/%d" % n_groups)
+    check(lib().gs_pool_mlp_backward_dp(ptr(table), table.shape[0], K, table.stride(0), ptr(row_ids), row0, n_groups, k,
+                                        ptr(ws), ptr(bias), hidden, ptr(dhp), dhp.stride(0), int(pool == "mean"), ptr(grad),
+                                        stream_ptr()))
+    _launched(1 if n_groups else 0, ev)
+    return grad
+
+
+def pool_mlp_backward_dw(table, n_groups, k, grad, dWm, dbm, row_ids=None, row0=0, K=None):
+    """B2 (gs_pool_mlp_backward_dw): dWm += X^T dP over the re-gathered rows and dbm += the column sums of dpre, both in
+    a fixed order.  dWm: contiguous float32 [K, hidden]; dbm: float32 [hidden]; grad: pool_mlp_backward_dp's buffer."""
+    require_cuda(table, grad, dWm, dbm, row_ids)
+    K = dWm.shape[0] if K is None else K
+    hidden = dWm.shape[1]
+    if dWm.dtype != torch.float32 or not dWm.is_contiguous() or dbm.dtype != torch.float32 or not dbm.is_contiguous() \
+            or dbm.numel() != hidden:
+        raise ValueError("dWm must be a contiguous float32 [K, hidden] matrix and dbm a contiguous float32 [hidden]")
+    nbytes = lib().gs_pool_mlp_dw_workspace_bytes(n_groups, k, K, hidden)
+    if nbytes < 0:
+        raise ValueError("pool_mlp_backward_dw: needs k <= 128 and hidden % 128 == 0 (k=%d hidden=%d)" % (k, hidden))
+    ws = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=table.device)
+    if row_ids is not None:
+        row_ids = _i32(row_ids.reshape(-1), "row_ids")
+    ev = _probe("pool_mlp_backward_dw/%d" % n_groups)
+    check(lib().gs_pool_mlp_backward_dw(ptr(table), table.shape[0], K, table.stride(0), ptr(row_ids), row0, n_groups, k,
+                                        hidden, ptr(grad), ptr(ws), nbytes, ptr(dWm), dWm.stride(0), ptr(dbm), stream_ptr()))
+    _launched(4 if n_groups else 0, ev)                 # the GEMM, then the dWm, dbm-group and dbm sums
+    return dWm, dbm
+
+
+def pool_mlp_backward_dx(grad, n_groups, k, W, packed_dx, out=None):
+    """B3 (gs_pool_mlp_backward_dx): dx = (dP Wm^T)[:, :cols] for the n_groups * k gathered rows, float32
+    [n_groups * k, cols] (cols = packed_dx.cols); packed_dx: a PackedMlpDxWeights."""
+    require_cuda(grad, W, out)
+    cols, hidden = packed_dx.cols, W.shape[1]
+    if out is None:
+        out = torch.empty((n_groups * k, pad_cols(cols)), dtype=torch.float32, device=grad.device)[:, :cols]
+    if out.dtype != torch.float32 or out.stride(1) != 1 or out.shape[0] < n_groups * k or out.shape[1] < cols:
+        raise ValueError("out must be a row-major float32 [>= %d, >= %d] matrix" % (n_groups * k, cols))
+    ws = packed_dx.get(W)
+    ev = _probe("pool_mlp_backward_dx/%d" % n_groups)
+    check(lib().gs_pool_mlp_backward_dx(n_groups, k, hidden, ptr(grad), ptr(ws), cols, ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n_groups else 0, ev)
+    return out
+
+
 def dropout_site(site):
     """(seed, call, rate) or (seed, call, rate, call_dev) -> the C descriptor; rate must lie in [0, 1) (the mask contract
     is in the header and oracle/dropout.py).  call_dev: None, or an int64 CUDA tensor whose first element the kernel adds to

@@ -260,6 +260,118 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
         return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
 
 
+FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K = 128, 640       # K4's limits (include/graphsage_b200.h)
+
+
+def refuse_fused_pool(model):
+    """The limits of the fused bf16 pooling branch (fused_pool=True) that are known once the aggregators exist."""
+    if not getattr(model, "fused_pool", False):
+        return
+    if not hasattr(model.aggregators[0], "mlp_layers"):
+        raise NotImplementedError("fused_pool=True applies to the maxpool and meanpool aggregators only")
+    if hasattr(model.features, "c_table"):
+        raise NotImplementedError("fused_pool=True with a node-partitioned (ShardedFeatures) table is not implemented")
+    if model.dropout_rate:
+        raise NotImplementedError("fused_pool=True with training dropout > 0 is not implemented (the MLP input would "
+                                  "have to be masked inside K4)")
+    for info in model.layer_infos:
+        if info.num_samples > FUSED_POOL_MAX_FANOUT:
+            raise NotImplementedError("fused_pool=True needs fanouts <= %d (got %d)" % (FUSED_POOL_MAX_FANOUT, info.num_samples))
+    for agg in model.aggregators:
+        if agg.neigh_input_dim > FUSED_POOL_MAX_K:
+            raise NotImplementedError("fused_pool=True needs layer input widths <= %d (got %d)"
+                                      % (FUSED_POOL_MAX_K, agg.neigh_input_dim))
+        if agg.hidden_dim % 128 != 0:
+            raise NotImplementedError("fused_pool=True needs a pooling hidden width that is a multiple of 128 (got %d)"
+                                      % agg.hidden_dim)
+        if len(agg.mlp_layers) != 1:
+            raise NotImplementedError("fused_pool=True supports one MLP layer")
+
+
+class _FusedPoolAggregateRowsFn(torch.autograd.Function):
+    """y = agg.aggregate_rows(src, segments) for MaxPoolingAggregator / MeanPoolingAggregator through the fused bf16
+    kernels (fused_pool=True): the pooled branch is K4 (ops.maxpool_mlp_fused) in the forward; the backward recomputes
+    the MLP tile instead of storing it (B1 ops.pool_mlp_backward_dp), then dWm / dbm (B2) and, where a source gradient
+    is needed, dX (B3).  bf16 operands with fp32 accumulation whatever agg.math is; the self branch and the Ws / Wn
+    gradients are those of _PoolAggregateRowsFn.  Saved: the self rows, the pooled rows, y, the weights and the bf16
+    operand table - neither the gathered neighbour rows nor the MLP activations."""
+
+    @staticmethod
+    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None, persistent=False):
+        """persistent: src is the model's feature table (layer 0), cast to bf16 once per table version; a layer >= 1
+        source is cast on every call and the cast is kept for the backward."""
+        code, post = act_code(agg.act)
+        if post is not None:
+            raise NotImplementedError("training supports act=relu or identity")
+        if hasattr(src, "c_table"):
+            raise NotImplementedError("fused_pool=True with a node-partitioned (ShardedFeatures) table is not implemented")
+        F_in, hid = src.shape[1], agg.hidden_dim
+        for s in segments:
+            if s.k > FUSED_POOL_MAX_FANOUT or F_in > FUSED_POOL_MAX_K or hid % 128 != 0:
+                raise NotImplementedError("fused_pool=True needs fanout <= %d, input width <= %d and hidden %% 128 == 0 "
+                                          "(k=%d K=%d hidden=%d)" % (FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, s.k, F_in, hid))
+        rows = max(s.out_row0 + s.n for s in segments)
+        with torch.no_grad():
+            table = agg._bf16_table(src, persistent)
+            if getattr(agg, "_packed_mlp", None) is None:
+                agg._packed_mlp = ops.PackedMlpWeights()
+            hp = torch.empty((rows, hid), dtype=torch.float32, device=src.device)
+            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
+            for s in segments:
+                ops.maxpool_mlp_fused(table, s.n, s.k, Wm, bm, agg._packed_mlp, row_ids=s.neigh_ids, row0=s.neigh_row0,
+                                      K=F_in, out=hp[s.out_row0:s.out_row0 + s.n], pool=agg.pool)
+                ops.gather_rows_f32(src, ids=None if s.self_ids is None else s.self_ids[:s.n], row0=s.self_row0, n=s.n,
+                                    out=xs[s.out_row0:s.out_row0 + s.n])
+            y = agg._finish([(xs, agg.input_dim, Ws), (hp, hid, Wn)], agg._combine())
+        ctx.agg, ctx.relu, ctx.concat = agg, code == ops.ACT_RELU, bool(agg.concat)
+        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
+        ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
+        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
+        ctx.save_for_backward(xs, hp, y, Ws, Wn, Wm, bm, table)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xs, hp, y, Ws, Wn, Wm, bm, table = ctx.saved_tensors
+        agg, F_in = ctx.agg, ctx.F_in
+        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
+        D = Ws.shape[1]
+        dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
+        dWs, dWn = xs.t() @ dz_s, hp.t() @ dz_n
+        dhp = (dz_n @ Wn.t()).contiguous()
+        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dy.dtype, device=dy.device)
+        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
+        dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
+        emb = ctx.emb_shape is not None
+        d = ctx.emb_shape[1] if emb else 0
+        es = dz_s @ Ws[:d].t() if emb else None
+        packed_dx = None
+        if ctx.src_needs_grad or emb:                        # dX columns: all of them for a previous layer, else [0, d)
+            cols = F_in if ctx.src_needs_grad else d
+            if getattr(agg, "_packed_dx", None) is None or agg._packed_dx.cols != cols:
+                agg._packed_dx = ops.PackedMlpDxWeights(cols)
+            packed_dx = agg._packed_dx
+        lists = []
+        for s in ctx.segments:                               # per hop, in order: B1 -> B2 (dWm, dbm) -> B3
+            n, k = s.n, s.k
+            rows = slice(s.out_row0, s.out_row0 + n)
+            grad = ops.pool_mlp_backward_dp(table, n, k, Wm, bm, agg._packed_mlp, dhp[rows], row_ids=s.neigh_ids,
+                                            row0=s.neigh_row0, K=F_in, pool=agg.pool)
+            ops.pool_mlp_backward_dw(table, n, k, grad, dWm, dbm, row_ids=s.neigh_ids, row0=s.neigh_row0, K=F_in)
+            if packed_dx is None:
+                continue
+            dxn = ops.pool_mlp_backward_dx(grad, n, k, Wm, packed_dx)
+            if emb:                                          # self id: dxs; neighbour id of gathered row r: dxn[r]
+                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dxn[:, :d], 1, 1.0)]
+            if ctx.src_needs_grad:
+                if s.self_ids is not None or s.neigh_ids is not None:
+                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
+                dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dxn
+                dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
+        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
+        return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
+
+
 def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     """sample -> aggregate (-> l2_normalize) with an autograd graph over the aggregator weights; `model` is a
     SampleAndAggregate whose .aggregators exist (reference models.py:347-350 / supervised_models.py:79-85).
@@ -267,7 +379,11 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     past them (p = 0 draws nothing and leaves the counter alone); model.dropout_call_dev, when set, is the device-side
     offset every site adds to its call number (graphed_training)."""
     dropout = check_dropout_rate(dropout)
+    fused = getattr(model, "fused_pool", False)
     if dropout:
+        if fused:
+            raise NotImplementedError("fused_pool=True with training dropout > 0 is not implemented (the MLP input would "
+                                      "have to be masked inside K4)")
         refuse_dropout_table(model.features)
     batch = batch.to(device=model.device, dtype=torch.int32).reshape(-1)
     n = batch.numel()
@@ -304,7 +420,11 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
             else:
                 sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
                          for h in range(hops)]
-        if pool:                                             # max-pool / mean-pool
+        if pool and fused:                                   # max-pool / mean-pool through the bf16 kernels
+            mlp = agg.mlp_layers[0].vars
+            src = _FusedPoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
+                                                  mlp["weights"], mlp["bias"], emb, layer == 0)
+        elif pool:                                           # max-pool / mean-pool
             mlp = agg.mlp_layers[0].vars
             src = _PoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
                                              mlp["weights"], mlp["bias"], emb, sites)
@@ -408,9 +528,11 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def __init__(self, num_classes, placeholders, features, adj, degrees, layer_infos, concat=True,
                  aggregator_type="mean", model_size="small", sigmoid_loss=False, identity_dim=0, learning_rate=0.01,
-                 weight_decay=0.0, device="cuda", distributed=False, group=None, dropout_seed=12345, **kwargs):
+                 weight_decay=0.0, device="cuda", distributed=False, group=None, dropout_seed=12345, fused_pool=False,
+                 **kwargs):
         """dropout_seed: key of the training dropout masks (placeholders['dropout'] > 0); with distributed=True each rank
-        uses dropout_seed + rank."""
+        uses dropout_seed + rank.  fused_pool: train the maxpool / meanpool branch through the fused bf16 kernels
+        (_FusedPoolAggregateRowsFn) instead of the materialised fp32 path."""
         refuse_distributed_embeddings(identity_dim, distributed)
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
@@ -422,7 +544,9 @@ class SupervisedGraphsage(SampleAndAggregate):
         self.sigmoid_loss = sigmoid_loss
         self.learning_rate, self.weight_decay = learning_rate, weight_decay
         self.distributed, self.group, self.last_allreduce_bytes = bool(distributed), group, 0
+        self.fused_pool = bool(fused_pool)
         self.build()
+        refuse_fused_pool(self)
 
     def build(self):
         from .inits import glorot, zeros

@@ -14,7 +14,8 @@ from .graphed_training import GraphedTrainStep
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
 from .supervised_models import (aggregator_parameters, build_aggregators, differentiable_outputs, embedding_parameters,
-                                init_dropout, refuse_distributed_embeddings, weight_decay_term)
+                                init_dropout, refuse_distributed_embeddings, refuse_fused_pool,
+                                weight_decay_term)
 
 
 class UnigramNegativeSampler(object):
@@ -37,9 +38,11 @@ class UnsupervisedGraphsage(SampleAndAggregate):
 
     def __init__(self, placeholders, features, adj, degrees, layer_infos, concat=True, aggregator_type="mean",
                  model_size="small", identity_dim=0, neg_sample_size=20, neg_sample_weights=1.0, learning_rate=0.00001,
-                 weight_decay=0.0, seed=123, device="cuda", distributed=False, group=None, dropout_seed=12345, **kwargs):
+                 weight_decay=0.0, seed=123, device="cuda", distributed=False, group=None, dropout_seed=12345,
+                 fused_pool=False, **kwargs):
         """dropout_seed: key of the training dropout masks (placeholders['dropout'] > 0); with distributed=True each rank
-        uses dropout_seed + rank."""
+        uses dropout_seed + rank.  fused_pool: train the maxpool / meanpool branch through the fused bf16 kernels (see
+        SupervisedGraphsage)."""
         refuse_distributed_embeddings(identity_dim, distributed)
         super(UnsupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                     aggregator_type=aggregator_type, model_size=model_size,
@@ -51,6 +54,8 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         self.learning_rate, self.weight_decay = learning_rate, weight_decay
         self.neg_sampler = UnigramNegativeSampler(degrees, 0.75, seed, device)      # models.py:336-343
         self.aggregators = build_aggregators(self)
+        self.fused_pool = bool(fused_pool)
+        refuse_fused_pool(self)
         dim_mult = 2 if self.concat else 1
         self.link_pred_layer = BipartiteEdgePredLayer(dim_mult * self.dims[-1], dim_mult * self.dims[-1], placeholders,
                                                       neg_sample_weights=self.neg_sample_weights, bilinear_weights=False,

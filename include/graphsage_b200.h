@@ -364,6 +364,39 @@ int32_t gs_meanpool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
                               float* out, int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Backward of the pooling branch through K4 (bf16 operands, fp32 accumulate; no atomics, deterministic).
+ * One hop: X = the n_groups*k gathered rows (addressed as in gs_maxpool_mlp_fused), pre = X Wm, b = bias,
+ * dhp [n_groups, hidden] = gradient of the pooled output.  Same limits as K4: k <= 128, K <= 640, hidden % 128 == 0
+ * (else GS_ERR_UNSUPPORTED).
+ *
+ * B1 gs_pool_mlp_backward_dp: recomputes pre with K4's main loop (128-row tiles of G = 128 / k groups), then
+ *   max:  hp = relu(max_j pre_j + b); if hp > 0, dpre_j = [fl(pre_j + b) == hp] * (dhp / count), count = number of
+ *         such j (ties split evenly: TensorFlow's reduce_max gradient times the ReLU mask); else dpre_j = 0
+ *   mean: dpre_j = (dhp / k) * [fl(pre_j + b) > 0]
+ *   and writes into dp (gs_pool_mlp_dp_bytes): dP = bf16(dpre) as tile images of dP^T, then the fp32 per-(tile,
+ *   column) sums of dpre (per parity of the group index: group sums in j order added in g order; then even + odd).
+ *   packed_weights: gs_maxpool_mlp_pack.
+ * B2 gs_pool_mlp_backward_dw: dWm += X^T dP (dWm [K, hidden] fp32, ldw == hidden) and dbm += the column sums of dpre,
+ *   X re-gathered from the table; both combined in a fixed order (workspace: gs_pool_mlp_dw_workspace_bytes).
+ * B3 gs_pool_mlp_backward_dx: dx[r, :Kd] = (dP Wm^T)[r, :Kd] for the n_groups*k gathered rows (fp32, overwritten);
+ *   packed: gs_pool_mlp_dx_pack(Wm) into gs_pool_mlp_dx_pack_bytes(Kd, hidden) bytes.
+ * --------------------------------------------------------------------------------------------- */
+int64_t gs_pool_mlp_dp_bytes(int64_t n_groups, int32_t k, int32_t hidden);
+int32_t gs_pool_mlp_backward_dp(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch,
+                                const int32_t* row_ids, int64_t row0, int64_t n_groups, int32_t k,
+                                const void* packed_weights, const float* bias, int32_t hidden, const float* dhp,
+                                int64_t lddhp, int32_t pool_mean, void* dp, void* stream);
+int64_t gs_pool_mlp_dw_workspace_bytes(int64_t n_groups, int32_t k, int32_t K, int32_t hidden);
+int32_t gs_pool_mlp_backward_dw(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch,
+                                const int32_t* row_ids, int64_t row0, int64_t n_groups, int32_t k, int32_t hidden,
+                                const void* dp, void* workspace, int64_t workspace_bytes, float* dWm, int64_t ldw,
+                                float* dbm, void* stream);
+int64_t gs_pool_mlp_dx_pack_bytes(int32_t Kd, int32_t hidden);
+int32_t gs_pool_mlp_dx_pack(const float* Wm, int64_t ldw, int32_t Kd, int32_t hidden, void* packed, void* stream);
+int32_t gs_pool_mlp_backward_dx(int64_t n_groups, int32_t k, int32_t hidden, const void* dp, const void* packed,
+                                int32_t Kd, float* dx, int64_t ldx, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * One pipelined step from HOST buffers in a single call (no per-kernel host work), on three streams:
  *   h2d_stream     : wait ev_done (this slot's previous step no longer reads ids_dev), copy ids host->device,
  *                    record ev_ids
