@@ -127,6 +127,11 @@ _SIGNATURES = {
                                           c_i64, c_vp, c_i64, c_vp]),
     "gs_embedding_sgd": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, ctypes.c_float, c_vp, c_i64, c_vp, c_i64,
                                  c_vp]),
+    "gs_seq_lengths": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, c_vp, c_vp]),
+    "gs_lstm_forward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64,
+                                c_vp, c_i64, c_vp]),
+    "gs_lstm_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i32, c_i32, c_vp, c_i64,
+                                 c_vp]),
     "gs_skipgram_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32]),
     "gs_skipgram_grad": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,
                                  c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),

@@ -1,5 +1,5 @@
-"""MeanAggregator / GCNAggregator / MaxPoolingAggregator - the surface of reference
-graphsage/aggregators.py:6-195 over the library's CUDA kernels.
+"""MeanAggregator / GCNAggregator / MaxPoolingAggregator / MeanPoolingAggregator / SeqAggregator - the surface of
+reference graphsage/aggregators.py over the library's CUDA kernels.
 
 Two entry points per aggregator:
   agg((self_vecs[n, in], neigh_vecs[n, k, neigh_in])) -> [n, out * (2 if concat else 1)]
@@ -314,3 +314,101 @@ class MeanPoolingAggregator(MaxPoolingAggregator):
     """act(concat_or_add(self @ Ws, mean_k(relu(neigh @ Wm + bm)) @ Wn)) - reference graphsage/aggregators.py:197-273.
     Same kernels as the max-pool aggregator with the pooling operator swapped (SURVEY section 8f row 4)."""
     pool = "mean"
+
+
+def refuse_seq_table(features):
+    """The seq aggregator reads a dense fp32 table (the projection GEMM and the length rule take fp32 rows)."""
+    if hasattr(features, "c_table"):
+        raise NotImplementedError("the seq aggregator with a node-partitioned (ShardedFeatures) table is not implemented")
+    if features is not None and features.dtype != torch.float32:
+        raise NotImplementedError("the seq aggregator with a %s feature table is not implemented (float32 only)"
+                                  % features.dtype)
+
+
+class LSTMCell(object):
+    """tf.contrib.rnn.BasicLSTMCell(H) of TF 1.8 (the reference's SeqAggregator.cell): `kernel` [K + H, 4H] - rows for the
+    input first, then for h; glorot uniform, the tf.get_variable default - and `bias` [4H], zeros.  Gate columns i, j, f, o;
+    the forget bias 1.0 is added at run time, not stored."""
+
+    def __init__(self, input_dim, hidden_dim, device="cuda"):
+        self.input_dim, self.hidden_dim = input_dim, hidden_dim
+        self.vars = {"kernel": glorot([input_dim + hidden_dim, 4 * hidden_dim], name="kernel", device=device),
+                     "bias": zeros([4 * hidden_dim], name="bias", device=device)}
+
+    @property
+    def W_x(self):
+        return self.vars["kernel"][:self.input_dim]
+
+    @property
+    def W_h(self):
+        return self.vars["kernel"][self.input_dim:]
+
+
+class SeqAggregator(_SageAggregator):
+    """act(concat_or_add(self @ Ws, h_len @ Wn)) - aggregators.py:363-449: an LSTM (`self.cell`, hidden 128 for "small",
+    256 for "big") runs over the first len_i neighbours of each node, len_i = max(1, number of neighbour rows that are not
+    all zero), and h after len_i steps is the neighbour summary.  The input projection X W_x + b is the library GEMM
+    (self.math), the recurrence the fp32 kernels gs_lstm_forward / gs_seq_lengths.  `dropout` is kept but never applied:
+    the reference's SeqAggregator._call draws no mask."""
+
+    def __init__(self, input_dim, output_dim, model_size="small", neigh_input_dim=None, dropout=0., bias=False, act=relu,
+                 name=None, concat=False, device="cuda", **kwargs):
+        super(SeqAggregator, self).__init__(**kwargs)
+        self.dropout = dropout
+        self.bias = bias
+        self.act = act
+        self.concat = concat
+        if neigh_input_dim is None:
+            neigh_input_dim = input_dim
+        if model_size == "small":
+            hidden_dim = self.hidden_dim = 128
+        elif model_size == "big":
+            hidden_dim = self.hidden_dim = 256
+        else:
+            raise ValueError("model_size must be 'small' or 'big'")
+        self.vars["neigh_weights"] = glorot([hidden_dim, output_dim], name="neigh_weights", device=device)
+        self.vars["self_weights"] = glorot([input_dim, output_dim], name="self_weights", device=device)
+        if self.bias:   # aggregators.py:395 reads self.output_dim before it is set; fixed as in MeanAggregator
+            self.vars["bias"] = zeros([output_dim * (2 if concat else 1)], name="bias", device=device)
+        self.input_dim = input_dim
+        self.output_dim = output_dim
+        self.neigh_input_dim = neigh_input_dim
+        self.math = _DEFAULT_MATH[0]
+        self.cell = LSTMCell(neigh_input_dim, hidden_dim, device=device)
+
+    def _combine(self):
+        return ops.COMBINE_CONCAT if self.concat else ops.COMBINE_ADD
+
+    def _neigh_hidden(self, X, n, k, out=None):
+        """h after len_i steps over the n sequences of k rows of X [n*k, neigh_input_dim]."""
+        lengths = ops.seq_lengths(X, n, k)
+        if getattr(self.cell, "_packed", None) is None:
+            self.cell._packed = ops.PackedWeights()
+        P = ops.sage_gemm([(X, self.neigh_input_dim, self.cell.W_x)], bias=self.cell.vars["bias"], math=self.math,
+                          packed=self.cell._packed)
+        return ops.lstm_forward(P, self.cell.W_h, lengths, n, k, out=out)
+
+    def _call(self, inputs):
+        self_vecs, neigh_vecs = inputs
+        n, k, d = neigh_vecs.shape
+        h = self._neigh_hidden(neigh_vecs.reshape(n * k, d), n, k)
+        return self._finish([(self_vecs, self.input_dim, self.vars["self_weights"]),
+                             (h, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
+
+    def aggregate_rows(self, src, segments, final=None, src_persistent=False):
+        refuse_seq_table(src)
+        rows = max(s.out_row0 + s.n for s in segments)
+        F_in = src.shape[1]
+        xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
+        h = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=src.device)
+        for s in segments:
+            n, k = s.n, s.k
+            X = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
+                src[s.neigh_row0:s.neigh_row0 + n * k]
+            self._neigh_hidden(X, n, k, out=h[s.out_row0:s.out_row0 + n])
+            if s.self_ids is not None:
+                ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
+            else:
+                xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
+        return self._finish([(xs, self.input_dim, self.vars["self_weights"]),
+                             (h, self.hidden_dim, self.vars["neigh_weights"])], self._combine())

@@ -9,7 +9,8 @@ from collections import namedtuple
 import torch
 
 from . import ops
-from .aggregators import GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator
+from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
+                          refuse_seq_table)
 from .layers import identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
@@ -20,7 +21,8 @@ SAGEInfo = namedtuple("SAGEInfo",
                        "output_dim"])     # the output (i.e., hidden) dimension
 
 _AGGREGATORS = {"mean": MeanAggregator, "maxpool": MaxPoolingAggregator, "gcn": GCNAggregator,
-                "meanpool": MeanPoolingAggregator}
+                "meanpool": MeanPoolingAggregator, "seq": SeqAggregator}
+_SIZED_AGGREGATORS = (MaxPoolingAggregator, SeqAggregator)       # take model_size (models.py:213-226)
 
 
 class SampleAndAggregate(object):
@@ -39,9 +41,6 @@ class SampleAndAggregate(object):
         for kwarg in kwargs.keys():
             assert kwarg in allowed_kwargs, "Invalid keyword argument: " + kwarg   # reference models.py:22-24
         if aggregator_type not in _AGGREGATORS:
-            if aggregator_type in ("seq",):
-                raise NotImplementedError("aggregator_type %r is outside the hot path (SURVEY section 2, row 5)"
-                                          % aggregator_type)
             raise ValueError("Unknown aggregator: %r" % (aggregator_type,))
         self.aggregator_cls = _AGGREGATORS[aggregator_type]
         if features is None and not identity_dim > 0:
@@ -105,6 +104,8 @@ class SampleAndAggregate(object):
         self.embeds = table[:, :d]
 
     def _finish_init(self, placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device):
+        if self.aggregator_cls is SeqAggregator:
+            refuse_seq_table(self.features)
         self.degrees = degrees
         self.concat = concat
         self.dims = [self.features.shape[1] + identity_dim]
@@ -162,10 +163,11 @@ class SampleAndAggregate(object):
                 act = identity if layer == L - 1 else relu                      # models.py:307-310
                 kw = dict(act=act, dropout=self.placeholders.get("dropout", 0.), name=name, concat=concat,
                           device=self.device)
-                if issubclass(self.aggregator_cls, MaxPoolingAggregator):
+                if issubclass(self.aggregator_cls, _SIZED_AGGREGATORS):
                     kw["model_size"] = model_size
                 aggregators.append(self.aggregator_cls(dim_mult * dims[layer], dims[layer + 1], **kw))
-        if any(getattr(a, "dropout", 0.) for a in aggregators):
+        # SeqAggregator keeps `dropout` but never applies it (aggregators.py:405-449): it stays on the gather-fused path
+        if any(getattr(a, "dropout", 0.) and not isinstance(a, SeqAggregator) for a in aggregators):
             return self._aggregate_materialised(samples, feats, dims, num_samples, support_sizes, batch_size,
                                                 aggregators, concat), aggregators
         # gather-fused recursion: hop h of a layer occupies rows [row0[h], row0[h] + batch*support[h])

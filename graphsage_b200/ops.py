@@ -870,6 +870,63 @@ def skipgram_grad(target, context, batch1, batch2, neg):
     return out
 
 
+def _rows_f32(t, name, cols):
+    require_cuda(t)
+    if t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1 or t.shape[1] < cols:
+        raise ValueError("%s must be a row-major float32 matrix with >= %d columns" % (name, cols))
+    return t
+
+
+def seq_lengths(x, n, k):
+    """The reference's sequence lengths (aggregators.py:411-414) of n sequences of k rows of x [n*k, K]: int32 [n],
+    max(1, number of rows with an element that is not zero)."""
+    _rows_f32(x, "x", 0)
+    if x.shape[0] != n * k:
+        raise ValueError("x has %d rows, expected n*k = %d" % (x.shape[0], n * k))
+    out = torch.empty((n,), dtype=torch.int32, device=x.device)
+    ev = _probe("seq_lengths/%d" % n)
+    check(lib().gs_seq_lengths(ptr(x), x.stride(0), n, k, x.shape[1], ptr(out), stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return out
+
+
+def lstm_forward(P, Wh, lengths, n, k, out=None, train=False):
+    """BasicLSTMCell under dynamic_rnn (aggregators.py:410-433): P [n*k, 4H] = X W_x + b, Wh [H, 4H] (a strided view is
+    fine), lengths int32 [n].  Returns h_last [n, H] (into `out` when given); with train=True (h_last, gates [n*k, 4H],
+    c [n*k, H], h_prev [n*k, H]) for lstm_backward and the weight gradients."""
+    H = Wh.shape[0]
+    _rows_f32(P, "P", 4 * H)
+    _rows_f32(Wh, "Wh", 4 * H)
+    lengths = _i32(lengths, "lengths")
+    dev = P.device
+    if out is None:
+        out = torch.empty((n, H), dtype=torch.float32, device=dev)
+    _rows_f32(out, "out", H)
+    saved = [torch.empty((n * k, w), dtype=torch.float32, device=dev) for w in (4 * H, H, H)] if train else [None] * 3
+    g, c, hp = saved
+    ev = _probe("lstm_forward/%d" % n)
+    check(lib().gs_lstm_forward(ptr(P), P.stride(0), ptr(Wh), Wh.stride(0), ptr(lengths), n, k, H, ptr(out), out.stride(0),
+                                ptr(g), 4 * H, ptr(c), H, ptr(hp), H, stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return (out, g, c, hp) if train else out
+
+
+def lstm_backward(dh_last, gates, c, lengths, Wh, n, k):
+    """Backpropagation through time of lstm_forward: dZ [n*k, 4H], the gradient of the gate pre-activations."""
+    H = Wh.shape[0]
+    _rows_f32(dh_last, "dh_last", H)
+    _rows_f32(gates, "gates", 4 * H)
+    _rows_f32(c, "c", H)
+    _rows_f32(Wh, "Wh", 4 * H)
+    lengths = _i32(lengths, "lengths")
+    dz = torch.empty((n * k, 4 * H), dtype=torch.float32, device=gates.device)
+    ev = _probe("lstm_backward/%d" % n)
+    check(lib().gs_lstm_backward(ptr(dh_last), dh_last.stride(0), ptr(gates), gates.stride(0), ptr(c), c.stride(0),
+                                 ptr(lengths), ptr(Wh), Wh.stride(0), n, k, H, ptr(dz), dz.stride(0), stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return dz
+
+
 def l2_normalize_rows_(x):
     """In-place tf.nn.l2_normalize(x, 1) - reference graphsage/models.py:368."""
     require_cuda(x)

@@ -20,7 +20,8 @@ import torch
 from . import ops
 from .graphed_training import GraphedTrainStep
 from .layers import act_code, identity, relu  # noqa: F401
-from .models import SampleAndAggregate
+from .aggregators import refuse_seq_table
+from .models import _SIZED_AGGREGATORS, SampleAndAggregate
 
 
 def _embedding_grad(emb_shape, lists, sites=None):
@@ -33,8 +34,10 @@ def dropout_site_plan(kind, n_layers, head=False):
     """The dropout sites of one forward pass in the reference's call order (models.py:303-328 calls each layer's
     aggregator once per hop): [(layer, hop, role)], role "neigh" then "self" for mean / gcn (aggregators.py:46-47,
     104-105), the one "mlp" input of the pools' Dense (layers.py:107), then (None, None, "head") for the supervised head
-    (supervised_models.py:88-90).  Site i of a pass draws with call = first call + i."""
+    (supervised_models.py:88-90); "seq" has no aggregator sites.  Site i of a pass draws with call = first call + i."""
     plan = []
+    if kind == "seq":                   # SeqAggregator._call applies no dropout (aggregators.py:405-449): the head only
+        n_layers = 0
     for layer in range(n_layers):
         for hop in range(n_layers - layer):
             plan += [(layer, hop, "mlp")] if kind in ("maxpool", "meanpool") else [(layer, hop, "neigh"), (layer, hop, "self")]
@@ -260,6 +263,85 @@ class _PoolAggregateRowsFn(torch.autograd.Function):
         return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
 
 
+class _SeqAggregateRowsFn(torch.autograd.Function):
+    """y = agg.aggregate_rows(src, segments) for SeqAggregator, differentiable w.r.t. Ws, Wn, the cell's kernel and bias,
+    (layers >= 1) src and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of src's first d columns.
+    Forward per hop: X (gathered rows, or the previous layer's row range) -> lengths (gs_seq_lengths) -> P = X W_x + b
+    (library GEMM, agg.math) -> gs_lstm_forward, keeping X, the lengths, the gates, c and h_{t-1}.  Backward per hop:
+    gs_lstm_backward gives dZ; dW_x = X^T dZ, dW_h = h_prev^T dZ, db = sum dZ and dX = dZ W_x^T are library matmuls."""
+
+    @staticmethod
+    def forward(ctx, agg, src, segments, Ws, Wn, kernel, cell_bias, emb=None):
+        code, post = act_code(agg.act)
+        if post is not None:
+            raise NotImplementedError("training supports act=relu or identity")
+        refuse_seq_table(src)
+        F_in, H = src.shape[1], agg.hidden_dim
+        rows = max(s.out_row0 + s.n for s in segments)
+        with torch.no_grad():
+            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
+            hl = torch.empty((rows, H), dtype=torch.float32, device=src.device)
+            Wx, Wh = kernel[:F_in], kernel[F_in:]
+            kept = []
+            for s in segments:
+                n, k = s.n, s.k
+                X = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
+                    src[s.neigh_row0:s.neigh_row0 + n * k]
+                lengths = ops.seq_lengths(X, n, k)
+                P = ops.sage_gemm([(X, F_in, Wx)], bias=cell_bias, math=agg.math)
+                _, gates, c, h_prev = ops.lstm_forward(P, Wh, lengths, n, k, out=hl[s.out_row0:s.out_row0 + n], train=True)
+                del P
+                if s.self_ids is not None:
+                    ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
+                else:
+                    xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
+                kept.extend([X, lengths, gates, c, h_prev])
+            y = agg._finish([(xs, agg.input_dim, Ws), (hl, H, Wn)], agg._combine())
+        ctx.relu, ctx.concat = code == ops.ACT_RELU, bool(agg.concat)
+        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
+        ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
+        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
+        ctx.save_for_backward(xs, hl, y, Ws, Wn, kernel, *kept)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xs, hl, y, Ws, Wn, kernel = ctx.saved_tensors[:6]
+        kept = ctx.saved_tensors[6:]
+        F_in = ctx.F_in
+        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
+        D = Ws.shape[1]
+        dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
+        dWs, dWn = xs.t() @ dz_s, hl.t() @ dz_n
+        dhl = (dz_n @ Wn.t()).contiguous()
+        Wx, Wh = kernel[:F_in], kernel[F_in:]
+        dWx, dWh = torch.zeros_like(Wx), torch.zeros_like(Wh)
+        db = torch.zeros(kernel.shape[1], dtype=dy.dtype, device=dy.device)
+        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
+        dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
+        emb = ctx.emb_shape is not None
+        d = ctx.emb_shape[1] if emb else 0
+        es = dz_s @ Ws[:d].t() if emb else None          # the embedding columns only need dZ @ W[:d]^T
+        lists = []
+        for i, s in enumerate(ctx.segments):
+            n, k = s.n, s.k
+            rows = slice(s.out_row0, s.out_row0 + n)
+            X, lengths, gates, c, h_prev = kept[5 * i:5 * i + 5]
+            dZ = ops.lstm_backward(dhl[rows], gates, c, lengths, Wh, n, k)
+            dWx += X.t() @ dZ
+            dWh += h_prev.t() @ dZ
+            db += dZ.sum(dim=0)
+            if emb:                                      # self id: dxs; neighbour id of gathered row r: dX[r]
+                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dZ @ Wx[:d].t(), 1, 1.0)]
+            if ctx.src_needs_grad:
+                if s.self_ids is not None or s.neigh_ids is not None:
+                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
+                dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dZ @ Wx.t()
+                dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
+        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
+        return None, dsrc, None, dWs, dWn, torch.cat([dWx, dWh]), db, demb
+
+
 FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K = 128, 640       # K4's limits (include/graphsage_b200.h)
 
 
@@ -394,7 +476,8 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     counts = [n * support[h] for h in range(L + 1)]
     src = model.features
     pool = hasattr(model.aggregators[0], "mlp_layers")
-    plan = dropout_site_plan("maxpool" if pool else "mean", L) if dropout else []
+    seq = hasattr(model.aggregators[0], "cell")
+    plan = dropout_site_plan("seq" if seq else "maxpool" if pool else "mean", L) if dropout else []
     call = {site: model.dropout_counter + i for i, site in enumerate(plan)}
     for layer in range(L):
         hops = L - layer
@@ -413,14 +496,18 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
         # deliver the scattered gradient as embeds.grad
         emb = getattr(model, "embeds", None) if layer == 0 else None
         sites = None
-        if dropout:                                          # per hop: the MLP-input site, or the (neighbour, self) pair
+        if dropout and not seq:                              # per hop: the MLP-input site, or the (neighbour, self) pair
             key, dev = model.dropout_key, model.dropout_call_dev
             if pool:
                 sites = [(key, call[(layer, h, "mlp")], dropout, dev) for h in range(hops)]
             else:
                 sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
                          for h in range(hops)]
-        if pool and fused:                                   # max-pool / mean-pool through the bf16 kernels
+        if seq:                                              # LSTM: draws no dropout mask
+            cell = agg.cell.vars
+            src = _SeqAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
+                                            cell["kernel"], cell["bias"], emb)
+        elif pool and fused:                                 # max-pool / mean-pool through the bf16 kernels
             mlp = agg.mlp_layers[0].vars
             src = _FusedPoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
                                                   mlp["weights"], mlp["bias"], emb, layer == 0)
@@ -477,7 +564,7 @@ def build_aggregators(model):
     for layer in range(L):
         dim_mult = 2 if model.concat and layer != 0 else 1
         act = identity if layer == L - 1 else relu
-        extra = {"model_size": model.model_size} if hasattr(model.aggregator_cls, "pool") else {}
+        extra = {"model_size": model.model_size} if issubclass(model.aggregator_cls, _SIZED_AGGREGATORS) else {}
         aggs.append(model.aggregator_cls(dim_mult * model.dims[layer], model.dims[layer + 1], act=act, dropout=0.,
                                          concat=model.concat, device=model.device, **extra))
     return aggs
@@ -486,9 +573,11 @@ def build_aggregators(model):
 def aggregator_parameters(aggregators):
     """(all trainable tensors, the subset the reference applies weight decay to).  The reference decays
     `aggregator.vars` only (supervised_models.py:103-105, models.py:385-387) - the pooling aggregators' Dense variables
-    live in `mlp_layers[0].vars` and are trained but not decayed."""
+    live in `mlp_layers[0].vars` and the seq aggregator's LSTM kernel and bias in `cell.vars`: both are trained but not
+    decayed."""
     decayed = [v for a in aggregators for v in a.vars.values()]
     extra = [v for a in aggregators for layer in getattr(a, "mlp_layers", []) for v in layer.vars.values()]
+    extra += [v for a in aggregators if hasattr(a, "cell") for v in a.cell.vars.values()]
     return decayed + extra, decayed
 
 
@@ -537,8 +626,8 @@ class SupervisedGraphsage(SampleAndAggregate):
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
                                                   identity_dim=identity_dim, device=device, **kwargs)
-        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool"):
-            raise NotImplementedError("training is implemented for the mean, gcn, maxpool and meanpool aggregators")
+        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool", "seq"):
+            raise NotImplementedError("training is implemented for the mean, gcn, maxpool, meanpool and seq aggregators")
         init_dropout(self, dropout_seed, distributed, group)
         self.num_classes = num_classes
         self.sigmoid_loss = sigmoid_loss

@@ -534,6 +534,34 @@ int32_t gs_skipgram_grad(const float* target, int64_t ldt, const float* context,
                          float* aff, float* neg_aff, float* gt, int64_t ldgt, float* gc_pos, float* gc_neg, int64_t ldgc,
                          void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * SeqAggregator (reference graphsage/aggregators.py:363-449): TF 1.8 BasicLSTMCell(H) under dynamic_rnn with
+ * sequence_length, over the k sampled neighbours of each of n nodes.  Gate column order i, j, f, o; with z = x·W_x + h·W_h + b
+ *     c' = c·σ(z_f + 1) + σ(z_i)·tanh(z_j),   h' = tanh(c')·σ(z_o),   h_0 = c_0 = 0
+ * Sequence i is rows i·k .. i·k + k - 1 of every [n·k, .] operand.  All three kernels are fp32 on the CUDA cores, read their
+ * loop bounds (the lengths) on the device, allocate nothing, use no atomics and only enqueue on `stream`: bit-identical on
+ * every call and capturable in a CUDA graph.
+ *
+ * gs_seq_lengths - the reference's length rule (:411-414): used[i, j] = 1 iff row x[(i·k + j)·ldx + 0..K) has an element
+ *   that is not zero (-0.0 is zero), len[i] = max(1, sum_j used[i, j]).  The LSTM runs over the FIRST len[i] positions,
+ *   whatever they hold.
+ * gs_lstm_forward - P [n·k, 4H] (ldp) = X·W_x + b from the input projection; Wh the [H, 4H] recurrent block W_h (the
+ *   kernel's bottom H rows, ldw).  Writes h_last[i] = h after len[i] steps ([n, H], ldh; len is clamped to k).
+ *   Training outputs, all three or none (NULL): gates [n·k, 4H] = (σ(z_i), tanh(z_j), σ(z_f + 1), σ(z_o)), c [n·k, H] = c_t,
+ *   h_prev [n·k, H] = h_{t-1} (zero at t = 0); rows t >= len[i] are zeros.  Limits: H in {128, 256}, k >= 1, n < 2^31.
+ * gs_lstm_backward - backpropagation through time from dh_last [n, H] (the gradient of h_last) with the forward's saved
+ *   gates and c: dZ [n·k, 4H], the gradient of the pre-activations z_t, zero for t >= len[i].  dh_{t-1} = dz_t·W_hᵀ is
+ *   carried inside the kernel (columns summed in ascending order).  Wh must be 16-byte aligned with ldw % 4 == 0.
+ *   The weight and input gradients are dW_x = Xᵀ·dZ, dW_h = h_prevᵀ·dZ, db = column sums of dZ, dX = dZ·W_xᵀ (the caller's).
+ * --------------------------------------------------------------------------------------------- */
+int32_t gs_seq_lengths(const float* x, int64_t ldx, int64_t n, int32_t k, int32_t K, int32_t* len, void* stream);
+int32_t gs_lstm_forward(const float* P, int64_t ldp, const float* Wh, int64_t ldw, const int32_t* len, int64_t n, int32_t k,
+                        int32_t H, float* h_last, int64_t ldh, float* gates, int64_t ldg, float* c, int64_t ldc,
+                        float* h_prev, int64_t ldhp, void* stream);
+int32_t gs_lstm_backward(const float* dh_last, int64_t lddh, const float* gates, int64_t ldg, const float* c, int64_t ldc,
+                         const int32_t* len, const float* Wh, int64_t ldw, int64_t n, int32_t k, int32_t H, float* dZ,
+                         int64_t ldz, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
