@@ -171,9 +171,9 @@ def _identity_train(args, model, seeds, labels, ms_base, dist, dev):
     seen = {}
     real = sm._embedding_grad
 
-    def keep(emb_shape, lists):
+    def keep(emb_shape, lists, sites=None):
         seen["lists"] = lists
-        return real(emb_shape, lists)
+        return real(emb_shape, lists, sites)
 
     sm._embedding_grad = keep
     try:

@@ -33,6 +33,27 @@ def _dense_segment(n, k):
     return [ops.make_segment(n, k)]
 
 
+def _rows(src, ids, row0, n, f32=False, out=None):
+    """Rows ids[:n] (or row0 .. row0 + n) of src: gathered by the library (gs_gather_rows_f32, which widens a bf16 table,
+    when f32 is set), or else a view of the row range (copied into `out` when given)."""
+    if f32:
+        return ops.gather_rows_f32(src, ids=None if ids is None else ids[:n], row0=row0, n=n, out=out)
+    if ids is not None:
+        return ops.gather_rows(src, ids[:n], out=out)
+    if out is None:
+        return src[row0:row0 + n]
+    out.copy_(src[row0:row0 + n])
+    return out
+
+
+# K4's limits (include/graphsage_b200.h): fanout, layer input width, multiple of the pooling hidden width
+FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, FUSED_POOL_HIDDEN_STEP = 128, 640, 128
+
+
+def fused_pool_fits(k, K, hidden):
+    return k <= FUSED_POOL_MAX_FANOUT and K <= FUSED_POOL_MAX_K and hidden % FUSED_POOL_HIDDEN_STEP == 0
+
+
 USE_GEMM_IMAGES = [False]     # opt-in: tf32x3 layers hand the gathered rows to the GEMM as tensor-core tile images
                               # (ops.gather_mean_images + ops.sage_gemm_img; bit-identical results).  Measured on the bench step:
                               # the GEMM's A side becomes one bulk copy per K-block, but the gather - the critical kernel -
@@ -41,6 +62,22 @@ USE_GEMM_IMAGES = [False]     # opt-in: tf32x3 layers hand the gathered rows to 
 
 
 class _SageAggregator(Layer):
+    def _combine(self):
+        return ops.COMBINE_CONCAT if self.concat and "self_weights" in self.vars else ops.COMBINE_ADD
+
+    def _summarise(self, src, segments, hop, f32_self=False):
+        """The GEMM parts [self rows, neighbour summary] of a layer whose neighbour branch is a per-hop summary of
+        hidden_dim columns (pools, seq): hop(i, s, out) writes the summary of segment i (s) into `out`, its rows of the
+        summary part; each hop's self rows are copied after it."""
+        rows = max(s.out_row0 + s.n for s in segments)
+        F_in = src.shape[1]
+        xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
+        h = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=src.device)
+        for i, s in enumerate(segments):
+            hop(i, s, h[s.out_row0:s.out_row0 + s.n])
+            _rows(src, s.self_ids, s.self_row0, s.n, f32_self, out=xs[s.out_row0:s.out_row0 + s.n])
+        return [(xs, self.input_dim, self.vars["self_weights"]), (h, self.hidden_dim, self.vars["neigh_weights"])]
+
     def _image_layer(self, src, segments, parts, combine, include_self, want_self):
         """gather + mean -> tile images -> wgmma GEMM (tf32x3); None when the image form does not apply."""
         code, post = act_code(self.act)
@@ -107,9 +144,6 @@ class MeanAggregator(_SageAggregator):
         self.output_dim = output_dim
         self.neigh_input_dim = neigh_input_dim
         self.math = _DEFAULT_MATH[0]
-
-    def _combine(self):
-        return ops.COMBINE_CONCAT if self.concat else ops.COMBINE_ADD
 
     def _call(self, inputs):
         self_vecs, neigh_vecs = inputs
@@ -215,16 +249,16 @@ class MaxPoolingAggregator(_SageAggregator):
         self.output_dim = output_dim
         self.neigh_input_dim = neigh_input_dim
 
-    def _combine(self):
-        return ops.COMBINE_CONCAT if self.concat else ops.COMBINE_ADD
-
     pool = "max"
 
-    def _pool(self, rows, n, k):
+    def _mlp(self, rows):
         h = rows
         for layer in self.mlp_layers:
             layer.math = self.math
             h = layer(h)
+        return h
+
+    def _pool(self, h, n, k):
         if self.pool == "mean":
             return ops.gather_mean(h, [ops.Seg(n, k)], want_self=False, out_pitch=h.shape[1])[1]
         return ops.segment_max(h, n, k)
@@ -232,7 +266,7 @@ class MaxPoolingAggregator(_SageAggregator):
     def _call(self, inputs):
         self_vecs, neigh_vecs = inputs
         n, k, d = neigh_vecs.shape
-        hmax = self._pool(neigh_vecs.reshape(n * k, d), n, k)
+        hmax = self._pool(self._mlp(neigh_vecs.reshape(n * k, d)), n, k)
         return self._finish([(self_vecs, self.input_dim, self.vars["self_weights"]),
                              (hmax, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
 
@@ -254,58 +288,51 @@ class MaxPoolingAggregator(_SageAggregator):
 
     def _fused_ok(self, src, segments):
         return (self.math == ops.MATH_BF16 and torch.is_tensor(src) and not self.dropout and len(self.mlp_layers) == 1
-                and self.neigh_input_dim <= 640 and self.hidden_dim % 128 == 0 and all(s.k <= 128 for s in segments)
+                and all(fused_pool_fits(s.k, self.neigh_input_dim, self.hidden_dim) for s in segments)
                 and self.mlp_layers[0].act is relu and "bias" in self.mlp_layers[0].vars)
 
-    def aggregate_rows(self, src, segments, final=None, src_persistent=False):
-        rows = max(s.out_row0 + s.n for s in segments)
-        dev = src.device
-        if self._fused_ok(src, segments):
-            # K4: gather -> MLP -> ReLU -> max over the fanout in one wgmma kernel per hop (bf16 operands).
-            # Every launch of this branch is one of the library's kernels (no torch copy / convert kernels in the step).
-            table = self._bf16_table(src, src_persistent)
-            if getattr(self, "_packed_mlp", None) is None:
-                self._packed_mlp = ops.PackedMlpWeights()
-            mlp = self.mlp_layers[0]
-            F_in = src.shape[1]
-            hmax = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=dev)
-            for s in segments:
-                ops.maxpool_mlp_fused(table, s.n, s.k, mlp.vars["weights"], mlp.vars["bias"], self._packed_mlp,
-                                      row_ids=s.neigh_ids, row0=s.neigh_row0, K=self.neigh_input_dim,
-                                      out=hmax[s.out_row0:s.out_row0 + s.n], pool=self.pool)
-            s0 = segments[0]
-            if len(segments) == 1 and s0.self_ids is None and s0.out_row0 == 0 and src.dtype == torch.float32:
-                xs = src[s0.self_row0:s0.self_row0 + s0.n]         # the self rows are already a dense fp32 row range
-            else:
-                xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=dev)[:, :F_in]
-                for s in segments:
-                    ops.gather_rows_f32(src, ids=None if s.self_ids is None else s.self_ids[:s.n], row0=s.self_row0,
-                                        n=s.n, out=xs[s.out_row0:s.out_row0 + s.n])
-            return self._finish([(xs, self.input_dim, self.vars["self_weights"]),
-                                 (hmax, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
-        # materialised form (fp32 / tf32 arithmetic, fanout > 128, wide inputs, sharded tables): the MLP is a plain GEMM over
-        # the gathered neighbour rows (widened to fp32 when the table is bf16), then the pooling kernel
-        xs = torch.empty((rows, ops.pad_cols(src.shape[1])), dtype=torch.float32, device=dev)[:, :src.shape[1]]
-        hmax = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=dev)
+    def _fused_hop(self, table, s, out):
+        """K4 for one hop: gather -> MLP -> ReLU -> pool over the fanout in one wgmma kernel (bf16 operands) into `out`."""
+        if getattr(self, "_packed_mlp", None) is None:
+            self._packed_mlp = ops.PackedMlpWeights()
+        mlp = self.mlp_layers[0].vars
+        ops.maxpool_mlp_fused(table, s.n, s.k, mlp["weights"], mlp["bias"], self._packed_mlp, row_ids=s.neigh_ids,
+                              row0=s.neigh_row0, K=self.neigh_input_dim, out=out, pool=self.pool)
+
+    def _pooled_parts(self, src, segments, kept=None, sites=None):
+        """The GEMM parts of the materialised form: per hop the neighbour rows (widened to fp32 from a bf16 table), with
+        training dropout the mask of sites[hop] applied to them, then the MLP and the pooling kernel.  `kept` (training)
+        receives each hop's MLP input and output."""
         widen = torch.is_tensor(src) and src.dtype != torch.float32
+
+        def hop(i, s, out):
+            xn = _rows(src, s.neigh_ids, s.neigh_row0, s.n * s.k, widen)
+            if sites is not None:                   # out of place: layer >= 1 rows belong to the previous layer
+                xn = ops.dropout_apply(xn, sites[i])
+            h = self._mlp(xn)
+            out.copy_(self._pool(h, s.n, s.k))
+            if kept is not None:
+                kept.extend([xn, h])
+        return self._summarise(src, segments, hop, widen)
+
+    def aggregate_rows(self, src, segments, final=None, src_persistent=False):
+        if not self._fused_ok(src, segments):
+            # materialised form (fp32 / tf32 arithmetic, fanout > 128, wide inputs, sharded tables)
+            return self._finish(self._pooled_parts(src, segments), self._combine())
+        # K4: every launch of this branch is one of the library's kernels (no torch copy / convert kernels in the step)
+        table = self._bf16_table(src, src_persistent)
+        rows = max(s.out_row0 + s.n for s in segments)
+        hmax = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=src.device)
         for s in segments:
-            n, k = s.n, s.k
-            if widen:
-                nrows = ops.gather_rows_f32(src, ids=None if s.neigh_ids is None else s.neigh_ids[:n * k],
-                                            row0=s.neigh_row0, n=n * k)
-                ops.gather_rows_f32(src, ids=None if s.self_ids is None else s.self_ids[:n], row0=s.self_row0, n=n,
-                                    out=xs[s.out_row0:s.out_row0 + n])
-                hmax[s.out_row0:s.out_row0 + n] = self._pool(nrows, n, k)
-                continue
-            if s.neigh_ids is not None:
-                nrows = ops.gather_rows(src, s.neigh_ids[:n * k])
-            else:
-                nrows = src[s.neigh_row0:s.neigh_row0 + n * k]
-            hmax[s.out_row0:s.out_row0 + n] = self._pool(nrows, n, k)
-            if s.self_ids is not None:
-                ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
-            else:
-                xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
+            self._fused_hop(table, s, hmax[s.out_row0:s.out_row0 + s.n])
+        s0 = segments[0]
+        if len(segments) == 1 and s0.self_ids is None and s0.out_row0 == 0 and src.dtype == torch.float32:
+            xs = src[s0.self_row0:s0.self_row0 + s0.n]             # the self rows are already a dense fp32 row range
+        else:
+            F_in = src.shape[1]
+            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
+            for s in segments:
+                _rows(src, s.self_ids, s.self_row0, s.n, True, out=xs[s.out_row0:s.out_row0 + s.n])
         return self._finish([(xs, self.input_dim, self.vars["self_weights"]),
                              (hmax, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
 
@@ -376,17 +403,19 @@ class SeqAggregator(_SageAggregator):
         self.math = _DEFAULT_MATH[0]
         self.cell = LSTMCell(neigh_input_dim, hidden_dim, device=device)
 
-    def _combine(self):
-        return ops.COMBINE_CONCAT if self.concat else ops.COMBINE_ADD
-
-    def _neigh_hidden(self, X, n, k, out=None):
-        """h after len_i steps over the n sequences of k rows of X [n*k, neigh_input_dim]."""
+    def _neigh_hidden(self, X, n, k, out=None, kept=None):
+        """h after len_i steps over the n sequences of k rows of X [n*k, neigh_input_dim]; `kept` (training) receives X,
+        the lengths, the gates, c and h_{t-1}."""
         lengths = ops.seq_lengths(X, n, k)
         if getattr(self.cell, "_packed", None) is None:
             self.cell._packed = ops.PackedWeights()
         P = ops.sage_gemm([(X, self.neigh_input_dim, self.cell.W_x)], bias=self.cell.vars["bias"], math=self.math,
                           packed=self.cell._packed)
-        return ops.lstm_forward(P, self.cell.W_h, lengths, n, k, out=out)
+        if kept is None:
+            return ops.lstm_forward(P, self.cell.W_h, lengths, n, k, out=out)
+        h, gates, c, h_prev = ops.lstm_forward(P, self.cell.W_h, lengths, n, k, out=out, train=True)
+        kept += [X, lengths, gates, c, h_prev]
+        return h
 
     def _call(self, inputs):
         self_vecs, neigh_vecs = inputs
@@ -395,20 +424,10 @@ class SeqAggregator(_SageAggregator):
         return self._finish([(self_vecs, self.input_dim, self.vars["self_weights"]),
                              (h, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
 
-    def aggregate_rows(self, src, segments, final=None, src_persistent=False):
+    def _seq_parts(self, src, segments, kept=None):
         refuse_seq_table(src)
-        rows = max(s.out_row0 + s.n for s in segments)
-        F_in = src.shape[1]
-        xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
-        h = torch.empty((rows, self.hidden_dim), dtype=torch.float32, device=src.device)
-        for s in segments:
-            n, k = s.n, s.k
-            X = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
-                src[s.neigh_row0:s.neigh_row0 + n * k]
-            self._neigh_hidden(X, n, k, out=h[s.out_row0:s.out_row0 + n])
-            if s.self_ids is not None:
-                ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
-            else:
-                xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
-        return self._finish([(xs, self.input_dim, self.vars["self_weights"]),
-                             (h, self.hidden_dim, self.vars["neigh_weights"])], self._combine())
+        return self._summarise(src, segments, lambda i, s, out: self._neigh_hidden(
+            _rows(src, s.neigh_ids, s.neigh_row0, s.n * s.k), s.n, s.k, out=out, kept=kept))
+
+    def aggregate_rows(self, src, segments, final=None, src_persistent=False):
+        return self._finish(self._seq_parts(src, segments), self._combine())

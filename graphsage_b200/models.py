@@ -25,6 +25,22 @@ _AGGREGATORS = {"mean": MeanAggregator, "maxpool": MaxPoolingAggregator, "gcn": 
 _SIZED_AGGREGATORS = (MaxPoolingAggregator, SeqAggregator)       # take model_size (models.py:213-226)
 
 
+def layer_segments(samples, counts, num_samples, layer):
+    """The segments of one layer of the gather-fused recursion: hop h holds counts[h] rows from row sum(counts[:h]) on;
+    layer 0 reads its self and neighbour rows by the sampled ids, a later layer by row ranges of the previous output."""
+    L = len(num_samples)
+    hops = L - layer
+    row0 = [sum(counts[:h]) for h in range(hops + 1)]
+    segs = []
+    for hop in range(hops):
+        k = num_samples[L - hop - 1]                                             # models.py:324
+        if layer == 0:
+            segs.append(ops.Seg(counts[hop], k, self_ids=samples[hop], neigh_ids=samples[hop + 1], out_row0=row0[hop]))
+        else:
+            segs.append(ops.Seg(counts[hop], k, self_row0=row0[hop], neigh_row0=row0[hop + 1], out_row0=row0[hop]))
+    return segs
+
+
 class SampleAndAggregate(object):
     """The sample -> K-hop gather -> aggregate recursion of GraphSAGE (reference models.py:187-330).
 
@@ -170,23 +186,11 @@ class SampleAndAggregate(object):
         if any(getattr(a, "dropout", 0.) and not isinstance(a, SeqAggregator) for a in aggregators):
             return self._aggregate_materialised(samples, feats, dims, num_samples, support_sizes, batch_size,
                                                 aggregators, concat), aggregators
-        # gather-fused recursion: hop h of a layer occupies rows [row0[h], row0[h] + batch*support[h])
         counts = [batch_size * support_sizes[h] for h in range(L + 1)]
         src = feats
         for layer in range(L):
-            hops = L - layer
-            row0 = [sum(counts[:h]) for h in range(hops + 1)]
-            segs = []
-            for hop in range(hops):
-                k = num_samples[L - hop - 1]                                     # models.py:324
-                if layer == 0:
-                    segs.append(ops.Seg(counts[hop], k, self_ids=samples[hop], neigh_ids=samples[hop + 1],
-                                        out_row0=row0[hop]))
-                else:
-                    segs.append(ops.Seg(counts[hop], k, self_row0=row0[hop], neigh_row0=row0[hop + 1],
-                                        out_row0=row0[hop]))
-            src = aggregators[layer].aggregate_rows(src, segs, final=_final if layer == L - 1 else None,
-                                                    src_persistent=(layer == 0))
+            src = aggregators[layer].aggregate_rows(src, layer_segments(samples, counts, num_samples, layer),
+                                                    final=_final if layer == L - 1 else None, src_persistent=(layer == 0))
         return src[:counts[0]], aggregators
 
     def _aggregate_materialised(self, samples, feats, dims, num_samples, support_sizes, batch_size, aggregators,

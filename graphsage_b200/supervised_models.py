@@ -20,8 +20,8 @@ import torch
 from . import ops
 from .graphed_training import GraphedTrainStep
 from .layers import act_code, identity, relu  # noqa: F401
-from .aggregators import refuse_seq_table
-from .models import _SIZED_AGGREGATORS, SampleAndAggregate
+from .aggregators import FUSED_POOL_HIDDEN_STEP, FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, fused_pool_fits
+from .models import _SIZED_AGGREGATORS, SampleAndAggregate, layer_segments
 
 
 def _embedding_grad(emb_shape, lists, sites=None):
@@ -57,106 +57,6 @@ class _DropoutFn(torch.autograd.Function):
         return ops.dropout_apply(dy.contiguous(), ctx.site), None
 
 
-class _AggregateRowsFn(torch.autograd.Function):
-    """y = agg.aggregate_rows(src, segments) for MeanAggregator / GCNAggregator, differentiable w.r.t. the
-    aggregator weights, (for layers >= 1, where rows are addressed by ranges) w.r.t. src, and (layer 0, identity_dim > 0)
-    w.r.t. `emb`, the [N+1, d] embedding view of src's first d columns."""
-
-    @staticmethod
-    def forward(ctx, agg, src, segments, emb, sites, *weights):
-        """sites: None, or one (neighbour site, self site) pair of (seed, call, rate) per segment (training dropout);
-        xs / xm are then the dropped self rows and the mean of the dropped rows, which is what dW = X^T dZ needs."""
-        kind = "gcn" if "weights" in agg.vars else "mean"
-        code, post = act_code(agg.act)
-        if post is not None:
-            raise NotImplementedError("training supports act=relu or identity")
-        with torch.no_grad():
-            if sites is not None:
-                ns, ss = [p[0] for p in sites], [p[1] for p in sites]
-                xs, xm = ops.gather_mean_dropout(src, segments, ns, ss, include_self=kind == "gcn", want_self=kind == "mean")
-            elif kind == "mean":
-                xs, xm = ops.gather_mean(src, segments, want_self=True)
-            else:
-                xs, xm = None, ops.gather_mean(src, segments, include_self=True, want_self=False)[1]
-            F_in = src.shape[1]
-            if kind == "mean":
-                parts = [(xs, F_in, weights[0]), (xm, F_in, weights[1])]
-                combine = ops.COMBINE_CONCAT if agg.concat else ops.COMBINE_ADD
-            else:
-                parts, combine = [(xm, F_in, weights[0])], ops.COMBINE_ADD
-            y = ops.sage_gemm(parts, combine=combine, bias=agg.vars.get("bias"), act=code, math=agg.math)
-        ctx.kind, ctx.relu, ctx.concat = kind, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in, ctx.sites = segments, tuple(src.shape), F_in, sites
-        ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
-        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
-        ctx.has_bias = "bias" in agg.vars
-        ctx.save_for_backward(xm if xs is None else xs, xm, y, *weights)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xs, xm, y = ctx.saved_tensors[:3]
-        weights = ctx.saved_tensors[3:]
-        F_in = ctx.F_in
-        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
-        grads_w, dsrc = [], None
-        if ctx.kind == "mean":
-            Ws, Wn = weights
-            D = Ws.shape[1]
-            dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
-            grads_w = [xs[:, :F_in].t() @ dz_s, xm[:, :F_in].t() @ dz_n]         # dW = X^T dZ  (library GEMM)
-            if ctx.src_needs_grad:
-                dxs, dxm = dz_s @ Ws.t(), dz_n @ Wn.t()
-        else:
-            (W,) = weights
-            grads_w = [xm[:, :F_in].t() @ dz]
-            if ctx.src_needs_grad:
-                dxm = dz @ W.t()
-                dxs = None
-        if ctx.src_needs_grad:
-            dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device)
-            for si, s in enumerate(ctx.segments):
-                if s.self_ids is not None or s.neigh_ids is not None:
-                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
-                n, k = s.n, s.k
-                rows = slice(s.out_row0, s.out_row0 + n)
-                div = float(k + (1 if ctx.kind == "gcn" else 0))
-                if ctx.sites is not None:
-                    # the masks regenerated: neighbour row i*k + j gets mask * dxm[i] / div / keep, the self row mask * dxs[i]
-                    # (gcn: mask * dxm[i] / div); launched in this fixed order, so dsrc is reproducible
-                    nsite, ssite = ctx.sites[si]
-                    ops.dropout_apply(dxm[rows], nsite, rows=n * k, group=k, scale=1.0 / div, accumulate=True,
-                                      out=dsrc[s.neigh_row0:s.neigh_row0 + n * k])
-                    self_g, self_scale = (dxm[rows], 1.0 / div) if ctx.kind == "gcn" else (dxs[rows], 1.0)
-                    ops.dropout_apply(self_g, ssite, scale=self_scale, accumulate=True, out=dsrc[s.self_row0:s.self_row0 + n])
-                    continue
-                dsrc[s.neigh_row0:s.neigh_row0 + n * k].view(n, k, -1).add_((dxm[rows] / div).unsqueeze(1))
-                if ctx.kind == "gcn":
-                    dsrc[s.self_row0:s.self_row0 + n].add_(dxm[rows] / div)
-                else:
-                    dsrc[s.self_row0:s.self_row0 + n].add_(dxs[rows])
-        demb = None
-        if ctx.emb_shape is not None:
-            d = ctx.emb_shape[1]
-            # the source gradient restricted to the embedding columns: dZ @ W[:d]^T (feature columns are not trainable)
-            if ctx.kind == "mean":
-                es, em = dz_s @ weights[0][:d].t(), dz_n @ weights[1][:d].t()
-            else:
-                es, em = None, dz @ weights[0][:d].t()
-            lists, sites = [], ([] if ctx.sites is not None else None)
-            for si, s in enumerate(ctx.segments):
-                n, k = s.n, s.k
-                rows = slice(s.out_row0, s.out_row0 + n)
-                if ctx.kind == "gcn":                       # mean over [neighbours, self]: every id gets dxm / (k + 1)
-                    lists += [(s.self_ids[:n], em[rows], 1, 1.0 / (k + 1)), (s.neigh_ids[:n * k], em[rows], k, 1.0 / (k + 1))]
-                else:                                       # self id: dxs; neighbour ids: dxm / k
-                    lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], em[rows], k, 1.0 / k)]
-                if sites is not None:                       # entry i of a list is position i of its site
-                    sites += [ctx.sites[si][1], ctx.sites[si][0]]
-            demb = _embedding_grad(ctx.emb_shape, lists, sites)
-        return (None, dsrc, None, demb, None) + tuple(grads_w)
-
-
 def pool_branch_backward(pool, xn, h, hp, dhp, Wm, k, need_dx):
     """Gradients through hp = pool_k(h), h = relu(xn @ Wm + bm) for one hop (reference aggregators.py:176-182 /
     :256-262 backwards).  xn [n*k, F], h [n*k, hid] (post-ReLU), hp / dhp [n, hid].
@@ -176,173 +76,167 @@ def pool_branch_backward(pool, xn, h, hp, dhp, Wm, k, need_dx):
     return dWm, dbm, (dpre @ Wm.t() if need_dx else None)
 
 
-class _PoolAggregateRowsFn(torch.autograd.Function):
-    """y = agg.aggregate_rows(src, segments) for MaxPoolingAggregator / MeanPoolingAggregator on the unfused fp32 path
-    (gather -> Dense(relu, bias) -> pool over the fanout -> both matmuls), differentiable w.r.t. the four weight tensors
-    and (layers >= 1) src, and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of src's first d columns.
-    The gathered neighbour rows and the MLP activations are kept for the backward pass."""
+class _LayerFn(torch.autograd.Function):
+    """y = agg.aggregate_rows(src, segments) for one aggregator layer, differentiable w.r.t. the layer's parameters,
+    (layers >= 1, where rows are addressed by ranges) src, and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding
+    view of src's first d columns.  The per-kind work is the branch's (_AggregateRowsFn, _PoolAggregateRowsFn,
+    _FusedPoolAggregateRowsFn, _SeqAggregateRowsFn; their apply is the layer's entry): its forward gives the GEMM parts
+    y = act(concat_or_add(x_p @ W_p) + bias) combines, its backward turns the gradients of its parts' inputs into the
+    gradients of its own parameters and the source-row contributions _source_grads routes."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None, sites=None):
-        """sites: None, or one (seed, call, rate) per segment for the MLP input (training dropout, layers.py:107; the self
-        rows are not dropped); the kept xn is the dropped input, which is what dWm = xn^T dpre needs."""
+    def forward(ctx, branch, src, emb, *params):
+        agg = branch.agg
         code, post = act_code(agg.act)
         if post is not None:
             raise NotImplementedError("training supports act=relu or identity")
-        if len(agg.mlp_layers) != 1 or agg.dropout:
-            raise NotImplementedError("training supports one MLP layer and dropout = 0")
-        F_in, hid = src.shape[1], agg.hidden_dim
-        rows = max(s.out_row0 + s.n for s in segments)
         with torch.no_grad():
-            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
-            hp = torch.empty((rows, hid), dtype=torch.float32, device=src.device)
             kept = []
-            for si, s in enumerate(segments):
-                n, k = s.n, s.k
-                xn = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
-                    src[s.neigh_row0:s.neigh_row0 + n * k]
-                if sites is not None:                        # out of place: layer >= 1 rows belong to the previous layer
-                    xn = ops.dropout_apply(xn, sites[si])
-                mlp = agg.mlp_layers[0]
-                mlp.math = agg.math
-                h = mlp(xn)
-                if agg.pool == "mean":
-                    hp[s.out_row0:s.out_row0 + n] = ops.gather_mean(h, [ops.Seg(n, k)], want_self=False, out_pitch=hid)[1]
-                else:
-                    hp[s.out_row0:s.out_row0 + n] = ops.segment_max(h, n, k)
-                if s.self_ids is not None:
-                    ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
-                else:
-                    xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
-                kept.extend([xn, h])
-            y = agg._finish([(xs, agg.input_dim, Ws), (hp, hid, Wn)], agg._combine())
-        ctx.pool, ctx.relu, ctx.concat = agg.pool, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in, ctx.sites = segments, tuple(src.shape), F_in, sites
+            parts = branch.forward(src, kept)
+            y = agg._finish(parts, agg._combine())
+        ctx.branch, ctx.relu, ctx.concat = branch, code == ops.ACT_RELU, bool(agg.concat)
+        ctx.src_shape, ctx.F_in, ctx.Ks = tuple(src.shape), src.shape[1], [K for _, K, _ in parts]
         ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
         ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
-        ctx.save_for_backward(xs, hp, y, Ws, Wn, Wm, *kept)
+        ctx.n_params = len(params)
+        ctx.save_for_backward(*[x for x, _, _ in parts], y, *params, *kept)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        xs, hp, y, Ws, Wn, Wm = ctx.saved_tensors[:6]
-        kept = ctx.saved_tensors[6:]
-        F_in = ctx.F_in
+        P = len(ctx.Ks)
+        saved = ctx.saved_tensors
+        xs, y, params, kept = saved[:P], saved[P], saved[P + 1:P + 1 + ctx.n_params], saved[P + 1 + ctx.n_params:]
         dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
-        D = Ws.shape[1]
-        dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
-        dWs, dWn = xs.t() @ dz_s, hp.t() @ dz_n
-        dhp = dz_n @ Wn.t()
-        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dy.dtype, device=dy.device)
-        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
-        dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
-        emb = ctx.emb_shape is not None
-        d = ctx.emb_shape[1] if emb else 0
-        # the embedding columns only need dZ @ W[:d]^T (feature columns are not trainable)
-        es = dz_s @ Ws[:d].t() if emb else None
-        W_dx = Wm if ctx.src_needs_grad else Wm[:d]
-        lists = []
-        for i, s in enumerate(ctx.segments):
-            n, k = s.n, s.k
-            rows = slice(s.out_row0, s.out_row0 + n)
-            xn, h = kept[2 * i][:, :F_in], kept[2 * i + 1]
-            g_wm, g_bm, dxn = pool_branch_backward(ctx.pool, xn, h, hp[rows], dhp[rows], W_dx, k,
-                                                   ctx.src_needs_grad or emb)
+        D = params[0].shape[1]
+        dzs = (dz[:, :D], dz[:, D:]) if P == 2 and ctx.concat else (dz,) * P
+        grads_w = [x[:, :K].t() @ g for x, K, g in zip(xs, ctx.Ks, dzs)]           # dW = X^T dZ  (library GEMM)
+        # the source rows need dX = dZ W^T: every column for a previous layer, only the embedding columns [0, d) of the
+        # layer-0 table (feature columns are not trainable); a part the branch computes itself always needs all of it
+        cols = ctx.F_in if ctx.src_needs_grad else ctx.emb_shape[1] if ctx.emb_shape is not None else 0
+        dxs = [g @ W.t() if p >= ctx.branch.row_parts else g @ W[:cols].t() if cols else None
+               for p, (g, W) in enumerate(zip(dzs, params))]
+        grads_own, contribs = ctx.branch.backward(xs, dxs, params[P:], kept, cols)
+        dsrc, demb = _source_grads(ctx, contribs, dy)
+        return (None, dsrc, demb) + tuple(grads_w) + tuple(grads_own)
+
+
+def _source_grads(ctx, contribs, dy):
+    """contribs: per segment (s, self contribution, neighbour contribution), each (grad rows, group, divisor, dropout site
+    or None): row r of s's self (neighbour) rows receives drop(grad[r // group] / divisor).  A layer >= 1 source takes
+    them into its row ranges, neighbour rows first, launched in this fixed order so dsrc is reproducible; the layer-0
+    embedding table through _embedding_grad, [self, neighbour] lists per segment."""
+    dsrc = demb = None
+    if ctx.src_needs_grad:
+        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device)
+        for s, cself, cneigh in contribs:
+            if s.self_ids is not None or s.neigh_ids is not None:
+                raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
+            for row0, rows, (g, group, div, site) in ((s.neigh_row0, s.n * s.k, cneigh), (s.self_row0, s.n, cself)):
+                out = dsrc[row0:row0 + rows]
+                if site is not None:                    # the mask regenerated
+                    ops.dropout_apply(g, site, rows=rows, group=group, scale=1.0 / div, accumulate=True, out=out)
+                else:
+                    out.view(rows // group, group, ctx.src_shape[1]).add_((g / div if div != 1 else g).unsqueeze(1))
+    if ctx.emb_shape is not None:
+        d = ctx.emb_shape[1]
+        lists, sites = [], []
+        for s, cself, cneigh in contribs:
+            for ids, rows, (g, group, div, site) in ((s.self_ids, s.n, cself), (s.neigh_ids, s.n * s.k, cneigh)):
+                lists.append((ids[:rows], g[:, :d], group, 1.0 / div))
+                sites.append(site)                      # entry i of a list is position i of its site
+        demb = _embedding_grad(ctx.emb_shape, lists, sites if any(x is not None for x in sites) else None)
+    return dsrc, demb
+
+
+class _AggregateRowsFn(object):
+    """The _LayerFn branch of MeanAggregator / GCNAggregator: the fused gather gives the self rows and the fanout mean, or
+    for GCN the mean over the k neighbours and the node itself.  sites: None, or one (neighbour site, self site) pair of
+    (seed, call, rate) per segment (training dropout): the gather then drops the rows it reads, so the parts are what
+    dW = X^T dZ needs."""
+
+    @staticmethod
+    def apply(agg, src, segments, emb, sites, *weights):
+        """weights: agg's [weights] (GCN) or [self_weights, neigh_weights]."""
+        return _LayerFn.apply(_AggregateRowsFn(agg, segments, sites), src, emb, *weights)
+
+    def __init__(self, agg, segments, sites):
+        self.agg, self.segments, self.sites = agg, segments, sites
+        self.gcn = "weights" in agg.vars
+        self.row_parts = 1 if self.gcn else 2
+
+    def forward(self, src, kept):
+        if self.sites is not None:
+            ns, ss = [p[0] for p in self.sites], [p[1] for p in self.sites]
+            xs, xm = ops.gather_mean_dropout(src, self.segments, ns, ss, include_self=self.gcn, want_self=not self.gcn)
+        else:
+            xs, xm = ops.gather_mean(src, self.segments, include_self=self.gcn, want_self=not self.gcn)
+        F_in, v = src.shape[1], self.agg.vars
+        if self.gcn:
+            return [(xm, F_in, v["weights"])]
+        return [(xs, F_in, v["self_weights"]), (xm, F_in, v["neigh_weights"])]
+
+    def backward(self, xs, dxs, params, kept, cols):
+        if not cols:
+            return [], []
+        dxm = dxs[-1]
+        contribs = []
+        for i, s in enumerate(self.segments):
+            rows = slice(s.out_row0, s.out_row0 + s.n)
+            nsite, ssite = self.sites[i] if self.sites is not None else (None, None)
+            div = float(s.k + (1 if self.gcn else 0))   # gcn: every row of the mean over [neighbours, self] gets dxm / (k + 1)
+            cself = (dxm[rows], 1, div, ssite) if self.gcn else (dxs[0][rows], 1, 1, ssite)
+            contribs.append((s, cself, (dxm[rows], s.k, div, nsite)))
+        return [], contribs
+
+
+class _SummaryBranch(object):
+    """The _LayerFn branches of the pools and seq: parts [self rows, per-hop neighbour summary]; the self rows receive
+    dZ_s Ws^T.  Their apply takes agg's self_weights, neigh_weights and the two tensors of the summary's own layer."""
+    row_parts = 1
+
+    def __init__(self, agg, segments):
+        self.agg, self.segments = agg, segments
+
+    def _contribs(self, dxs, neigh_grads):
+        return [(s, (dxs[s.out_row0:s.out_row0 + s.n], 1, 1, None), (g, 1, 1, None))
+                for s, g in zip(self.segments, neigh_grads)]
+
+
+class _PoolAggregateRowsFn(_SummaryBranch):
+    """MaxPoolingAggregator / MeanPoolingAggregator, materialised on the fp32 kernels: gather -> Dense(relu, bias) ->
+    pool over the fanout, keeping the gathered neighbour rows and the MLP activations for pool_branch_backward.
+    sites: None, or one (seed, call, rate) per segment for the MLP input (training dropout, layers.py:107; the self rows
+    are not dropped); the kept rows are the dropped input, which is what dWm = xn^T dpre needs."""
+
+    @staticmethod
+    def apply(agg, src, segments, Ws, Wn, Wm, bm, emb=None, sites=None):
+        return _LayerFn.apply(_PoolAggregateRowsFn(agg, segments, sites), src, emb, Ws, Wn, Wm, bm)
+
+    def __init__(self, agg, segments, sites):
+        _SummaryBranch.__init__(self, agg, segments)
+        self.sites = sites
+
+    def forward(self, src, kept):
+        if len(self.agg.mlp_layers) != 1 or self.agg.dropout:
+            raise NotImplementedError("training supports one MLP layer and dropout = 0")
+        self.F_in = src.shape[1]
+        return self.agg._pooled_parts(src, self.segments, kept, self.sites)
+
+    def backward(self, xs, dxs, params, kept, cols):
+        (Wm, _), hp, dhp = params, xs[1], dxs[1]
+        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dhp.dtype, device=dhp.device)
+        dxn_all = []
+        for i, s in enumerate(self.segments):
+            rows = slice(s.out_row0, s.out_row0 + s.n)
+            xn, h = kept[2 * i][:, :self.F_in], kept[2 * i + 1]
+            g_wm, g_bm, dxn = pool_branch_backward(self.agg.pool, xn, h, hp[rows], dhp[rows], Wm[:cols], s.k, cols > 0)
             dWm += g_wm
             dbm += g_bm
-            if dxn is not None and ctx.sites is not None:    # through the input mask, regenerated
-                dxn = ops.dropout_apply(dxn, ctx.sites[i])
-            if emb:                                          # self id: dxs; neighbour id of gathered row r: dxn[r]
-                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dxn[:, :d], 1, 1.0)]
-            if ctx.src_needs_grad:
-                if s.self_ids is not None or s.neigh_ids is not None:
-                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
-                dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dxn
-                dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
-        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
-        return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
-
-
-class _SeqAggregateRowsFn(torch.autograd.Function):
-    """y = agg.aggregate_rows(src, segments) for SeqAggregator, differentiable w.r.t. Ws, Wn, the cell's kernel and bias,
-    (layers >= 1) src and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of src's first d columns.
-    Forward per hop: X (gathered rows, or the previous layer's row range) -> lengths (gs_seq_lengths) -> P = X W_x + b
-    (library GEMM, agg.math) -> gs_lstm_forward, keeping X, the lengths, the gates, c and h_{t-1}.  Backward per hop:
-    gs_lstm_backward gives dZ; dW_x = X^T dZ, dW_h = h_prev^T dZ, db = sum dZ and dX = dZ W_x^T are library matmuls."""
-
-    @staticmethod
-    def forward(ctx, agg, src, segments, Ws, Wn, kernel, cell_bias, emb=None):
-        code, post = act_code(agg.act)
-        if post is not None:
-            raise NotImplementedError("training supports act=relu or identity")
-        refuse_seq_table(src)
-        F_in, H = src.shape[1], agg.hidden_dim
-        rows = max(s.out_row0 + s.n for s in segments)
-        with torch.no_grad():
-            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
-            hl = torch.empty((rows, H), dtype=torch.float32, device=src.device)
-            Wx, Wh = kernel[:F_in], kernel[F_in:]
-            kept = []
-            for s in segments:
-                n, k = s.n, s.k
-                X = ops.gather_rows(src, s.neigh_ids[:n * k]) if s.neigh_ids is not None else \
-                    src[s.neigh_row0:s.neigh_row0 + n * k]
-                lengths = ops.seq_lengths(X, n, k)
-                P = ops.sage_gemm([(X, F_in, Wx)], bias=cell_bias, math=agg.math)
-                _, gates, c, h_prev = ops.lstm_forward(P, Wh, lengths, n, k, out=hl[s.out_row0:s.out_row0 + n], train=True)
-                del P
-                if s.self_ids is not None:
-                    ops.gather_rows(src, s.self_ids[:n], out=xs[s.out_row0:s.out_row0 + n])
-                else:
-                    xs[s.out_row0:s.out_row0 + n] = src[s.self_row0:s.self_row0 + n]
-                kept.extend([X, lengths, gates, c, h_prev])
-            y = agg._finish([(xs, agg.input_dim, Ws), (hl, H, Wn)], agg._combine())
-        ctx.relu, ctx.concat = code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
-        ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
-        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
-        ctx.save_for_backward(xs, hl, y, Ws, Wn, kernel, *kept)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xs, hl, y, Ws, Wn, kernel = ctx.saved_tensors[:6]
-        kept = ctx.saved_tensors[6:]
-        F_in = ctx.F_in
-        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
-        D = Ws.shape[1]
-        dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
-        dWs, dWn = xs.t() @ dz_s, hl.t() @ dz_n
-        dhl = (dz_n @ Wn.t()).contiguous()
-        Wx, Wh = kernel[:F_in], kernel[F_in:]
-        dWx, dWh = torch.zeros_like(Wx), torch.zeros_like(Wh)
-        db = torch.zeros(kernel.shape[1], dtype=dy.dtype, device=dy.device)
-        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
-        dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
-        emb = ctx.emb_shape is not None
-        d = ctx.emb_shape[1] if emb else 0
-        es = dz_s @ Ws[:d].t() if emb else None          # the embedding columns only need dZ @ W[:d]^T
-        lists = []
-        for i, s in enumerate(ctx.segments):
-            n, k = s.n, s.k
-            rows = slice(s.out_row0, s.out_row0 + n)
-            X, lengths, gates, c, h_prev = kept[5 * i:5 * i + 5]
-            dZ = ops.lstm_backward(dhl[rows], gates, c, lengths, Wh, n, k)
-            dWx += X.t() @ dZ
-            dWh += h_prev.t() @ dZ
-            db += dZ.sum(dim=0)
-            if emb:                                      # self id: dxs; neighbour id of gathered row r: dX[r]
-                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dZ @ Wx[:d].t(), 1, 1.0)]
-            if ctx.src_needs_grad:
-                if s.self_ids is not None or s.neigh_ids is not None:
-                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
-                dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dZ @ Wx.t()
-                dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
-        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
-        return None, dsrc, None, dWs, dWn, torch.cat([dWx, dWh]), db, demb
-
-
-FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K = 128, 640       # K4's limits (include/graphsage_b200.h)
+            if dxn is not None and self.sites is not None:    # through the input mask, regenerated
+                dxn = ops.dropout_apply(dxn, self.sites[i])
+            dxn_all.append(dxn)
+        return [dWm, dbm], (self._contribs(dxs[0], dxn_all) if cols else [])
 
 
 def refuse_fused_pool(model):
@@ -363,95 +257,106 @@ def refuse_fused_pool(model):
         if agg.neigh_input_dim > FUSED_POOL_MAX_K:
             raise NotImplementedError("fused_pool=True needs layer input widths <= %d (got %d)"
                                       % (FUSED_POOL_MAX_K, agg.neigh_input_dim))
-        if agg.hidden_dim % 128 != 0:
-            raise NotImplementedError("fused_pool=True needs a pooling hidden width that is a multiple of 128 (got %d)"
-                                      % agg.hidden_dim)
+        if agg.hidden_dim % FUSED_POOL_HIDDEN_STEP != 0:
+            raise NotImplementedError("fused_pool=True needs a pooling hidden width that is a multiple of %d (got %d)"
+                                      % (FUSED_POOL_HIDDEN_STEP, agg.hidden_dim))
         if len(agg.mlp_layers) != 1:
             raise NotImplementedError("fused_pool=True supports one MLP layer")
 
 
-class _FusedPoolAggregateRowsFn(torch.autograd.Function):
-    """y = agg.aggregate_rows(src, segments) for MaxPoolingAggregator / MeanPoolingAggregator through the fused bf16
-    kernels (fused_pool=True): the pooled branch is K4 (ops.maxpool_mlp_fused) in the forward; the backward recomputes
-    the MLP tile instead of storing it (B1 ops.pool_mlp_backward_dp), then dWm / dbm (B2) and, where a source gradient
-    is needed, dX (B3).  bf16 operands with fp32 accumulation whatever agg.math is; the self branch and the Ws / Wn
-    gradients are those of _PoolAggregateRowsFn.  Saved: the self rows, the pooled rows, y, the weights and the bf16
-    operand table - neither the gathered neighbour rows nor the MLP activations."""
+class _FusedPoolAggregateRowsFn(_SummaryBranch):
+    """MaxPoolingAggregator / MeanPoolingAggregator through the fused bf16 kernels (fused_pool=True): K4
+    (ops.maxpool_mlp_fused) in the forward; the backward recomputes the MLP tile instead of storing it (B1
+    ops.pool_mlp_backward_dp), then dWm / dbm (B2) and, where a source gradient is needed, dX (B3).  bf16 operands with
+    fp32 accumulation whatever agg.math is.  Kept: the bf16 operand table - neither the gathered neighbour rows nor the
+    MLP activations.  persistent: src is the model's feature table (layer 0), cast to bf16 once per table version; a
+    layer >= 1 source is cast on every call."""
 
     @staticmethod
-    def forward(ctx, agg, src, segments, Ws, Wn, Wm, bm, emb=None, persistent=False):
-        """persistent: src is the model's feature table (layer 0), cast to bf16 once per table version; a layer >= 1
-        source is cast on every call and the cast is kept for the backward."""
-        code, post = act_code(agg.act)
-        if post is not None:
-            raise NotImplementedError("training supports act=relu or identity")
+    def apply(agg, src, segments, Ws, Wn, Wm, bm, emb=None, persistent=False):
+        return _LayerFn.apply(_FusedPoolAggregateRowsFn(agg, segments, persistent), src, emb, Ws, Wn, Wm, bm)
+
+    def __init__(self, agg, segments, persistent):
+        _SummaryBranch.__init__(self, agg, segments)
+        self.persistent = persistent
+
+    def forward(self, src, kept):
+        agg = self.agg
         if hasattr(src, "c_table"):
             raise NotImplementedError("fused_pool=True with a node-partitioned (ShardedFeatures) table is not implemented")
         F_in, hid = src.shape[1], agg.hidden_dim
-        for s in segments:
-            if s.k > FUSED_POOL_MAX_FANOUT or F_in > FUSED_POOL_MAX_K or hid % 128 != 0:
-                raise NotImplementedError("fused_pool=True needs fanout <= %d, input width <= %d and hidden %% 128 == 0 "
-                                          "(k=%d K=%d hidden=%d)" % (FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, s.k, F_in, hid))
-        rows = max(s.out_row0 + s.n for s in segments)
-        with torch.no_grad():
-            table = agg._bf16_table(src, persistent)
-            if getattr(agg, "_packed_mlp", None) is None:
-                agg._packed_mlp = ops.PackedMlpWeights()
-            hp = torch.empty((rows, hid), dtype=torch.float32, device=src.device)
-            xs = torch.empty((rows, ops.pad_cols(F_in)), dtype=torch.float32, device=src.device)[:, :F_in]
-            for s in segments:
-                ops.maxpool_mlp_fused(table, s.n, s.k, Wm, bm, agg._packed_mlp, row_ids=s.neigh_ids, row0=s.neigh_row0,
-                                      K=F_in, out=hp[s.out_row0:s.out_row0 + s.n], pool=agg.pool)
-                ops.gather_rows_f32(src, ids=None if s.self_ids is None else s.self_ids[:s.n], row0=s.self_row0, n=s.n,
-                                    out=xs[s.out_row0:s.out_row0 + s.n])
-            y = agg._finish([(xs, agg.input_dim, Ws), (hp, hid, Wn)], agg._combine())
-        ctx.agg, ctx.relu, ctx.concat = agg, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.segments, ctx.src_shape, ctx.F_in = segments, tuple(src.shape), F_in
-        ctx.src_needs_grad = bool(torch.is_tensor(src) and src.requires_grad)
-        ctx.emb_shape = tuple(emb.shape) if emb is not None and emb.requires_grad else None
-        ctx.save_for_backward(xs, hp, y, Ws, Wn, Wm, bm, table)
-        return y
+        for s in self.segments:
+            if not fused_pool_fits(s.k, F_in, hid):
+                raise NotImplementedError("fused_pool=True needs fanout <= %d, input width <= %d and hidden %% %d == 0 "
+                                          "(k=%d K=%d hidden=%d)" % (FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K,
+                                                                     FUSED_POOL_HIDDEN_STEP, s.k, F_in, hid))
+        self.F_in = F_in
+        table = agg._bf16_table(src, self.persistent)
+        kept.append(table)
+        return agg._summarise(src, self.segments, lambda i, s, out: agg._fused_hop(table, s, out), f32_self=True)
+
+    def backward(self, xs, dxs, params, kept, cols):
+        (Wm, bm), dhp, (table,), agg = params, dxs[1], kept, self.agg
+        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dhp.dtype, device=dhp.device)
+        if cols and (getattr(agg, "_packed_dx", None) is None or agg._packed_dx.cols != cols):
+            agg._packed_dx = ops.PackedMlpDxWeights(cols)
+        dxn_all = []
+        for s in self.segments:                               # per hop, in order: B1 -> B2 (dWm, dbm) -> B3
+            n, k = s.n, s.k
+            grad = ops.pool_mlp_backward_dp(table, n, k, Wm, bm, agg._packed_mlp, dhp[s.out_row0:s.out_row0 + n],
+                                            row_ids=s.neigh_ids, row0=s.neigh_row0, K=self.F_in, pool=agg.pool)
+            ops.pool_mlp_backward_dw(table, n, k, grad, dWm, dbm, row_ids=s.neigh_ids, row0=s.neigh_row0, K=self.F_in)
+            if cols:
+                dxn_all.append(ops.pool_mlp_backward_dx(grad, n, k, Wm, agg._packed_dx))
+        return [dWm, dbm], (self._contribs(dxs[0], dxn_all) if cols else [])
+
+
+class _SeqAggregateRowsFn(_SummaryBranch):
+    """SeqAggregator.  Forward per hop: X (gathered rows, or the previous layer's row range) -> lengths (gs_seq_lengths)
+    -> P = X W_x + b (library GEMM, agg.math) -> gs_lstm_forward, keeping X, the lengths, the gates, c and h_{t-1}.
+    Backward per hop: gs_lstm_backward gives dZ; dW_x = X^T dZ, dW_h = h_prev^T dZ, db = sum dZ and dX = dZ W_x^T are
+    library matmuls."""
 
     @staticmethod
-    def backward(ctx, dy):
-        xs, hp, y, Ws, Wn, Wm, bm, table = ctx.saved_tensors
-        agg, F_in = ctx.agg, ctx.F_in
-        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
-        D = Ws.shape[1]
-        dz_s, dz_n = (dz[:, :D], dz[:, D:]) if ctx.concat else (dz, dz)
-        dWs, dWn = xs.t() @ dz_s, hp.t() @ dz_n
-        dhp = (dz_n @ Wn.t()).contiguous()
-        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dy.dtype, device=dy.device)
-        dsrc = torch.zeros(ctx.src_shape, dtype=dy.dtype, device=dy.device) if ctx.src_needs_grad else None
-        dxs = dz_s @ Ws.t() if ctx.src_needs_grad else None
-        emb = ctx.emb_shape is not None
-        d = ctx.emb_shape[1] if emb else 0
-        es = dz_s @ Ws[:d].t() if emb else None
-        packed_dx = None
-        if ctx.src_needs_grad or emb:                        # dX columns: all of them for a previous layer, else [0, d)
-            cols = F_in if ctx.src_needs_grad else d
-            if getattr(agg, "_packed_dx", None) is None or agg._packed_dx.cols != cols:
-                agg._packed_dx = ops.PackedMlpDxWeights(cols)
-            packed_dx = agg._packed_dx
-        lists = []
-        for s in ctx.segments:                               # per hop, in order: B1 -> B2 (dWm, dbm) -> B3
-            n, k = s.n, s.k
-            rows = slice(s.out_row0, s.out_row0 + n)
-            grad = ops.pool_mlp_backward_dp(table, n, k, Wm, bm, agg._packed_mlp, dhp[rows], row_ids=s.neigh_ids,
-                                            row0=s.neigh_row0, K=F_in, pool=agg.pool)
-            ops.pool_mlp_backward_dw(table, n, k, grad, dWm, dbm, row_ids=s.neigh_ids, row0=s.neigh_row0, K=F_in)
-            if packed_dx is None:
-                continue
-            dxn = ops.pool_mlp_backward_dx(grad, n, k, Wm, packed_dx)
-            if emb:                                          # self id: dxs; neighbour id of gathered row r: dxn[r]
-                lists += [(s.self_ids[:n], es[rows], 1, 1.0), (s.neigh_ids[:n * k], dxn[:, :d], 1, 1.0)]
-            if ctx.src_needs_grad:
-                if s.self_ids is not None or s.neigh_ids is not None:
-                    raise NotImplementedError("gradient w.r.t. an id-addressed source (trainable features) is out of scope")
-                dsrc[s.neigh_row0:s.neigh_row0 + n * k] += dxn
-                dsrc[s.self_row0:s.self_row0 + n] += dxs[rows]
-        demb = _embedding_grad(ctx.emb_shape, lists) if emb else None
-        return None, dsrc, None, dWs, dWn, dWm, dbm, demb, None
+    def apply(agg, src, segments, Ws, Wn, kernel, cell_bias, emb=None):
+        return _LayerFn.apply(_SeqAggregateRowsFn(agg, segments), src, emb, Ws, Wn, kernel, cell_bias)
+
+    def forward(self, src, kept):
+        self.F_in = src.shape[1]
+        return self.agg._seq_parts(src, self.segments, kept)
+
+    def backward(self, xs, dxs, params, kept, cols):
+        kernel, dhl = params[0], dxs[1]
+        Wx, Wh = kernel[:self.F_in], kernel[self.F_in:]
+        dWx, dWh = torch.zeros_like(Wx), torch.zeros_like(Wh)
+        db = torch.zeros(kernel.shape[1], dtype=dhl.dtype, device=dhl.device)
+        dX_all = []
+        for i, s in enumerate(self.segments):
+            X, lengths, gates, c, h_prev = kept[5 * i:5 * i + 5]
+            dZ = ops.lstm_backward(dhl[s.out_row0:s.out_row0 + s.n], gates, c, lengths, Wh, s.n, s.k)
+            dWx += X.t() @ dZ
+            dWh += h_prev.t() @ dZ
+            db += dZ.sum(dim=0)
+            if cols:
+                dX_all.append(dZ @ Wx[:cols].t())
+        return [torch.cat([dWx, dWh]), db], (self._contribs(dxs[0], dX_all) if cols else [])
+
+
+def train_layer(agg, src, segments, emb=None, sites=None, fused=False, persistent=False):
+    """agg.aggregate_rows(src, segments) with an autograd graph (_LayerFn): through the seq, the materialised or (fused)
+    the fused bf16 pooling branch, or the mean / GCN one.  sites: training dropout of the mean / GCN and materialised
+    pooling branches (see their classes); persistent: src is the model's layer-0 feature table."""
+    v = agg.vars
+    if hasattr(agg, "cell"):
+        cell = agg.cell.vars
+        return _SeqAggregateRowsFn.apply(agg, src, segments, v["self_weights"], v["neigh_weights"], cell["kernel"],
+                                         cell["bias"], emb)
+    if hasattr(agg, "mlp_layers"):
+        mlp = agg.mlp_layers[0].vars
+        fn, extra = (_FusedPoolAggregateRowsFn, persistent) if fused else (_PoolAggregateRowsFn, sites)
+        return fn.apply(agg, src, segments, v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"], emb, extra)
+    ws = (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
+    return _AggregateRowsFn.apply(agg, src, segments, emb, sites, *ws)
 
 
 def differentiable_outputs(model, batch, normalize=True, dropout=0.):
@@ -481,17 +386,6 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     call = {site: model.dropout_counter + i for i, site in enumerate(plan)}
     for layer in range(L):
         hops = L - layer
-        row0 = [sum(counts[:h]) for h in range(hops + 1)]
-        segs = []
-        for hop in range(hops):
-            k = num_samples[L - hop - 1]
-            if layer == 0:
-                segs.append(ops.Seg(counts[hop], k, self_ids=samples[hop], neigh_ids=samples[hop + 1],
-                                    out_row0=row0[hop]))
-            else:
-                segs.append(ops.Seg(counts[hop], k, self_row0=row0[hop], neigh_row0=row0[hop + 1],
-                                    out_row0=row0[hop]))
-        agg = model.aggregators[layer]
         # layer 0 reads the embedding table (identity_dim > 0) through src; handing it over as an input lets autograd
         # deliver the scattered gradient as embeds.grad
         emb = getattr(model, "embeds", None) if layer == 0 else None
@@ -503,21 +397,8 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
             else:
                 sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
                          for h in range(hops)]
-        if seq:                                              # LSTM: draws no dropout mask
-            cell = agg.cell.vars
-            src = _SeqAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
-                                            cell["kernel"], cell["bias"], emb)
-        elif pool and fused:                                 # max-pool / mean-pool through the bf16 kernels
-            mlp = agg.mlp_layers[0].vars
-            src = _FusedPoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
-                                                  mlp["weights"], mlp["bias"], emb, layer == 0)
-        elif pool:                                           # max-pool / mean-pool
-            mlp = agg.mlp_layers[0].vars
-            src = _PoolAggregateRowsFn.apply(agg, src, segs, agg.vars["self_weights"], agg.vars["neigh_weights"],
-                                             mlp["weights"], mlp["bias"], emb, sites)
-        else:
-            ws = (agg.vars["weights"],) if "weights" in agg.vars else (agg.vars["self_weights"], agg.vars["neigh_weights"])
-            src = _AggregateRowsFn.apply(agg, src, segs, emb, sites, *ws)
+        src = train_layer(model.aggregators[layer], src, layer_segments(samples, counts, num_samples, layer), emb, sites,
+                          fused, layer == 0)
     model.dropout_counter += len(plan)
     out = src[:counts[0]]
     if normalize:
