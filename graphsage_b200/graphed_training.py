@@ -109,9 +109,10 @@ class GraphedTrainStep(object):
                     setattr(o, d, None)                         # eager calls keep the host-numbered sequence
         torch.cuda.current_stream(dev).wait_stream(self.stream)
         ops.CACHE_EPOCH[0] += 1                                 # the restore changed the weights behind the caches' keys
-        # what the step leaves on the model for mrr() (the affinities) and neg_samples: the graph's tensors, re-bound after
-        # every replay because an eager step in between binds its own
-        self.bound = {k: getattr(model, k) for k in ("_last", "neg_samples") if getattr(model, k, None) is not None}
+        # what the step leaves on the model for mrr() (the affinities), last_predictions() (the logits) and neg_samples:
+        # the graph's tensors, re-bound after every replay because an eager step in between binds its own
+        self.bound = {k: getattr(model, k) for k in ("_last", "_last_logits", "neg_samples")
+                      if getattr(model, k, None) is not None}
         self.replays = 0
 
     def _snapshot(self, optimizer):

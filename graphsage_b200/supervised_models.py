@@ -555,6 +555,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         """supervised_models.py:101-118: weight decay * l2_loss(var) over aggregator + head variables, then the
         mean of the per-element sigmoid xent (multi-label) or the mean of the per-node softmax xent."""
         logits = self.logits(batch, dropout=dropout) if dropout else self.logits(batch)    # overrides take (batch)
+        self._last_logits = logits.detach()
         labels = labels.to(device=logits.device, dtype=torch.float32)
         loss = classification_loss(logits, labels, self.sigmoid_loss)
         if self.weight_decay:
@@ -582,5 +583,14 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def predict(self, batch):
         with torch.no_grad():
-            lg = self.logits(batch)
-            return torch.sigmoid(lg) if self.sigmoid_loss else torch.softmax(lg, dim=1)
+            return self._predictions(self.logits(batch))
+
+    def last_predictions(self):
+        """model.preds of the last loss() / train_step() call (supervised_models.py:120-126): the predictions from that
+        call's own logits - before its update, at its dropout rate - without another forward pass (which would draw new
+        samples and masks).  After a replay of graphed_train_step, the replay's."""
+        with torch.no_grad():
+            return self._predictions(self._last_logits)
+
+    def _predictions(self, logits):
+        return torch.sigmoid(logits) if self.sigmoid_loss else torch.softmax(logits, dim=1)
