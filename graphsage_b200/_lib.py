@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgraphsage_b200.so")
 
 ABI_VERSION = 2          # GS_ABI_VERSION of include/graphsage_b200.h this binding was written against
-GS_F32, GS_BF16 = 0, 1
+GS_F32, GS_BF16, GS_F64 = 0, 1, 2
 ACT_NONE, ACT_RELU = 0, 1
 COMBINE_ADD, COMBINE_CONCAT = 0, 1
 MATH_FP32_SIMT, MATH_TF32X3, MATH_TF32, MATH_BF16 = 0, 1, 2, 3
@@ -135,6 +135,9 @@ _SIGNATURES = {
     "gs_skipgram_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32]),
     "gs_skipgram_grad": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,
                                  c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "gs_sgd_orders": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_vp, c_vp]),
+    "gs_sgd_fit": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, ctypes.c_double, ctypes.c_double,
+                           c_vp, c_i64, c_vp, c_vp]),
 }
 
 _lib = None

@@ -35,7 +35,7 @@ typedef enum {
   GS_ERR_UNSUPPORTED = -3
 } gs_status;
 
-typedef enum { GS_F32 = 0, GS_BF16 = 1 } gs_dtype;
+typedef enum { GS_F32 = 0, GS_BF16 = 1, GS_F64 = 2 } gs_dtype;   /* GS_F64: gs_sgd_fit's X only */
 typedef enum { GS_ACT_NONE = 0, GS_ACT_RELU = 1 } gs_act;
 /* how the neighbour part and the self part are combined */
 typedef enum {
@@ -561,6 +561,42 @@ int32_t gs_lstm_forward(const float* P, int64_t ldp, const float* Wh, int64_t ld
 int32_t gs_lstm_backward(const float* dh_last, int64_t lddh, const float* gates, int64_t ldg, const float* c, int64_t ldc,
                          const int32_t* len, const float* Wh, int64_t ldw, int64_t n, int32_t k, int32_t H, float* dZ,
                          int64_t ldz, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The logistic classifier of the reference's eval scripts (eval_scripts/{ppi,reddit,citation}_eval.py:
+ * SGDClassifier(loss="log")): scikit-learn's plain SGD loop (_sgd_fast.pyx.tp, _plain_sgd) for the log loss, an L2
+ * penalty alpha, an intercept, the "optimal" learning rate, no averaging and no class or sample weights, in fp64, over P
+ * independent binary problems that share one X.  Contract: oracle/sgd.py.  Neither entry needs a workspace.
+ *
+ * gs_sgd_orders - the sample order of every epoch.  Problem p's permutation sigma is the Fisher-Yates shuffle of arange(n)
+ *   with our_rand_r (xorshift32; a zero state becomes 1; draw = state % 2^31) from seeds[p] (device uint32 [P]):
+ *   for i < n - 1: j = i + draw % (n - i); swap(ind[i], ind[j]).  scikit-learn passes the seed by value, so every epoch
+ *   applies the same swaps to the previous epoch's order:  orders[p, 0, k] = sigma[k],
+ *   orders[p, e, k] = sigma[orders[p, e - 1, k]].  orders is int32 [P, epochs, n].  sigma is one sequential chain per
+ *   problem (one thread); the later epochs are a parallel gather.
+ * gs_sgd_fit - problem p learns w (d fp64 weights, wscale = 1) and b = 0 from X [n, d] (row stride ldx, GS_F32 or GS_F64,
+ *   every element widened exactly to fp64) with labels[p * ldy + row] (> 0: positive, else negative; y = 1 or 0) in
+ *   the order orders[p] (all epochs, t = 1, 2, ... across epochs):
+ *     pred   = fl(dot * wscale) + b                       dot: see below
+ *     eta    = 1 / (alpha * ((optimal_init + t) - 1))
+ *     g      = ((1 - y) - y e) / (1 + e), e = exp(-pred)   if pred > -37, else exp(pred) - y; clipped to +-1e12
+ *     update = -eta * g
+ *     wscale = wscale * max(0, 1 - eta * alpha);  wscale < 1e-9: w = wscale * w, wscale = 1
+ *     update != 0:  w = w + x * (update / wscale),  b = b + update
+ *   coef[p * ldc + j] = wscale * w[j] (fp64), intercept[p] = b.  Every product and sum is rounded separately (no FMA).
+ *   Dot-product order: lane l (0..31) sums w[j] * x[j] for j = l, l + 32, l + 64, ... (< d) left to right from 0.0; the 32
+ *   partial sums are then combined by the xor butterfly v += shuffle_xor(v, m) for m = 16, 8, 4, 2, 1.  exp is CUDA's
+ *   double exp (not correctly rounded): results are close to, not bit-identical with, a correctly rounded restatement.
+ *   One warp per problem with w in registers; the rows of upcoming steps are prefetched with cp.async into a shared ring.
+ * Limits (else GS_ERR_UNSUPPORTED): d <= GS_SGD_MAX_D, P <= GS_SGD_MAX_PROBLEMS, epochs <= GS_SGD_MAX_EPOCHS, n < 2^31.
+ * --------------------------------------------------------------------------------------------- */
+#define GS_SGD_MAX_D 1024
+#define GS_SGD_MAX_PROBLEMS 65535
+#define GS_SGD_MAX_EPOCHS 1024
+int32_t gs_sgd_orders(const uint32_t* seeds, int32_t P, int64_t n, int32_t epochs, int32_t* orders, void* stream);
+int32_t gs_sgd_fit(const void* x, int32_t dtype, int64_t n, int32_t d, int64_t ldx, const int32_t* labels, int64_t ldy,
+                   const int32_t* orders, int32_t P, int32_t epochs, double alpha, double optimal_init, double* coef,
+                   int64_t ldc, double* intercept, void* stream);
 
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
