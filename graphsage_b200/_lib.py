@@ -41,6 +41,8 @@ class GemmPart(ctypes.Structure):
 MAX_EMBED_LISTS = 8
 MAX_UNIQUE_SAMPLED = 1024          # GS_MAX_UNIQUE_SAMPLED
 UNIQUE_DRAW_BUDGET = 1 << 20       # GS_UNIQUE_DRAW_BUDGET
+WALK_MAX_WALKS = 1 << 20           # GS_WALK_MAX_WALKS
+WALK_MAX_LEN = 33                  # GS_WALK_MAX_LEN
 
 
 class EmbedGradList(ctypes.Structure):
@@ -138,6 +140,9 @@ _SIGNATURES = {
     "gs_sgd_orders": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_vp, c_vp]),
     "gs_sgd_fit": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, ctypes.c_double, ctypes.c_double,
                            c_vp, c_i64, c_vp, c_vp]),
+    "gs_random_walks_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32]),
+    "gs_random_walks": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_i64, c_vp, c_i64, c_vp, c_vp]),
+    "gs_random_walks_emit": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp]),
 }
 
 _lib = None

@@ -133,6 +133,7 @@ constexpr uint32_t kStreamCsr = 0x40000000u;
 constexpr uint32_t kStreamUnigram = 0x20000000u;
 constexpr uint32_t kStreamBuild = 0x10000000u;
 constexpr uint32_t kStreamUnigramUnique = 0x30000000u;
+constexpr uint32_t kStreamWalk = 0x50000000u;
 
 // ---- PTX wrappers (mbarrier / bulk copy) ---------------------------------------------------
 #ifdef __CUDACC__

@@ -155,6 +155,40 @@ def sample_csr(indptr, indices, ids, k, seed, counter, replace_if_short=True, pa
     return out
 
 
+def random_walks(indptr, indices, starts, num_walks, walk_len, seed, counter=0, start_offset=0):
+    """Co-occurrence pairs of uniform random walks (gs_random_walks; reference graphsage/utils.py:77-92): num_walks walks
+    of walk_len - 1 steps from every start, (starts[t], visited id) for every visited id other than the start, ordered
+    by start, walk and step.  Contract: oracle/walks.py (start_offset is the global position of starts[0], so chunks
+    with the right offsets give the pairs of one call).  Returns an int32 CUDA tensor [P, 2].
+    P is read back to size the output: one device-to-host copy (and so a synchronisation) per call - start-up work,
+    not meant for capture."""
+    require_cuda(indptr, indices, starts)
+    if indptr.dtype != torch.int64:
+        raise TypeError("indptr must be int64")
+    indptr, indices, starts = indptr.contiguous(), _i32(indices, "indices"), _i32(starts.reshape(-1), "starts")
+    num_walks, walk_len, start_offset = int(num_walks), int(walk_len), int(start_offset)
+    if not 1 <= num_walks <= _lib.WALK_MAX_WALKS:
+        raise ValueError("num_walks must be in [1, %d] (got %d)" % (_lib.WALK_MAX_WALKS, num_walks))
+    if not 2 <= walk_len <= _lib.WALK_MAX_LEN:
+        raise ValueError("walk_len must be in [2, %d] (got %d)" % (_lib.WALK_MAX_LEN, walk_len))
+    n = starts.numel()
+    if not (start_offset >= 0 and start_offset + n <= 2**32):
+        raise ValueError("start_offset + len(starts) must be in [0, 2^32] (got %d + %d)" % (start_offset, n))
+    nbytes = lib().gs_random_walks_workspace_bytes(n, num_walks, walk_len)
+    if nbytes < 0:
+        check(-1)
+    dev = starts.device
+    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev)
+    n_pairs = torch.empty((1,), dtype=torch.int64, device=dev)
+    ev = _probe("random_walks/%d" % (n * num_walks))
+    check(lib().gs_random_walks(ptr(indptr), ptr(indices), indptr.numel() - 1, ptr(starts), n, num_walks, walk_len,
+                                seed & _U64, counter & _U64, start_offset, ptr(ws), nbytes, ptr(n_pairs), stream_ptr()))
+    out = torch.empty((int(n_pairs.item()), 2), dtype=torch.int32, device=dev)
+    check(lib().gs_random_walks_emit(ptr(starts), n, num_walks, walk_len, ptr(ws), nbytes, ptr(out), stream_ptr()))
+    _launched(3 if n else 0, ev)                  # walk, emit (+ CUB's scan passes)
+    return out
+
+
 def _dtype_code(t):
     if t.dtype == torch.float32:
         return _lib.GS_F32

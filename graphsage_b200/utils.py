@@ -93,6 +93,58 @@ def run_random_walks(G, nodes, num_walks=N_WALKS, rng=None):
     return pairs
 
 
+WALK_CHUNK = 1 << 16  # starts per device call of run_random_walks_device: bounds the device memory a call needs
+
+
+def run_random_walks_device(G, nodes, num_walks=N_WALKS, seed=123, device=None, counter=0):
+    """run_random_walks on the GPU (ops.random_walks, contract oracle/walks.py): the same list of (node, context) tuples
+    of node names, with the reference's loop and WALK_LEN, drawn from the seeded Philox stream instead of `random`.
+    Row k of the CSR is G.neighbors(node) in order, so neighbour k is what rng.choice's index k would pick.  The starts
+    are walked in chunks of WALK_CHUNK, each copied back before the next, so the pairs need not fit in device memory."""
+    import torch
+
+    from . import ops
+    from .graph import to_csr
+    names = G.nodes()
+    pos = {n: i for i, n in enumerate(names)}
+    csr = to_csr(G, pos)
+    dev = torch.device("cuda") if device is None else torch.device(device)
+    indptr = torch.from_numpy(csr["indptr"]).to(dev)
+    indices = torch.from_numpy(csr["indices"]).to(dev)
+    starts = np.array([pos[n] for n in nodes], dtype=np.int32)
+    pairs = []
+    for c0 in range(0, len(starts), WALK_CHUNK):
+        chunk = torch.from_numpy(starts[c0:c0 + WALK_CHUNK]).to(dev)
+        idx = ops.random_walks(indptr, indices, chunk, num_walks, WALK_LEN, seed, counter, start_offset=c0).cpu().numpy()
+        pairs += [(names[a], names[b]) for a, b in idx.tolist()]
+    return pairs
+
+
+def format_walks(pairs):
+    """The `<prefix>-walks.txt` text the reference's script writes (utils.py:103-104): one `start<TAB>context` line per
+    pair, no trailing newline."""
+    return "\n".join([str(p[0]) + "\t" + str(p[1]) for p in pairs])
+
+
+def main(argv=None, walker=None):
+    """`python -m graphsage_b200.utils <graph_file> <out_file>` (reference utils.py:94-104): the walks file of the train
+    subgraph (nodes that are neither val nor test), 50 walks of WALK_LEN per node, seed 123 and counter 0.
+    walker(G, nodes) -> pairs replaces run_random_walks_device (tests supply pairs without a device)."""
+    import sys
+    argv = sys.argv[1:] if argv is None else list(argv)
+    if len(argv) != 2:
+        raise SystemExit("usage: python -m graphsage_b200.utils <graph_file> <out_file>")
+    graph_file, out_file = argv
+    with open(graph_file) as fp:
+        G = node_link_graph(json.load(fp))
+    nodes = [n for n in G.nodes() if not G.node[n]["val"] and not G.node[n]["test"]]
+    G = G.subgraph(nodes)
+    pairs = (run_random_walks_device if walker is None else walker)(G, nodes)
+    with open(out_file, "w") as fp:
+        fp.write(format_walks(pairs))
+    return pairs
+
+
 def write_dataset(prefix, G, feats, id_map, class_map, walks=None):
     """Write a dataset in the same on-disk format (used by tests and synthetic data generators)."""
     nodes = G.nodes()
@@ -113,5 +165,9 @@ def write_dataset(prefix, G, feats, id_map, class_map, walks=None):
             fp.write("\n".join("%s\t%s" % (a, b) for a, b in walks))
 
 
-__all__ = ["Graph", "node_link_graph", "load_data", "run_random_walks", "standard_scale", "write_dataset", "WALK_LEN",
-           "N_WALKS"]
+__all__ = ["Graph", "node_link_graph", "load_data", "run_random_walks", "run_random_walks_device", "format_walks",
+           "standard_scale", "write_dataset", "WALK_LEN", "N_WALKS"]
+
+
+if __name__ == "__main__":
+    main()

@@ -598,6 +598,36 @@ int32_t gs_sgd_fit(const void* x, int32_t dtype, int64_t n, int32_t d, int64_t l
                    const int32_t* orders, int32_t P, int32_t epochs, double alpha, double optimal_init, double* coef,
                    int64_t ldc, double* intercept, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * run_random_walks         reference graphsage/utils.py:77-92 (the `<prefix>-walks.txt` co-occurrence pairs)
+ *   For start position t < n (global position i = start_offset + t) and walk w < num_walks (W), with L = walk_len:
+ *     node = starts[t];  curr = node;  for j = 0 .. L-1:
+ *       if curr != node: emit (node, curr)
+ *       if j < L-1: curr = indices[indptr[curr] + mulhi32(draw_j, deg(curr))]   (the reference's L-th choice is unused)
+ *   draw_s is word s % 4 of philox4x32_10(ctr = (counter_lo, counter_hi, i, 0x50000000 + w * ceil((L-1)/4) + s / 4),
+ *   key = (seed_lo, seed_hi)); mulhi32(a, b) = (a * b) >> 32.  A start outside [0, n_nodes) or without neighbours emits
+ *   nothing.  A walk that reaches a node without neighbours, or a neighbour id outside [0, n_nodes), emits it and stops
+ *   (the reference would raise; its undirected graphs never get there).  Pairs are ordered by t, then w, then j.
+ *   Bit-identical to oracle/walks.py; the draws depend only on (i, w, s), so calls over consecutive chunks of starts with
+ *   the matching start_offset give the pairs of one call.
+ * gs_random_walks_workspace_bytes - workspace for (n, num_walks, walk_len); -1 (see gs_last_error_string) outside the
+ *   limits: 1 <= num_walks <= GS_WALK_MAX_WALKS, 2 <= walk_len <= GS_WALK_MAX_LEN, n * num_walks < 2^31 - 1.
+ * gs_random_walks - runs every walk (one thread each; the visited ids and per-walk counts go to the workspace), scans the
+ *   counts (CUB, integer: deterministic) and writes the pair count P to the device word *n_pairs.  Also requires
+ *   start_offset + n <= 2^32 and n_nodes < 2^31 - 1.
+ * gs_random_walks_emit - with the same workspace after gs_random_walks on the same stream: out int32 [P, 2] =
+ *   (starts[t], visited id) pairs.  The caller reads *n_pairs to size out (one device-to-host read per call), so the
+ *   pair is not meant for CUDA-graph capture.  No atomics: every pair's position is its walk's scanned offset.
+ * --------------------------------------------------------------------------------------------- */
+#define GS_WALK_MAX_WALKS (1 << 20)
+#define GS_WALK_MAX_LEN 33
+int64_t gs_random_walks_workspace_bytes(int64_t n, int32_t num_walks, int32_t walk_len);
+int32_t gs_random_walks(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, const int32_t* starts, int64_t n,
+                        int32_t num_walks, int32_t walk_len, uint64_t seed, uint64_t counter, int64_t start_offset,
+                        void* workspace, int64_t workspace_bytes, int64_t* n_pairs, void* stream);
+int32_t gs_random_walks_emit(const int32_t* starts, int64_t n, int32_t num_walks, int32_t walk_len, const void* workspace,
+                             int64_t workspace_bytes, int32_t* out, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
