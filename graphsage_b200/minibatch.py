@@ -122,6 +122,22 @@ class _TableOwner(object):
         c = self._csr()
         return construct_test_adj(c["indptr"], c["indices"], self.max_degree, c["node_order"], self.rng)
 
+    def neighbor_csr(self, test=False):
+        """(indptr int64 [N+1], indices int32) over node indices: the rows and edges construct_adj (test=False: the train
+        graph - val/test nodes have empty rows, train_removed edges are dropped) or construct_test_adj (test=True: every
+        edge) samples from, kept whole: no padding, no subsampling.  The input of full_neighbor_embeddings."""
+        c = self._csr()
+        indptr = np.asarray(c["indptr"], dtype=np.int64)
+        indices = np.asarray(c["indices"], dtype=np.int32)
+        if test:
+            return indptr.copy(), indices.copy()
+        n = len(indptr) - 1
+        row = np.repeat(np.arange(n), np.diff(indptr))
+        keep = ~np.asarray(c["edge_removed"], dtype=bool) & ~np.asarray(c["val_or_test"], dtype=bool)[row]
+        out = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.bincount(row[keep], minlength=n), out=out[1:])
+        return out, indices[keep]
+
     def _is_train(self, n):
         a = self.G.node[n]
         return not a["test"] and not a["val"]

@@ -6,12 +6,13 @@ The TF placeholders / FLAGS the reference threads through become explicit argume
 """
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import ops
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
-                          refuse_seq_table)
-from .layers import identity, relu  # noqa: F401
+                          _rows, refuse_seq_table)
+from .layers import act_code, identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
 SAGEInfo = namedtuple("SAGEInfo",
@@ -230,6 +231,75 @@ class SampleAndAggregate(object):
             with open(out_prefix + ".txt", "w") as fp:
                 fp.write("\n".join(str(int(x)) for x in ids.tolist()))
         return emb
+
+    def full_neighbor_embeddings(self, indptr, indices, node_ids=None, normalize=True):
+        """Deterministic embeddings over WHOLE neighbourhoods, layer by layer (contract: oracle/full_neighbor.py): layer l
+        computes every node's row of h^{l+1} once - the last layer only the rows of `node_ids` (default: all N nodes) -
+        from its CSR row (indptr int64 [N+1], indices int32; an empty row uses the dummy node N, as the padded table does).
+        The neighbour reductions are gs_csr_aggregate, the combine the aggregator's own GEMM (_finish); the pooling
+        aggregators run their MLP once per node.  No sampling and no dropout: two calls give the same bits.  Returns fp32
+        [len(node_ids), out_w], l2-normalised like forward().  Peak memory: two fp32 [N+1, width] layer buffers, plus the
+        pools' [N+1, hidden] MLP output."""
+        if self.aggregator_cls is SeqAggregator:
+            raise NotImplementedError("full-neighbourhood inference is not implemented for the seq aggregator (its "
+                                      "neighbour order is the sampled order)")
+        if hasattr(self.features, "c_table"):
+            raise NotImplementedError("full-neighbourhood inference with a node-partitioned (ShardedFeatures) table is "
+                                      "not implemented")
+        n_rows = int(self.features.shape[0])
+        indptr, indices = self._csr_input(indptr, torch.int64, "indptr"), self._csr_input(indices, torch.int32, "indices")
+        if indptr.dim() != 1 or indptr.numel() != n_rows:
+            raise ValueError("indptr must have N + 1 = %d entries (one row per node of the [N+1, .] table, plus the end)"
+                             % n_rows)
+        ids = None if node_ids is None else torch.as_tensor(node_ids).to(device=self.device, dtype=torch.int32).reshape(-1)
+        if ids is None:
+            ids = torch.arange(n_rows - 1, dtype=torch.int32, device=self.device)
+        if self.aggregators is None:
+            from .supervised_models import build_aggregators
+            self.aggregators = build_aggregators(self)
+        h = self.features
+        L = len(self.aggregators)
+        with torch.no_grad():
+            for layer, agg in enumerate(self.aggregators):
+                rows = ids if layer == L - 1 else None          # None: all N+1 rows (the dummy node's row last)
+                if isinstance(agg, GCNAggregator):
+                    m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=rows)
+                    h = agg._finish([(m, agg.neigh_input_dim, agg.vars["weights"])], ops.COMBINE_ADD)
+                    continue
+                widen = h.dtype != torch.float32
+                n = h.shape[0] if rows is None else rows.numel()
+                hs = _rows(h, rows, 0, n, widen) if (widen or rows is not None) else h
+                if isinstance(agg, MaxPoolingAggregator):
+                    z = _rows(h, None, 0, h.shape[0], True) if widen else h
+                    for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116)
+                        code, post = act_code(dense.act)
+                        if getattr(dense, "_packed", None) is None:
+                            dense._packed = ops.PackedWeights()
+                        z = ops.sage_gemm([(z, dense.input_dim, dense.vars["weights"])], bias=dense.vars.get("bias"),
+                                          act=code, math=agg.math, packed=dense._packed)
+                        z = post(z) if post else z
+                    p = ops.csr_aggregate(z, indptr, indices, "max" if agg.pool == "max" else "mean", rows=rows)
+                    parts = [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
+                else:
+                    m = ops.csr_aggregate(h, indptr, indices, "mean", rows=rows)
+                    parts = [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
+                h = agg._finish(parts, agg._combine())
+            if normalize:
+                h = ops.l2_normalize_rows_(h.contiguous())
+        return h
+
+    def _csr_input(self, t, dtype, name):
+        """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""
+        if not torch.is_tensor(t):
+            arr = np.asarray(t)
+            if arr.dtype != {torch.int64: np.int64, torch.int32: np.int32}[dtype]:
+                raise TypeError("%s must be %s (got %s)" % (name, dtype, arr.dtype))
+            return torch.as_tensor(arr, device=self.device)
+        if t.dtype != dtype:
+            raise TypeError("%s must be %s (got %s)" % (name, dtype, t.dtype))
+        if t.device != self.device and not (t.is_cuda and self.device.type == "cuda" and self.device.index is None):
+            raise ValueError("%s is on %s, the model on %s" % (name, t.device, self.device))
+        return t.contiguous()
 
     def forward(self, batch, normalize=True):
         """sample -> aggregate -> l2_normalize (reference models.py:347-350, 368) for one id batch."""

@@ -473,6 +473,41 @@ def segment_max(x, n, k):
     return out
 
 
+CSR_OPS = {"mean": _lib.CSR_MEAN, "mean_self": _lib.CSR_MEAN_SELF, "max": _lib.CSR_MAX}
+
+
+def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
+    """The reduction of each node's whole CSR row (gs_csr_aggregate; contract in oracle/full_neighbor.py): output row i is
+    for node v = rows[i] - or, without rows, for every node 0 .. N-1 and then the dummy node N (N = len(indptr) - 1: the
+    [N+1, .] layout of the tables it reads) - over the source rows indices[indptr[v] .. indptr[v+1]) in CSR order - op "mean", "mean_self"
+    (GCN: v's own row joins the sum, divisor count + 1) or "max".  An empty row, or v outside [0, len(indptr) - 1), reduces
+    over the last source row (the dummy) alone; entries outside the table read it too.  src: fp32 or bf16 [R, F] CUDA table.
+    Returns fp32 [n, F], a view of an [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed)."""
+    require_cuda(src, indptr, indices, rows, out)
+    if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
+        raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
+    if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
+        raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
+    if op not in CSR_OPS:
+        raise ValueError("op must be one of %s (got %r)" % (sorted(CSR_OPS), op))
+    indptr, indices = indptr.contiguous(), _i32(indices.reshape(-1), "indices")
+    if indices.numel() == 0:
+        indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
+    n_nodes = indptr.numel() - 1
+    if rows is not None:
+        rows = _i32(rows.reshape(-1), "rows")
+    n, F = (n_nodes + 1 if rows is None else rows.numel()), src.shape[1]
+    if out is None:
+        out = torch.empty((n, pad_cols(F)), dtype=torch.float32, device=src.device)
+    if out.dtype != torch.float32 or out.dim() != 2 or out.stride(1) != 1 or out.shape[0] < n:
+        raise ValueError("out must be a row-major float32 [>= %d, .] CUDA matrix" % n)
+    ev = _probe("csr_aggregate/%d" % n)
+    check(lib().gs_csr_aggregate(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), ptr(indptr), ptr(indices),
+                                 n_nodes, ptr(rows), n, CSR_OPS[op], ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return out[:n, :F]
+
+
 def _gemm_parts(parts):
     M = parts[0][0].shape[0] if parts[0][0] is not None else 0
     arr = (GemmPart * len(parts))()

@@ -585,6 +585,13 @@ class SupervisedGraphsage(SampleAndAggregate):
         with torch.no_grad():
             return self._predictions(self.logits(batch))
 
+    def full_neighbor_predict(self, indptr, indices, node_ids):
+        """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on
+        full_neighbor_embeddings(indptr, indices, node_ids) - deterministic, no sampling, no dropout."""
+        with torch.no_grad():
+            out = self.full_neighbor_embeddings(indptr, indices, node_ids, normalize=True)
+            return self._predictions(out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"])
+
     def last_predictions(self):
         """model.preds of the last loss() / train_step() call (supervised_models.py:120-126): the predictions from that
         call's own logits - before its update, at its dropout rate - without another forward pass (which would draw new

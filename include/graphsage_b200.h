@@ -628,6 +628,26 @@ int32_t gs_random_walks(const int64_t* indptr, const int32_t* indices, int64_t n
 int32_t gs_random_walks_emit(const int32_t* starts, int64_t n, int32_t num_walks, int32_t walk_len, const void* workspace,
                              int64_t workspace_bytes, int32_t* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Full-neighbourhood reduction over CSR rows (layer-wise inference, SampleAndAggregate.full_neighbor_embeddings): the
+ * fixed-fanout reductions of gs_gather_mean / gs_segment_max (aggregators.py:48, 106-107, 182) with k made per row.
+ * Contract: oracle/full_neighbor.py.  Output row i is for node v = rows ? rows[i] : i; its entries are
+ * indices[indptr[v] .. indptr[v+1]) in CSR order.  An entry outside [0, n_src_rows) reads row n_src_rows - 1 (the clamp
+ * of gs_gather_mean); a node with no entries, or v outside [0, n_nodes), reduces over that row alone (the dummy).
+ *   GS_CSR_MEAN      acc = +0; acc += x_j in order; out = acc / (float)count
+ *   GS_CSR_MEAN_SELF the same, then acc += src[v] (v clamped like an entry); out = acc / (float)(count + 1)   (GCN)
+ *   GS_CSR_MAX       m = x_0; m = fmaxf(m, x_j) in order                                       (gs_segment_max)
+ * A CSR whose rows are a fixed-fanout sample gives the bits of gs_gather_mean / gs_segment_max.  dtype GS_F32, or GS_BF16
+ * widened to fp32 (pitch % 8 == 0, out_pitch % 8 == 0, 16-byte-aligned src and out).  Output fp32 [n, out_pitch]; columns
+ * F..out_pitch-1 are zeroed.  No allocation, no atomics, no host synchronisation: each output element is one sequential
+ * chain, so two calls give the same bits.  Rows with more than 256 entries are spread over CTAs by 32-column slices.
+ * --------------------------------------------------------------------------------------------- */
+typedef enum { GS_CSR_MEAN = 0, GS_CSR_MEAN_SELF = 1, GS_CSR_MAX = 2 } gs_csr_op;
+int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                         const int64_t* indptr, const int32_t* indices, int64_t n_nodes,
+                         const int32_t* rows /* may be NULL */, int64_t n, int32_t op,
+                         float* out, int64_t out_pitch, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
