@@ -39,6 +39,14 @@ class GemmPart(ctypes.Structure):
     _fields_ = [("A", c_vp), ("lda", c_i64), ("K", c_i32), ("B", c_vp), ("ldb", c_i64), ("N", c_i32)]
 
 
+class RowRange(ctypes.Structure):
+    _fields_ = [("ids", c_vp), ("row0", c_i64), ("n", c_i64)]
+
+
+class GemmRowIds(ctypes.Structure):
+    _fields_ = [("n_table_rows", c_i64), ("n_ranges", c_i32), ("_pad", c_i32), ("ranges", RowRange * MAX_SEGMENTS)]
+
+
 MAX_EMBED_LISTS = 8
 MAX_UNIQUE_SAMPLED = 1024          # GS_MAX_UNIQUE_SAMPLED
 UNIQUE_DRAW_BUDGET = 1 << 20       # GS_UNIQUE_DRAW_BUDGET
@@ -95,6 +103,8 @@ _SIGNATURES = {
     "gs_sage_gemm_pack": (c_i32, [ctypes.POINTER(GemmPart), c_i32, c_i32, c_vp, c_vp]),
     "gs_sage_gemm_prepacked": (c_i32, [c_i64, ctypes.POINTER(GemmPart), c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_i64,
                                        c_vp, c_vp]),
+    "gs_sage_gemm_rows": (c_i32, [c_i64, ctypes.POINTER(GemmPart), ctypes.POINTER(GemmRowIds), c_i32, c_i32, c_vp, c_i32, c_i32,
+                                  c_vp, c_i64, c_vp, c_vp]),
     "gs_gather_mean_img_bytes": (c_i64, [c_i64, c_i32, c_i32]),
     "gs_gather_mean_img": (c_i32, [c_vp, c_i64, ctypes.POINTER(ShardedTable), c_i32, c_vp, c_i32, c_i64, ctypes.POINTER(Segment),
                                    c_i32, c_i32, c_i32, c_vp, c_vp]),

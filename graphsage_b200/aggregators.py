@@ -167,7 +167,13 @@ class MeanAggregator(_SageAggregator):
                               self._combine(), False, True)
         if y is not None:
             return y
-        xs, xm = ops.gather_mean(src, segments, want_self=True)
+        if torch.is_tensor(src) and src.is_cuda and src.dtype == torch.float32 and all(s.self_ids is not None for s in segments):
+            # the self rows only feed the GEMM: it reads them from the table by id, so the gather neither fetches them nor
+            # writes a copy (same operand values, same bits)
+            _, xm = ops.gather_mean(src, segments, want_self=False)
+            xs = ops.TableRows(src, [(s.self_ids[:s.n], s.out_row0) for s in segments], xm.shape[0])
+        else:
+            xs, xm = ops.gather_mean(src, segments, want_self=True)
         return self._finish([(xs, self.input_dim, self.vars["self_weights"]),
                              (xm, self.neigh_input_dim, self.vars["neigh_weights"])], self._combine())
 

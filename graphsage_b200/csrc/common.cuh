@@ -197,6 +197,22 @@ __device__ __forceinline__ float4 ldg_nc_f4(const float4* p) {
                : "l"(p));
   return r;
 }
+
+// the A row that operand row r of a GEMM part reads (gs_sage_gemm_rows): r itself for a dense part, else the clamped id
+// its range holds; -1 = a zero row (r >= M, or no range covers r)
+__device__ __forceinline__ int64_t gemm_a_row(const gs_gemm_row_ids& R, int64_t M, int64_t r) {
+  if (r >= M) return -1;
+  if (R.n_ranges == 0) return r;
+#pragma unroll
+  for (int s = 0; s < GS_MAX_SEGMENTS; ++s) {
+    const gs_row_range& g = R.ranges[s];
+    if (s < R.n_ranges && r >= g.row0 && r - g.row0 < g.n) {
+      const int64_t id = g.ids[r - g.row0];
+      return (id < 0 || id >= R.n_table_rows) ? R.n_table_rows - 1 : id;
+    }
+  }
+  return -1;
+}
 #endif  // __CUDACC__
 
 }  // namespace gs

@@ -306,8 +306,10 @@ __device__ __forceinline__ void gather_img_store(const GatherImg& im, int part, 
 
 // kDrop: every gathered row is dropped in registers before it is summed (gs_gather_mean_dropout); the kDrop = false
 // instantiation is the plain gather.
+// min 3 CTAs per SM: what the two-buffer ring's shared memory allows at F = 602 (2 x 13 rows x 2,432 B); without the hint
+// ptxas caps the kernel at 64 registers and spills
 template <class Rows, bool kDrop>
-__global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_constant__ Rows rows_of, int F,
+__global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_constant__ Rows rows_of, int F,
                                                                const __grid_constant__ SegTable tab,
                                                                int include_self, float* __restrict__ out_self,
                                                                float* __restrict__ out_mean, int64_t out_pitch,
@@ -331,6 +333,9 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
   const int ncol4 = (int)(out_pitch >> 2);
   const int row_f4 = row_bytes >> 4;
   const size_t buf_bytes = (size_t)kGroupRows * row_bytes;
+  // a node's self row is fetched only when something reads it: the GCN sum, out_self or the self image.  The mean layer
+  // whose GEMM reads the self rows by id (gs_sage_gemm_rows) asks for none of them and so moves k rows per node, not k + 1.
+  const int self_rows = (include_self || out_self || (img.base && img.want_self)) ? 1 : 0;
 
   // work items of this CTA: (node r, group g); enumerate lazily
   int64_t r_issue = blockIdx.x;      // node whose groups are being issued
@@ -340,7 +345,7 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
     int64_t i;
     const gs_segment& sg = tab.s[find_segment(tab, r_issue, i)];
     const int k = sg.k;
-    const int rows_total = k + 1;                         // neighbours then self
+    const int rows_total = k + self_rows;                 // neighbours, then self
     const int first = g_issue * kGroupRows;
     const int cnt = min(kGroupRows, rows_total - first);
     if (threadIdx.x < 32) {
@@ -371,14 +376,14 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
     const int si = find_segment(tab, r, i);
     const gs_segment& sg = tab.s[si];
     const int k = sg.k;
-    const int rows_total = k + 1;
+    const int rows_total = k + self_rows;
     const int first = g * kGroupRows;
     const int cnt = min(kGroupRows, rows_total - first);
     const bool last = first + cnt >= rows_total;
     mbar_wait(&bar[buf], phase[buf]);
     phase[buf] ^= 1u;
     const float4* rows = reinterpret_cast<const float4*>(smem + buf * buf_bytes);
-    const int nn = last ? cnt - 1 : cnt;                  // neighbour rows in this group (the self row is the node's last row)
+    const int nn = last ? cnt - self_rows : cnt;          // neighbour rows in this group (the self row is the node's last row)
     DropSite nsite{};
     if constexpr (kDrop) nsite = with_call_offset(drop.neigh[si], drop_off[si]);
 #pragma unroll
@@ -404,8 +409,10 @@ __global__ void __launch_bounds__(192) gather_mean_tma2_kernel(const __grid_cons
           float4 a = make_float4(0.f, 0.f, 0.f, 0.f), sv = a;
           if (c < ncol4 && c * 4 < F) {
             a = acc[q];
-            sv = rows[(cnt - 1) * row_f4 + c];
-            if constexpr (kDrop) sv = drop4(with_call_offset(drop.self[si], drop_off[GS_MAX_SEGMENTS + si]), i, (uint32_t)c, sv);
+            if (self_rows) {
+              sv = rows[(cnt - 1) * row_f4 + c];
+              if constexpr (kDrop) sv = drop4(with_call_offset(drop.self[si], drop_off[GS_MAX_SEGMENTS + si]), i, (uint32_t)c, sv);
+            }
             const float div = (float)(k + (include_self ? 1 : 0));
             if (include_self) { a.x += sv.x; a.y += sv.y; a.z += sv.z; a.w += sv.w; }
             a.x /= div; a.y /= div; a.z /= div; a.w /= div;

@@ -11,6 +11,7 @@ struct GemmParts {
   gs_gemm_part p[2];
   int32_t n_parts;
   int32_t combine;
+  gs_gemm_row_ids rid[2];   // part p's A rows by id (gs_sage_gemm_rows); n_ranges == 0: dense A
 };
 
 constexpr int BM = 64, BN = 64, BK = 16;
@@ -41,15 +42,17 @@ __global__ void __launch_bounds__(256) sage_gemm_simt_kernel(int64_t M, const __
 
   for (int pi = part_lo; pi < part_hi; ++pi) {
     const gs_gemm_part& P = gp.p[pi];
+    int64_t arow[4];                     // A row behind this thread's four A-tile rows (-1: zero row)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) arow[e] = gemm_a_row(gp.rid[pi], M, m0 + ((threadIdx.x + e * 256) >> 4));
     for (int k0 = 0; k0 < P.K; k0 += BK) {
       // A tile: 64 rows x 16 k  (256 threads x 4 elements)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         int idx = threadIdx.x + e * 256;
         int r = idx >> 4, kk = idx & 15;
-        int64_t gm = m0 + r;
         int gk = k0 + kk;
-        As[kk][r] = (gm < M && gk < P.K) ? P.A[gm * P.lda + gk] : 0.f;
+        As[kk][r] = (arow[e] >= 0 && gk < P.K) ? P.A[arow[e] * P.lda + gk] : 0.f;
       }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
@@ -90,13 +93,14 @@ __global__ void __launch_bounds__(256) sage_gemm_simt_kernel(int64_t M, const __
   }
 }
 
-int32_t sage_gemm_simt(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias,
-                       int32_t act, float* out, int64_t ldo, cudaStream_t st) {
+int32_t sage_gemm_simt(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids* row_ids, int32_t n_parts,
+                       int32_t combine, const float* bias, int32_t act, float* out, int64_t ldo, cudaStream_t st) {
   GemmParts gp;
   memset(&gp, 0, sizeof(gp));
   gp.n_parts = n_parts;
   gp.combine = combine;
   for (int i = 0; i < n_parts; ++i) gp.p[i] = parts[i];
+  for (int i = 0; row_ids && i < n_parts; ++i) gp.rid[i] = row_ids[i];
   int tiles_n0 = (parts[0].N + BN - 1) / BN;
   int tiles_n = tiles_n0;
   if (combine == GS_COMBINE_CONCAT && n_parts == 2) tiles_n += (parts[1].N + BN - 1) / BN;

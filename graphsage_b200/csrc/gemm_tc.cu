@@ -11,7 +11,9 @@
 //   B (weights): pre-swizzled tile images of W^T (built per weight update by pack_b_kernel into the caller's
 //                workspace), one cp.async.bulk per K-block into a ring of stages, completion on an mbarrier.
 //   A          : register form - every thread loads its 16-byte chunks of the next K-block from global memory while
-//                the current K-block's wgmmas run, then splits / converts them and stores the SW128 tile image;
+//                the current K-block's wgmmas run, then splits / converts them and stores the SW128 tile image; a part
+//                may name its rows by id into a table (gs_sage_gemm_rows: the mean layer-0 self rows straight from the
+//                feature table), resolved once per tile, so only the address of the load changes;
 //                image form (tf32x3 only) - the fused gather already wrote the tf32 hi / lo tile images
 //                (gs_gather_mean_img), so A arrives by bulk copy like B.  Both forms run the same MMAs in the same
 //                order, so their results are bit-identical.
@@ -47,6 +49,7 @@ struct TcParams {
   const unsigned char* a_img;   // image form: A operands as tf32 hi/lo tile images (gs_gather_mean_img)
   int32_t a_mtiles;             // 128-row tiles in the A images
   int32_t a_part0;              // A-image part that feeds GEMM part 0 (GEMM part p reads A part a_part0 + p)
+  gs_gemm_row_ids rid[2];       // register form: part p's A rows by id (gs_sage_gemm_rows); n_ranges == 0: dense A
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -110,12 +113,12 @@ struct TcCfg {
 };
 
 template <int MODE>
-__device__ __forceinline__ void load_a_chunk(const TcPart& P, int64_t M, int64_t grow, int gcol, bool vec, float (&v)[8]) {
+__device__ __forceinline__ void load_a_chunk(const TcPart& P, int64_t arow, int gcol, bool vec, float (&v)[8]) {
   constexpr int EPC = MODE == 2 ? 8 : 4;
 #pragma unroll
   for (int e = 0; e < 8; ++e) v[e] = 0.f;
-  if (grow >= M) return;
-  const float* src = P.A + grow * P.lda + gcol;
+  if (arow < 0) return;                          // zero row (gemm_a_row)
+  const float* src = P.A + arow * P.lda + gcol;
   if (vec && gcol + EPC <= P.K) {
     float4 a = ldg_nc_f4(reinterpret_cast<const float4*>(src));
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
@@ -198,6 +201,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
       bulk_g2s(st, prm.a_img + (((int64_t)(prm.a_part0 + pi) * prm.a_mtiles + blockIdx.x) * P.kblocks + kb) * C::IMG_BYTES,
                C::IMG_BYTES, &full[s]);
   };
+  // the A row behind each of this thread's chunks, for the tile's first and second part: fixed over the K loop, so a part
+  // whose rows come by id looks each id up once per tile, not once per K-block
+  int64_t arow_lo[C::CPT], arow_hi[C::CPT];
+  if constexpr (!kImg) {
+#pragma unroll
+    for (int i = 0; i < C::CPT; ++i) {
+      const int64_t r = m0 + ((tid + TC_THREADS * i) >> 3);
+      arow_lo[i] = gemm_a_row(prm.rid[part_lo], prm.M, r);
+      arow_hi[i] = part_hi - part_lo == 2 ? gemm_a_row(prm.rid[part_lo + 1], prm.M, r) : -1;
+    }
+  }
   float cur[C::CPT][8];
   auto fetch = [&](int it) {
     int pi, kb;
@@ -207,7 +221,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
 #pragma unroll
     for (int i = 0; i < C::CPT; ++i) {
       const int q = tid + TC_THREADS * i;
-      load_a_chunk<MODE>(P, prm.M, m0 + (q >> 3), kb * C::BK + (q & 7) * (MODE == 2 ? 8 : 4), vec, cur[i]);
+      load_a_chunk<MODE>(P, pi == part_lo ? arow_lo[i] : arow_hi[i], kb * C::BK + (q & 7) * (MODE == 2 ? 8 : 4), vec, cur[i]);
     }
   };
 
@@ -361,13 +375,15 @@ int32_t sage_gemm_tc_img(int64_t M, const gs_gemm_part* parts, int32_t n_parts, 
   return launch_tc<0, true>(prm, (const unsigned char*)workspace, st);
 }
 
-int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias,
-                     int32_t act, int32_t math, float* out, int64_t ldo, const void* workspace, cudaStream_t st) {
+int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids* row_ids, int32_t n_parts, int32_t combine,
+                     const float* bias, int32_t act, int32_t math, float* out, int64_t ldo, const void* workspace,
+                     cudaStream_t st) {
   GS_REQUIRE(workspace != nullptr, "gs_sage_gemm: tensor-core math modes need the workspace (gs_sage_gemm_workspace_bytes)");
   GS_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 127u) == 0, "gs_sage_gemm: workspace must be 128-byte aligned");
   const int mode = mode_of(math);
   TcParams prm;
   fill_parts(prm, M, parts, n_parts, mode);
+  for (int i = 0; row_ids && i < n_parts; ++i) prm.rid[i] = row_ids[i];
   prm.combine = combine;
   prm.bias = bias;
   prm.act = act;

@@ -4,7 +4,7 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_NONE, ACT_RELU, COMBINE_ADD, COMBINE_CONCAT, MATH_FP32_SIMT, MATH_TF32X3, MATH_TF32,
-                   MATH_BF16, GemmPart, Segment, check, lib, ptr, require_cuda, stream_ptr)
+                   MATH_BF16, GemmPart, GemmRowIds, RowRange, Segment, check, lib, ptr, require_cuda, stream_ptr)
 
 _U64 = 2**64 - 1
 
@@ -508,15 +508,49 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
     return out[:n, :F]
 
 
+class TableRows(object):
+    """A sage_gemm A operand of M rows read by id from a row table (gs_sage_gemm_rows), for rows that only feed the GEMM:
+    for each (ids, row0) of `ranges`, operand row row0 + i is table[ids[i]].  Ids outside [0, table rows) read the table's
+    last row (the zero dummy row), rows no range covers are zero.  The result equals sage_gemm on the gathered rows, bit for
+    bit, in every math."""
+    __slots__ = ("table", "ranges", "M")
+
+    def __init__(self, table, ranges, M):
+        require_cuda(table)
+        if table.dtype != torch.float32 or table.dim() != 2 or table.stride(1) != 1:
+            raise ValueError("the row table must be a row-major float32 matrix")
+        if len(ranges) > _lib.MAX_SEGMENTS:
+            raise ValueError("at most %d id ranges" % _lib.MAX_SEGMENTS)
+        self.table, self.M = table, int(M)
+        self.ranges = [(_i32(ids.reshape(-1), "ids"), int(row0)) for ids, row0 in ranges]
+        require_cuda(*[ids for ids, _ in self.ranges])
+
+    @property
+    def device(self):
+        return self.table.device
+
+    def c_struct(self):
+        r = GemmRowIds(self.table.shape[0], len(self.ranges), 0)
+        for s, (ids, row0) in enumerate(self.ranges):
+            r.ranges[s] = RowRange(ptr(ids), row0, ids.numel())
+        return r
+
+
 def _gemm_parts(parts):
-    M = parts[0][0].shape[0] if parts[0][0] is not None else 0
+    A0 = parts[0][0]
+    M = A0.M if isinstance(A0, TableRows) else (A0.shape[0] if A0 is not None else 0)
     arr = (GemmPart * len(parts))()
     keep = []
     for i, (A, K, B) in enumerate(parts):
+        by_id = isinstance(A, TableRows)
+        if by_id:
+            if A.M != M:
+                raise ValueError("bad A operand for part %d" % i)
+            A = A.table
         require_cuda(A, B)
         if (A is not None and A.dtype != torch.float32) or B.dtype != torch.float32:
             raise TypeError("sage_gemm operands must be float32")
-        if A is not None and (A.stride(1) != 1 or A.shape[0] != M or A.shape[1] < K):
+        if A is not None and (A.stride(1) != 1 or (A.shape[0] != M and not by_id) or A.shape[1] < K):
             raise ValueError("bad A operand for part %d" % i)
         B = B.contiguous()
         if B.shape[0] != K:
@@ -555,27 +589,42 @@ class PackedWeights(object):
 
 
 def sage_gemm(parts, combine=COMBINE_ADD, bias=None, act=ACT_NONE, math=MATH_FP32_SIMT, out=None, packed=None):
-    """parts: [(A[M, >=K] (row stride used as lda), K, B[K, N])] (1 or 2).  act(concat_or_add(A_p[:, :K] @ B_p) + bias).
+    """parts: [(A[M, >=K] (row stride used as lda) or a TableRows, K, B[K, N])] (1 or 2).
+    act(concat_or_add(A_p[:, :K] @ B_p) + bias).
     packed: optional PackedWeights cache (tensor-core modes) so the weight images are built once, not per call."""
     M, arr, keep = _gemm_parts(parts)
+    rid = None
+    if any(isinstance(p[0], TableRows) for p in parts):
+        rid = (GemmRowIds * len(parts))()
+        for i, p in enumerate(parts):
+            if isinstance(p[0], TableRows):
+                rid[i] = p[0].c_struct()
     ntot = sum(p[2].shape[1] for p in parts) if (combine == COMBINE_CONCAT) else parts[0][2].shape[1]
     dev = parts[0][0].device
     if out is None:
         out = torch.empty((M, ntot), dtype=torch.float32, device=dev)
+
+    def run(ws):
+        if rid is None:
+            return lib().gs_sage_gemm_prepacked(M, arr, len(parts), combine, ptr(bias), act, math, ptr(out), out.stride(0),
+                                                ptr(ws), stream_ptr())
+        return lib().gs_sage_gemm_rows(M, arr, rid, len(parts), combine, ptr(bias), act, math, ptr(out), out.stride(0),
+                                       ptr(ws), stream_ptr())
+
     if math == MATH_FP32_SIMT or packed is None:
         ws_bytes = lib().gs_sage_gemm_workspace_bytes(M, arr, len(parts), math)
         if ws_bytes < 0:
             check(-1)
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
         ev = _probe("sage_gemm/%d" % M)
-        check(lib().gs_sage_gemm(M, arr, len(parts), combine, ptr(bias), act, math, ptr(out), out.stride(0), ptr(ws),
-                                 stream_ptr()))
+        if M and ws is not None:             # gs_sage_gemm = pack + prepacked
+            check(lib().gs_sage_gemm_pack(arr, len(parts), math, ptr(ws), stream_ptr()))
+        check(run(ws))
         _launched((2 if ws is not None else 1) if M else 0, ev)
         return out
     ws = packed.get(parts, arr, math, dev)
     ev = _probe("sage_gemm/%d" % M)
-    check(lib().gs_sage_gemm_prepacked(M, arr, len(parts), combine, ptr(bias), act, math, ptr(out), out.stride(0),
-                                       ptr(ws), stream_ptr()))
+    check(run(ws))
     _launched(1 if M else 0, ev)
     return out
 

@@ -297,6 +297,31 @@ int32_t gs_sage_gemm_prepacked(int64_t M, const gs_gemm_part* parts_host, int32_
                                const float* bias, int32_t act, int32_t math, float* out, int64_t ldo,
                                const void* workspace, void* stream);
 
+/* gs_sage_gemm_prepacked with the A rows of a part read BY ID from a row table, so rows that only feed the GEMM need no
+ * gathered copy (the mean layer-0 self rows: their ids index the feature table).  row_ids_host[p] (p < n_parts; the array
+ * or an entry may be NULL, and an entry with n_ranges == 0 means the same) turns parts[p].A into a table of
+ * n_table_rows rows (row stride lda):
+ *   operand row r of part p = parts[p].A[ranges[s].ids[r - ranges[s].row0] * lda + 0:K]  for the first range s with
+ *   row0 <= r < row0 + n;  ids outside [0, n_table_rows) read row n_table_rows - 1 (the zero dummy row: the rule of
+ *   gs_gather_mean);  rows no range covers are zero.
+ * The loaded values, the operand split and the MMA order are those of the dense form, so the result is bit-identical to
+ * gs_sage_gemm_prepacked on the gathered rows, in every math (workspace as for gs_sage_gemm_prepacked; none for
+ * GS_MATH_FP32_SIMT).  Limits: n_ranges <= GS_MAX_SEGMENTS, 1 <= n_table_rows < 2^31. */
+typedef struct {
+  const int32_t* ids;   /* device, n ids */
+  int64_t row0;         /* first operand row they feed */
+  int64_t n;
+} gs_row_range;
+typedef struct {
+  int64_t n_table_rows;
+  int32_t n_ranges;
+  int32_t _pad;
+  gs_row_range ranges[GS_MAX_SEGMENTS];
+} gs_gemm_row_ids;
+int32_t gs_sage_gemm_rows(int64_t M, const gs_gemm_part* parts_host, const gs_gemm_row_ids* row_ids_host, int32_t n_parts,
+                          int32_t combine, const float* bias, int32_t act, int32_t math, float* out, int64_t ldo,
+                          const void* workspace, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * The mean / GCN layer-0 pair with the A operand handed over as tensor-core tile images (tf32x3 arithmetic):
  *   gs_gather_mean_img : the fused gather + fanout mean of gs_gather_mean / gs_gather_mean_sharded (same segments, same
