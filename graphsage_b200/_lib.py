@@ -16,7 +16,7 @@ GS_F32, GS_BF16, GS_F64 = 0, 1, 2
 ACT_NONE, ACT_RELU = 0, 1
 COMBINE_ADD, COMBINE_CONCAT = 0, 1
 MATH_FP32_SIMT, MATH_TF32X3, MATH_TF32, MATH_BF16 = 0, 1, 2, 3
-CSR_MEAN, CSR_MEAN_SELF, CSR_MAX = 0, 1, 2
+CSR_MEAN, CSR_MEAN_SELF, CSR_MAX, CSR_SUM = 0, 1, 2, 3
 MAX_SEGMENTS = 4
 
 c_i32, c_i64, c_u64, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64, ctypes.c_void_p
@@ -155,6 +155,10 @@ _SIGNATURES = {
     "gs_random_walks": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_random_walks_emit": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp]),
     "gs_csr_aggregate": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp]),
+    "gs_csr_transpose_workspace_bytes": (c_i64, [c_i64, c_i64, c_i32]),
+    "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "gs_csr_max_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64,
+                                    c_vp, c_i64, c_vp]),
 }
 
 _lib = None

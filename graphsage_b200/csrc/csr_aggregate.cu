@@ -3,7 +3,8 @@
 //   reference: tf.reduce_mean(neigh_vecs, axis=1)              graphsage/aggregators.py:48
 //              mean(concat([neigh, self]), 1)  (GCN)           graphsage/aggregators.py:106-107
 //              tf.reduce_max(neigh_h, axis=1)                  graphsage/aggregators.py:182
-// with the fanout k made per row.  Every output element is ONE sequential chain over the row's entries in CSR order
+// with the fanout k made per row, and the plain sum GS_CSR_SUM, the backward of the means over the transposed graph
+// (SupervisedGraphsage.full_neighbor_train_step; contract in oracle/full_neighbor_grad.py).  Every output element is ONE sequential chain over the row's entries in CSR order
 // (the order of gs_gather_mean / gs_segment_max), so no work split may cut a row along its entries.  Two roles share
 // one launch of 256-thread CTAs:
 //   hub role (the first hub_blocks CTAs): rows with more than kCsrLong entries.  Work item = (chunk of 256 rows, slice of
@@ -103,17 +104,17 @@ __device__ __forceinline__ float load_scalar(const CsrArgs& a, int64_t r, int c)
   else return __ldg(static_cast<const float*>(a.src) + r * a.pitch + c);
 }
 
-// one step of the chain after its first entry (the max starts from x_0 itself, the means from +0)
+// one step of the chain after its first entry (the max starts from x_0 itself, the means and the sum from +0)
 template <int OP>
 __device__ __forceinline__ float csr_step(float acc, float x) {
   if constexpr (OP == GS_CSR_MAX) return fmaxf(acc, x);
   else return acc + x;
 }
 
-// the chain's end: the mean's division (after the self row for GS_CSR_MEAN_SELF)
+// the chain's end: the mean's division (after the self row for GS_CSR_MEAN_SELF); the max and the sum end as they are
 template <int OP>
 __device__ __forceinline__ float csr_final(float acc, int64_t count, float self) {
-  if constexpr (OP == GS_CSR_MAX) return acc;
+  if constexpr (OP == GS_CSR_MAX || OP == GS_CSR_SUM) return acc;
   if constexpr (OP == GS_CSR_MEAN_SELF) return (acc + self) / (float)(count + 1);
   return acc / (float)count;
 }
@@ -199,7 +200,8 @@ __device__ void short_role(const CsrArgs& a, int64_t block) {
 #pragma unroll
     for (int q = 0; q < V; ++q) acc[q] = 0.f;
     if (c0 < a.F) {
-      const int64_t count = cnt > 0 ? cnt : 1;              // an empty row: the dummy row alone
+      // an empty row: the dummy row alone, except for the sum, whose empty row is +0 (a node nobody points to)
+      const int64_t count = OP == GS_CSR_SUM ? cnt : cnt > 0 ? cnt : 1;
       int64_t e = 0;
       if constexpr (OP == GS_CSR_MAX) {
         float x0[V];
@@ -247,7 +249,8 @@ template <typename T, int V>
 static void launch_csr(int32_t op, unsigned blocks, const CsrArgs& a, cudaStream_t st) {
   if (op == GS_CSR_MEAN) csr_aggregate_kernel<T, V, GS_CSR_MEAN><<<blocks, kCsrThreads, 0, st>>>(a);
   else if (op == GS_CSR_MEAN_SELF) csr_aggregate_kernel<T, V, GS_CSR_MEAN_SELF><<<blocks, kCsrThreads, 0, st>>>(a);
-  else csr_aggregate_kernel<T, V, GS_CSR_MAX><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if (op == GS_CSR_MAX) csr_aggregate_kernel<T, V, GS_CSR_MAX><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if constexpr (sizeof(T) == 4) csr_aggregate_kernel<T, V, GS_CSR_SUM><<<blocks, kCsrThreads, 0, st>>>(a);   // fp32 only
 }
 
 }  // namespace gs
@@ -258,8 +261,10 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
                          const int32_t* indices, int64_t n_nodes, const int32_t* rows, int64_t n, int32_t op, float* out,
                          int64_t out_pitch, void* stream) {
   const char* who = "gs_csr_aggregate";
-  GS_REQUIRE(op == GS_CSR_MEAN || op == GS_CSR_MEAN_SELF || op == GS_CSR_MAX, "%s: unknown op %d", who, (int)op);
+  GS_REQUIRE(op == GS_CSR_MEAN || op == GS_CSR_MEAN_SELF || op == GS_CSR_MAX || op == GS_CSR_SUM, "%s: unknown op %d", who,
+             (int)op);
   GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16, "%s: dtype must be GS_F32 or GS_BF16", who);
+  GS_REQUIRE(op != GS_CSR_SUM || dtype == GS_F32, "%s: GS_CSR_SUM reads fp32 sources only", who);
   GS_REQUIRE(n >= 0 && n_nodes >= 0 && F >= 1 && pitch >= F && out_pitch >= F, "%s: bad sizes", who);
   GS_REQUIRE(out_pitch < (1LL << 30), "%s: out_pitch must be < 2^30", who);
   if (n == 0) return GS_OK;

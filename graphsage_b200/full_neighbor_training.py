@@ -1,0 +1,233 @@
+"""Full-batch training over whole neighbourhoods: the differentiable form of SampleAndAggregate.full_neighbor_embeddings
+(contract: oracle/full_neighbor_grad.py).
+
+One torch.autograd.Function per layer (_FullLayerFn, the layer-wise counterpart of supervised_models._LayerFn).  Its
+forward is full_neighbor_embeddings' layer, launch for launch, so the values are the same bits.  Its backward:
+  - weight gradients dW = X^T dZ as library matmuls, as in the sampled path;
+  - source gradients through the CSR kernels over the transposed graph (ops.csr_transpose, built once per CSR and cached
+    on the model): the means' backward is ops.csr_aggregate(op="sum") of g / count, the max-pool's ops.csr_max_backward;
+  - the last layer reads only the rows of node_ids (duplicates allowed): their gradients are scattered into a dense
+    [N+1, w] gradient by ops.embedding_grad (group 1) first.
+The pools run their MLP once per node, as full_neighbor_embeddings does, whatever fused_pool says: the MLP input is the
+layer's whole [N+1, in] table, so its gradient dZ Wm^T needs no transpose.  Layer-0 feature columns are not trainable:
+with identity_dim = 0 layer 0 computes no source gradient (the pools still compute dWm, dbm); with identity_dim = d > 0 it
+computes columns [0, d) only, which autograd delivers as model.embeds.grad (a dense [N+1, d] tensor).
+"""
+import torch
+
+from . import ops
+from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, _rows
+from .layers import act_code
+
+
+class FullNeighborGraph(object):
+    """The transposes and divisors of one CSR, built on first use.  `key` identifies the CSR tensors (data_ptr, numel,
+    _version of both); the tensors themselves are held, so their memory cannot be reused by a different CSR while cached."""
+
+    def __init__(self, indptr, indices):
+        self.indptr, self.indices = indptr, indices
+        self.key = FullNeighborGraph.key_of(indptr, indices)
+        self.n_rows = indptr.numel()                 # N + 1
+        self._t, self._counts = {}, {}
+
+    @staticmethod
+    def key_of(indptr, indices):
+        return tuple((t.data_ptr(), t.numel(), t._version) for t in (indptr, indices))
+
+    def transpose(self, with_self):
+        if with_self not in self._t:
+            self._t[with_self] = ops.csr_transpose(self.indptr, self.indices, with_self=with_self)
+        return self._t[with_self]
+
+    def counts(self, with_self):
+        """The forward's divisors for the N + 1 effective rows (max(degree, 1), + 1 for GCN), fp32 [N + 1, 1]."""
+        if with_self not in self._counts:
+            deg = (self.indptr[1:] - self.indptr[:-1]).clamp(min=1)
+            one = torch.ones((1,), dtype=deg.dtype, device=deg.device)
+            self._counts[with_self] = (torch.cat([deg, one]) + int(with_self)).to(torch.float32).unsqueeze(1)
+        return self._counts[with_self]
+
+    def mean_backward(self, g, with_self):
+        """d(source) of the mean over the effective rows for their gradient g [N + 1, w]: sum of g / count over the
+        transposed rows."""
+        t_indptr, t_indices = self.transpose(with_self)
+        return ops.csr_aggregate((g / self.counts(with_self)).contiguous(), t_indptr, t_indices, "sum")
+
+
+class _FullLayer(object):
+    """One aggregator layer over every node: rows None computes all N + 1 rows, else (the last layer) the rows of `rows`."""
+
+    def __init__(self, agg, graph, rows):
+        self.agg, self.graph, self.rows = agg, graph, rows
+        self.gcn = isinstance(agg, GCNAggregator)
+        self.pool = isinstance(agg, MaxPoolingAggregator)
+
+    def dense(self, x):
+        """The [N+1, w] gradient of the rows this layer outputs: x itself, or the scatter of x into rows' ids."""
+        if self.rows is None:
+            return x
+        return ops.embedding_grad([(self.rows, x.contiguous(), 1, 1.0)], self.graph.n_rows, x.shape[1])
+
+    def forward(self, h, kept):
+        """The GEMM parts of full_neighbor_embeddings' layer; `kept` receives what the backward reads besides them."""
+        agg, g, rows = self.agg, self.graph, self.rows
+        indptr, indices = g.indptr, g.indices
+        if self.gcn:
+            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=rows)
+            return [(m, agg.neigh_input_dim, agg.vars["weights"])]
+        widen = h.dtype != torch.float32
+        n = h.shape[0] if rows is None else rows.numel()
+        hs = _rows(h, rows, 0, n, widen) if (widen or rows is not None) else h
+        if not self.pool:
+            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=rows)
+            return [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
+        x = _rows(h, None, 0, h.shape[0], True) if widen else h
+        z = x
+        for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116), once per node
+            code, post = act_code(dense.act)
+            if getattr(dense, "_packed", None) is None:
+                dense._packed = ops.PackedWeights()
+            z = ops.sage_gemm([(z, dense.input_dim, dense.vars["weights"])], bias=dense.vars.get("bias"), act=code,
+                              math=agg.math, packed=dense._packed)
+            z = post(z) if post else z
+        op = "max" if agg.pool == "max" else "mean"
+        if op == "max" and rows is not None:         # the backward needs every row's max: the same chains, then the rows
+            p_all = ops.csr_aggregate(z, indptr, indices, "max")
+            p = p_all.index_select(0, rows)
+        else:
+            p = p_all = ops.csr_aggregate(z, indptr, indices, op, rows=rows)
+        kept.extend([x, z, p_all])
+        return [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
+
+    def backward(self, xs, dzs, params, kept, cols):
+        """(gradients of the branch's own parameters, d(source) [N + 1, cols] or None)."""
+        if self.gcn:
+            if not cols:
+                return [], None
+            return [], self.graph.mean_backward(self.dense(dzs[0] @ params[0][:cols].t()), True)
+        Ws, Wn = params[0], params[1]
+        dself = self.dense(dzs[0] @ Ws[:cols].t()) if cols else None
+        if not self.pool:
+            if not cols:
+                return [], None
+            return [], self.graph.mean_backward(self.dense(dzs[1] @ Wn[:cols].t()), False) + dself
+        Wm = params[2]
+        x, z, p_all = kept
+        dp = self.dense(dzs[1] @ Wn.t())
+        if self.agg.pool == "max":
+            t_indptr, t_indices = self.graph.transpose(False)
+            dzp = ops.csr_max_backward(z, p_all, dp, self.graph.indptr, self.graph.indices, t_indptr, t_indices)
+        else:
+            dzp = self.graph.mean_backward(dp, False) * (z > 0).to(dp.dtype)    # the ReLU of the Dense layer
+        K = Wm.shape[0]
+        grads = [x[:, :K].t() @ dzp, dzp.sum(dim=0)]
+        return grads, (dzp @ Wm[:cols].t() + dself if cols else None)
+
+
+class _FullLayerFn(torch.autograd.Function):
+    """y = the layer of full_neighbor_embeddings, differentiable w.r.t. the layer's parameters, its source h (layers >= 1)
+    and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of the table's first d columns."""
+
+    @staticmethod
+    def forward(ctx, layer, h, emb, *params):
+        agg = layer.agg
+        code, post = act_code(agg.act)
+        if post is not None:
+            raise NotImplementedError("training supports act=relu or identity")
+        with torch.no_grad():
+            kept = []
+            parts = layer.forward(h, kept)
+            y = agg._finish(parts, agg._combine())
+        ctx.layer, ctx.relu, ctx.concat = layer, code == ops.ACT_RELU, bool(agg.concat)
+        ctx.F_in, ctx.Ks = h.shape[1], [K for _, K, _ in parts]
+        ctx.src_needs_grad = bool(h.requires_grad)
+        ctx.emb_d = emb.shape[1] if emb is not None and emb.requires_grad else 0
+        ctx.n_params = len(params)
+        ctx.save_for_backward(*[x for x, _, _ in parts], y, *params, *kept)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        P = len(ctx.Ks)
+        saved = ctx.saved_tensors
+        xs, y, params, kept = saved[:P], saved[P], saved[P + 1:P + 1 + ctx.n_params], saved[P + 1 + ctx.n_params:]
+        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
+        D = params[0].shape[1]
+        dzs = (dz[:, :D], dz[:, D:]) if P == 2 and ctx.concat else (dz,) * P
+        grads_w = [x[:, :K].t() @ g for x, K, g in zip(xs, ctx.Ks, dzs)]           # dW = X^T dZ  (library GEMM)
+        cols = ctx.F_in if ctx.src_needs_grad else ctx.emb_d
+        grads_own, dsrc = ctx.layer.backward(xs, dzs, params, kept, cols)
+        dh = dsrc if ctx.src_needs_grad else None
+        demb = dsrc[:, :ctx.emb_d] if ctx.emb_d and dsrc is not None else None
+        return (None, dh, demb) + tuple(grads_w) + tuple(grads_own)
+
+
+class _L2NormalizeFn(torch.autograd.Function):
+    """tf.nn.l2_normalize(x, 1) through gs_l2_normalize_rows (the bits of full_neighbor_embeddings); the backward is the
+    formula's gradient."""
+
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return ops.l2_normalize_rows_(x.detach().contiguous().clone())
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        with torch.enable_grad():
+            xx = x.detach().requires_grad_(True)
+            out = xx / torch.sqrt(torch.clamp((xx * xx).sum(dim=1, keepdim=True), min=1e-12))
+            return torch.autograd.grad(out, xx, dy)[0]
+
+
+def refuse_full_neighbor_training(model):
+    if model.aggregator_cls is SeqAggregator:
+        raise NotImplementedError("full-neighbourhood training is not implemented for the seq aggregator (its neighbour "
+                                  "order is the sampled order)")
+    if hasattr(model.features, "c_table"):
+        raise NotImplementedError("full-neighbourhood training with a node-partitioned (ShardedFeatures) table is not "
+                                  "implemented")
+    if getattr(model, "distributed", False):
+        raise NotImplementedError("full-neighbourhood training with distributed=True is not implemented")
+    if getattr(model, "dropout_rate", 0.):
+        raise NotImplementedError("full-neighbourhood training with dropout > 0 is not implemented (the masks are "
+                                  "defined per sampled copy of a row; a whole neighbourhood has no such copies)")
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise NotImplementedError("a full-neighbourhood training step cannot be captured in a CUDA graph")
+
+
+def full_neighbor_graph(model, indptr, indices):
+    """The model's cached FullNeighborGraph for this CSR (rebuilt when the CSR tensors change)."""
+    g = getattr(model, "_full_neighbor_graph", None)
+    if g is None or g.key != FullNeighborGraph.key_of(indptr, indices):
+        g = model._full_neighbor_graph = FullNeighborGraph(indptr, indices)
+    return g
+
+
+def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True):
+    """full_neighbor_embeddings(indptr, indices, node_ids, normalize) with an autograd graph over the aggregator
+    weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
+    refuse_full_neighbor_training(model)
+    n_rows = int(model.features.shape[0])
+    indptr, indices = model._csr_input(indptr, torch.int64, "indptr"), model._csr_input(indices, torch.int32, "indices")
+    if indptr.dim() != 1 or indptr.numel() != n_rows:
+        raise ValueError("indptr must have N + 1 = %d entries (one row per node of the [N+1, .] table, plus the end)"
+                         % n_rows)
+    ids = torch.as_tensor(node_ids).to(device=model.device, dtype=torch.int32).reshape(-1)
+    # an id outside [0, N) reads the dummy node N in the forward; naming it N routes its gradient there too (same bits)
+    ids = torch.where((ids < 0) | (ids >= n_rows - 1), torch.full_like(ids, n_rows - 1), ids)
+    graph = full_neighbor_graph(model, indptr, indices)
+    h = model.features
+    L = len(model.aggregators)
+    for layer, agg in enumerate(model.aggregators):
+        v = agg.vars
+        if hasattr(agg, "mlp_layers"):
+            if len(agg.mlp_layers) != 1:
+                raise NotImplementedError("training supports one MLP layer")
+            mlp = agg.mlp_layers[0].vars
+            params = (v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"])
+        else:
+            params = (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
+        emb = getattr(model, "embeds", None) if layer == 0 else None
+        h = _FullLayerFn.apply(_FullLayer(agg, graph, ids if layer == L - 1 else None), h, emb, *params)
+    return _L2NormalizeFn.apply(h) if normalize else h

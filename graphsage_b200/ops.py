@@ -473,7 +473,7 @@ def segment_max(x, n, k):
     return out
 
 
-CSR_OPS = {"mean": _lib.CSR_MEAN, "mean_self": _lib.CSR_MEAN_SELF, "max": _lib.CSR_MAX}
+CSR_OPS = {"mean": _lib.CSR_MEAN, "mean_self": _lib.CSR_MEAN_SELF, "max": _lib.CSR_MAX, "sum": _lib.CSR_SUM}
 
 
 def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
@@ -481,8 +481,11 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
     for node v = rows[i] - or, without rows, for every node 0 .. N-1 and then the dummy node N (N = len(indptr) - 1: the
     [N+1, .] layout of the tables it reads) - over the source rows indices[indptr[v] .. indptr[v+1]) in CSR order - op "mean", "mean_self"
     (GCN: v's own row joins the sum, divisor count + 1) or "max".  An empty row, or v outside [0, len(indptr) - 1), reduces
-    over the last source row (the dummy) alone; entries outside the table read it too.  src: fp32 or bf16 [R, F] CUDA table.
-    Returns fp32 [n, F], a view of an [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed)."""
+    over the last source row (the dummy) alone; entries outside the table read it too.  op "sum" (fp32 src only): the plain
+    sum in CSR order, +0 for an empty row - the backward of the means over csr_transpose's graph
+    (oracle/full_neighbor_grad.py); its CSR has one row per source row (len(indptr) = R + 1), and without rows the output
+    is those R rows, with no extra dummy row.  src: fp32 or bf16 [R, F] CUDA table.  Returns fp32 [n, F], a view of an
+    [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed)."""
     require_cuda(src, indptr, indices, rows, out)
     if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
         raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
@@ -490,13 +493,20 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
         raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
     if op not in CSR_OPS:
         raise ValueError("op must be one of %s (got %r)" % (sorted(CSR_OPS), op))
+    if op == "sum" and src.dtype != torch.float32:
+        raise ValueError("op 'sum' reads float32 sources only")
+    if op == "sum" and indptr.numel() != src.shape[0] + 1:
+        # the sum runs over a square graph such as csr_transpose's: one CSR row per source row (the forward CSR of an
+        # [N+1, .] table has only N)
+        raise ValueError("op 'sum' needs one CSR row per source row: indptr of %d entries for %d source rows (got %d) - "
+                         "the layout of csr_transpose" % (src.shape[0] + 1, src.shape[0], indptr.numel()))
     indptr, indices = indptr.contiguous(), _i32(indices.reshape(-1), "indices")
     if indices.numel() == 0:
         indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
     n_nodes = indptr.numel() - 1
     if rows is not None:
         rows = _i32(rows.reshape(-1), "rows")
-    n, F = (n_nodes + 1 if rows is None else rows.numel()), src.shape[1]
+    n, F = (n_nodes + (op != "sum") if rows is None else rows.numel()), src.shape[1]
     if out is None:
         out = torch.empty((n, pad_cols(F)), dtype=torch.float32, device=src.device)
     if out.dtype != torch.float32 or out.dim() != 2 or out.stride(1) != 1 or out.shape[0] < n:
@@ -506,6 +516,71 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
                                  n_nodes, ptr(rows), n, CSR_OPS[op], ptr(out), out.stride(0), stream_ptr()))
     _launched(1 if n else 0, ev)
     return out[:n, :F]
+
+
+def _csr_args(indptr, indices):
+    require_cuda(indptr, indices)
+    if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
+        raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
+    return indptr.contiguous(), _i32(indices.reshape(-1), "indices")
+
+
+def csr_transpose(indptr, indices, with_self=False):
+    """The transpose of the effective CSR of the full-neighbourhood forward (gs_csr_transpose; contract in
+    oracle/full_neighbor_grad.py): over N + 1 rows (N = len(indptr) - 1), entries outside [0, N] read as N, an empty row and
+    the dummy row N as {N}, with_self (GCN) appending each row's own id.  Row j of the result lists, in ascending order,
+    the rows i with an entry j (once per entry).  Returns (t_indptr int64 [N + 2], t_indices int32 [capacity]): entries
+    past t_indptr[-1] are unspecified.  Built on the device - the entry count is not read back."""
+    indptr, indices = _csr_args(indptr, indices)
+    n_nodes, nnz, ws_self = indptr.numel() - 1, indices.numel(), int(bool(with_self))
+    nbytes = lib().gs_csr_transpose_workspace_bytes(n_nodes, nnz, ws_self)
+    if nbytes < 0:
+        check(-1)
+    cap = nnz + (n_nodes + 1) * (1 + ws_self)
+    t_indptr = torch.empty((n_nodes + 2,), dtype=torch.int64, device=indptr.device)
+    t_indices = torch.empty((cap,), dtype=torch.int32, device=indptr.device)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=indptr.device)
+    ev = _probe("csr_transpose/%d" % cap)
+    check(lib().gs_csr_transpose(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ws_self, ptr(t_indptr),
+                                 ptr(t_indices), ptr(ws), nbytes, stream_ptr()))
+    _launched(4, ev)                     # counts, fill, indptr (+ CUB's scan and sort passes)
+    return t_indptr, t_indices
+
+
+def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out=None):
+    """The gradient of m = csr_aggregate(z, indptr, indices, "max") over all N + 1 rows, through the ReLU that made z
+    (gs_csr_max_backward; oracle/full_neighbor_grad.py): s = dm / tie count per (row, column), then per node j the sum, in
+    transposed order, of s[i] over the rows i that read j where z[j] attains m[i]; +0 where z[j] <= 0.  z, m, dm: fp32
+    [N + 1, F] CUDA matrices with unit column stride; (t_indptr, t_indices) = csr_transpose(indptr, indices).  s: optional
+    [N + 1, >= F] scratch (the scale of phase (a), kept for inspection).  Returns fp32 [N + 1, F]."""
+    indptr, indices = _csr_args(indptr, indices)
+    t_indptr, t_indices = _csr_args(t_indptr, t_indices)
+    rows = indptr.numel()
+    if t_indptr.numel() != rows + 1:
+        raise ValueError("t_indptr must have N + 2 = %d entries" % (rows + 1))
+    for name, t in (("z", z), ("m", m), ("dm", dm)):
+        _fp32_table(t, name, 1)
+        if t.shape[0] != rows:
+            raise ValueError("%s must have N + 1 = %d rows" % (name, rows))
+    F = z.shape[1]
+    if m.shape[1] != F or dm.shape[1] != F:
+        raise ValueError("z, m and dm must have the same width")
+    if s is None:
+        s = torch.empty((rows, pad_cols(F)), dtype=torch.float32, device=z.device)
+    if out is None:
+        out = torch.empty((rows, pad_cols(F)), dtype=torch.float32, device=z.device)
+    for name, t in (("s", s), ("out", out)):
+        _fp32_table(t, name, F)
+        if t.shape[0] != rows:
+            raise ValueError("%s must have N + 1 = %d rows" % (name, rows))
+    if indices.numel() == 0:
+        indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
+    ev = _probe("csr_max_backward/%d" % rows)
+    check(lib().gs_csr_max_backward(ptr(z), z.stride(0), ptr(m), m.stride(0), ptr(dm), dm.stride(0), F, ptr(indptr),
+                                    ptr(indices), ptr(t_indptr), ptr(t_indices), rows - 1, ptr(s), s.stride(0), ptr(out),
+                                    out.stride(0), stream_ptr()))
+    _launched(2, ev)
+    return out[:, :F]
 
 
 class TableRows(object):

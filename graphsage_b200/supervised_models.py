@@ -585,6 +585,38 @@ class SupervisedGraphsage(SampleAndAggregate):
         with torch.no_grad():
             return self._predictions(self.logits(batch))
 
+    def full_neighbor_outputs(self, indptr, indices, node_ids):
+        """outputs() over whole neighbourhoods: full_neighbor_embeddings(indptr, indices, node_ids) - the same bits -
+        with an autograd graph over the aggregator weights and (identity_dim > 0) the node embeddings, for any head to
+        compose (contract: oracle/full_neighbor_grad.py).  The CSR's transposes are built on first use and cached on the
+        model, keyed by the CSR tensors' data_ptr, numel and _version.  Refused (NotImplementedError): the seq aggregator,
+        ShardedFeatures, distributed=True, training dropout > 0, CUDA-graph capture."""
+        from .full_neighbor_training import full_neighbor_outputs
+        return full_neighbor_outputs(self, indptr, indices, node_ids)
+
+    def full_neighbor_loss(self, indptr, indices, node_ids, labels):
+        """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids."""
+        out = self.full_neighbor_outputs(indptr, indices, node_ids)
+        logits = out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
+        self._last_logits = logits.detach()
+        labels = torch.as_tensor(labels).to(device=logits.device, dtype=torch.float32)
+        loss = classification_loss(logits, labels, self.sigmoid_loss)
+        if self.weight_decay:
+            loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)
+        return loss
+
+    def full_neighbor_train_step(self, indptr, indices, node_ids, labels):
+        """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling, no
+        dropout), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host synchronisation."""
+        loss = self.full_neighbor_loss(indptr, indices, node_ids, labels)
+        self.optimizer.zero_grad(set_to_none=True)
+        loss.backward()
+        for p in self.parameters():                                              # clip_by_value(grad, -5, 5)  :93-94
+            if p.grad is not None:
+                p.grad.clamp_(-5.0, 5.0)
+        self.optimizer.step()
+        return loss.detach()
+
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on
         full_neighbor_embeddings(indptr, indices, node_ids) - deterministic, no sampling, no dropout."""

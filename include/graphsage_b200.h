@@ -662,16 +662,54 @@ int32_t gs_random_walks_emit(const int32_t* starts, int64_t n, int32_t num_walks
  *   GS_CSR_MEAN      acc = +0; acc += x_j in order; out = acc / (float)count
  *   GS_CSR_MEAN_SELF the same, then acc += src[v] (v clamped like an entry); out = acc / (float)(count + 1)   (GCN)
  *   GS_CSR_MAX       m = x_0; m = fmaxf(m, x_j) in order                                       (gs_segment_max)
+ *   GS_CSR_SUM       see the backward below (fp32 only)
  * A CSR whose rows are a fixed-fanout sample gives the bits of gs_gather_mean / gs_segment_max.  dtype GS_F32, or GS_BF16
  * widened to fp32 (pitch % 8 == 0, out_pitch % 8 == 0, 16-byte-aligned src and out).  Output fp32 [n, out_pitch]; columns
  * F..out_pitch-1 are zeroed.  No allocation, no atomics, no host synchronisation: each output element is one sequential
  * chain, so two calls give the same bits.  Rows with more than 256 entries are spread over CTAs by 32-column slices.
  * --------------------------------------------------------------------------------------------- */
-typedef enum { GS_CSR_MEAN = 0, GS_CSR_MEAN_SELF = 1, GS_CSR_MAX = 2 } gs_csr_op;
+typedef enum { GS_CSR_MEAN = 0, GS_CSR_MEAN_SELF = 1, GS_CSR_MAX = 2, GS_CSR_SUM = 3 } gs_csr_op;
 int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
                          const int64_t* indptr, const int32_t* indices, int64_t n_nodes,
                          const int32_t* rows /* may be NULL */, int64_t n, int32_t op,
                          float* out, int64_t out_pitch, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Backward of the full-neighbourhood reductions (SupervisedGraphsage.full_neighbor_train_step).  Contract:
+ * oracle/full_neighbor_grad.py.  Nodes 0 .. N-1 have CSR rows; the dummy node N closes every [N+1, .] table.
+ *
+ * GS_CSR_SUM (op of gs_csr_aggregate above, GS_F32 only): acc = +0; acc += x_j in CSR order; out = acc.  A row with no
+ *   entries, or v outside [0, n_nodes), is +0 - not the dummy row.  With the transposed CSR below it is the backward of the
+ *   means: dsrc[j] = sum over the rows i that read j of g[i] / count_i, in ascending i.
+ *
+ * The EFFECTIVE CSR of the forward (N + 1 rows): row i < N holds its entries in CSR order, an entry outside [0, N] replaced
+ *   by N (the forward's clamp); an empty row (indptr[i+1] <= indptr[i]) holds {N}; the dummy row N holds {N}.  with_self
+ *   appends the row's own id i to every row (GS_CSR_MEAN_SELF).
+ * gs_csr_transpose - its transpose, on the device: t_indptr int64 [N + 2], t_indices int32 [capacity]; row j of the
+ *   transpose holds the source rows i of every effective entry equal to j, in ascending i, entries of one row in CSR
+ *   order (what a stable sort by destination gives: CUB's radix sort of (destination, source row) pairs in (i, position)
+ *   order).  t_indptr[N + 1] is the effective entry count; t_indices past it are unspecified.  capacity = nnz +
+ *   (N + 1) * (1 + with_self), nnz the length of `indices`, which every row's entries must lie in.  Integer work only, no
+ *   host synchronisation: the count stays on the device.  workspace: gs_csr_transpose_workspace_bytes(...) bytes;
+ *   -1 (see gs_last_error_string) outside the limits n_nodes < 2^31 - 2, capacity < 2^31.
+ * gs_csr_max_backward - the gradient of m = GS_CSR_MAX(z) (TensorFlow's reduce_max gradient: split evenly among ties),
+ *   then the ReLU of the Dense layer that made z (z = relu(.) >= 0):
+ *   (a) for every effective forward row i <= N and column c: cnt = #{entries e of row i : z[e][c] == m[i][c]}
+ *       (duplicates counted), s[i][c] = dm[i][c] / (float)cnt;
+ *   (b) for every node j <= N: acc = +0; for i in transposed row j, in order: if z[j][c] == m[i][c], acc += s[i][c];
+ *       dz[j][c] = z[j][c] > 0 ? acc : +0.
+ *   z, m, dm, s, dz: fp32 [N + 1, F] with their own row pitches (only columns 0..F-1 are read or written).  s is the
+ *   caller's scratch, read by (b).  Each output element is
+ *   one sequential chain; rows longer than 256 entries are spread over CTAs by 32-column slices (gs_csr_aggregate's hub
+ *   split).  No allocation, no atomics, no host synchronisation: two calls give the same bits.
+ * --------------------------------------------------------------------------------------------- */
+int64_t gs_csr_transpose_workspace_bytes(int64_t n_nodes, int64_t nnz, int32_t with_self);
+int32_t gs_csr_transpose(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t with_self,
+                         int64_t* t_indptr, int32_t* t_indices, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm, int64_t lddm,
+                            int32_t F, const int64_t* indptr, const int32_t* indices, const int64_t* t_indptr,
+                            const int32_t* t_indices, int64_t n_nodes, float* s, int64_t lds, float* dz, int64_t lddz,
+                            void* stream);
 
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
