@@ -52,6 +52,7 @@ MAX_UNIQUE_SAMPLED = 1024          # GS_MAX_UNIQUE_SAMPLED
 UNIQUE_DRAW_BUDGET = 1 << 20       # GS_UNIQUE_DRAW_BUDGET
 WALK_MAX_WALKS = 1 << 20           # GS_WALK_MAX_WALKS
 WALK_MAX_LEN = 33                  # GS_WALK_MAX_LEN
+MAX_BLOCK_LAYERS = 8               # GS_MAX_BLOCK_LAYERS
 
 
 class EmbedGradList(ctypes.Structure):
@@ -159,6 +160,11 @@ _SIGNATURES = {
     "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gs_csr_max_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64,
                                     c_vp, c_i64, c_vp]),
+    "gs_csr_blocks_workspace_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i32]),
+    "gs_csr_blocks_plan": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp]),
+    "gs_csr_blocks_fill": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, ctypes.POINTER(c_i64),
+                                   ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
+                                   c_vp]),
 }
 
 _lib = None

@@ -12,6 +12,13 @@ The pools run their MLP once per node, as full_neighbor_embeddings does, whateve
 layer's whole [N+1, in] table, so its gradient dZ Wm^T needs no transpose.  Layer-0 feature columns are not trainable:
 with identity_dim = 0 layer 0 computes no source gradient (the pools still compute dWm, dbm); with identity_dim = d > 0 it
 computes columns [0, d) only, which autograd delivers as model.embeds.grad (a dense [N+1, d] tensor).
+
+Minibatches (full_neighbor_minibatch_outputs; contract: oracle/full_neighbor_blocks.py) run the same layers over the
+seeds' receptive field: ops.csr_blocks builds one block per layer - a local CSR over V_l, the nodes layer l reads - and
+layer l runs over its block with the block's rows, exactly as the whole-graph layers run over the whole CSR.  Layer 0
+reads the global table: the means through the global CSR with rows = V_1, the pools' MLP on V_0's rows only (read by id,
+ops.TableRows), reduced through block 0.  Same bits as the whole-graph pass for the seeds; every buffer is block-sized.
+The blocks and their transposes are built per call, not cached.
 """
 import torch
 
@@ -55,12 +62,17 @@ class FullNeighborGraph(object):
 
 
 class _FullLayer(object):
-    """One aggregator layer over every node: rows None computes all N + 1 rows, else (the last layer) the rows of `rows`."""
+    """One aggregator layer over a graph's rows: rows None computes all of them, else the rows of `rows` (ids of the
+    graph's nodes).  A block's layer 0 (src_ids = V_0's global ids) reads the global [N+1, .] table instead: its reductions
+    of the table through table_csr = (global indptr, global indices, V_1's global ids), the pools' MLP on V_0's rows;
+    everything after the MLP, and the whole backward, is in the graph's (block 0's) local space."""
 
-    def __init__(self, agg, graph, rows):
+    def __init__(self, agg, graph, rows, src_ids=None, table_csr=None):
         self.agg, self.graph, self.rows = agg, graph, rows
+        self.src_ids, self.table_csr = src_ids, table_csr
         self.gcn = isinstance(agg, GCNAggregator)
         self.pool = isinstance(agg, MaxPoolingAggregator)
+        self.table = None
 
     def dense(self, x):
         """The [N+1, w] gradient of the rows this layer outputs: x itself, or the scatter of x into rows' ids."""
@@ -68,21 +80,32 @@ class _FullLayer(object):
             return x
         return ops.embedding_grad([(self.rows, x.contiguous(), 1, 1.0)], self.graph.n_rows, x.shape[1])
 
+    def table_grad(self, d):
+        """The gradient of the layer's source table from d, the source gradient in the graph's row space."""
+        if self.src_ids is None:
+            return d
+        return ops.embedding_grad([(self.src_ids, d, 1, 1.0)], self.table.shape[0], d.shape[1])
+
     def forward(self, h, kept):
         """The GEMM parts of full_neighbor_embeddings' layer; `kept` receives what the backward reads besides them."""
         agg, g, rows = self.agg, self.graph, self.rows
-        indptr, indices = g.indptr, g.indices
+        self.table = h if self.src_ids is not None else None
+        indptr, indices, h_rows = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows)
         if self.gcn:
-            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=rows)
+            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=h_rows)
             return [(m, agg.neigh_input_dim, agg.vars["weights"])]
         widen = h.dtype != torch.float32
-        n = h.shape[0] if rows is None else rows.numel()
-        hs = _rows(h, rows, 0, n, widen) if (widen or rows is not None) else h
+        n = h.shape[0] if h_rows is None else h_rows.numel()
+        hs = _rows(h, h_rows, 0, n, widen) if (widen or h_rows is not None) else h
         if not self.pool:
-            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=rows)
+            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=h_rows)
             return [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
-        x = _rows(h, None, 0, h.shape[0], True) if widen else h
-        z = x
+        if self.src_ids is None:
+            x = z = _rows(h, None, 0, h.shape[0], True) if widen else h
+        elif widen:
+            x = z = ops.gather_rows_f32(h, self.src_ids)             # V_0's rows, widened
+        else:                                                        # V_0's rows read by id: no gathered copy
+            x, z = None, ops.TableRows(h, [(self.src_ids, 0)], self.src_ids.numel())
         for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116), once per node
             code, post = act_code(dense.act)
             if getattr(dense, "_packed", None) is None:
@@ -92,10 +115,10 @@ class _FullLayer(object):
             z = post(z) if post else z
         op = "max" if agg.pool == "max" else "mean"
         if op == "max" and rows is not None:         # the backward needs every row's max: the same chains, then the rows
-            p_all = ops.csr_aggregate(z, indptr, indices, "max")
+            p_all = ops.csr_aggregate(z, g.indptr, g.indices, "max")
             p = p_all.index_select(0, rows)
         else:
-            p = p_all = ops.csr_aggregate(z, indptr, indices, op, rows=rows)
+            p = p_all = ops.csr_aggregate(z, g.indptr, g.indices, op, rows=rows)
         kept.extend([x, z, p_all])
         return [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
 
@@ -113,6 +136,8 @@ class _FullLayer(object):
             return [], self.graph.mean_backward(self.dense(dzs[1] @ Wn[:cols].t()), False) + dself
         Wm = params[2]
         x, z, p_all = kept
+        if x is None:                                # the MLP read V_0's rows by id: gather them for dWm
+            x = ops.gather_rows_f32(self.table, self.src_ids)
         dp = self.dense(dzs[1] @ Wn.t())
         if self.agg.pool == "max":
             t_indptr, t_indices = self.graph.transpose(False)
@@ -158,7 +183,7 @@ class _FullLayerFn(torch.autograd.Function):
         cols = ctx.F_in if ctx.src_needs_grad else ctx.emb_d
         grads_own, dsrc = ctx.layer.backward(xs, dzs, params, kept, cols)
         dh = dsrc if ctx.src_needs_grad else None
-        demb = dsrc[:, :ctx.emb_d] if ctx.emb_d and dsrc is not None else None
+        demb = ctx.layer.table_grad(dsrc[:, :ctx.emb_d]) if ctx.emb_d and dsrc is not None else None
         return (None, dh, demb) + tuple(grads_w) + tuple(grads_own)
 
 
@@ -180,6 +205,11 @@ class _L2NormalizeFn(torch.autograd.Function):
             return torch.autograd.grad(out, xx, dy)[0]
 
 
+def refuse_capture(what):
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise NotImplementedError("%s cannot be captured in a CUDA graph" % what)
+
+
 def refuse_full_neighbor_training(model):
     if model.aggregator_cls is SeqAggregator:
         raise NotImplementedError("full-neighbourhood training is not implemented for the seq aggregator (its neighbour "
@@ -192,8 +222,7 @@ def refuse_full_neighbor_training(model):
     if getattr(model, "dropout_rate", 0.):
         raise NotImplementedError("full-neighbourhood training with dropout > 0 is not implemented (the masks are "
                                   "defined per sampled copy of a row; a whole neighbourhood has no such copies)")
-    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
-        raise NotImplementedError("a full-neighbourhood training step cannot be captured in a CUDA graph")
+    refuse_capture("a full-neighbourhood training step")
 
 
 def full_neighbor_graph(model, indptr, indices):
@@ -204,30 +233,80 @@ def full_neighbor_graph(model, indptr, indices):
     return g
 
 
-def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True):
-    """full_neighbor_embeddings(indptr, indices, node_ids, normalize) with an autograd graph over the aggregator
-    weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
-    refuse_full_neighbor_training(model)
+def _inputs(model, indptr, indices, node_ids):
+    """(indptr, indices, ids): the CSR on the model's device, checked, and node_ids as int32 with every id outside [0, N)
+    named N - it reads the dummy node in the forward; naming it N routes its gradient there too (same bits)."""
     n_rows = int(model.features.shape[0])
     indptr, indices = model._csr_input(indptr, torch.int64, "indptr"), model._csr_input(indices, torch.int32, "indices")
     if indptr.dim() != 1 or indptr.numel() != n_rows:
         raise ValueError("indptr must have N + 1 = %d entries (one row per node of the [N+1, .] table, plus the end)"
                          % n_rows)
     ids = torch.as_tensor(node_ids).to(device=model.device, dtype=torch.int32).reshape(-1)
-    # an id outside [0, N) reads the dummy node N in the forward; naming it N routes its gradient there too (same bits)
     ids = torch.where((ids < 0) | (ids >= n_rows - 1), torch.full_like(ids, n_rows - 1), ids)
-    graph = full_neighbor_graph(model, indptr, indices)
+    return indptr, indices, ids
+
+
+def _params(agg):
+    v = agg.vars
+    if hasattr(agg, "mlp_layers"):
+        if len(agg.mlp_layers) != 1:
+            raise NotImplementedError("training supports one MLP layer")
+        mlp = agg.mlp_layers[0].vars
+        return v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"]
+    return (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
+
+
+def _outputs(model, layers, normalize):
     h = model.features
-    L = len(model.aggregators)
-    for layer, agg in enumerate(model.aggregators):
-        v = agg.vars
-        if hasattr(agg, "mlp_layers"):
-            if len(agg.mlp_layers) != 1:
-                raise NotImplementedError("training supports one MLP layer")
-            mlp = agg.mlp_layers[0].vars
-            params = (v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"])
-        else:
-            params = (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
+    for layer, fl in enumerate(layers):
         emb = getattr(model, "embeds", None) if layer == 0 else None
-        h = _FullLayerFn.apply(_FullLayer(agg, graph, ids if layer == L - 1 else None), h, emb, *params)
+        h = _FullLayerFn.apply(fl, h, emb, *_params(fl.agg))
     return _L2NormalizeFn.apply(h) if normalize else h
+
+
+def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True):
+    """full_neighbor_embeddings(indptr, indices, node_ids, normalize) with an autograd graph over the aggregator
+    weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
+    refuse_full_neighbor_training(model)
+    indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
+    graph = full_neighbor_graph(model, indptr, indices)
+    L = len(model.aggregators)
+    return _outputs(model, [_FullLayer(agg, graph, ids if layer == L - 1 else None)
+                            for layer, agg in enumerate(model.aggregators)], normalize)
+
+
+def minibatch_layers(aggregators, indptr, indices, ids):
+    """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped)."""
+    L = len(aggregators)
+    blocks = ops.csr_blocks(indptr, indices, ids, L)
+    layers = []
+    for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
+        graph = FullNeighborGraph(b.indptr, b.indices)
+        if layer == 0:
+            v1 = blocks[1].src_ids if L > 1 else ids
+            layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
+        else:
+            layers.append(_FullLayer(agg, graph, b.rows))
+    return layers
+
+
+def full_neighbor_minibatch_outputs(model, indptr, indices, node_ids, normalize=True):
+    """full_neighbor_outputs(indptr, indices, node_ids, normalize) over the receptive-field blocks of node_ids: the same
+    values, bit for bit, with buffers sized by the blocks instead of the graph.  Reads the block sizes back once."""
+    refuse_full_neighbor_training(model)
+    indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
+    return _outputs(model, minibatch_layers(model.aggregators, indptr, indices, ids), normalize)
+
+
+def full_neighbor_minibatch_embeddings(model, indptr, indices, node_ids, normalize=True):
+    """SampleAndAggregate.full_neighbor_embeddings(indptr, indices, node_ids, normalize) over the receptive-field blocks
+    of node_ids, without autograd: the same bits."""
+    refuse_capture("full_neighbor_minibatch_embeddings (it reads the block sizes back)")
+    indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
+    h = model.features
+    with torch.no_grad():
+        for fl in minibatch_layers(model.aggregators, indptr, indices, ids):
+            h = fl.agg._finish(fl.forward(h, []), fl.agg._combine())
+        if normalize:
+            h = ops.l2_normalize_rows_(h.contiguous())
+    return h

@@ -288,6 +288,25 @@ class SampleAndAggregate(object):
                 h = ops.l2_normalize_rows_(h.contiguous())
         return h
 
+    def full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True):
+        """full_neighbor_embeddings(indptr, indices, node_ids, normalize) - torch.equal to it - computed over the
+        receptive field of node_ids only (contract: oracle/full_neighbor_blocks.py): ops.csr_blocks builds, on the
+        device, one block per layer holding the nodes that layer must compute, and each layer runs over its block.  Cost
+        and memory follow the blocks, not the graph: use it when node_ids' receptive field is a small part of the graph
+        (serving, evaluating a split in batches).  Reads the block sizes back once per call (a synchronisation), so it
+        cannot be captured in a CUDA graph.  Same refusals as full_neighbor_embeddings."""
+        if self.aggregator_cls is SeqAggregator:
+            raise NotImplementedError("full-neighbourhood inference is not implemented for the seq aggregator (its "
+                                      "neighbour order is the sampled order)")
+        if hasattr(self.features, "c_table"):
+            raise NotImplementedError("full-neighbourhood inference with a node-partitioned (ShardedFeatures) table is "
+                                      "not implemented")
+        if self.aggregators is None:
+            from .supervised_models import build_aggregators
+            self.aggregators = build_aggregators(self)
+        from .full_neighbor_training import full_neighbor_minibatch_embeddings
+        return full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize)
+
     def _csr_input(self, t, dtype, name):
         """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""
         if not torch.is_tensor(t):

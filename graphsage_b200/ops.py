@@ -1,5 +1,7 @@
 """Functional wrappers: torch CUDA tensors in, torch CUDA tensors out, all work done by
 libgraphsage_b200.so on the current CUDA stream.  torch only owns memory and streams here."""
+import collections
+
 import torch
 
 from . import _lib
@@ -581,6 +583,46 @@ def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out
                                     out.stride(0), stream_ptr()))
     _launched(2, ev)
     return out[:, :F]
+
+
+CsrBlock = collections.namedtuple("CsrBlock", ["src_ids", "indptr", "indices", "rows"])   # one layer of csr_blocks
+
+
+def csr_blocks(indptr, indices, seeds, n_layers):
+    """The receptive field of `seeds` over n_layers layers of whole neighbourhoods (gs_csr_blocks_plan / _fill; contract
+    in oracle/full_neighbor_blocks.py): a list, index l = layer l, of CsrBlock(src_ids int32 V_l, indptr int64 [|V_l|],
+    indices int32, rows int32).  A block is a CSR over |V_l| - 1 local nodes whose last local row is the dummy, so
+    csr_aggregate(table of V_l's rows, indptr, indices, rows=rows) gives the whole-graph layer's rows of the next level.
+    Built on the device; the 2L sizes are read back once to allocate the outputs - one device-to-host copy (and so a
+    synchronisation) per call, not meant for capture."""
+    require_cuda(indptr, indices, seeds)
+    if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
+        raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
+    indptr, indices, seeds = indptr.contiguous(), _i32(indices.reshape(-1), "indices"), _i32(seeds.reshape(-1), "seeds")
+    L = int(n_layers)
+    if not 1 <= L <= _lib.MAX_BLOCK_LAYERS:
+        raise ValueError("n_layers must be in [1, %d] (got %d)" % (_lib.MAX_BLOCK_LAYERS, L))
+    n_nodes, nnz, n = indptr.numel() - 1, indices.numel(), seeds.numel()
+    nbytes = lib().gs_csr_blocks_workspace_bytes(n_nodes, nnz, n, L)
+    if nbytes < 0:
+        check(-1)
+    dev = indptr.device
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+    counts = torch.empty((2 * L,), dtype=torch.int64, device=dev)
+    ev = _probe("csr_blocks/%d" % n)
+    check(lib().gs_csr_blocks_plan(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L,
+                                   ptr(ws), nbytes, ptr(counts), stream_ptr()))
+    sizes = [int(x) for x in counts.tolist()]                # the one device-to-host read
+    out_rows = [sizes[2 * l + 2] for l in range(L - 1)] + [n]
+    blocks = [CsrBlock(torch.empty((sizes[2 * l],), dtype=torch.int32, device=dev),
+                       torch.empty((sizes[2 * l],), dtype=torch.int64, device=dev),
+                       torch.empty((sizes[2 * l + 1],), dtype=torch.int32, device=dev),
+                       torch.empty((out_rows[l],), dtype=torch.int32, device=dev)) for l in range(L)]
+    arrs = [(_lib.c_vp * L)(*[ptr(b[k]) if b[k].numel() else 0 for b in blocks]) for k in range(4)]
+    check(lib().gs_csr_blocks_fill(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L,
+                                   ptr(ws), nbytes, (_lib.c_i64 * (2 * L))(*sizes), *arrs, stream_ptr()))
+    _launched(6 * L + 4, ev)           # plan: mark, compact, size, degrees per level; fill: degrees, fill, rows (+ CUB)
+    return blocks
 
 
 class TableRows(object):

@@ -596,7 +596,9 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def full_neighbor_loss(self, indptr, indices, node_ids, labels):
         """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids."""
-        out = self.full_neighbor_outputs(indptr, indices, node_ids)
+        return self._head_loss(self.full_neighbor_outputs(indptr, indices, node_ids), labels)
+
+    def _head_loss(self, out, labels):
         logits = out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
         self._last_logits = logits.detach()
         labels = torch.as_tensor(labels).to(device=logits.device, dtype=torch.float32)
@@ -608,7 +610,9 @@ class SupervisedGraphsage(SampleAndAggregate):
     def full_neighbor_train_step(self, indptr, indices, node_ids, labels):
         """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling, no
         dropout), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host synchronisation."""
-        loss = self.full_neighbor_loss(indptr, indices, node_ids, labels)
+        return self._clipped_step(self.full_neighbor_loss(indptr, indices, node_ids, labels))
+
+    def _clipped_step(self, loss):
         self.optimizer.zero_grad(set_to_none=True)
         loss.backward()
         for p in self.parameters():                                              # clip_by_value(grad, -5, 5)  :93-94
@@ -616,6 +620,23 @@ class SupervisedGraphsage(SampleAndAggregate):
                 p.grad.clamp_(-5.0, 5.0)
         self.optimizer.step()
         return loss.detach()
+
+    def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids):
+        """full_neighbor_outputs over the receptive field of node_ids only: the same values, bit for bit, with per-layer
+        blocks built on the device by ops.csr_blocks (contract: oracle/full_neighbor_blocks.py) and their transposes built
+        per call, not cached.  Cost and memory follow the blocks, not the graph: the minibatch form of exact-neighbourhood
+        training.  Reads the block sizes back once per call.  Same refusals as full_neighbor_outputs."""
+        from .full_neighbor_training import full_neighbor_minibatch_outputs
+        return full_neighbor_minibatch_outputs(self, indptr, indices, node_ids)
+
+    def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels):
+        """full_neighbor_loss over full_neighbor_minibatch_outputs: the same head, cross-entropy and weight decay."""
+        return self._head_loss(self.full_neighbor_minibatch_outputs(indptr, indices, node_ids), labels)
+
+    def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels):
+        """full_neighbor_train_step for a minibatch: one Adam step on full_neighbor_minibatch_loss, gradients clipped to
+        +-5.  Returns the detached loss."""
+        return self._clipped_step(self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels))
 
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on

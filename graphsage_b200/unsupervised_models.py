@@ -113,6 +113,38 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         self.optimizer.step()
         return loss.detach()
 
+    def full_neighbor_minibatch_loss(self, indptr, indices, batch1, batch2):
+        """loss() with every embedding computed over whole neighbourhoods (contract: oracle/full_neighbor_blocks.py): the
+        negatives are drawn first, as _passes draws them (one neg_sampler call); ONE set of receptive-field blocks is
+        built over cat(batch1, batch2, negatives) and its outputs split; then the same link-prediction loss and weight
+        decay, divided by len(batch1), and the affinities for mrr().  Reads the block sizes back once per call.  Refused
+        (NotImplementedError): the seq aggregator, ShardedFeatures, distributed=True, training dropout > 0, CUDA-graph
+        capture."""
+        from .full_neighbor_training import full_neighbor_minibatch_outputs, refuse_full_neighbor_training
+        refuse_full_neighbor_training(self)
+        neg = self.neg_sampler(self.neg_sample_size)
+        b1, b2 = (torch.as_tensor(b).to(device=self.device, dtype=torch.int32).reshape(-1) for b in (batch1, batch2))
+        out = full_neighbor_minibatch_outputs(self, indptr, indices, torch.cat([b1, b2, neg]))
+        o1, o2, on = torch.split(out, [b1.numel(), b2.numel(), neg.numel()])
+        loss = self.link_pred_layer.loss(o1, o2, on)
+        if self.weight_decay:
+            loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)
+        with torch.no_grad():
+            self._last = (self.link_pred_layer.affinity(o1, o2), self.link_pred_layer.neg_cost(o1, on))
+        return loss / float(o1.shape[0])
+
+    def full_neighbor_minibatch_train_step(self, indptr, indices, batch1, batch2):
+        """One Adam step on full_neighbor_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the
+        detached loss."""
+        loss = self.full_neighbor_minibatch_loss(indptr, indices, batch1, batch2)
+        self.optimizer.zero_grad(set_to_none=True)
+        loss.backward()
+        for p in self.parameters():
+            if p.grad is not None:
+                p.grad.clamp_(-5.0, 5.0)                                             # models.py:380-381
+        self.optimizer.step()
+        return loss.detach()
+
     def graphed_train_step(self, batch_size):
         """train_step for a fixed batch size captured in one CUDA graph: returns step(batch1, batch2) -> loss, a static 0-d
         CUDA tensor (see graphed_training.GraphedTrainStep; a short last batch runs through the eager train_step)."""

@@ -711,6 +711,34 @@ int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t
                             const int32_t* t_indices, int64_t n_nodes, float* s, int64_t lds, float* dz, int64_t lddz,
                             void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Receptive-field blocks of a minibatch over whole neighbourhoods (full_neighbor_minibatch_*).  Contract:
+ * oracle/full_neighbor_blocks.py.  For a CSR over nodes 0 .. N-1 (N = n_nodes; the dummy node is N), seeds clamped to
+ * [0, N] (an id outside [0, N) is N) and L = n_layers: V_L = the seeds; V_l (l = L-1 .. 0) = the sorted-unique union of
+ * V_{l+1}, the clamped entries of V_{l+1}'s raw rows, and {N}.  Block l: src_ids int32 [|V_l|] = V_l; indptr int64
+ * [|V_l|] - one row per local node but the last (the dummy), V_{l+1}'s members holding their raw rows relabelled to
+ * positions in V_l, every other row empty; indices int32 [entries]; rows int32 = the positions in V_l of V_{l+1}
+ * (l < L-1, ascending) or of the clamped seeds (l = L-1, in seed order).  gs_csr_aggregate over a block with its rows
+ * gives the whole-graph layer's bits for those nodes.
+ * gs_csr_blocks_plan - device only: builds every V_l and writes counts_dev int64 [2L] = (|V_l|, entries of block l) for
+ *   l = 0 .. L-1.  No host synchronisation inside; the caller reads counts_dev once to size the outputs.
+ * gs_csr_blocks_fill - with the same workspace, after gs_csr_blocks_plan on the same stream, and counts = a HOST copy of
+ *   counts_dev: writes the blocks into the caller's arrays (one pointer per block; n_out = |V_{l+1}| or n_seeds rows).
+ * Integer work only, no atomics: two calls give the same bytes.  workspace: gs_csr_blocks_workspace_bytes(...) bytes,
+ *   (L + 1) id arrays and position maps of N + 2 int32, a flag array, an int64 degree array and CUB's temporary storage;
+ *   -1 (see gs_last_error_string) outside n_nodes < 2^31 - 3, n_seeds < 2^31, 1 <= n_layers <= GS_MAX_BLOCK_LAYERS.
+ * --------------------------------------------------------------------------------------------- */
+#define GS_MAX_BLOCK_LAYERS 8
+int64_t gs_csr_blocks_workspace_bytes(int64_t n_nodes, int64_t nnz, int64_t n_seeds, int32_t n_layers);
+int32_t gs_csr_blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers, void* workspace,
+                           int64_t workspace_bytes, int64_t* counts_dev, void* stream);
+int32_t gs_csr_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers, void* workspace,
+                           int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
+                           int64_t* const* indptr_out, int32_t* const* indices_out, int32_t* const* rows_out,
+                           void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
