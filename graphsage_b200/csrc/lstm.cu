@@ -48,14 +48,15 @@ __global__ void __launch_bounds__(256) seq_lengths_kernel(const float* __restric
   }
 }
 
-// Sets lens[] (0 for rows past n, clamped to k) and returns the tile's longest length.  Ends with a barrier.
+// Sets lens[] (len clamped to [0, k]; 0 for rows past n) and returns the tile's longest length.  Ends with a barrier.
+// The clamp below 0 keeps `L - 1` (the backward's dh_last step) free of overflow for any int32 length.
 template <int S>
 __device__ __forceinline__ int load_tile_lengths(const int32_t* __restrict__ len, int64_t s0, int64_t n, int32_t k,
                                                  int* lens, int* tile_len) {
   if (threadIdx.x < S) {
     const int64_t i = s0 + threadIdx.x;
     const int L = i < n ? len[i] : 0;
-    lens[threadIdx.x] = L < k ? L : k;
+    lens[threadIdx.x] = L < 0 ? 0 : L < k ? L : k;
   }
   __syncthreads();
   if (threadIdx.x == 0) {

@@ -571,7 +571,9 @@ int32_t gs_skipgram_grad(const float* target, int64_t ldt, const float* context,
  *   that is not zero (-0.0 is zero), len[i] = max(1, sum_j used[i, j]).  The LSTM runs over the FIRST len[i] positions,
  *   whatever they hold.
  * gs_lstm_forward - P [n·k, 4H] (ldp) = X·W_x + b from the input projection; Wh the [H, 4H] recurrent block W_h (the
- *   kernel's bottom H rows, ldw).  Writes h_last[i] = h after len[i] steps ([n, H], ldh; len is clamped to k).
+ *   kernel's bottom H rows, ldw).  Writes h_last[i] = h after len[i] steps ([n, H], ldh).  Both kernels clamp len[i]
+ *   to [0, k]: a length above k runs k steps; a length <= 0 runs none (h_last[i] = 0, every saved row and every dZ
+ *   row of sequence i zero; its P rows and dh_last row are not read).  P rows t >= len[i] are never read either.
  *   Training outputs, all three or none (NULL): gates [n·k, 4H] = (σ(z_i), tanh(z_j), σ(z_f + 1), σ(z_o)), c [n·k, H] = c_t,
  *   h_prev [n·k, H] = h_{t-1} (zero at t = 0); rows t >= len[i] are zeros.  Limits: H in {128, 256}, k >= 1, n < 2^31.
  * gs_lstm_backward - backpropagation through time from dh_last [n, H] (the gradient of h_last) with the forward's saved
