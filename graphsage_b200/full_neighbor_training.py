@@ -1,9 +1,10 @@
-"""Full-batch training over whole neighbourhoods: the differentiable form of SampleAndAggregate.full_neighbor_embeddings
-(contract: oracle/full_neighbor_grad.py).
+"""Whole-neighbourhood layers: SampleAndAggregate.full_neighbor_embeddings (contract: oracle/full_neighbor.py) and its
+differentiable form, full-batch training (contract: oracle/full_neighbor_grad.py).
 
-One torch.autograd.Function per layer (_FullLayerFn, the layer-wise counterpart of supervised_models._LayerFn).  Its
-forward is full_neighbor_embeddings' layer, launch for launch, so the values are the same bits.  Its backward:
-  - weight gradients dW = X^T dZ as library matmuls, as in the sampled path;
+One layer implementation, _FullLayer, serves both.  Inference runs its forward under no_grad; training runs it as a
+branch of supervised_models._LayerFn, the autograd Function of every aggregator, so the training forward is the
+inference layer and the values are the same bits.  The backward:
+  - weight gradients dW = X^T dZ as library matmuls, as in the sampled path (_LayerFn);
   - source gradients through the CSR kernels over the transposed graph (ops.csr_transpose, built once per CSR and cached
     on the model): the means' backward is ops.csr_aggregate(op="sum") of g / count, the max-pool's ops.csr_max_backward;
   - the last layer reads only the rows of node_ids (duplicates allowed): their gradients are scattered into a dense
@@ -13,7 +14,7 @@ layer's whole [N+1, in] table, so its gradient dZ Wm^T needs no transpose.  Laye
 with identity_dim = 0 layer 0 computes no source gradient (the pools still compute dWm, dbm); with identity_dim = d > 0 it
 computes columns [0, d) only, which autograd delivers as model.embeds.grad (a dense [N+1, d] tensor).
 
-Minibatches (full_neighbor_minibatch_outputs; contract: oracle/full_neighbor_blocks.py) run the same layers over the
+Minibatches (minibatch=True; contract: oracle/full_neighbor_blocks.py) run the same layers over the
 seeds' receptive field: ops.csr_blocks builds one block per layer - a local CSR over V_l, the nodes layer l reads - and
 layer l runs over its block with the block's rows, exactly as the whole-graph layers run over the whole CSR.  Layer 0
 reads the global table: the means through the global CSR with rows = V_1, the pools' MLP on V_0's rows only (read by id,
@@ -25,6 +26,7 @@ import torch
 from . import ops
 from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, _rows
 from .layers import act_code
+from .supervised_models import _LayerFn, build_aggregators, layer_params
 
 
 class FullNeighborGraph(object):
@@ -62,16 +64,18 @@ class FullNeighborGraph(object):
 
 
 class _FullLayer(object):
-    """One aggregator layer over a graph's rows: rows None computes all of them, else the rows of `rows` (ids of the
-    graph's nodes).  A block's layer 0 (src_ids = V_0's global ids) reads the global [N+1, .] table instead: its reductions
-    of the table through table_csr = (global indptr, global indices, V_1's global ids), the pools' MLP on V_0's rows;
-    everything after the MLP, and the whole backward, is in the graph's (block 0's) local space."""
+    """One aggregator layer over a graph's rows, and the _LayerFn branch that trains it: rows None computes all of them,
+    else the rows of `rows` (ids of the graph's nodes).  A block's layer 0 (src_ids = V_0's global ids) reads the global
+    [N+1, .] table instead: its reductions of the table through table_csr = (global indptr, global indices, V_1's global
+    ids), the pools' MLP on V_0's rows; everything after the MLP, and the whole backward, is in the graph's (block 0's)
+    local space."""
 
     def __init__(self, agg, graph, rows, src_ids=None, table_csr=None):
         self.agg, self.graph, self.rows = agg, graph, rows
         self.src_ids, self.table_csr = src_ids, table_csr
         self.gcn = isinstance(agg, GCNAggregator)
         self.pool = isinstance(agg, MaxPoolingAggregator)
+        self.row_parts = 1 if self.gcn or self.pool else 2      # the GEMM parts that are rows of the source
         self.table = None
 
     def dense(self, x):
@@ -87,7 +91,8 @@ class _FullLayer(object):
         return ops.embedding_grad([(self.src_ids, d, 1, 1.0)], self.table.shape[0], d.shape[1])
 
     def forward(self, h, kept):
-        """The GEMM parts of full_neighbor_embeddings' layer; `kept` receives what the backward reads besides them."""
+        """The GEMM parts of the layer.  kept: None for inference, else a list that receives what the backward reads
+        besides the parts."""
         agg, g, rows = self.agg, self.graph, self.rows
         self.table = h if self.src_ids is not None else None
         indptr, indices, h_rows = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows)
@@ -114,31 +119,29 @@ class _FullLayer(object):
                               math=agg.math, packed=dense._packed)
             z = post(z) if post else z
         op = "max" if agg.pool == "max" else "mean"
-        if op == "max" and rows is not None:         # the backward needs every row's max: the same chains, then the rows
+        if kept is not None and op == "max" and rows is not None:
+            # training: the backward needs every row's max - the same chains, then the rows
             p_all = ops.csr_aggregate(z, g.indptr, g.indices, "max")
             p = p_all.index_select(0, rows)
         else:
             p = p_all = ops.csr_aggregate(z, g.indptr, g.indices, op, rows=rows)
-        kept.extend([x, z, p_all])
+        if kept is not None:
+            kept.extend([x, z, p_all])
         return [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
 
-    def backward(self, xs, dzs, params, kept, cols):
-        """(gradients of the branch's own parameters, d(source) [N + 1, cols] or None)."""
+    def backward(self, xs, dxs, params, kept, cols):
+        """(gradients of the pools' Wm, bm, d(source) [N + 1, cols] or None) from dxs, the gradients of the parts' rows."""
+        for p in range(len(dxs)):                    # made dense in place: each row gradient is freed once scattered
+            if dxs[p] is not None:
+                dxs[p] = self.dense(dxs[p])
         if self.gcn:
-            if not cols:
-                return [], None
-            return [], self.graph.mean_backward(self.dense(dzs[0] @ params[0][:cols].t()), True)
-        Ws, Wn = params[0], params[1]
-        dself = self.dense(dzs[0] @ Ws[:cols].t()) if cols else None
+            return [], (self.graph.mean_backward(dxs[0], True) if cols else None)
+        dself = dxs[0]
         if not self.pool:
-            if not cols:
-                return [], None
-            return [], self.graph.mean_backward(self.dense(dzs[1] @ Wn[:cols].t()), False) + dself
-        Wm = params[2]
-        x, z, p_all = kept
+            return [], (self.graph.mean_backward(dxs[1], False) + dself if cols else None)
+        (Wm, _), (x, z, p_all), dp = params, kept, dxs[1]
         if x is None:                                # the MLP read V_0's rows by id: gather them for dWm
             x = ops.gather_rows_f32(self.table, self.src_ids)
-        dp = self.dense(dzs[1] @ Wn.t())
         if self.agg.pool == "max":
             t_indptr, t_indices = self.graph.transpose(False)
             dzp = ops.csr_max_backward(z, p_all, dp, self.graph.indptr, self.graph.indices, t_indptr, t_indices)
@@ -148,43 +151,10 @@ class _FullLayer(object):
         grads = [x[:, :K].t() @ dzp, dzp.sum(dim=0)]
         return grads, (dzp @ Wm[:cols].t() + dself if cols else None)
 
-
-class _FullLayerFn(torch.autograd.Function):
-    """y = the layer of full_neighbor_embeddings, differentiable w.r.t. the layer's parameters, its source h (layers >= 1)
-    and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding view of the table's first d columns."""
-
-    @staticmethod
-    def forward(ctx, layer, h, emb, *params):
-        agg = layer.agg
-        code, post = act_code(agg.act)
-        if post is not None:
-            raise NotImplementedError("training supports act=relu or identity")
-        with torch.no_grad():
-            kept = []
-            parts = layer.forward(h, kept)
-            y = agg._finish(parts, agg._combine())
-        ctx.layer, ctx.relu, ctx.concat = layer, code == ops.ACT_RELU, bool(agg.concat)
-        ctx.F_in, ctx.Ks = h.shape[1], [K for _, K, _ in parts]
-        ctx.src_needs_grad = bool(h.requires_grad)
-        ctx.emb_d = emb.shape[1] if emb is not None and emb.requires_grad else 0
-        ctx.n_params = len(params)
-        ctx.save_for_backward(*[x for x, _, _ in parts], y, *params, *kept)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        P = len(ctx.Ks)
-        saved = ctx.saved_tensors
-        xs, y, params, kept = saved[:P], saved[P], saved[P + 1:P + 1 + ctx.n_params], saved[P + 1 + ctx.n_params:]
-        dz = dy * (y > 0).to(dy.dtype) if ctx.relu else dy
-        D = params[0].shape[1]
-        dzs = (dz[:, :D], dz[:, D:]) if P == 2 and ctx.concat else (dz,) * P
-        grads_w = [x[:, :K].t() @ g for x, K, g in zip(xs, ctx.Ks, dzs)]           # dW = X^T dZ  (library GEMM)
-        cols = ctx.F_in if ctx.src_needs_grad else ctx.emb_d
-        grads_own, dsrc = ctx.layer.backward(xs, dzs, params, kept, cols)
-        dh = dsrc if ctx.src_needs_grad else None
-        demb = ctx.layer.table_grad(dsrc[:, :ctx.emb_d]) if ctx.emb_d and dsrc is not None else None
-        return (None, dh, demb) + tuple(grads_w) + tuple(grads_own)
+    def source_grads(self, ctx, dsrc, dy):
+        """(d(h) of a layer >= 1, d(embeddings) of layer 0 with identity_dim > 0) from the source gradient dsrc."""
+        demb = self.table_grad(dsrc[:, :ctx.emb_shape[1]]) if ctx.emb_shape is not None and dsrc is not None else None
+        return (dsrc if ctx.src_needs_grad else None), demb
 
 
 class _L2NormalizeFn(torch.autograd.Function):
@@ -210,13 +180,17 @@ def refuse_capture(what):
         raise NotImplementedError("%s cannot be captured in a CUDA graph" % what)
 
 
-def refuse_full_neighbor_training(model):
+def refuse_full_neighbor(model, training):
+    """The NotImplementedErrors of the full-neighbourhood entry points; training adds those of the training paths."""
+    what = "training" if training else "inference"
     if model.aggregator_cls is SeqAggregator:
-        raise NotImplementedError("full-neighbourhood training is not implemented for the seq aggregator (its neighbour "
-                                  "order is the sampled order)")
+        raise NotImplementedError("full-neighbourhood %s is not implemented for the seq aggregator (its neighbour "
+                                  "order is the sampled order)" % what)
     if hasattr(model.features, "c_table"):
-        raise NotImplementedError("full-neighbourhood training with a node-partitioned (ShardedFeatures) table is not "
-                                  "implemented")
+        raise NotImplementedError("full-neighbourhood %s with a node-partitioned (ShardedFeatures) table is not "
+                                  "implemented" % what)
+    if not training:
+        return
     if getattr(model, "distributed", False):
         raise NotImplementedError("full-neighbourhood training with distributed=True is not implemented")
     if getattr(model, "dropout_rate", 0.):
@@ -234,45 +208,19 @@ def full_neighbor_graph(model, indptr, indices):
 
 
 def _inputs(model, indptr, indices, node_ids):
-    """(indptr, indices, ids): the CSR on the model's device, checked, and node_ids as int32 with every id outside [0, N)
-    named N - it reads the dummy node in the forward; naming it N routes its gradient there too (same bits)."""
+    """(indptr, indices, ids): the CSR on the model's device, checked, and node_ids (None: all N nodes) as int32 with
+    every id outside [0, N) named N - it reads the dummy node in the forward; naming it N routes its gradient there too
+    (same bits)."""
     n_rows = int(model.features.shape[0])
     indptr, indices = model._csr_input(indptr, torch.int64, "indptr"), model._csr_input(indices, torch.int32, "indices")
     if indptr.dim() != 1 or indptr.numel() != n_rows:
         raise ValueError("indptr must have N + 1 = %d entries (one row per node of the [N+1, .] table, plus the end)"
                          % n_rows)
+    if node_ids is None:
+        return indptr, indices, torch.arange(n_rows - 1, dtype=torch.int32, device=model.device)
     ids = torch.as_tensor(node_ids).to(device=model.device, dtype=torch.int32).reshape(-1)
     ids = torch.where((ids < 0) | (ids >= n_rows - 1), torch.full_like(ids, n_rows - 1), ids)
     return indptr, indices, ids
-
-
-def _params(agg):
-    v = agg.vars
-    if hasattr(agg, "mlp_layers"):
-        if len(agg.mlp_layers) != 1:
-            raise NotImplementedError("training supports one MLP layer")
-        mlp = agg.mlp_layers[0].vars
-        return v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"]
-    return (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
-
-
-def _outputs(model, layers, normalize):
-    h = model.features
-    for layer, fl in enumerate(layers):
-        emb = getattr(model, "embeds", None) if layer == 0 else None
-        h = _FullLayerFn.apply(fl, h, emb, *_params(fl.agg))
-    return _L2NormalizeFn.apply(h) if normalize else h
-
-
-def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True):
-    """full_neighbor_embeddings(indptr, indices, node_ids, normalize) with an autograd graph over the aggregator
-    weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
-    refuse_full_neighbor_training(model)
-    indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
-    graph = full_neighbor_graph(model, indptr, indices)
-    L = len(model.aggregators)
-    return _outputs(model, [_FullLayer(agg, graph, ids if layer == L - 1 else None)
-                            for layer, agg in enumerate(model.aggregators)], normalize)
 
 
 def minibatch_layers(aggregators, indptr, indices, ids):
@@ -290,23 +238,39 @@ def minibatch_layers(aggregators, indptr, indices, ids):
     return layers
 
 
-def full_neighbor_minibatch_outputs(model, indptr, indices, node_ids, normalize=True):
-    """full_neighbor_outputs(indptr, indices, node_ids, normalize) over the receptive-field blocks of node_ids: the same
-    values, bit for bit, with buffers sized by the blocks instead of the graph.  Reads the block sizes back once."""
-    refuse_full_neighbor_training(model)
+def _layers(model, indptr, indices, node_ids, training, minibatch):
+    """The checked layers of one call: over the receptive-field blocks of node_ids (minibatch; reads the block sizes
+    back once), else over the whole CSR - the model's cached FullNeighborGraph when training, an uncached one otherwise
+    (inference builds no transposes, and must not evict the ones a training CSR has cached)."""
+    refuse_full_neighbor(model, training)
+    if minibatch:
+        refuse_capture("a full-neighbourhood minibatch (it reads the block sizes back)")
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
-    return _outputs(model, minibatch_layers(model.aggregators, indptr, indices, ids), normalize)
+    if model.aggregators is None:
+        model.aggregators = build_aggregators(model)
+    if minibatch:
+        return minibatch_layers(model.aggregators, indptr, indices, ids)
+    graph = full_neighbor_graph(model, indptr, indices) if training else FullNeighborGraph(indptr, indices)
+    L = len(model.aggregators)
+    return [_FullLayer(agg, graph, ids if layer == L - 1 else None) for layer, agg in enumerate(model.aggregators)]
 
 
-def full_neighbor_minibatch_embeddings(model, indptr, indices, node_ids, normalize=True):
-    """SampleAndAggregate.full_neighbor_embeddings(indptr, indices, node_ids, normalize) over the receptive-field blocks
-    of node_ids, without autograd: the same bits."""
-    refuse_capture("full_neighbor_minibatch_embeddings (it reads the block sizes back)")
-    indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
+def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False):
+    """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings), without autograd."""
     h = model.features
     with torch.no_grad():
-        for fl in minibatch_layers(model.aggregators, indptr, indices, ids):
-            h = fl.agg._finish(fl.forward(h, []), fl.agg._combine())
+        for fl in _layers(model, indptr, indices, node_ids, False, minibatch):
+            h = fl.agg._finish(fl.forward(h, None), fl.agg._combine())
         if normalize:
             h = ops.l2_normalize_rows_(h.contiguous())
     return h
+
+
+def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False):
+    """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch) with an autograd graph over the
+    aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
+    h = model.features
+    for layer, fl in enumerate(_layers(model, indptr, indices, node_ids, True, minibatch)):
+        emb = getattr(model, "embeds", None) if layer == 0 else None
+        h = _LayerFn.apply(fl, h, emb, *layer_params(fl.agg))
+    return _L2NormalizeFn.apply(h) if normalize else h

@@ -11,8 +11,8 @@ import torch
 
 from . import ops
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
-                          _rows, refuse_seq_table)
-from .layers import act_code, identity, relu  # noqa: F401
+                          refuse_seq_table)
+from .layers import identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
 SAGEInfo = namedtuple("SAGEInfo",
@@ -240,53 +240,8 @@ class SampleAndAggregate(object):
         aggregators run their MLP once per node.  No sampling and no dropout: two calls give the same bits.  Returns fp32
         [len(node_ids), out_w], l2-normalised like forward().  Peak memory: two fp32 [N+1, width] layer buffers, plus the
         pools' [N+1, hidden] MLP output."""
-        if self.aggregator_cls is SeqAggregator:
-            raise NotImplementedError("full-neighbourhood inference is not implemented for the seq aggregator (its "
-                                      "neighbour order is the sampled order)")
-        if hasattr(self.features, "c_table"):
-            raise NotImplementedError("full-neighbourhood inference with a node-partitioned (ShardedFeatures) table is "
-                                      "not implemented")
-        n_rows = int(self.features.shape[0])
-        indptr, indices = self._csr_input(indptr, torch.int64, "indptr"), self._csr_input(indices, torch.int32, "indices")
-        if indptr.dim() != 1 or indptr.numel() != n_rows:
-            raise ValueError("indptr must have N + 1 = %d entries (one row per node of the [N+1, .] table, plus the end)"
-                             % n_rows)
-        ids = None if node_ids is None else torch.as_tensor(node_ids).to(device=self.device, dtype=torch.int32).reshape(-1)
-        if ids is None:
-            ids = torch.arange(n_rows - 1, dtype=torch.int32, device=self.device)
-        if self.aggregators is None:
-            from .supervised_models import build_aggregators
-            self.aggregators = build_aggregators(self)
-        h = self.features
-        L = len(self.aggregators)
-        with torch.no_grad():
-            for layer, agg in enumerate(self.aggregators):
-                rows = ids if layer == L - 1 else None          # None: all N+1 rows (the dummy node's row last)
-                if isinstance(agg, GCNAggregator):
-                    m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=rows)
-                    h = agg._finish([(m, agg.neigh_input_dim, agg.vars["weights"])], ops.COMBINE_ADD)
-                    continue
-                widen = h.dtype != torch.float32
-                n = h.shape[0] if rows is None else rows.numel()
-                hs = _rows(h, rows, 0, n, widen) if (widen or rows is not None) else h
-                if isinstance(agg, MaxPoolingAggregator):
-                    z = _rows(h, None, 0, h.shape[0], True) if widen else h
-                    for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116)
-                        code, post = act_code(dense.act)
-                        if getattr(dense, "_packed", None) is None:
-                            dense._packed = ops.PackedWeights()
-                        z = ops.sage_gemm([(z, dense.input_dim, dense.vars["weights"])], bias=dense.vars.get("bias"),
-                                          act=code, math=agg.math, packed=dense._packed)
-                        z = post(z) if post else z
-                    p = ops.csr_aggregate(z, indptr, indices, "max" if agg.pool == "max" else "mean", rows=rows)
-                    parts = [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
-                else:
-                    m = ops.csr_aggregate(h, indptr, indices, "mean", rows=rows)
-                    parts = [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
-                h = agg._finish(parts, agg._combine())
-            if normalize:
-                h = ops.l2_normalize_rows_(h.contiguous())
-        return h
+        from .full_neighbor_training import full_neighbor_embeddings
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize)
 
     def full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True):
         """full_neighbor_embeddings(indptr, indices, node_ids, normalize) - torch.equal to it - computed over the
@@ -295,17 +250,8 @@ class SampleAndAggregate(object):
         and memory follow the blocks, not the graph: use it when node_ids' receptive field is a small part of the graph
         (serving, evaluating a split in batches).  Reads the block sizes back once per call (a synchronisation), so it
         cannot be captured in a CUDA graph.  Same refusals as full_neighbor_embeddings."""
-        if self.aggregator_cls is SeqAggregator:
-            raise NotImplementedError("full-neighbourhood inference is not implemented for the seq aggregator (its "
-                                      "neighbour order is the sampled order)")
-        if hasattr(self.features, "c_table"):
-            raise NotImplementedError("full-neighbourhood inference with a node-partitioned (ShardedFeatures) table is "
-                                      "not implemented")
-        if self.aggregators is None:
-            from .supervised_models import build_aggregators
-            self.aggregators = build_aggregators(self)
-        from .full_neighbor_training import full_neighbor_minibatch_embeddings
-        return full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize)
+        from .full_neighbor_training import full_neighbor_embeddings
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True)
 
     def _csr_input(self, t, dtype, name):
         """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""

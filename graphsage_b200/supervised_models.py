@@ -80,9 +80,10 @@ class _LayerFn(torch.autograd.Function):
     """y = agg.aggregate_rows(src, segments) for one aggregator layer, differentiable w.r.t. the layer's parameters,
     (layers >= 1, where rows are addressed by ranges) src, and (layer 0, identity_dim > 0) `emb`, the [N+1, d] embedding
     view of src's first d columns.  The per-kind work is the branch's (_AggregateRowsFn, _PoolAggregateRowsFn,
-    _FusedPoolAggregateRowsFn, _SeqAggregateRowsFn; their apply is the layer's entry): its forward gives the GEMM parts
-    y = act(concat_or_add(x_p @ W_p) + bias) combines, its backward turns the gradients of its parts' inputs into the
-    gradients of its own parameters and the source-row contributions _source_grads routes."""
+    _FusedPoolAggregateRowsFn, _SeqAggregateRowsFn, whose apply is the layer's entry, and the whole-neighbourhood
+    full_neighbor_training._FullLayer): its forward gives the GEMM parts y = act(concat_or_add(x_p @ W_p) + bias)
+    combines, its backward turns the gradients of its parts' inputs into the gradients of its own parameters and the
+    source gradient its source_grads routes (the sampled branches: per-segment contributions, _source_grads)."""
 
     @staticmethod
     def forward(ctx, branch, src, emb, *params):
@@ -117,7 +118,7 @@ class _LayerFn(torch.autograd.Function):
         dxs = [g @ W.t() if p >= ctx.branch.row_parts else g @ W[:cols].t() if cols else None
                for p, (g, W) in enumerate(zip(dzs, params))]
         grads_own, contribs = ctx.branch.backward(xs, dxs, params[P:], kept, cols)
-        dsrc, demb = _source_grads(ctx, contribs, dy)
+        dsrc, demb = ctx.branch.source_grads(ctx, contribs, dy)
         return (None, dsrc, demb) + tuple(grads_w) + tuple(grads_own)
 
 
@@ -154,6 +155,7 @@ class _AggregateRowsFn(object):
     for GCN the mean over the k neighbours and the node itself.  sites: None, or one (neighbour site, self site) pair of
     (seed, call, rate) per segment (training dropout): the gather then drops the rows it reads, so the parts are what
     dW = X^T dZ needs."""
+    source_grads = staticmethod(_source_grads)
 
     @staticmethod
     def apply(agg, src, segments, emb, sites, *weights):
@@ -194,6 +196,7 @@ class _SummaryBranch(object):
     """The _LayerFn branches of the pools and seq: parts [self rows, per-hop neighbour summary]; the self rows receive
     dZ_s Ws^T.  Their apply takes agg's self_weights, neigh_weights and the two tensors of the summary's own layer."""
     row_parts = 1
+    source_grads = staticmethod(_source_grads)
 
     def __init__(self, agg, segments):
         self.agg, self.segments = agg, segments
@@ -342,21 +345,32 @@ class _SeqAggregateRowsFn(_SummaryBranch):
         return [torch.cat([dWx, dWh]), db], (self._contribs(dxs[0], dX_all) if cols else [])
 
 
+def layer_params(agg):
+    """The tensors a layer trains, in _LayerFn's order: the GEMM parts' weights ([weights] for GCN, else [self_weights,
+    neigh_weights]), then the branch's own - the pools' MLP weights and bias, the seq cell's kernel and bias."""
+    v = agg.vars
+    if hasattr(agg, "cell"):
+        cell = agg.cell.vars
+        return v["self_weights"], v["neigh_weights"], cell["kernel"], cell["bias"]
+    if hasattr(agg, "mlp_layers"):
+        if len(agg.mlp_layers) != 1:
+            raise NotImplementedError("training supports one MLP layer")
+        mlp = agg.mlp_layers[0].vars
+        return v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"]
+    return (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
+
+
 def train_layer(agg, src, segments, emb=None, sites=None, fused=False, persistent=False):
     """agg.aggregate_rows(src, segments) with an autograd graph (_LayerFn): through the seq, the materialised or (fused)
     the fused bf16 pooling branch, or the mean / GCN one.  sites: training dropout of the mean / GCN and materialised
     pooling branches (see their classes); persistent: src is the model's layer-0 feature table."""
-    v = agg.vars
+    params = layer_params(agg)
     if hasattr(agg, "cell"):
-        cell = agg.cell.vars
-        return _SeqAggregateRowsFn.apply(agg, src, segments, v["self_weights"], v["neigh_weights"], cell["kernel"],
-                                         cell["bias"], emb)
+        return _SeqAggregateRowsFn.apply(agg, src, segments, *params, emb)
     if hasattr(agg, "mlp_layers"):
-        mlp = agg.mlp_layers[0].vars
         fn, extra = (_FusedPoolAggregateRowsFn, persistent) if fused else (_PoolAggregateRowsFn, sites)
-        return fn.apply(agg, src, segments, v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"], emb, extra)
-    ws = (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
-    return _AggregateRowsFn.apply(agg, src, segments, emb, sites, *ws)
+        return fn.apply(agg, src, segments, *params, emb, extra)
+    return _AggregateRowsFn.apply(agg, src, segments, emb, sites, *params)
 
 
 def differentiable_outputs(model, batch, normalize=True, dropout=0.):
@@ -491,6 +505,22 @@ def weight_decay_term(params, weight_decay):
     return total
 
 
+def clipped_step(model, loss):
+    """One optimiser step of the supervised and unsupervised models on `loss`: gradients, their mean over the ranks when
+    model.distributed (data parallel), clip_by_value(grad, -5, 5) (supervised_models.py:93-94, models.py:380-381), Adam.
+    Returns the detached loss."""
+    model.optimizer.zero_grad(set_to_none=True)
+    loss.backward()
+    if model.distributed:
+        from .parallel import allreduce_gradients
+        model.last_allreduce_bytes = allreduce_gradients(model.parameters(), model.group)
+    for p in model.parameters():
+        if p.grad is not None:
+            p.grad.clamp_(-5.0, 5.0)
+    model.optimizer.step()
+    return loss.detach()
+
+
 class SupervisedGraphsage(SampleAndAggregate):
     """Supervised GraphSAGE (reference graphsage/supervised_models.py:10-126): the hot path, then
     l2_normalize -> Dense(-> num_classes) -> sigmoid / softmax cross-entropy (+ weight decay), gradients clipped to
@@ -549,14 +579,21 @@ class SupervisedGraphsage(SampleAndAggregate):
         if check_dropout_rate(dropout):
             out = _DropoutFn.apply(out, (self.dropout_key, self.dropout_counter, dropout, self.dropout_call_dev))
             self.dropout_counter += 1
+        return self._node_pred(out)
+
+    def _node_pred(self, out):
         return out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
 
     def loss(self, batch, labels, dropout=0.):
         """supervised_models.py:101-118: weight decay * l2_loss(var) over aggregator + head variables, then the
         mean of the per-element sigmoid xent (multi-label) or the mean of the per-node softmax xent."""
         logits = self.logits(batch, dropout=dropout) if dropout else self.logits(batch)    # overrides take (batch)
+        return self._logits_loss(logits, labels)
+
+    def _logits_loss(self, logits, labels):
+        """loss()'s tail on the head's logits, shared with the full-neighbourhood losses."""
         self._last_logits = logits.detach()
-        labels = labels.to(device=logits.device, dtype=torch.float32)
+        labels = torch.as_tensor(labels).to(device=logits.device, dtype=torch.float32)
         loss = classification_loss(logits, labels, self.sigmoid_loss)
         if self.weight_decay:
             loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)
@@ -564,17 +601,7 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def train_step(self, batch, labels):
         """One Adam step at the training dropout rate placeholders['dropout'] (supervised_train.py:271)."""
-        self.optimizer.zero_grad(set_to_none=True)
-        loss = self.loss(batch, labels, dropout=self.dropout_rate)
-        loss.backward()
-        if self.distributed:                                                     # data parallel: mean gradient over ranks
-            from .parallel import allreduce_gradients
-            self.last_allreduce_bytes = allreduce_gradients(self.parameters(), self.group)
-        for p in self.parameters():                                              # clip_by_value(grad, -5, 5)  :93-94
-            if p.grad is not None:
-                p.grad.clamp_(-5.0, 5.0)
-        self.optimizer.step()
-        return loss.detach()
+        return clipped_step(self, self.loss(batch, labels, dropout=self.dropout_rate))
 
     def graphed_train_step(self, batch_size):
         """train_step for a fixed batch size captured in one CUDA graph: returns step(batch, labels) -> loss, a static 0-d
@@ -596,54 +623,35 @@ class SupervisedGraphsage(SampleAndAggregate):
 
     def full_neighbor_loss(self, indptr, indices, node_ids, labels):
         """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids."""
-        return self._head_loss(self.full_neighbor_outputs(indptr, indices, node_ids), labels)
-
-    def _head_loss(self, out, labels):
-        logits = out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"]
-        self._last_logits = logits.detach()
-        labels = torch.as_tensor(labels).to(device=logits.device, dtype=torch.float32)
-        loss = classification_loss(logits, labels, self.sigmoid_loss)
-        if self.weight_decay:
-            loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)
-        return loss
+        return self._logits_loss(self._node_pred(self.full_neighbor_outputs(indptr, indices, node_ids)), labels)
 
     def full_neighbor_train_step(self, indptr, indices, node_ids, labels):
         """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling, no
         dropout), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host synchronisation."""
-        return self._clipped_step(self.full_neighbor_loss(indptr, indices, node_ids, labels))
-
-    def _clipped_step(self, loss):
-        self.optimizer.zero_grad(set_to_none=True)
-        loss.backward()
-        for p in self.parameters():                                              # clip_by_value(grad, -5, 5)  :93-94
-            if p.grad is not None:
-                p.grad.clamp_(-5.0, 5.0)
-        self.optimizer.step()
-        return loss.detach()
+        return clipped_step(self, self.full_neighbor_loss(indptr, indices, node_ids, labels))
 
     def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids):
         """full_neighbor_outputs over the receptive field of node_ids only: the same values, bit for bit, with per-layer
         blocks built on the device by ops.csr_blocks (contract: oracle/full_neighbor_blocks.py) and their transposes built
         per call, not cached.  Cost and memory follow the blocks, not the graph: the minibatch form of exact-neighbourhood
         training.  Reads the block sizes back once per call.  Same refusals as full_neighbor_outputs."""
-        from .full_neighbor_training import full_neighbor_minibatch_outputs
-        return full_neighbor_minibatch_outputs(self, indptr, indices, node_ids)
+        from .full_neighbor_training import full_neighbor_outputs
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True)
 
     def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels):
         """full_neighbor_loss over full_neighbor_minibatch_outputs: the same head, cross-entropy and weight decay."""
-        return self._head_loss(self.full_neighbor_minibatch_outputs(indptr, indices, node_ids), labels)
+        return self._logits_loss(self._node_pred(self.full_neighbor_minibatch_outputs(indptr, indices, node_ids)), labels)
 
     def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels):
         """full_neighbor_train_step for a minibatch: one Adam step on full_neighbor_minibatch_loss, gradients clipped to
         +-5.  Returns the detached loss."""
-        return self._clipped_step(self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels))
+        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels))
 
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on
         full_neighbor_embeddings(indptr, indices, node_ids) - deterministic, no sampling, no dropout."""
         with torch.no_grad():
-            out = self.full_neighbor_embeddings(indptr, indices, node_ids, normalize=True)
-            return self._predictions(out @ self.node_pred_vars["weights"] + self.node_pred_vars["bias"])
+            return self._predictions(self._node_pred(self.full_neighbor_embeddings(indptr, indices, node_ids)))
 
     def last_predictions(self):
         """model.preds of the last loss() / train_step() call (supervised_models.py:120-126): the predictions from that

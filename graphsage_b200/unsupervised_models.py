@@ -13,8 +13,8 @@ from . import ops
 from .graphed_training import GraphedTrainStep
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
-from .supervised_models import (aggregator_parameters, build_aggregators, differentiable_outputs, embedding_parameters,
-                                init_dropout, refuse_distributed_embeddings, refuse_fused_pool,
+from .supervised_models import (aggregator_parameters, build_aggregators, clipped_step, differentiable_outputs,
+                                embedding_parameters, init_dropout, refuse_distributed_embeddings, refuse_fused_pool,
                                 weight_decay_term)
 
 
@@ -89,6 +89,11 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         (models.py:378).  The edge-prediction layer has no dropout (models.py:363-366)."""
         # at dropout 0 the two-argument form, which overrides of _passes implement
         o1, o2, on, _ = self._passes(batch1, batch2, dropout) if dropout else self._passes(batch1, batch2)
+        return self._pairs_loss(o1, o2, on)
+
+    def _pairs_loss(self, o1, o2, on):
+        """loss()'s tail on the three passes' outputs, shared with full_neighbor_minibatch_loss; keeps the affinities
+        for mrr()."""
         loss = self.link_pred_layer.loss(o1, o2, on)
         if self.weight_decay:
             loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)       # models.py:385-387
@@ -101,17 +106,7 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         return mrr_from_affinities(*self._last)
 
     def train_step(self, batch1, batch2):
-        self.optimizer.zero_grad(set_to_none=True)
-        loss = self.loss(batch1, batch2, dropout=self.dropout_rate)                 # unsupervised_train.py:269
-        loss.backward()
-        if self.distributed:                                                         # data parallel: mean gradient over ranks
-            from .parallel import allreduce_gradients
-            self.last_allreduce_bytes = allreduce_gradients(self.parameters(), self.group)
-        for p in self.parameters():
-            if p.grad is not None:
-                p.grad.clamp_(-5.0, 5.0)                                             # models.py:380-381
-        self.optimizer.step()
-        return loss.detach()
+        return clipped_step(self, self.loss(batch1, batch2, dropout=self.dropout_rate))   # unsupervised_train.py:269
 
     def full_neighbor_minibatch_loss(self, indptr, indices, batch1, batch2):
         """loss() with every embedding computed over whole neighbourhoods (contract: oracle/full_neighbor_blocks.py): the
@@ -120,30 +115,17 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         decay, divided by len(batch1), and the affinities for mrr().  Reads the block sizes back once per call.  Refused
         (NotImplementedError): the seq aggregator, ShardedFeatures, distributed=True, training dropout > 0, CUDA-graph
         capture."""
-        from .full_neighbor_training import full_neighbor_minibatch_outputs, refuse_full_neighbor_training
-        refuse_full_neighbor_training(self)
+        from .full_neighbor_training import full_neighbor_outputs, refuse_full_neighbor
+        refuse_full_neighbor(self, training=True)                                    # before drawing the negatives
         neg = self.neg_sampler(self.neg_sample_size)
         b1, b2 = (torch.as_tensor(b).to(device=self.device, dtype=torch.int32).reshape(-1) for b in (batch1, batch2))
-        out = full_neighbor_minibatch_outputs(self, indptr, indices, torch.cat([b1, b2, neg]))
-        o1, o2, on = torch.split(out, [b1.numel(), b2.numel(), neg.numel()])
-        loss = self.link_pred_layer.loss(o1, o2, on)
-        if self.weight_decay:
-            loss = loss + weight_decay_term(self.decayed_parameters(), self.weight_decay)
-        with torch.no_grad():
-            self._last = (self.link_pred_layer.affinity(o1, o2), self.link_pred_layer.neg_cost(o1, on))
-        return loss / float(o1.shape[0])
+        out = full_neighbor_outputs(self, indptr, indices, torch.cat([b1, b2, neg]), minibatch=True)
+        return self._pairs_loss(*torch.split(out, [b1.numel(), b2.numel(), neg.numel()]))
 
     def full_neighbor_minibatch_train_step(self, indptr, indices, batch1, batch2):
         """One Adam step on full_neighbor_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the
         detached loss."""
-        loss = self.full_neighbor_minibatch_loss(indptr, indices, batch1, batch2)
-        self.optimizer.zero_grad(set_to_none=True)
-        loss.backward()
-        for p in self.parameters():
-            if p.grad is not None:
-                p.grad.clamp_(-5.0, 5.0)                                             # models.py:380-381
-        self.optimizer.step()
-        return loss.detach()
+        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, batch1, batch2))
 
     def graphed_train_step(self, batch_size):
         """train_step for a fixed batch size captured in one CUDA graph: returns step(batch1, batch2) -> loss, a static 0-d

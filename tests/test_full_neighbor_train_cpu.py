@@ -358,3 +358,27 @@ def test_autograd_wiring_matches_the_oracle(cpu_kernels, kind, concat, d):
     assert fnt.full_neighbor_graph(model, g0.indptr, g0.indices) is g0
     g0.indptr.add_(0)                                                        # a new _version: rebuilt
     assert fnt.full_neighbor_graph(model, g0.indptr, g0.indices) is not g0
+
+
+@pytest.mark.parametrize("kind", ["mean", "gcn", "maxpool", "meanpool"])
+def test_inference_is_the_training_forward_and_leaves_the_cache_alone(cpu_kernels, kind):
+    r = np.random.RandomState(12)
+    indptr, indices = messy_graph(seed=6)
+    N, F = len(indptr) - 1, 6
+    feats = np.vstack([r.randn(N, F).astype(np.float32), np.zeros((1, F), np.float32)])
+    infos = [gs.SAGEInfo("node", None, 3, 8), gs.SAGEInfo("node", None, 3, 8)]
+    model = SupervisedGraphsage(3, {}, torch.from_numpy(feats), torch.zeros((N + 1, 3), dtype=torch.int32), None, infos,
+                                concat=kind != "gcn", aggregator_type=kind, device="cpu")
+    model.aggregator_type = kind
+    for a in model.aggregators:
+        a.math = ops.MATH_FP32_SIMT
+    node_ids = np.array([1, 4, 4, 7, 2, 20, -3, N + 5], np.int64)          # duplicates, an empty row, out of range
+    emb = model.full_neighbor_embeddings(indptr, indices, node_ids)
+    ref = fn.full_neighbor_embeddings(feats, indptr, indices, oracle_dicts(model), kind != "gcn", node_ids)
+    assert emb.shape == ref.shape and np.abs(_np(emb) - ref).max() <= 1e-5
+    assert not hasattr(model, "_full_neighbor_graph")                        # inference caches no transposes
+    out = model.full_neighbor_outputs(indptr, indices, node_ids)
+    g0 = model._full_neighbor_graph
+    assert torch.equal(emb, out.detach())
+    assert torch.equal(model.full_neighbor_embeddings(indptr, indices, node_ids), emb)
+    assert model._full_neighbor_graph is g0                                  # nor evicts the training CSR's
