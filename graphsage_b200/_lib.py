@@ -106,11 +106,6 @@ _SIGNATURES = {
                                        c_vp, c_vp]),
     "gs_sage_gemm_rows": (c_i32, [c_i64, ctypes.POINTER(GemmPart), ctypes.POINTER(GemmRowIds), c_i32, c_i32, c_vp, c_i32, c_i32,
                                   c_vp, c_i64, c_vp, c_vp]),
-    "gs_gather_mean_img_bytes": (c_i64, [c_i64, c_i32, c_i32]),
-    "gs_gather_mean_img": (c_i32, [c_vp, c_i64, ctypes.POINTER(ShardedTable), c_i32, c_vp, c_i32, c_i64, ctypes.POINTER(Segment),
-                                   c_i32, c_i32, c_i32, c_vp, c_vp]),
-    "gs_sage_gemm_img": (c_i32, [c_i64, ctypes.POINTER(GemmPart), c_i32, c_i32, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_i32,
-                                 c_vp]),
     "gs_sage_layer_small": (c_i32, [c_vp, c_i64, c_i32, c_i64, ctypes.POINTER(Segment), c_i32, ctypes.POINTER(GemmPart),
                                     c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_i64, c_vp, c_u64, c_vp]),
     "gs_maxpool_mlp_workspace_bytes": (c_i64, [c_i32, c_i32]),

@@ -54,13 +54,6 @@ def fused_pool_fits(k, K, hidden):
     return k <= FUSED_POOL_MAX_FANOUT and K <= FUSED_POOL_MAX_K and hidden % FUSED_POOL_HIDDEN_STEP == 0
 
 
-USE_GEMM_IMAGES = [False]     # opt-in: tf32x3 layers hand the gathered rows to the GEMM as tensor-core tile images
-                              # (ops.gather_mean_images + ops.sage_gemm_img; bit-identical results).  Measured on the bench step:
-                              # the GEMM's A side becomes one bulk copy per K-block, but the gather - the critical kernel -
-                              # writes hi + lo images of both parts (55 MB instead of 27 MB): 59.3 us instead of 55.4, and the
-                              # pipelined step went from 74.1 to 76.3 us.  Kept off.
-
-
 class _SageAggregator(Layer):
     def _combine(self):
         return ops.COMBINE_CONCAT if self.concat and "self_weights" in self.vars else ops.COMBINE_ADD
@@ -77,21 +70,6 @@ class _SageAggregator(Layer):
             hop(i, s, h[s.out_row0:s.out_row0 + s.n])
             _rows(src, s.self_ids, s.self_row0, s.n, f32_self, out=xs[s.out_row0:s.out_row0 + s.n])
         return [(xs, self.input_dim, self.vars["self_weights"]), (h, self.hidden_dim, self.vars["neigh_weights"])]
-
-    def _image_layer(self, src, segments, parts, combine, include_self, want_self):
-        """gather + mean -> tile images -> wgmma GEMM (tf32x3); None when the image form does not apply."""
-        code, post = act_code(self.act)
-        if not USE_GEMM_IMAGES[0] or self.math != ops.MATH_TF32X3 or post is not None or self.dropout \
-                or any(K != src.shape[1] for (_, K, _) in parts):
-            return None
-        res = ops.gather_mean_images(src, segments, include_self=include_self, want_self=want_self)
-        if res is None:
-            return None
-        images, rows = res
-        if getattr(self, "_packed", None) is None:
-            self._packed = ops.PackedWeights()
-        return ops.sage_gemm_img(rows, images, parts, combine=combine, bias=self.vars.get("bias"), act=code,
-                                 packed=self._packed)
 
     def _finish(self, parts, combine):
         code, post = act_code(self.act)
@@ -162,11 +140,6 @@ class MeanAggregator(_SageAggregator):
                               self._combine(), False, final)
         if y is not None:
             return y
-        y = self._image_layer(src, segments, [(None, self.input_dim, self.vars["self_weights"]),
-                                              (None, self.neigh_input_dim, self.vars["neigh_weights"])],
-                              self._combine(), False, True)
-        if y is not None:
-            return y
         if torch.is_tensor(src) and src.is_cuda and src.dtype == torch.float32 and all(s.self_ids is not None for s in segments):
             # the self rows only feed the GEMM: it reads them from the table by id, so the gather neither fetches them nor
             # writes a copy (same operand values, same bits)
@@ -216,9 +189,6 @@ class GCNAggregator(_SageAggregator):
             raise NotImplementedError("dropout > 0 uses the dense call path")
         y = self._small_layer(src, segments, [(None, self.neigh_input_dim, self.vars["weights"])], ops.COMBINE_ADD, True,
                               final)
-        if y is not None:
-            return y
-        y = self._image_layer(src, segments, [(None, self.neigh_input_dim, self.vars["weights"])], ops.COMBINE_ADD, True, False)
         if y is not None:
             return y
         _, means = ops.gather_mean(src, segments, include_self=True, want_self=False)

@@ -278,32 +278,6 @@ struct ShardRows {
 // ------------------------------------------------------------------------------------------
 constexpr int kGroupRows = 13;
 
-// A-operand images for the wgmma GEMM that follows (gs_sage_gemm_img, tf32x3): instead of (or besides) the fp32 rows,
-// the kernel writes each result row already SPLIT into tf32 hi / lo and laid out as the K-major SWIZZLE_128B tile
-// images the GEMM multiplies - part p (0 = self rows, 1 = mean rows), 128-row tile mt, 32-column K-block kb:
-//   img + ((((p * n_mtiles + mt) * kblocks + kb) * 2 + hl) * 16 KB) + sw128_off(row % 128, chunk),  hl = 0 hi / 1 lo,
-// so the GEMM's A operand is one 32 KB bulk copy per K-block (no producer warps, no register round trip, no proxy fence).
-struct GatherImg {
-  unsigned char* base;          // NULL: no images
-  int32_t kblocks, n_mtiles;
-  int32_t want_self;            // part 0 present (Mean); 0: only the mean part (GCN) at p = 0
-};
-
-__device__ __forceinline__ void gather_img_store(const GatherImg& im, int part, int64_t orow, int c, float4 v) {
-  const int kb = c >> 3, chunk = c & 7;
-  const int64_t mt = orow >> 7;
-  const int r = (int)(orow & 127);
-  unsigned char* dst = im.base + ((((int64_t)part * im.n_mtiles + mt) * im.kblocks + kb) * 2) * 16384 +
-                       (uint32_t)(r * 128 + ((chunk ^ (r & 7)) << 4));
-  uint4 hi, lo;
-  hi.x = __float_as_uint(v.x) & 0xFFFFE000u; hi.y = __float_as_uint(v.y) & 0xFFFFE000u;
-  hi.z = __float_as_uint(v.z) & 0xFFFFE000u; hi.w = __float_as_uint(v.w) & 0xFFFFE000u;
-  lo.x = __float_as_uint(v.x - __uint_as_float(hi.x)) & 0xFFFFE000u; lo.y = __float_as_uint(v.y - __uint_as_float(hi.y)) & 0xFFFFE000u;
-  lo.z = __float_as_uint(v.z - __uint_as_float(hi.z)) & 0xFFFFE000u; lo.w = __float_as_uint(v.w - __uint_as_float(hi.w)) & 0xFFFFE000u;
-  *reinterpret_cast<uint4*>(dst) = hi;
-  *reinterpret_cast<uint4*>(dst + 16384) = lo;
-}
-
 // kDrop: every gathered row is dropped in registers before it is summed (gs_gather_mean_dropout); the kDrop = false
 // instantiation is the plain gather.
 // min 3 CTAs per SM: what the two-buffer ring's shared memory allows at F = 602 (2 x 13 rows x 2,432 B); without the hint
@@ -313,8 +287,7 @@ __global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_c
                                                                const __grid_constant__ SegTable tab,
                                                                int include_self, float* __restrict__ out_self,
                                                                float* __restrict__ out_mean, int64_t out_pitch,
-                                                               int row_bytes, const __grid_constant__ GatherImg img,
-                                                               const __grid_constant__ DropTab drop) {
+                                                               int row_bytes, const __grid_constant__ DropTab drop) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t bar[2];
   __shared__ uint32_t drop_off[2 * GS_MAX_SEGMENTS];      // kDrop: the device-side call offsets, neighbour sites then self
@@ -333,9 +306,9 @@ __global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_c
   const int ncol4 = (int)(out_pitch >> 2);
   const int row_f4 = row_bytes >> 4;
   const size_t buf_bytes = (size_t)kGroupRows * row_bytes;
-  // a node's self row is fetched only when something reads it: the GCN sum, out_self or the self image.  The mean layer
-  // whose GEMM reads the self rows by id (gs_sage_gemm_rows) asks for none of them and so moves k rows per node, not k + 1.
-  const int self_rows = (include_self || out_self || (img.base && img.want_self)) ? 1 : 0;
+  // a node's self row is fetched only when something reads it: the GCN sum or out_self.  The mean layer whose GEMM reads
+  // the self rows by id (gs_sage_gemm_rows) asks for neither and so moves k rows per node, not k + 1.
+  const int self_rows = (include_self || out_self) ? 1 : 0;
 
   // work items of this CTA: (node r, group g); enumerate lazily
   int64_t r_issue = blockIdx.x;      // node whose groups are being issued
@@ -401,13 +374,12 @@ __global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_c
     }
     if (last) {
       const int64_t orow = sg.out_row0 + i;
-      const int ncol_img = img.base ? img.kblocks * 8 : 0;          // images are whole K-blocks: zero chunks past the row
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int c = threadIdx.x + q * blockDim.x;
-        if (c < ncol4 || c < ncol_img) {
+        if (c < ncol4) {
           float4 a = make_float4(0.f, 0.f, 0.f, 0.f), sv = a;
-          if (c < ncol4 && c * 4 < F) {
+          if (c * 4 < F) {
             a = acc[q];
             if (self_rows) {
               sv = rows[(cnt - 1) * row_f4 + c];
@@ -419,15 +391,9 @@ __global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_c
             a = mask_tail(a, c * 4, F);
             sv = mask_tail(sv, c * 4, F);
           }
-          if (c < ncol4) {
-            if (out_mean) reinterpret_cast<float4*>(out_mean + orow * out_pitch)[c] = a;
-            if (out_self) reinterpret_cast<float4*>(out_self + orow * out_pitch)[c] = sv;
-          }
-          if (c < ncol_img) {
-            if (img.want_self) gather_img_store(img, 0, orow, c, sv);
-            gather_img_store(img, img.want_self ? 1 : 0, orow, c, a);
-          }
-          if (c < ncol4) acc[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (out_mean) reinterpret_cast<float4*>(out_mean + orow * out_pitch)[c] = a;
+          if (out_self) reinterpret_cast<float4*>(out_self + orow * out_pitch)[c] = sv;
+          acc[q] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
       r += gridDim.x;
@@ -924,10 +890,10 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 
 
 namespace gs {
-// launch of the grouped double-buffered bulk-copy gather (dense or sharded resolver), with or without A-operand images
+// launch of the grouped double-buffered bulk-copy gather (dense or sharded resolver)
 template <class Rows, bool kDrop = false>
 static int32_t launch_gather_tma2(const Rows& rows_of, int F, const SegTable& tab, int include_self, float* out_self, float* out_mean,
-                                  int64_t out_pitch, const GatherImg& img, cudaStream_t st, const DropTab* drop = nullptr) {
+                                  int64_t out_pitch, cudaStream_t st, const DropTab* drop = nullptr) {
   const int32_t rc_attr = ensure_dyn_smem((const void*)gather_mean_tma2_kernel<Rows, kDrop>, 200 * 1024);
   if (rc_attr != GS_OK) return rc_attr;
   const int ncol4 = (int)(out_pitch / 4);
@@ -946,11 +912,25 @@ static int32_t launch_gather_tma2(const Rows& rows_of, int F, const SegTable& ta
   DropTab no_drop;
   memset(&no_drop, 0, sizeof(no_drop));
   gather_mean_tma2_kernel<Rows, kDrop><<<(unsigned)blocks, threads, smem2, st>>>(rows_of, F, tab, include_self, out_self,
-                                                                                 out_mean, out_pitch, row_bytes, img,
+                                                                                 out_mean, out_pitch, row_bytes,
                                                                                  drop ? *drop : no_drop);
   return launch_check("gather_mean_tma2_kernel");
 }
 }  // namespace gs
+
+// copies the caller's segments into `tab`, checks each one and sums total_rows; raises *kmax (if given) to the largest fanout
+static int32_t fill_seg_table(const gs_segment* segments_host, int32_t n_segments, gs::SegTable& tab, const char* who,
+                              int* kmax = nullptr) {
+  memset(&tab, 0, sizeof(tab));
+  tab.n_segments = n_segments;
+  for (int s = 0; s < n_segments; ++s) {
+    tab.s[s] = segments_host[s];
+    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "%s: segment %d has n=%lld k=%d", who, s, (long long)tab.s[s].n, tab.s[s].k);
+    tab.total_rows += tab.s[s].n;
+    if (kmax && tab.s[s].k > *kmax) *kmax = tab.s[s].k;
+  }
+  return GS_OK;
+}
 
 extern "C" {
 
@@ -1002,16 +982,9 @@ int32_t gs_gather_mean(const void* src, int32_t dtype, int64_t n_src_rows, int32
              GS_MAX_SEGMENTS);
   GS_REQUIRE(segments_host || n_segments == 0, "gs_gather_mean: segments_host is NULL");
   gs::SegTable tab;
-  memset(&tab, 0, sizeof(tab));
-  tab.n_segments = n_segments;
   int kmax = 0;
-  for (int s = 0; s < n_segments; ++s) {
-    tab.s[s] = segments_host[s];
-    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "gs_gather_mean: segment %d has n=%lld k=%d", s, (long long)tab.s[s].n,
-               tab.s[s].k);
-    tab.total_rows += tab.s[s].n;
-    if (tab.s[s].k > kmax) kmax = tab.s[s].k;
-  }
+  const int32_t rc = fill_seg_table(segments_host, n_segments, tab, "gs_gather_mean", &kmax);
+  if (rc != GS_OK) return rc;
   if (tab.total_rows == 0) return GS_OK;
   GS_REQUIRE(src && out_mean, "gs_gather_mean: NULL pointer");
   GS_REQUIRE(F > 0 && pitch >= F && out_pitch >= F && n_src_rows > 0, "gs_gather_mean: bad F/pitch");
@@ -1064,9 +1037,7 @@ int32_t gs_gather_mean(const void* src, int32_t dtype, int64_t n_src_rows, int32
   const int variant = gs::tuning("gather_variant", 2);   // 2: grouped double-buffered TMA (default), 1: whole-node TMA, 0: LDG
   if (variant == 2 && ncol4 <= 2 * 160) {
     const gs::DenseRows rows_of{fsrc, n_src_rows, pitch};
-    gs::GatherImg img;
-    memset(&img, 0, sizeof(img));
-    return gs::launch_gather_tma2(rows_of, F, tab, include_self, (float*)out_self, (float*)out_mean, out_pitch, img, st);
+    return gs::launch_gather_tma2(rows_of, F, tab, include_self, (float*)out_self, (float*)out_mean, out_pitch, st);
   }
   if (variant >= 1 && smem <= 200 * 1024) {
     {
@@ -1169,20 +1140,16 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
   GS_REQUIRE((segments_host && neigh_sites_host && self_sites_host) || n_segments == 0,
              "gs_gather_mean_dropout: segments / sites are NULL");
   gs::SegTable tab;
-  memset(&tab, 0, sizeof(tab));
+  int32_t rc = fill_seg_table(segments_host, n_segments, tab, "gs_gather_mean_dropout");
+  if (rc != GS_OK) return rc;
   gs::DropTab drop;
   memset(&drop, 0, sizeof(drop));
-  tab.n_segments = n_segments;
   for (int s = 0; s < n_segments; ++s) {
-    tab.s[s] = segments_host[s];
-    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "gs_gather_mean_dropout: segment %d has n=%lld k=%d", s,
-               (long long)tab.s[s].n, tab.s[s].k);
-    int32_t rc = check_site(neigh_sites_host[s], "gs_gather_mean_dropout");
+    rc = check_site(neigh_sites_host[s], "gs_gather_mean_dropout");
     if (rc == GS_OK) rc = check_site(self_sites_host[s], "gs_gather_mean_dropout");
     if (rc != GS_OK) return rc;
     drop.neigh[s] = gs::make_drop_site(neigh_sites_host[s]);
     drop.self[s] = gs::make_drop_site(self_sites_host[s]);
-    tab.total_rows += tab.s[s].n;
   }
   if (tab.total_rows == 0) return GS_OK;
   GS_REQUIRE(src && out_mean, "gs_gather_mean_dropout: NULL pointer");
@@ -1193,10 +1160,7 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
                       pitch % 4 == 0 && out_pitch % 4 == 0 && ((F + 3) / 4) * 4 <= pitch;
   if (vec_ok && ncol4 <= 2 * 160) {
     const gs::DenseRows rows_of{src, n_src_rows, pitch};
-    gs::GatherImg img;
-    memset(&img, 0, sizeof(img));
-    return gs::launch_gather_tma2<gs::DenseRows, true>(rows_of, F, tab, include_self, out_self, out_mean, out_pitch, img, st,
-                                                       &drop);
+    return gs::launch_gather_tma2<gs::DenseRows, true>(rows_of, F, tab, include_self, out_self, out_mean, out_pitch, st, &drop);
   }
   int64_t blocks = tab.total_rows;
   int64_t cap = (int64_t)gs::sm_count() * 8;
@@ -1284,57 +1248,6 @@ int32_t gs_translate_ids(const gs_sharded_table* table_host, const int32_t* ids,
   return gs::launch_check("translate_ids_kernel");
 }
 
-int64_t gs_gather_mean_img_bytes(int64_t rows, int32_t F, int32_t want_self) {
-  if (rows < 0 || F < 1) return -1;
-  const int64_t n_mtiles = (rows + 127) / 128, kblocks = (F + 31) / 32;
-  return (want_self ? 2 : 1) * n_mtiles * kblocks * 2 * 16384;
-}
-
-int32_t gs_gather_mean_img(const void* src, int64_t n_src_rows, const gs_sharded_table* table_host, int32_t ids_are_locators,
-                           const void* staging, int32_t F, int64_t pitch, const gs_segment* segments_host, int32_t n_segments,
-                           int32_t include_self, int32_t want_self, void* images, void* stream) {
-  GS_REQUIRE((src != nullptr) != (table_host != nullptr), "gs_gather_mean_img: pass either a dense table or a sharded one");
-  GS_REQUIRE(n_segments >= 0 && n_segments <= GS_MAX_SEGMENTS && (segments_host || n_segments == 0),
-             "gs_gather_mean_img: bad segments");
-  gs::SegTable tab;
-  memset(&tab, 0, sizeof(tab));
-  tab.n_segments = n_segments;
-  int64_t rows = 0;
-  for (int s = 0; s < n_segments; ++s) {
-    tab.s[s] = segments_host[s];
-    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "gs_gather_mean_img: segment %d has n=%lld k=%d", s, (long long)tab.s[s].n,
-               tab.s[s].k);
-    tab.total_rows += tab.s[s].n;
-    if (tab.s[s].out_row0 + tab.s[s].n > rows) rows = tab.s[s].out_row0 + tab.s[s].n;
-  }
-  if (tab.total_rows == 0) return GS_OK;
-  GS_REQUIRE(images && (reinterpret_cast<uintptr_t>(images) & 1023u) == 0, "gs_gather_mean_img: images must be 1024-byte aligned");
-  const int64_t out_pitch = ((int64_t)F + 7) / 8 * 8;
-  const int ncol4 = (int)(out_pitch / 4);
-  if (ncol4 > 2 * 160 || F < 1 || pitch % 4 != 0 || pitch < ((F + 3) / 4) * 4 || gs::tuning("gather_variant", 2) != 2) {
-    gs::set_error("gs_gather_mean_img: needs F <= 1280, 16-byte row pitch and the bulk-copy gather (F=%d pitch=%lld)", F, (long long)pitch);
-    return GS_ERR_UNSUPPORTED;
-  }
-  gs::GatherImg img;
-  img.base = (unsigned char*)images;
-  img.kblocks = (F + 31) / 32;
-  img.n_mtiles = (int32_t)((rows + 127) / 128);
-  img.want_self = want_self ? 1 : 0;
-  if (src) {
-    GS_REQUIRE(gs::aligned16(src) && n_src_rows > 0, "gs_gather_mean_img: table must be 16-byte aligned");
-    const gs::DenseRows rows_of{(const float*)src, n_src_rows, pitch};
-    return gs::launch_gather_tma2(rows_of, F, tab, include_self, nullptr, nullptr, out_pitch, img, (cudaStream_t)stream);
-  }
-  gs::ShardRows sr;
-  int32_t rc = fill_shard_tab(table_host, sr, pitch, "gs_gather_mean_img");
-  if (rc != GS_OK) return rc;
-  GS_REQUIRE(ids_are_locators >= 0 && ids_are_locators <= 2 && (ids_are_locators != 2 || staging != nullptr),
-             "gs_gather_mean_img: ids_are_locators = 2 needs the staging buffer");
-  sr.locators = ids_are_locators;
-  sr.staging = (const float*)staging;
-  return gs::launch_gather_tma2(sr, F, tab, include_self, nullptr, nullptr, out_pitch, img, (cudaStream_t)stream);
-}
-
 int32_t gs_halo_begin(int32_t* claim, int64_t n_global_rows, int32_t* count, void* stream) {
   GS_REQUIRE(claim && count && n_global_rows > 0, "gs_halo_begin: bad arguments");
   GS_CUDA(cudaMemsetAsync(claim, 0xff, (size_t)n_global_rows * 4, (cudaStream_t)stream));     // every entry = -1
@@ -1405,14 +1318,8 @@ int32_t gs_gather_mean_sharded(const gs_sharded_table* table_host, int32_t dtype
   sr.locators = ids_are_locators;
   sr.staging = (const float*)staging;
   gs::SegTable tab;
-  memset(&tab, 0, sizeof(tab));
-  tab.n_segments = n_segments;
-  for (int s = 0; s < n_segments; ++s) {
-    tab.s[s] = segments_host[s];
-    GS_REQUIRE(tab.s[s].n >= 0 && tab.s[s].k >= 1, "gs_gather_mean_sharded: segment %d has n=%lld k=%d", s,
-               (long long)tab.s[s].n, tab.s[s].k);
-    tab.total_rows += tab.s[s].n;
-  }
+  rc = fill_seg_table(segments_host, n_segments, tab, "gs_gather_mean_sharded");
+  if (rc != GS_OK) return rc;
   if (tab.total_rows == 0) return GS_OK;
   GS_REQUIRE(out_mean && gs::aligned16(out_mean) && (!out_self || gs::aligned16(out_self)) && out_pitch % 4 == 0 &&
                  F > 0 && pitch >= ((F + 3) / 4) * 4 && out_pitch >= F,
@@ -1420,12 +1327,8 @@ int32_t gs_gather_mean_sharded(const gs_sharded_table* table_host, int32_t dtype
   const int ncol4 = (int)(out_pitch / 4);
   // default: the grouped double-buffered bulk-copy kernel of the dense table with peer-mapped row addresses - a
   // remote row is one cp.async.bulk over NVLink straight into this SM's shared memory (gather_variant=0: 128-bit loads)
-  if (gs::tuning("gather_variant", 2) != 0 && ncol4 <= 2 * 160) {
-    gs::GatherImg img;
-    memset(&img, 0, sizeof(img));
-    return gs::launch_gather_tma2(sr, F, tab, include_self, (float*)out_self, (float*)out_mean, out_pitch, img,
-                                  (cudaStream_t)stream);
-  }
+  if (gs::tuning("gather_variant", 2) != 0 && ncol4 <= 2 * 160)
+    return gs::launch_gather_tma2(sr, F, tab, include_self, (float*)out_self, (float*)out_mean, out_pitch, (cudaStream_t)stream);
   int threads = ((ncol4 + 31) / 32) * 32;
   if (threads > 256) threads = 256;
   int64_t blocks = tab.total_rows;

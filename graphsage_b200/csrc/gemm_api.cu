@@ -5,8 +5,6 @@ namespace gs {
 int32_t sage_gemm_simt(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids* row_ids, int32_t n_parts,
                        int32_t combine, const float* bias, int32_t act, float* out, int64_t ldo, cudaStream_t st);
 int64_t sage_gemm_tc_workspace(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t math);
-int32_t sage_gemm_tc_img(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias, int32_t act,
-                         float* out, int64_t ldo, const void* workspace, const void* a_images, int32_t a_part0, cudaStream_t st);
 int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids* row_ids, int32_t n_parts, int32_t combine,
                      const float* bias, int32_t act, int32_t math, float* out, int64_t ldo, const void* workspace,
                      cudaStream_t st);
@@ -79,25 +77,6 @@ int32_t gs_sage_gemm_prepacked(int64_t M, const gs_gemm_part* parts_host, int32_
                                const float* bias, int32_t act, int32_t math, float* out, int64_t ldo,
                                const void* workspace, void* stream) {
   return gs_sage_gemm_rows(M, parts_host, nullptr, n_parts, combine, bias, act, math, out, ldo, workspace, stream);
-}
-
-int32_t gs_sage_gemm_img(int64_t M, const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
-                         int32_t act, float* out, int64_t ldo, const void* workspace, const void* a_images,
-                         int32_t a_part0, void* stream) {
-  GS_REQUIRE(parts_host && n_parts >= 1 && n_parts <= 2, "gs_sage_gemm_img: n_parts must be 1 or 2");
-  for (int i = 0; i < n_parts; ++i)
-    GS_REQUIRE(parts_host[i].B && parts_host[i].K >= 1 && parts_host[i].N >= 1 && parts_host[i].ldb >= parts_host[i].N,
-               "gs_sage_gemm_img: bad part %d", i);
-  GS_REQUIRE(combine == GS_COMBINE_CONCAT || n_parts == 1 || parts_host[0].N == parts_host[1].N,
-             "gs_sage_gemm_img: ADD needs equal output widths");
-  if (M == 0) return GS_OK;
-  GS_REQUIRE(M > 0 && out, "gs_sage_gemm_img: bad M / out");
-  int ntot = parts_host[0].N + ((n_parts == 2 && combine == GS_COMBINE_CONCAT) ? parts_host[1].N : 0);
-  GS_REQUIRE(ldo >= ntot, "gs_sage_gemm_img: ldo=%lld < output width %d", (long long)ldo, ntot);
-  GS_REQUIRE(act == GS_ACT_NONE || act == GS_ACT_RELU, "gs_sage_gemm_img: act=%d", act);
-  GS_REQUIRE(a_part0 >= 0 && a_part0 <= 1, "gs_sage_gemm_img: a_part0=%d", a_part0);
-  return gs::sage_gemm_tc_img(M, parts_host, n_parts, combine, bias, act, out, ldo, workspace, a_images, a_part0,
-                              (cudaStream_t)stream);
 }
 
 int32_t gs_sage_gemm(int64_t M, const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,

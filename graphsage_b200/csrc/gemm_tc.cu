@@ -10,13 +10,10 @@
 // Structure (one CTA = one 128 x 128 output tile, two warpgroups of 128 threads, each owning 64 output rows):
 //   B (weights): pre-swizzled tile images of W^T (built per weight update by pack_b_kernel into the caller's
 //                workspace), one cp.async.bulk per K-block into a ring of stages, completion on an mbarrier.
-//   A          : register form - every thread loads its 16-byte chunks of the next K-block from global memory while
-//                the current K-block's wgmmas run, then splits / converts them and stores the SW128 tile image; a part
-//                may name its rows by id into a table (gs_sage_gemm_rows: the mean layer-0 self rows straight from the
-//                feature table), resolved once per tile, so only the address of the load changes;
-//                image form (tf32x3 only) - the fused gather already wrote the tf32 hi / lo tile images
-//                (gs_gather_mean_img), so A arrives by bulk copy like B.  Both forms run the same MMAs in the same
-//                order, so their results are bit-identical.
+//   A          : every thread loads its 16-byte chunks of the next K-block from global memory while the current
+//                K-block's wgmmas run, then splits / converts them and stores the SW128 tile image; a part may name its
+//                rows by id into a table (gs_sage_gemm_rows: the mean layer-0 self rows straight from the feature
+//                table), resolved once per tile, so only the address of the load changes.
 // A goes through registers on purpose: the hi/lo split (and the bf16 rounding) is arithmetic on the operand.
 #include "tc_common.cuh"
 
@@ -46,10 +43,7 @@ struct TcParams {
   float* out;
   int64_t ldo;
   int32_t tiles_n0;    // number of N tiles of part 0 (CONCAT tile -> part mapping)
-  const unsigned char* a_img;   // image form: A operands as tf32 hi/lo tile images (gs_gather_mean_img)
-  int32_t a_mtiles;             // 128-row tiles in the A images
-  int32_t a_part0;              // A-image part that feeds GEMM part 0 (GEMM part p reads A part a_part0 + p)
-  gs_gemm_row_ids rid[2];       // register form: part p's A rows by id (gs_sage_gemm_rows); n_ranges == 0: dense A
+  gs_gemm_row_ids rid[2];       // part p's A rows by id (gs_sage_gemm_rows); n_ranges == 0: dense A
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -134,32 +128,30 @@ __device__ __forceinline__ void load_a_chunk(const TcPart& P, int64_t arow, int 
 }
 
 template <int MODE>
-__device__ __forceinline__ void store_a_chunk(unsigned char* a_img, int row, int c, const float (&v)[8]) {
+__device__ __forceinline__ void store_a_chunk(unsigned char* tile, int row, int c, const float (&v)[8]) {
   const uint32_t off = sw128_off(row, c);
   if constexpr (MODE == 2) {
     __nv_bfloat162 h[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
-    *reinterpret_cast<uint4*>(a_img + off) = *reinterpret_cast<uint4*>(h);
+    *reinterpret_cast<uint4*>(tile + off) = *reinterpret_cast<uint4*>(h);
   } else {
     uint4 hi;
     hi.x = tf32_mask(v[0]); hi.y = tf32_mask(v[1]); hi.z = tf32_mask(v[2]); hi.w = tf32_mask(v[3]);
-    *reinterpret_cast<uint4*>(a_img + off) = hi;
+    *reinterpret_cast<uint4*>(tile + off) = hi;
     if constexpr (MODE == 0) {
       uint4 lo;
       lo.x = tf32_mask(v[0] - __uint_as_float(hi.x)); lo.y = tf32_mask(v[1] - __uint_as_float(hi.y));
       lo.z = tf32_mask(v[2] - __uint_as_float(hi.z)); lo.w = tf32_mask(v[3] - __uint_as_float(hi.w));
-      *reinterpret_cast<uint4*>(a_img + TC_TILE_BYTES + off) = lo;
+      *reinterpret_cast<uint4*>(tile + TC_TILE_BYTES + off) = lo;
     }
   }
 }
 
-// kImg: A from the gather's tile images (MODE 0 only) instead of the fp32 rows
-template <int MODE, bool kImg>
+template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __grid_constant__ TcParams prm,
                                                                      const unsigned char* __restrict__ ws) {
   using C = TcCfg<MODE>;
-  static_assert(!kImg || MODE == 0, "the image form carries tf32 hi / lo images");
   extern __shared__ unsigned char smem_raw[];
   __shared__ __align__(8) uint64_t full[C::STAGES];
 
@@ -187,7 +179,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
   }
   __syncthreads();
 
-  // one thread posts the bulk copies of K-block `it` (B, and A in the image form) into its stage
+  // one thread posts the bulk copy of K-block `it`'s B images into its stage
   auto post = [&](int it) {
     if (tid != 0 || it >= total_it) return;
     int pi, kb;
@@ -195,22 +187,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
     const TcPart& P = prm.p[pi];
     const int s = it % C::STAGES;
     unsigned char* st = smem + (size_t)s * C::STAGE_BYTES;
-    mbar_expect_tx(&full[s], kImg ? 2 * C::IMG_BYTES : C::IMG_BYTES);
+    mbar_expect_tx(&full[s], C::IMG_BYTES);
     bulk_g2s(st + C::IMG_BYTES, ws + P.img_off + ((int64_t)ntile * P.kblocks + kb) * C::IMG_BYTES, C::IMG_BYTES, &full[s]);
-    if constexpr (kImg)
-      bulk_g2s(st, prm.a_img + (((int64_t)(prm.a_part0 + pi) * prm.a_mtiles + blockIdx.x) * P.kblocks + kb) * C::IMG_BYTES,
-               C::IMG_BYTES, &full[s]);
   };
   // the A row behind each of this thread's chunks, for the tile's first and second part: fixed over the K loop, so a part
   // whose rows come by id looks each id up once per tile, not once per K-block
   int64_t arow_lo[C::CPT], arow_hi[C::CPT];
-  if constexpr (!kImg) {
 #pragma unroll
-    for (int i = 0; i < C::CPT; ++i) {
-      const int64_t r = m0 + ((tid + TC_THREADS * i) >> 3);
-      arow_lo[i] = gemm_a_row(prm.rid[part_lo], prm.M, r);
-      arow_hi[i] = part_hi - part_lo == 2 ? gemm_a_row(prm.rid[part_lo + 1], prm.M, r) : -1;
-    }
+  for (int i = 0; i < C::CPT; ++i) {
+    const int64_t r = m0 + ((tid + TC_THREADS * i) >> 3);
+    arow_lo[i] = gemm_a_row(prm.rid[part_lo], prm.M, r);
+    arow_hi[i] = part_hi - part_lo == 2 ? gemm_a_row(prm.rid[part_lo + 1], prm.M, r) : -1;
   }
   float cur[C::CPT][8];
   auto fetch = [&](int it) {
@@ -226,7 +213,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
   };
 
   for (int j = 0; j < C::STAGES - 1; ++j) post(j);
-  if constexpr (!kImg) fetch(0);
+  fetch(0);
 
   float acc[64];
 #pragma unroll
@@ -234,19 +221,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) sage_gemm_tc_kernel(const __gri
   for (int it = 0; it < total_it; ++it) {
     const int s = it % C::STAGES;
     unsigned char* st = smem + (size_t)s * C::STAGE_BYTES;
-    if constexpr (!kImg) {
 #pragma unroll
-      for (int i = 0; i < C::CPT; ++i) {
-        const int q = tid + TC_THREADS * i;
-        store_a_chunk<MODE>(st, q >> 3, q & 7, cur[i]);
-      }
-      fence_proxy_async();                       // generic-proxy stores -> visible to wgmma (async proxy)
+    for (int i = 0; i < C::CPT; ++i) {
+      const int q = tid + TC_THREADS * i;
+      store_a_chunk<MODE>(st, q >> 3, q & 7, cur[i]);
     }
+    fence_proxy_async();                         // generic-proxy stores -> visible to wgmma (async proxy)
     __syncthreads();                             // A stored; every warpgroup is done with K-block it - 1's stage
     post(it + C::STAGES - 1);                    // ... which is the stage this refills
-    if constexpr (!kImg) {
-      if (it + 1 < total_it) fetch(it + 1);      // next K-block's loads fly under this one's MMAs
-    }
+    if (it + 1 < total_it) fetch(it + 1);        // next K-block's loads fly under this one's MMAs
     mbar_wait(&full[s], (uint32_t)(it / C::STAGES) & 1u);
     const uint32_t a_base = smem_u32(st) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(st + C::IMG_BYTES);
     const uint64_t a_hi = make_smem_desc(a_base), b_hi = make_smem_desc(b_base);
@@ -333,15 +316,15 @@ static int32_t launch_pack(const TcParams& prm, unsigned char* ws, cudaStream_t 
   return launch_check("pack_b_kernel");
 }
 
-template <int MODE, bool kImg>
+template <int MODE>
 static int32_t launch_tc(const TcParams& prm, const unsigned char* ws, cudaStream_t st) {
   using C = TcCfg<MODE>;
-  const int32_t rc_attr = ensure_dyn_smem((const void*)sage_gemm_tc_kernel<MODE, kImg>, C::SMEM_BYTES);
+  const int32_t rc_attr = ensure_dyn_smem((const void*)sage_gemm_tc_kernel<MODE>, C::SMEM_BYTES);
   if (rc_attr != GS_OK) return rc_attr;
   int tiles_n = prm.p[0].ntiles;
   if (prm.combine == GS_COMBINE_CONCAT && prm.n_parts == 2) tiles_n += prm.p[1].ntiles;
   dim3 grid((unsigned)((prm.M + TC_BM - 1) / TC_BM), (unsigned)tiles_n);
-  sage_gemm_tc_kernel<MODE, kImg><<<grid, TC_THREADS, C::SMEM_BYTES, st>>>(prm, ws);
+  sage_gemm_tc_kernel<MODE><<<grid, TC_THREADS, C::SMEM_BYTES, st>>>(prm, ws);
   return launch_check("sage_gemm_tc_kernel");
 }
 
@@ -355,24 +338,6 @@ int32_t sage_gemm_tc_pack(const gs_gemm_part* parts, int32_t n_parts, int32_t ma
   if (mode == 0) return launch_pack<0>(prm, ws, st);
   if (mode == 1) return launch_pack<1>(prm, ws, st);
   return launch_pack<2>(prm, ws, st);
-}
-
-int32_t sage_gemm_tc_img(int64_t M, const gs_gemm_part* parts, int32_t n_parts, int32_t combine, const float* bias, int32_t act,
-                         float* out, int64_t ldo, const void* workspace, const void* a_images, int32_t a_part0,
-                         cudaStream_t st) {
-  GS_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 127u) == 0,
-             "gs_sage_gemm_img: packed weights missing or not 128-byte aligned");
-  GS_REQUIRE(a_images != nullptr && (reinterpret_cast<uintptr_t>(a_images) & 1023u) == 0,
-             "gs_sage_gemm_img: A images missing or not 1024-byte aligned");
-  TcParams prm;
-  fill_parts(prm, M, parts, n_parts, 0);
-  for (int i = 1; i < n_parts; ++i)
-    GS_REQUIRE(prm.p[i].K == prm.p[0].K, "gs_sage_gemm_img: every part must have the K of the gathered rows");
-  prm.combine = combine; prm.bias = bias; prm.act = act; prm.out = out; prm.ldo = ldo;
-  prm.a_img = (const unsigned char*)a_images;
-  prm.a_mtiles = (int32_t)((M + TC_BM - 1) / TC_BM);
-  prm.a_part0 = a_part0;
-  return launch_tc<0, true>(prm, (const unsigned char*)workspace, st);
 }
 
 int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids* row_ids, int32_t n_parts, int32_t combine,
@@ -390,9 +355,9 @@ int32_t sage_gemm_tc(int64_t M, const gs_gemm_part* parts, const gs_gemm_row_ids
   prm.out = out;
   prm.ldo = ldo;
   const unsigned char* ws = (const unsigned char*)workspace;
-  if (mode == 0) return launch_tc<0, false>(prm, ws, st);
-  if (mode == 1) return launch_tc<1, false>(prm, ws, st);
-  return launch_tc<2, false>(prm, ws, st);
+  if (mode == 0) return launch_tc<0>(prm, ws, st);
+  if (mode == 1) return launch_tc<1>(prm, ws, st);
+  return launch_tc<2>(prm, ws, st);
 }
 
 }  // namespace gs

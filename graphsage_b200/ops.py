@@ -413,59 +413,6 @@ def _gather_mean_sharded(src, segments, include_self, want_self, out_pitch, out_
     return (out_self if want_self else None), out_mean
 
 
-def gather_mean_images(src, segments, include_self=False, want_self=True):
-    """gs_gather_mean_img: the fused gather + fanout mean whose result is written as tf32 hi/lo tensor-core tile images (the A
-    operand of sage_gemm_img).  Returns (images uint8 tensor, rows) or None when the image form does not apply."""
-    sharded = hasattr(src, "c_table")
-    if not sharded:
-        require_cuda(src)
-        if src.dtype != torch.float32 or src.dim() != 2 or src.stride(1) != 1:
-            return None
-    F = src.shape[1]
-    pitch = src.pitch if sharded else src.stride(0)
-    if F > 1280 or pitch % 4 != 0 or (not sharded and src.data_ptr() % 16 != 0):
-        return None
-    rows = max([s.out_row0 + s.n for s in segments] + [0])
-    if rows == 0:
-        return None
-    nbytes = lib().gs_gather_mean_img_bytes(rows, F, int(bool(want_self)))
-    dev = src.device
-    buf = torch.empty((nbytes + 1024,), dtype=torch.uint8, device=dev)
-    off = (-buf.data_ptr()) % 1024
-    images = buf[off:off + nbytes]
-    locators, staging = 0, None
-    if sharded:
-        segments, locators, staging = _shard_prepare(src, segments)
-    arr = (Segment * max(len(segments), 1))(*[s.c_struct() for s in segments])
-    ev = _probe("gather_mean/%d" % rows)
-    rc = lib().gs_gather_mean_img(0 if sharded else ptr(src), 0 if sharded else src.shape[0], src.c_table() if sharded else None,
-                                  locators, ptr(staging), F, pitch, arr, len(segments), int(bool(include_self)),
-                                  int(bool(want_self)), ptr(images), stream_ptr())
-    if rc == -3:                       # GS_ERR_UNSUPPORTED: the caller uses the fp32 pair
-        return None
-    check(rc)
-    _launched(1, ev)
-    return images, rows
-
-
-def sage_gemm_img(M, images, parts, combine=COMBINE_ADD, bias=None, act=ACT_NONE, packed=None, a_part0=0, out=None):
-    """gs_sage_gemm_img: act(concat_or_add(A_p @ B_p) + bias) in tf32x3 arithmetic with the A operands taken from the tile
-    images gather_mean_images wrote (part p reads image part a_part0 + p).  parts: [(None, K, B[K, N])]."""
-    _, arr, keep = _gemm_parts([(None, K, B) for (_, K, B) in parts])
-    ntot = sum(p[2].shape[1] for p in parts) if (combine == COMBINE_CONCAT) else parts[0][2].shape[1]
-    dev = images.device
-    if out is None:
-        out = torch.empty((M, ntot), dtype=torch.float32, device=dev)
-    if packed is None:
-        packed = PackedWeights()
-    ws = packed.get(parts, arr, MATH_TF32X3, dev)
-    ev = _probe("sage_gemm/%d" % M)
-    check(lib().gs_sage_gemm_img(M, arr, len(parts), combine, ptr(bias), act, ptr(out), out.stride(0), ptr(ws), ptr(images),
-                                 int(a_part0), stream_ptr()))
-    _launched(1 if M else 0, ev)
-    return out
-
-
 def segment_max(x, n, k):
     require_cuda(x)
     C = x.shape[1]

@@ -3,8 +3,8 @@
 One process per GPU (torch.distributed for bootstrap, seed routing, barriers and the training step's one gradient
 all-reduce).  Rank r owns the feature rows of the global nodes [row_start[r], row_start[r+1]) - equal ranges
 (`uniform_bounds`) or cuts moved to community starts (`community_bounds`); every rank maps every shard through CUDA IPC
-(NVLink / NVSwitch peer memory), and the gather kernels (gs_gather_mean_sharded / gs_gather_rows_sharded /
-gs_gather_mean_img) resolve each id to `base[owner] + (id - row_start[owner]) * pitch`: remote rows are pulled by the
+(NVLink / NVSwitch peer memory), and the gather kernels (gs_gather_mean_sharded / gs_gather_rows_sharded) resolve
+each id to `base[owner] + (id - row_start[owner]) * pitch`: remote rows are pulled by the
 consuming kernel's own bulk copies, so no collective sits on the data path.  A rank may also keep replicas of the
 remote rows its batches read most (`hot_remote_rows`, `hot_remote_rows_csr`) behind its own rows; ids are then resolved
 once per step to locators (ops.translate_ids) and replica hits are local reads.  GS_HALO_STAGING=1 switches to the

@@ -323,29 +323,6 @@ int32_t gs_sage_gemm_rows(int64_t M, const gs_gemm_part* parts_host, const gs_ge
                           const void* workspace, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * The mean / GCN layer-0 pair with the A operand handed over as tensor-core tile images (tf32x3 arithmetic):
- *   gs_gather_mean_img : the fused gather + fanout mean of gs_gather_mean / gs_gather_mean_sharded (same segments, same
- *       table forms: pass `src` (dense fp32 [n_src_rows, pitch]) or `table_host` (node-partitioned; ids_are_locators /
- *       staging as in gs_gather_mean_sharded)), whose result rows are written ALREADY SPLIT into tf32 hi / lo and laid
- *       out as K-major SWIZZLE_128B tensor-core tile images: part p (0 = self rows, 1 = mean rows when want_self; only the mean
- *       part when !want_self), 128-row tile mt, 32-column K-block kb at
- *       images + (((p * n_mtiles + mt) * kblocks + kb) * 2 + hl) * 16384, hl = 0 hi / 1 lo.  images: device buffer of
- *       gs_gather_mean_img_bytes(rows, F, want_self) bytes, 1024-byte aligned; rows = max(out_row0 + n).
- *       GS_ERR_UNSUPPORTED when the bulk-copy gather does not apply (F > 1280, unaligned pitch): use the fp32 pair.
- *   gs_sage_gemm_img : gs_sage_gemm_prepacked(math = GS_MATH_TF32X3) with part p's A operand = image part a_part0 + p
- *       (parts[].A / lda are ignored; every part's K = F).  Bit-identical results to the fp32-operand form.
- * Reference ops: tf.nn.embedding_lookup + reduce_mean + matmul + concat/add_n + relu (models.py:299,
- * aggregators.py:48-64 / 106-116).
- * --------------------------------------------------------------------------------------------- */
-int64_t gs_gather_mean_img_bytes(int64_t rows, int32_t F, int32_t want_self);
-int32_t gs_gather_mean_img(const void* src, int64_t n_src_rows, const gs_sharded_table* table_host, int32_t ids_are_locators,
-                           const void* staging, int32_t F, int64_t pitch, const gs_segment* segments_host,
-                           int32_t n_segments, int32_t include_self, int32_t want_self, void* images, void* stream);
-int32_t gs_sage_gemm_img(int64_t M, const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
-                         int32_t act, float* out, int64_t ldo, const void* workspace, const void* a_images,
-                         int32_t a_part0, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
  * One whole aggregator layer for a SMALL number of output rows (the last layers of the recursion:
  * 512 rows at batch 512) in one launch, exact fp32 FFMA:
  *   mean over the fanout (gs_gather_mean semantics, one segment) -> two (or one) matmuls ->

@@ -336,7 +336,7 @@ def test_gather_mean_emulated(gs, layout, F, gv, variant):
             emu.close()
 
 
-def test_gather_mean_refuses_mixed_addressing(gs):
+def test_sharded_gather_mean_refuses_mixed_addressing(gs):
     """With replicas or halo staging the id lists are translated to locators, which a row-range segment cannot carry: a
     call that mixes both forms must be refused (before, the replica form read its row ranges as local row indices)."""
     row_start = LAYOUTS["unequal3"]
@@ -352,60 +352,11 @@ def test_gather_mean_refuses_mixed_addressing(gs):
         else:
             with pytest.raises(ValueError, match="by ids"):
                 gs.ops.gather_mean(emu, segs)
-            with pytest.raises(ValueError, match="by ids"):
-                gs.ops.gather_mean_images(emu, segs)
         emu.close()
 
 
-# ---------------------------------------------------------------- gs_gather_mean_img with a table + gs_sage_gemm_img
-SEGS_IMG = [(140, 25), (0, 13), (9, 128), (17, 14)]
-
-
-@pytest.mark.parametrize("F", [602, 50])
-@pytest.mark.parametrize("kind", ["mean_concat", "mean_add", "gcn"])
-def test_gather_mean_images_emulated(gs, kind, F):
-    ops = gs.ops
-    row_start = LAYOUTS["unequal3"]
-    feats = features(F, 21)
-    dense = dense_table(feats)
-    segs = id_segments(gs, id_pool(row_start), SEGS_IMG, 22)
-    rs = np.random.RandomState(23)
-    D = 64
-    W = [dev((rs.randn(F, D) * 0.1).astype(np.float32)) for _ in range(2)]
-    gcn = kind == "gcn"
-    combine = ops.COMBINE_CONCAT if kind == "mean_concat" else ops.COMBINE_ADD
-    bias = dev(rs.randn(D if combine == ops.COMBINE_ADD else 2 * D).astype(np.float32))
-    img_parts = [(None, F, W[0])] if gcn else [(None, F, W[0]), (None, F, W[1])]
-
-    def image_pair(table):
-        res = ops.gather_mean_images(table, segs, include_self=gcn, want_self=not gcn)
-        assert res is not None
-        images, rows = res
-        return ops.sage_gemm_img(rows, images, img_parts, combine=combine, bias=bias, act=ops.ACT_RELU)
-
-    want = image_pair(dense)
-    for my in range(3):
-        for mode in ("plain", "replicas", "halo"):
-            emu = emulate(feats, row_start, my, mode)
-            got = image_pair(emu)
-            assert torch.equal(got, want), (kind, F, my, mode)
-            xs, xm = ops.gather_mean(emu, segs, include_self=gcn, want_self=not gcn)
-            parts = [(xm, F, W[0])] if gcn else [(xs, F, W[0]), (xm, F, W[1])]
-            fp32_pair = ops.sage_gemm(parts, combine=combine, bias=bias, act=ops.ACT_RELU, math=ops.MATH_TF32X3)
-            assert torch.equal(got, fp32_pair), (kind, F, my, mode)
-            emu.close()
-
-
-def test_gather_mean_images_refuse_wide_rows(gs):
-    F = 1500                                                # ncol4 > 320: the image form does not apply
-    emu = emulate(features(F), LAYOUTS["unequal3"], 1, "halo")
-    segs = id_segments(gs, id_pool(LAYOUTS["unequal3"]), [(10, 13)], 24)
-    assert gs.ops.gather_mean_images(emu, segs, want_self=True) is None
-    emu.close()
-
-
 # ---------------------------------------------------------------- refusals: errors, not launches
-def test_sharded_entry_points_refuse_bad_tables(gs):
+def test_sharded_entry_points_refuse_bad_shard_tables(gs):
     lib, ptr, check, stream = gs._lib.lib(), gs._lib.ptr, gs._lib.check, gs._lib.stream_ptr()
     F = 50
     row_start = LAYOUTS["unequal3"]
@@ -421,10 +372,6 @@ def test_sharded_entry_points_refuse_bad_tables(gs):
     locs = torch.full((n,), -7, dtype=torch.int32, device="cuda")
     seg = gs.ops.Seg(4, 13, self_ids=ids[:4], neigh_ids=ids[4:56])
     arr = (gs._lib.Segment * 1)(seg.c_struct())
-    nbytes = lib.gs_gather_mean_img_bytes(4, F, 1)
-    img_buf = torch.full((nbytes + 1024,), 7, dtype=torch.uint8, device="cuda")
-    off = (-img_buf.data_ptr()) % 1024
-    images = img_buf[off:off + nbytes]
 
     def entries(t, locators=0, staging_ptr=None):
         return {
@@ -432,8 +379,6 @@ def test_sharded_entry_points_refuse_bad_tables(gs):
                                                                          stream),
             "gs_gather_mean_sharded": lambda: lib.gs_gather_mean_sharded(t, gs._lib.GS_F32, F, pitch, arr, 1, 0, locators,
                                                                          staging_ptr, ptr(out), ptr(out), pitch, stream),
-            "gs_gather_mean_img": lambda: lib.gs_gather_mean_img(None, 0, t, locators, staging_ptr, F, pitch, arr, 1, 0, 1,
-                                                                 ptr(images), stream),
             "gs_halo_claim": lambda: lib.gs_halo_claim(t, ptr(ids), n, ptr(claim), ptr(count), ptr(stage_ids), n, stream),
             "gs_halo_translate": lambda: lib.gs_halo_translate(t, ptr(ids), n, ptr(claim), ptr(locs), stream),
             "gs_halo_fetch": lambda: lib.gs_halo_fetch(t, F, pitch, ptr(stage_ids), ptr(count), n, ptr(staging), pitch, stream),
@@ -464,22 +409,21 @@ def test_sharded_entry_points_refuse_bad_tables(gs):
         for name, call in entries(ctypes.byref(t)).items():
             with pytest.raises(RuntimeError, match=re.escape("%s: %s" % (name, msg))):
                 check(call())
-    for name in ("gs_gather_mean_sharded", "gs_gather_mean_img"):
-        with pytest.raises(RuntimeError, match=re.escape("%s: ids_are_locators = 2 needs the staging buffer" % name)):
-            check(entries(emu.c_table(), locators=2)[name]())
+    with pytest.raises(RuntimeError, match=re.escape("gs_gather_mean_sharded: ids_are_locators = 2 needs the staging buffer")):
+        check(entries(emu.c_table(), locators=2)["gs_gather_mean_sharded"]())
     plain = emulate(features(F), row_start, 1, "plain")
     with pytest.raises(RuntimeError, match=re.escape("gs_translate_ids: the table has no remap (no replicas)")):
         gs.ops.translate_ids(plain, ids)
     torch.cuda.synchronize()
     # nothing was launched: every buffer a kernel would have written still holds its sentinel
     assert bool((out == -7).all()) and bool((staging == -7).all()) and bool((stage_ids == -7).all())
-    assert bool((locs == -7).all()) and bool((claim == -1).all()) and int(count.item()) == 0 and bool((images == 7).all())
+    assert bool((locs == -7).all()) and bool((claim == -1).all()) and int(count.item()) == 0
     plain.close()
     emu.close()
 
 
 # ---------------------------------------------------------------- every sharded entry point launches its own kernel
-def test_sharded_kernels_recorded_by_profiler(gs, variant):
+def test_sharded_kernels_each_recorded_by_profiler(gs, variant):
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
     row_start = LAYOUTS["unequal3"]
@@ -496,7 +440,6 @@ def test_sharded_kernels_recorded_by_profiler(gs, variant):
             gs.ops.translate_ids(emus["replicas"], ids)
             for mode, e in emus.items():
                 gs.ops.gather_mean(e, segs)
-                gs.ops.gather_mean_images(e, segs)
             variant(0)
             gs.ops.gather_mean(emus["halo"], segs)
             variant(2)
