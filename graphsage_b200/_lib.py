@@ -131,7 +131,8 @@ _SIGNATURES = {
     "gs_embedding_grad": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "gs_gather_mean_dropout": (c_i32, [c_vp, c_i64, c_i32, c_i64, ctypes.POINTER(Segment), c_i32, ctypes.POINTER(DropoutSite),
                                        ctypes.POINTER(DropoutSite), c_i32, c_vp, c_vp, c_i64, c_vp]),
-    "gs_dropout_apply": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, ctypes.c_float, DropoutSite, c_i32, c_vp, c_i64, c_vp]),
+    "gs_dropout_apply": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, ctypes.c_float, DropoutSite, c_i32, c_vp, c_i64, c_vp,
+                                 c_vp]),
     "gs_embedding_grad_dropout": (c_i32, [ctypes.POINTER(EmbedGradList), ctypes.POINTER(DropoutSite), c_i32, c_i64, c_i32, c_vp,
                                           c_i64, c_vp, c_i64, c_vp]),
     "gs_embedding_sgd": (c_i32, [ctypes.POINTER(EmbedGradList), c_i32, c_i64, c_i32, ctypes.c_float, c_vp, c_i64, c_vp, c_i64,
@@ -151,8 +152,10 @@ _SIGNATURES = {
     "gs_random_walks": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_random_walks_emit": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp]),
     "gs_csr_aggregate": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp]),
+    "gs_csr_aggregate_dropout": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32,
+                                         DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "gs_csr_transpose_workspace_bytes": (c_i64, [c_i64, c_i64, c_i32]),
-    "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gs_csr_max_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64,
                                     c_vp, c_i64, c_vp]),
     "gs_csr_blocks_workspace_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i32]),

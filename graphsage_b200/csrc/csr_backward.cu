@@ -56,7 +56,9 @@ __global__ void __launch_bounds__(kBwdThreads) eff_count_kernel(const int64_t* _
   cnt[i] = i <= n_nodes ? c + with_self : 0;
 }
 
-// one warp per effective row: its (destination, source row) pairs at its scanned slots, in CSR order, the self entry last
+// one warp per effective row: its (destination, source row) pairs at its scanned slots, in CSR order, the self entry last.
+// kSlots: the value is the slot itself, from which slot_rows_kernel derives both the source row and the entry offset.
+template <bool kSlots>
 __global__ void __launch_bounds__(kBwdThreads) eff_fill_kernel(const int64_t* __restrict__ indptr,
                                                                const int32_t* __restrict__ indices, int64_t n_nodes,
                                                                int32_t with_self, const int64_t* __restrict__ slot,
@@ -77,17 +79,17 @@ __global__ void __launch_bounds__(kBwdThreads) eff_fill_kernel(const int64_t* __
         d = (d < 0 || d > n_nodes) ? n_nodes : d;
         if (base + e < cap) {
           keys[base + e] = (uint32_t)d;
-          vals[base + e] = (int32_t)i;
+          vals[base + e] = kSlots ? (int32_t)(base + e) : (int32_t)i;
         }
       }
     } else if (lane == 0 && base < cap) {        // an empty row and the dummy row: {N}
       keys[base] = (uint32_t)n_nodes;
-      vals[base] = (int32_t)i;
+      vals[base] = kSlots ? (int32_t)base : (int32_t)i;
     }
     const int64_t at = base + (c > 0 ? c : 1);
     if (with_self && lane == 0 && at < cap) {
       keys[at] = (uint32_t)i;
-      vals[at] = (int32_t)i;
+      vals[at] = kSlots ? (int32_t)at : (int32_t)i;
     }
   }
 }
@@ -104,6 +106,29 @@ __global__ void __launch_bounds__(kBwdThreads) t_indptr_kernel(const uint32_t* _
     else hi = mid;
   }
   t_indptr[j] = lo;
+}
+
+// after a kSlots sort: t_indices[k] holds the effective slot s of transposed entry k; write its source row i (the row
+// whose scanned slots hold s) to t_indices[k] and its offset in that row to t_slot[k]: j for entry j of the row's CSR
+// entries, -1 for the implicit {N} entry of an empty row or the dummy row, -2 for the with_self entry.  The unused tail
+// holds slot 0, so it becomes row 0 as without t_slot.
+__global__ void __launch_bounds__(kBwdThreads) slot_rows_kernel(const int64_t* __restrict__ slot,
+                                                                const int64_t* __restrict__ indptr, int64_t n_nodes,
+                                                                int64_t cap, int32_t* __restrict__ t_indices,
+                                                                int32_t* __restrict__ t_slot) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < cap; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t s = t_indices[k];
+    int64_t lo = 0, hi = n_nodes;               // the last row i <= N with slot[i] <= s (every row has >= 1 entry)
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (slot[mid] <= s) lo = mid;
+      else hi = mid - 1;
+    }
+    const int64_t j = s - slot[lo];
+    const int64_t c = lo < n_nodes ? indptr[lo + 1] - indptr[lo] : 0;
+    t_indices[k] = (int32_t)lo;
+    t_slot[k] = j >= (c > 0 ? c : 1) ? -2 : c > 0 ? (int32_t)j : -1;
+  }
 }
 
 static int32_t make_transpose_plan(int64_t n_nodes, int64_t nnz, int32_t with_self, TransposePlan& P, const char* who) {
@@ -299,7 +324,8 @@ int64_t gs_csr_transpose_workspace_bytes(int64_t n_nodes, int64_t nnz, int32_t w
 }
 
 int32_t gs_csr_transpose(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t with_self,
-                         int64_t* t_indptr, int32_t* t_indices, void* workspace, int64_t workspace_bytes, void* stream) {
+                         int64_t* t_indptr, int32_t* t_indices, int32_t* t_slot, void* workspace, int64_t workspace_bytes,
+                         void* stream) {
   const char* who = "gs_csr_transpose";
   gs::TransposePlan P;
   int32_t rc = gs::make_transpose_plan(n_nodes, nnz, with_self, P, who);
@@ -325,8 +351,12 @@ int32_t gs_csr_transpose(const int64_t* indptr, const int32_t* indices, int64_t 
   GS_CUDA(cudaMemsetAsync(kin, 0xFF, (size_t)P.cap * 4, st));       // unused slots: destination 0xFFFFFFFF, sorted last
   GS_CUDA(cudaMemsetAsync(vin, 0, (size_t)P.cap * 4, st));
   const int64_t fill_blocks = std::min<int64_t>((P.rows + 7) / 8, (int64_t)gs::sm_count() * 8 * 16);
-  gs::eff_fill_kernel<<<(unsigned)fill_blocks, gs::kBwdThreads, 0, st>>>(indptr, indices, n_nodes, with_self, slot, P.cap,
-                                                                       kin, vin);
+  if (t_slot)
+    gs::eff_fill_kernel<true><<<(unsigned)fill_blocks, gs::kBwdThreads, 0, st>>>(indptr, indices, n_nodes, with_self, slot,
+                                                                               P.cap, kin, vin);
+  else
+    gs::eff_fill_kernel<false><<<(unsigned)fill_blocks, gs::kBwdThreads, 0, st>>>(indptr, indices, n_nodes, with_self, slot,
+                                                                                P.cap, kin, vin);
   rc = gs::launch_check("eff_fill_kernel");
   if (rc != GS_OK) return rc;
   cub_bytes = P.cub_bytes;
@@ -334,7 +364,11 @@ int32_t gs_csr_transpose(const int64_t* indptr, const int32_t* indices, int64_t 
                                               t_indices, (int)P.cap, 0, P.end_bit, st);
   if (e != cudaSuccess) return gs::cuda_fail(e, "cub::DeviceRadixSort::SortPairs");
   gs::t_indptr_kernel<<<row_blocks, gs::kBwdThreads, 0, st>>>(kout, P.cap, n_nodes, t_indptr);
-  return gs::launch_check("t_indptr_kernel");
+  rc = gs::launch_check("t_indptr_kernel");
+  if (rc != GS_OK || !t_slot) return rc;
+  const int64_t slot_blocks = std::min<int64_t>((P.cap + gs::kBwdThreads - 1) / gs::kBwdThreads, (int64_t)gs::sm_count() * 16);
+  gs::slot_rows_kernel<<<(unsigned)slot_blocks, gs::kBwdThreads, 0, st>>>(slot, indptr, n_nodes, P.cap, t_indices, t_slot);
+  return gs::launch_check("slot_rows_kernel");
 }
 
 int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm, int64_t lddm,

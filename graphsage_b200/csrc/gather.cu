@@ -668,18 +668,20 @@ __global__ void __launch_bounds__(256) cast_rows_bf16_scalar_kernel(const float*
   }
 }
 
-// out[r, c] (+)= keep(site, r, c) ? (x[r / group, c] * scale) / keep : 0 - one thread per 4 columns of a row (one Philox
-// block), so every element is read and written by one thread (out may alias x when group == 1)
+// out[r, c] (+)= keep(site, pos, c) ? (x[r / group, c] * scale) / keep : 0, pos = kIds ? pos_ids[r] : r - one thread per
+// 4 columns of a row (one Philox block), so every element is read and written by one thread (out may alias x when
+// group == 1)
+template <bool kIds>
 __global__ void __launch_bounds__(256) dropout_apply_kernel(const float* x, int64_t ldx, int64_t rows, int F, int group,
                                                             float scale, DropSite site, int accumulate, float* out,
-                                                            int64_t ldo) {
+                                                            int64_t ldo, const int32_t* pos_ids) {
   const int nc4 = (F + 3) >> 2;
   const int64_t total = rows * nc4;
   site.call += drop_call_offset(site);
   for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = q / nc4;
     const int c4 = (int)(q - r * nc4);
-    const u32x4 w = drop_words(site, r, (uint32_t)c4);
+    const u32x4 w = drop_words(site, kIds ? (int64_t)__ldg(pos_ids + r) : r, (uint32_t)c4);
     const float* xr = x + (r / group) * ldx;
     float* orow = out + r * ldo;
 #pragma unroll
@@ -1171,7 +1173,8 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
 }
 
 int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, int32_t group, float scale,
-                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, void* stream) {
+                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, const int32_t* pos_ids,
+                         void* stream) {
   int32_t rc = check_site(site, "gs_dropout_apply");
   if (rc != GS_OK) return rc;
   GS_REQUIRE(rows >= 0 && F >= 0 && group >= 1, "gs_dropout_apply: bad sizes (rows=%lld F=%d group=%d)", (long long)rows, F,
@@ -1184,8 +1187,14 @@ int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, i
   int64_t blocks = (total + 255) / 256;
   int64_t cap = (int64_t)gs::sm_count() * 16;
   if (blocks > cap) blocks = cap;
-  gs::dropout_apply_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, F, group, scale,
-                                                                                gs::make_drop_site(site), accumulate, out, ldo);
+  if (pos_ids)
+    gs::dropout_apply_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, F, group, scale,
+                                                                                      gs::make_drop_site(site), accumulate,
+                                                                                      out, ldo, pos_ids);
+  else
+    gs::dropout_apply_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, F, group, scale,
+                                                                                       gs::make_drop_site(site), accumulate,
+                                                                                       out, ldo, nullptr);
   return gs::launch_check("dropout_apply_kernel");
 }
 

@@ -20,21 +20,32 @@ layer l runs over its block with the block's rows, exactly as the whole-graph la
 reads the global table: the means through the global CSR with rows = V_1, the pools' MLP on V_0's rows only (read by id,
 ops.TableRows), reduced through block 0.  Same bits as the whole-graph pass for the seeds; every buffer is block-sized.
 The blocks and their transposes are built per call, not cached.
+
+Training dropout (dropout=p > 0; contract: oracle/full_neighbor_dropout.py) masks by global identities: per CSR entry for
+the means' neighbour branch (gs_csr_aggregate_dropout, the entry's global CSR position), per node for the mean's self
+rows, GCN's own row and the pools' MLP input (ops.dropout_apply by id).  Each graph carries the position map of its
+kernels - (indptr, None, nnz) for the whole graph, (global indptr, src_ids, global nnz) for a block - so a block masks every
+element as the whole-graph pass does.  The backward regenerates every mask: the transposed sum reads the transpose's
+t_slot (ops.csr_transpose(slots=True)) to find each entry's forward position.
 """
 import torch
 
 from . import ops
 from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, _rows
 from .layers import act_code
-from .supervised_models import _LayerFn, build_aggregators, layer_params
+from .supervised_models import (_LayerFn, build_aggregators, check_full_neighbor_dropout, full_neighbor_site_plan,
+                                layer_params)
 
 
 class FullNeighborGraph(object):
     """The transposes and divisors of one CSR, built on first use.  `key` identifies the CSR tensors (data_ptr, numel,
     _version of both); the tensors themselves are held, so their memory cannot be reused by a different CSR while cached."""
 
-    def __init__(self, indptr, indices):
+    def __init__(self, indptr, indices, pos_map=None):
+        """pos_map: (pos_indptr, pos_ids or None, pos_nnz), how the masks name this CSR's rows and entries globally
+        (default: the CSR is the global one)."""
         self.indptr, self.indices = indptr, indices
+        self.pos_map = pos_map if pos_map is not None else (indptr, None, indices.numel())
         self.key = FullNeighborGraph.key_of(indptr, indices)
         self.n_rows = indptr.numel()                 # N + 1
         self._t, self._counts = {}, {}
@@ -43,7 +54,14 @@ class FullNeighborGraph(object):
     def key_of(indptr, indices):
         return tuple((t.data_ptr(), t.numel(), t._version) for t in (indptr, indices))
 
-    def transpose(self, with_self):
+    def transpose(self, with_self, slots=False):
+        """(t_indptr, t_indices), or with slots (t_indptr, t_indices, t_slot); a slotted transpose serves both."""
+        if (with_self, True) in self._t:
+            return self._t[(with_self, True)] if slots else self._t[(with_self, True)][:2]
+        if slots:
+            self._t.pop(with_self, None)
+            self._t[(with_self, True)] = ops.csr_transpose(self.indptr, self.indices, with_self=with_self, slots=True)
+            return self._t[(with_self, True)]
         if with_self not in self._t:
             self._t[with_self] = ops.csr_transpose(self.indptr, self.indices, with_self=with_self)
         return self._t[with_self]
@@ -56,11 +74,22 @@ class FullNeighborGraph(object):
             self._counts[with_self] = (torch.cat([deg, one]) + int(with_self)).to(torch.float32).unsqueeze(1)
         return self._counts[with_self]
 
-    def mean_backward(self, g, with_self):
+    def mean_backward(self, g, with_self, sites=None):
         """d(source) of the mean over the effective rows for their gradient g [N + 1, w]: sum of g / count over the
-        transposed rows."""
-        t_indptr, t_indices = self.transpose(with_self)
-        return ops.csr_aggregate((g / self.counts(with_self)).contiguous(), t_indptr, t_indices, "sum")
+        transposed rows; sites = (neighbour, self): the forward's masks, regenerated through t_slot."""
+        gp = (g / self.counts(with_self)).contiguous()
+        if sites is None:
+            t_indptr, t_indices = self.transpose(with_self)
+            return ops.csr_aggregate(gp, t_indptr, t_indices, "sum")
+        t_indptr, t_indices, t_slot = self.transpose(with_self, slots=True)
+        return ops.csr_aggregate(gp, t_indptr, t_indices, "sum", dropout=(sites[0], sites[1], self.pos_map), t_slot=t_slot)
+
+    def node_ids(self, rows):
+        """The global node ids of local rows (None: every row) for the per-node masks; None when they are the rows."""
+        ids = self.pos_map[1]
+        if rows is None:
+            return ids
+        return rows if ids is None else ids.index_select(0, rows.long())
 
 
 class _FullLayer(object):
@@ -73,6 +102,7 @@ class _FullLayer(object):
     def __init__(self, agg, graph, rows, src_ids=None, table_csr=None):
         self.agg, self.graph, self.rows = agg, graph, rows
         self.src_ids, self.table_csr = src_ids, table_csr
+        self.sites = None                       # training dropout: {"neigh", "self"} or {"mlp"} -> (seed, call, rate)
         self.gcn = isinstance(agg, GCNAggregator)
         self.pool = isinstance(agg, MaxPoolingAggregator)
         self.row_parts = 1 if self.gcn or self.pool else 2      # the GEMM parts that are rows of the source
@@ -96,21 +126,29 @@ class _FullLayer(object):
         agg, g, rows = self.agg, self.graph, self.rows
         self.table = h if self.src_ids is not None else None
         indptr, indices, h_rows = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows)
+        s = self.sites
+        # the means' masks: the table CSR is the global one (positions by node id), else the graph's own map
+        tgraph = FullNeighborGraph(indptr, indices) if self.table_csr is not None else g
+        drop = {} if s is None or self.pool else {"dropout": (s["neigh"], s["self"], tgraph.pos_map)}
         if self.gcn:
-            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=h_rows)
+            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=h_rows, **drop)
             return [(m, agg.neigh_input_dim, agg.vars["weights"])]
         widen = h.dtype != torch.float32
         n = h.shape[0] if h_rows is None else h_rows.numel()
         hs = _rows(h, h_rows, 0, n, widen) if (widen or h_rows is not None) else h
         if not self.pool:
-            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=h_rows)
+            if s is not None:                                        # the self rows by node id, after widening
+                hs = ops.dropout_apply(hs, s["self"], pos_ids=tgraph.node_ids(h_rows), out=None if hs is h else hs)
+            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=h_rows, **drop)
             return [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
         if self.src_ids is None:
             x = z = _rows(h, None, 0, h.shape[0], True) if widen else h
-        elif widen:
+        elif widen or s is not None:
             x = z = ops.gather_rows_f32(h, self.src_ids)             # V_0's rows, widened
         else:                                                        # V_0's rows read by id: no gathered copy
             x, z = None, ops.TableRows(h, [(self.src_ids, 0)], self.src_ids.numel())
+        if s is not None:                                            # the MLP input, once per node, by node id
+            x = z = ops.dropout_apply(x, s["mlp"], pos_ids=g.node_ids(None), out=None if x is h else x)
         for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116), once per node
             code, post = act_code(dense.act)
             if getattr(dense, "_packed", None) is None:
@@ -134,11 +172,16 @@ class _FullLayer(object):
         for p in range(len(dxs)):                    # made dense in place: each row gradient is freed once scattered
             if dxs[p] is not None:
                 dxs[p] = self.dense(dxs[p])
+        s, g = self.sites, self.graph
         if self.gcn:
-            return [], (self.graph.mean_backward(dxs[0], True) if cols else None)
+            return [], (g.mean_backward(dxs[0], True, s and (s["neigh"], s["self"])) if cols else None)
         dself = dxs[0]
         if not self.pool:
-            return [], (self.graph.mean_backward(dxs[1], False) + dself if cols else None)
+            if not cols:
+                return [], None
+            if s is not None:
+                dself = ops.dropout_apply(dself, s["self"], pos_ids=g.node_ids(None), out=dself)
+            return [], g.mean_backward(dxs[1], False, s and (s["neigh"], s["self"])) + dself
         (Wm, _), (x, z, p_all), dp = params, kept, dxs[1]
         if x is None:                                # the MLP read V_0's rows by id: gather them for dWm
             x = ops.gather_rows_f32(self.table, self.src_ids)
@@ -149,7 +192,12 @@ class _FullLayer(object):
             dzp = self.graph.mean_backward(dp, False) * (z > 0).to(dp.dtype)    # the ReLU of the Dense layer
         K = Wm.shape[0]
         grads = [x[:, :K].t() @ dzp, dzp.sum(dim=0)]
-        return grads, (dzp @ Wm[:cols].t() + dself if cols else None)
+        if not cols:
+            return grads, None
+        dx = dzp @ Wm[:cols].t()
+        if s is not None:                                            # through the MLP input's node mask
+            dx = ops.dropout_apply(dx, s["mlp"], pos_ids=g.node_ids(None), out=dx)
+        return grads, dx + dself
 
     def source_grads(self, ctx, dsrc, dy):
         """(d(h) of a layer >= 1, d(embeddings) of layer 0 with identity_dim > 0) from the source gradient dsrc."""
@@ -180,8 +228,9 @@ def refuse_capture(what):
         raise NotImplementedError("%s cannot be captured in a CUDA graph" % what)
 
 
-def refuse_full_neighbor(model, training):
-    """The NotImplementedErrors of the full-neighbourhood entry points; training adds those of the training paths."""
+def refuse_full_neighbor(model, training, dropout=None):
+    """The NotImplementedErrors of the full-neighbourhood entry points; training adds those of the training paths.
+    dropout: the training call's explicit rate (None: the model's dropout_rate must be 0)."""
     what = "training" if training else "inference"
     if model.aggregator_cls is SeqAggregator:
         raise NotImplementedError("full-neighbourhood %s is not implemented for the seq aggregator (its neighbour "
@@ -193,9 +242,11 @@ def refuse_full_neighbor(model, training):
         return
     if getattr(model, "distributed", False):
         raise NotImplementedError("full-neighbourhood training with distributed=True is not implemented")
-    if getattr(model, "dropout_rate", 0.):
+    if dropout is None and getattr(model, "dropout_rate", 0.):
         raise NotImplementedError("full-neighbourhood training with dropout > 0 is not implemented (the masks are "
-                                  "defined per sampled copy of a row; a whole neighbourhood has no such copies)")
+                                  "defined per sampled copy of a row; a whole neighbourhood has no such copies) - pass "
+                                  "dropout=model.dropout_rate for the full-neighbourhood masks, one per CSR entry and "
+                                  "per node")
     refuse_capture("a full-neighbourhood training step")
 
 
@@ -229,7 +280,7 @@ def minibatch_layers(aggregators, indptr, indices, ids):
     blocks = ops.csr_blocks(indptr, indices, ids, L)
     layers = []
     for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
-        graph = FullNeighborGraph(b.indptr, b.indices)
+        graph = FullNeighborGraph(b.indptr, b.indices, pos_map=(indptr, b.src_ids, indices.numel()))
         if layer == 0:
             v1 = blocks[1].src_ids if L > 1 else ids
             layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
@@ -238,11 +289,11 @@ def minibatch_layers(aggregators, indptr, indices, ids):
     return layers
 
 
-def _layers(model, indptr, indices, node_ids, training, minibatch):
+def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None):
     """The checked layers of one call: over the receptive-field blocks of node_ids (minibatch; reads the block sizes
     back once), else over the whole CSR - the model's cached FullNeighborGraph when training, an uncached one otherwise
     (inference builds no transposes, and must not evict the ones a training CSR has cached)."""
-    refuse_full_neighbor(model, training)
+    refuse_full_neighbor(model, training, dropout)
     if minibatch:
         refuse_capture("a full-neighbourhood minibatch (it reads the block sizes back)")
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
@@ -266,11 +317,21 @@ def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=Tr
     return h
 
 
-def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False):
+def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False, dropout=None):
     """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch) with an autograd graph over the
-    aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit."""
+    aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
+    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them."""
+    p = check_full_neighbor_dropout(dropout)
+    layers = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p)
+    if p:
+        pool = isinstance(layers[0].agg, MaxPoolingAggregator)
+        plan = full_neighbor_site_plan("maxpool" if pool else "mean", len(layers))
+        for i, (layer, role) in enumerate(plan):
+            layers[layer].sites = layers[layer].sites or {}
+            layers[layer].sites[role] = (model.dropout_key, model.dropout_counter + i, p)
+        model.dropout_counter += len(plan)
     h = model.features
-    for layer, fl in enumerate(_layers(model, indptr, indices, node_ids, True, minibatch)):
+    for layer, fl in enumerate(layers):
         emb = getattr(model, "embeds", None) if layer == 0 else None
         h = _LayerFn.apply(fl, h, emb, *layer_params(fl.agg))
     return _L2NormalizeFn.apply(h) if normalize else h

@@ -425,7 +425,7 @@ def segment_max(x, n, k):
 CSR_OPS = {"mean": _lib.CSR_MEAN, "mean_self": _lib.CSR_MEAN_SELF, "max": _lib.CSR_MAX, "sum": _lib.CSR_SUM}
 
 
-def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
+def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t_slot=None):
     """The reduction of each node's whole CSR row (gs_csr_aggregate; contract in oracle/full_neighbor.py): output row i is
     for node v = rows[i] - or, without rows, for every node 0 .. N-1 and then the dummy node N (N = len(indptr) - 1: the
     [N+1, .] layout of the tables it reads) - over the source rows indices[indptr[v] .. indptr[v+1]) in CSR order - op "mean", "mean_self"
@@ -434,7 +434,10 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
     sum in CSR order, +0 for an empty row - the backward of the means over csr_transpose's graph
     (oracle/full_neighbor_grad.py); its CSR has one row per source row (len(indptr) = R + 1), and without rows the output
     is those R rows, with no extra dummy row.  src: fp32 or bf16 [R, F] CUDA table.  Returns fp32 [n, F], a view of an
-    [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed)."""
+    [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed).
+    dropout: None, or (neighbour site, self site, (pos_indptr, pos_ids or None, pos_nnz)) - full-neighbourhood training
+    dropout (gs_csr_aggregate_dropout; contract in oracle/full_neighbor_dropout.py) for ops "mean", "mean_self" and "sum";
+    "sum" then also takes t_slot, the slots of csr_transpose(..., slots=True)."""
     require_cuda(src, indptr, indices, rows, out)
     if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
         raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
@@ -460,6 +463,28 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None):
         out = torch.empty((n, pad_cols(F)), dtype=torch.float32, device=src.device)
     if out.dtype != torch.float32 or out.dim() != 2 or out.stride(1) != 1 or out.shape[0] < n:
         raise ValueError("out must be a row-major float32 [>= %d, .] CUDA matrix" % n)
+    if dropout is not None:
+        neigh, self_site, (pos_indptr, pos_ids, pos_nnz) = dropout
+        if op == "max":
+            raise ValueError("dropout applies to the ops 'mean', 'mean_self' and 'sum'")
+        if op == "sum" and (t_slot is None or t_slot.dtype != torch.int32 or t_slot.numel() < indices.numel()):
+            raise ValueError("op 'sum' with dropout needs t_slot, int32 with one slot per transposed entry")
+        require_cuda(pos_indptr, pos_ids, t_slot)
+        if pos_indptr.dtype != torch.int64 or pos_indptr.dim() != 1:
+            raise TypeError("pos_indptr must be a 1-D int64 tensor")
+        if pos_ids is not None:
+            pos_ids = _i32(pos_ids.reshape(-1), "pos_ids")
+            need = n_nodes if op == "sum" else n_nodes + 1         # the sum's CSR has a row per source row already
+            if pos_ids.numel() < need:
+                raise ValueError("pos_ids needs one id per local row: %d, got %d" % (need, pos_ids.numel()))
+        ev = _probe("csr_aggregate_dropout/%d" % n)
+        check(lib().gs_csr_aggregate_dropout(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), ptr(indptr),
+                                             ptr(indices), ptr(t_slot) if op == "sum" else 0, n_nodes, ptr(rows), n,
+                                             CSR_OPS[op], dropout_site(neigh), dropout_site(self_site),
+                                             ptr(pos_indptr.contiguous()), ptr(pos_ids), int(pos_nnz), ptr(out),
+                                             out.stride(0), stream_ptr()))
+        _launched(1 if n else 0, ev)
+        return out[:n, :F]
     ev = _probe("csr_aggregate/%d" % n)
     check(lib().gs_csr_aggregate(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), ptr(indptr), ptr(indices),
                                  n_nodes, ptr(rows), n, CSR_OPS[op], ptr(out), out.stride(0), stream_ptr()))
@@ -474,12 +499,14 @@ def _csr_args(indptr, indices):
     return indptr.contiguous(), _i32(indices.reshape(-1), "indices")
 
 
-def csr_transpose(indptr, indices, with_self=False):
+def csr_transpose(indptr, indices, with_self=False, slots=False):
     """The transpose of the effective CSR of the full-neighbourhood forward (gs_csr_transpose; contract in
     oracle/full_neighbor_grad.py): over N + 1 rows (N = len(indptr) - 1), entries outside [0, N] read as N, an empty row and
     the dummy row N as {N}, with_self (GCN) appending each row's own id.  Row j of the result lists, in ascending order,
     the rows i with an entry j (once per entry).  Returns (t_indptr int64 [N + 2], t_indices int32 [capacity]): entries
-    past t_indptr[-1] are unspecified.  Built on the device - the entry count is not read back."""
+    past t_indptr[-1] are unspecified.  Built on the device - the entry count is not read back.  slots: also return
+    t_slot int32 [capacity], where each transposed entry sits in its forward row (j, -1 for the implicit {N} entry, -2 for
+    the with_self entry) - what the masked backward sum reads; t_indptr and t_indices are the same bytes."""
     indptr, indices = _csr_args(indptr, indices)
     n_nodes, nnz, ws_self = indptr.numel() - 1, indices.numel(), int(bool(with_self))
     nbytes = lib().gs_csr_transpose_workspace_bytes(n_nodes, nnz, ws_self)
@@ -488,12 +515,13 @@ def csr_transpose(indptr, indices, with_self=False):
     cap = nnz + (n_nodes + 1) * (1 + ws_self)
     t_indptr = torch.empty((n_nodes + 2,), dtype=torch.int64, device=indptr.device)
     t_indices = torch.empty((cap,), dtype=torch.int32, device=indptr.device)
+    t_slot = torch.empty((cap,), dtype=torch.int32, device=indptr.device) if slots else None
     ws = torch.empty((nbytes,), dtype=torch.uint8, device=indptr.device)
     ev = _probe("csr_transpose/%d" % cap)
     check(lib().gs_csr_transpose(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ws_self, ptr(t_indptr),
-                                 ptr(t_indices), ptr(ws), nbytes, stream_ptr()))
-    _launched(4, ev)                     # counts, fill, indptr (+ CUB's scan and sort passes)
-    return t_indptr, t_indices
+                                 ptr(t_indices), ptr(t_slot), ptr(ws), nbytes, stream_ptr()))
+    _launched(5 if slots else 4, ev)     # counts, fill, indptr (+ CUB's scan and sort passes), slots
+    return (t_indptr, t_indices, t_slot) if slots else (t_indptr, t_indices)
 
 
 def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out=None):
@@ -901,12 +929,12 @@ def gather_mean_dropout(src, segments, neigh_sites, self_sites, include_self=Fal
     return out_self, out_mean
 
 
-def dropout_apply(x, site, rows=None, group=1, scale=1.0, out=None, accumulate=False):
-    """Masked scale (gs_dropout_apply): out[r, c] (+)= keep(site, r, c) ? (x[r // group, c] * scale) / keep : 0 for
-    r < rows (default x.shape[0] * group).  x, out: float32 CUDA matrices with unit column stride (strided rows are fine).
-    Forward dropout (x -> drop(x)) and every dropout backward (the same mask applied to the incoming gradient).
-    Returns out (a new [rows, F] tensor unless given)."""
-    require_cuda(x, out)
+def dropout_apply(x, site, rows=None, group=1, scale=1.0, out=None, accumulate=False, pos_ids=None):
+    """Masked scale (gs_dropout_apply): out[r, c] (+)= keep(site, pos, c) ? (x[r // group, c] * scale) / keep : 0 for
+    r < rows (default x.shape[0] * group), pos = pos_ids[r] (an int32 CUDA tensor of >= rows ids) or r.  x, out: float32
+    CUDA matrices with unit column stride (strided rows are fine).  Forward dropout (x -> drop(x)) and every dropout
+    backward (the same mask applied to the incoming gradient).  Returns out (a new [rows, F] tensor unless given)."""
+    require_cuda(x, out, pos_ids)
     group = int(group)
     if group < 1:
         raise ValueError("group must be >= 1")
@@ -927,9 +955,13 @@ def dropout_apply(x, site, rows=None, group=1, scale=1.0, out=None, accumulate=F
     ldx, ldo = max(x.stride(0), F), max(out.stride(0), F)
     if out.data_ptr() == x.data_ptr() and (group != 1 or ldx != ldo):
         raise ValueError("in-place dropout_apply needs group == 1 and equal row strides")
+    if pos_ids is not None:
+        pos_ids = _i32(pos_ids.reshape(-1), "pos_ids")
+        if pos_ids.numel() < rows:
+            raise ValueError("pos_ids has %d ids, %d rows" % (pos_ids.numel(), rows))
     ev = _probe("dropout_apply/%d" % rows)
     check(lib().gs_dropout_apply(ptr(x), ldx, rows, F, group, float(scale), c_site, int(bool(accumulate)), ptr(out), ldo,
-                                 stream_ptr()))
+                                 ptr(pos_ids), stream_ptr()))
     _launched(1 if rows * F else 0, ev)
     return out
 

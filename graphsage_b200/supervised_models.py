@@ -44,6 +44,25 @@ def dropout_site_plan(kind, n_layers, head=False):
     return plan + ([(None, None, "head")] if head else [])
 
 
+def full_neighbor_site_plan(kind, n_layers, head=False):
+    """The dropout sites of one full-neighbourhood training pass (contract: oracle/full_neighbor_dropout.py): [(layer,
+    role)], per layer "neigh" then "self" for mean / gcn - one mask per CSR entry, one per node - or the one per-node
+    "mlp" input of the pools (the full path runs the MLP once per node), then (None, "head") for the supervised head.  Site
+    i draws with call = first call + i."""
+    roles = ("mlp",) if kind in ("maxpool", "meanpool") else ("neigh", "self")
+    return [(layer, role) for layer in range(n_layers) for role in roles] + ([(None, "head")] if head else [])
+
+
+def check_full_neighbor_dropout(dropout):
+    """The `dropout` argument of the full_neighbor_* training methods: None (no masks; a model whose dropout_rate > 0 is
+    refused), or a rate p in [0, 1) applied as asked - p = 0 draws nothing.  Anything else is a ValueError."""
+    if dropout is None:
+        return None
+    if isinstance(dropout, bool) or not isinstance(dropout, (int, float)) or not 0.0 <= float(dropout) < 1.0:
+        raise ValueError("dropout must be None or a rate in [0, 1) (got %r)" % (dropout,))
+    return float(dropout)
+
+
 class _DropoutFn(torch.autograd.Function):
     """y = drop(x) for one site (the supervised head's input, layers.py:107); the backward applies the same mask."""
 
@@ -612,40 +631,59 @@ class SupervisedGraphsage(SampleAndAggregate):
         with torch.no_grad():
             return self._predictions(self.logits(batch))
 
-    def full_neighbor_outputs(self, indptr, indices, node_ids):
+    def full_neighbor_outputs(self, indptr, indices, node_ids, dropout=None):
         """outputs() over whole neighbourhoods: full_neighbor_embeddings(indptr, indices, node_ids) - the same bits -
         with an autograd graph over the aggregator weights and (identity_dim > 0) the node embeddings, for any head to
         compose (contract: oracle/full_neighbor_grad.py).  The CSR's transposes are built on first use and cached on the
-        model, keyed by the CSR tensors' data_ptr, numel and _version.  Refused (NotImplementedError): the seq aggregator,
-        ShardedFeatures, distributed=True, training dropout > 0, CUDA-graph capture."""
+        model, keyed by the CSR tensors' data_ptr, numel and _version.  dropout: None (no masks), or a training rate
+        p in [0, 1) - callers pass dropout=model.dropout_rate.  The full-neighbourhood masks follow their own contract
+        (one per CSR entry and per node, keyed by global ids: oracle/full_neighbor_dropout.py), not the sampled one, so
+        they are applied only when asked for; p = 0 gives the bits of dropout=None.  Refused (NotImplementedError): the
+        seq aggregator, ShardedFeatures, distributed=True, CUDA-graph capture, and dropout=None on a model whose
+        dropout_rate > 0."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, dropout=dropout)
 
-    def full_neighbor_loss(self, indptr, indices, node_ids, labels):
-        """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids."""
-        return self._logits_loss(self._node_pred(self.full_neighbor_outputs(indptr, indices, node_ids)), labels)
+    def _full_neighbor_logits(self, out, dropout):
+        """The head on full-neighbourhood outputs; with p > 0 its input is dropped at the site after the layers'."""
+        p = check_full_neighbor_dropout(dropout)
+        if p:
+            out = _DropoutFn.apply(out, (self.dropout_key, self.dropout_counter, p, None))
+            self.dropout_counter += 1
+        return self._node_pred(out)
 
-    def full_neighbor_train_step(self, indptr, indices, node_ids, labels):
-        """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling, no
-        dropout), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host synchronisation."""
-        return clipped_step(self, self.full_neighbor_loss(indptr, indices, node_ids, labels))
+    def full_neighbor_loss(self, indptr, indices, node_ids, labels, dropout=None):
+        """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids.
+        dropout: as full_neighbor_outputs; p > 0 also drops the head input (row r of node_ids at position r)."""
+        check_full_neighbor_dropout(dropout)
+        out = self.full_neighbor_outputs(indptr, indices, node_ids, dropout=dropout)
+        return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids):
+    def full_neighbor_train_step(self, indptr, indices, node_ids, labels, dropout=None):
+        """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling;
+        dropout as full_neighbor_loss), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host
+        synchronisation."""
+        return clipped_step(self, self.full_neighbor_loss(indptr, indices, node_ids, labels, dropout=dropout))
+
+    def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids, dropout=None):
         """full_neighbor_outputs over the receptive field of node_ids only: the same values, bit for bit, with per-layer
         blocks built on the device by ops.csr_blocks (contract: oracle/full_neighbor_blocks.py) and their transposes built
         per call, not cached.  Cost and memory follow the blocks, not the graph: the minibatch form of exact-neighbourhood
-        training.  Reads the block sizes back once per call.  Same refusals as full_neighbor_outputs."""
+        training.  Reads the block sizes back once per call.  dropout and refusals as full_neighbor_outputs: the masks are
+        keyed by global ids, so the rows equal the whole-graph pass's from the same counter."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, dropout=dropout)
 
-    def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels):
+    def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None):
         """full_neighbor_loss over full_neighbor_minibatch_outputs: the same head, cross-entropy and weight decay."""
-        return self._logits_loss(self._node_pred(self.full_neighbor_minibatch_outputs(indptr, indices, node_ids)), labels)
+        check_full_neighbor_dropout(dropout)
+        out = self.full_neighbor_minibatch_outputs(indptr, indices, node_ids, dropout=dropout)
+        return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels):
+    def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None):
         """full_neighbor_train_step for a minibatch: one Adam step on full_neighbor_minibatch_loss, gradients clipped to
         +-5.  Returns the detached loss."""
-        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels))
+        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
 
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on

@@ -485,12 +485,15 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
                                float* out_mean, int64_t out_pitch, void* stream);
 
 /* Masked scale, elementwise over a [rows, F] block:
- *   v = keep(site, pos = r, c) ? (x[(r / group) * ldx + c] * scale) / keep : 0
+ *   v = keep(site, pos, c) ? (x[(r / group) * ldx + c] * scale) / keep : 0,  pos = pos_ids ? pos_ids[r] : r
  *   out[r * ldo + c] = accumulate ? out[r * ldo + c] + v : v
  * group >= 1 repeats each x row for `group` consecutive output rows (the fanout mean's backward).  out may alias x when
- * group == 1 and ldo == ldx.  Each element is read and written by one thread: bit-identical on every call. */
+ * group == 1 and ldo == ldx.  pos_ids (device int32 [rows], may be NULL) names each row's position by id: the
+ * full-neighbourhood self rows and MLP inputs of a minibatch block, masked by their global node ids.  Each element is read
+ * and written by one thread: bit-identical on every call. */
 int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, int32_t group, float scale,
-                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, void* stream);
+                         gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, const int32_t* pos_ids,
+                         void* stream);
 
 /* gs_embedding_grad with a dropout site per list (sites_host[l]; NULL: no masks): contribution i of list l adds
  *   keep(site_l, pos = i, c) ? (l.scale * l.grad[(i / l.group) * l.ldg + c]) / keep : 0
@@ -653,6 +656,28 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
                          const int32_t* rows /* may be NULL */, int64_t n, int32_t op,
                          float* out, int64_t out_pitch, void* stream);
 
+/* gs_csr_aggregate with full-neighbourhood training dropout (contract: oracle/full_neighbor_dropout.py), op GS_CSR_MEAN,
+ * GS_CSR_MEAN_SELF or GS_CSR_SUM.  Every element a chain reads is masked first - drop(x) = keep ? x / keep : 0 with the
+ * sites' Philox rule (gs_dropout_site), bf16 sources after widening - and the chain, its order and its divisor are
+ * gs_csr_aggregate's.  Positions come from the map (pos_indptr int64, pos_ids int32 or NULL, pos_nnz): local row r is
+ * global node g(r) = pos_ids ? pos_ids[r] : r (r clamped to the dummy row n_nodes first; pos_ids then has n_nodes + 1
+ * entries, n_nodes for GS_CSR_SUM, whose rows are the source rows), and
+ *   GS_CSR_MEAN / _MEAN_SELF  entry j of node v = rows ? rows[i] : i: neigh_site at pos_indptr[g(v)] + j; the implicit
+ *                             dummy entry of an empty row (or of a v outside [0, n_nodes)): neigh_site at pos_nnz + g(v);
+ *                             the GCN self row: self_site at g(v);
+ *   GS_CSR_SUM (fp32)         over gs_csr_transpose's graph with its t_slot: the entry from forward row i at slot s is
+ *                             masked as that forward entry was - neigh_site at pos_indptr[g(i)] + s (s >= 0) or
+ *                             pos_nnz + g(i) (s = -1), self_site at g(i) (s = -2).
+ * The whole graph passes (indptr, NULL, len(indices)); a minibatch block (gs_csr_blocks_fill) passes (the global indptr,
+ * the block's src_ids, the global nnz), so a block masks every element as the whole-graph pass does.  Both rates 0: the
+ * plain gs_csr_aggregate kernel runs.  No allocation, no atomics, no host synchronisation: two calls give the same bits. */
+int32_t gs_csr_aggregate_dropout(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                 const int64_t* indptr, const int32_t* indices, const int32_t* t_slot /* GS_CSR_SUM */,
+                                 int64_t n_nodes, const int32_t* rows /* may be NULL */, int64_t n, int32_t op,
+                                 gs_dropout_site neigh_site, gs_dropout_site self_site, const int64_t* pos_indptr,
+                                 const int32_t* pos_ids /* may be NULL */, int64_t pos_nnz, float* out, int64_t out_pitch,
+                                 void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Backward of the full-neighbourhood reductions (SupervisedGraphsage.full_neighbor_train_step).  Contract:
  * oracle/full_neighbor_grad.py.  Nodes 0 .. N-1 have CSR rows; the dummy node N closes every [N+1, .] table.
@@ -671,6 +696,10 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
  *   (N + 1) * (1 + with_self), nnz the length of `indices`, which every row's entries must lie in.  Integer work only, no
  *   host synchronisation: the count stays on the device.  workspace: gs_csr_transpose_workspace_bytes(...) bytes;
  *   -1 (see gs_last_error_string) outside the limits n_nodes < 2^31 - 2, capacity < 2^31.
+ *   t_slot (int32 [capacity], may be NULL): for each transposed entry, where it sits in its forward row i = t_indices[.]:
+ *   j for the row's CSR entry j, -1 for the implicit {N} entry (empty row, dummy row), -2 for the with_self entry - the
+ *   positions gs_csr_aggregate_dropout's GS_CSR_SUM masks by.  It comes from the same sort (the slot is sorted as the
+ *   value and both outputs are derived from it), so t_indptr and t_indices are the bytes of a call without it.
  * gs_csr_max_backward - the gradient of m = GS_CSR_MAX(z) (TensorFlow's reduce_max gradient: split evenly among ties),
  *   then the ReLU of the Dense layer that made z (z = relu(.) >= 0):
  *   (a) for every effective forward row i <= N and column c: cnt = #{entries e of row i : z[e][c] == m[i][c]}
@@ -684,7 +713,8 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
  * --------------------------------------------------------------------------------------------- */
 int64_t gs_csr_transpose_workspace_bytes(int64_t n_nodes, int64_t nnz, int32_t with_self);
 int32_t gs_csr_transpose(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t with_self,
-                         int64_t* t_indptr, int32_t* t_indices, void* workspace, int64_t workspace_bytes, void* stream);
+                         int64_t* t_indptr, int32_t* t_indices, int32_t* t_slot /* may be NULL */, void* workspace,
+                         int64_t workspace_bytes, void* stream);
 int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm, int64_t lddm,
                             int32_t F, const int64_t* indptr, const int32_t* indices, const int64_t* t_indptr,
                             const int32_t* t_indices, int64_t n_nodes, float* s, int64_t lds, float* dz, int64_t lddz,
