@@ -1,14 +1,15 @@
 """GPU: training the max-pool / mean-pool branch through the fused bf16 kernels (fused_pool=True).
 
 B1 (gs_pool_mlp_backward_dp) is checked bit for bit against oracle/pool_grad.py on grid-valued inputs (multiples of 2^-4:
-exact in bf16, and every fp32 sum of their products is exact), B2 / B3 against fp64 products of the kernel's own dP,
-and the whole step against torch-CPU autograd on bf16-rounded operands with dP rounded to bf16 where the kernel rounds
-it.  Also: determinism, CUDA-graph capture, training quality, peak memory and the refusals."""
+exact in bf16, and every fp32 sum of their products is exact), B2 / B3 against fp64 products of the kernel's own dP
+within oracle/numerics.py's GEMM bounds, and the whole step against torch-CPU autograd on bf16-rounded operands with dP
+rounded to bf16 where the kernel rounds it.  Also: determinism, CUDA-graph capture, training quality, peak memory and the refusals."""
 import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden
+from oracle import numerics as nu
 from oracle import pool_grad
 
 pytestmark = pytest.mark.gpu
@@ -74,14 +75,25 @@ def test_b2_b3_match_fp64_products_of_the_kernels_dp(pool, k, K, hidden, n, by_i
     dWm = torch.ones((K, hidden), dtype=torch.float32, device="cuda")          # B2 adds into the caller's buffers
     dbm = torch.full((hidden,), 0.5, dtype=torch.float32, device="cuda")
     gs.ops.pool_mlp_backward_dw(c["table"], n, k, c["grad"], dWm, dbm, row_ids=c["row_ids"], row0=c["row0"], K=K)
-    ref_w = c["X"].astype(np.float64).T @ dP.astype(np.float64)
-    assert _norm_rel(dWm.cpu().numpy() - 1.0, ref_w) <= 1e-5
+    dW0 = torch.zeros((K, hidden), dtype=torch.float32, device="cuda")
+    gs.ops.pool_mlp_backward_dw(c["table"], n, k, c["grad"], dW0, torch.zeros_like(dbm), row_ids=c["row_ids"],
+                                row0=c["row0"], K=K)
+    # the sum over the rows is added to dWm once: fl32(1 + the sum), and the sum is held to numerics.check_gemm
+    assert np.array_equal(dWm.cpu().numpy(), dW0.cpu().numpy() + np.float32(1))
+    _check_dw(dW0, c["X"], dP)
     assert np.array_equal(dbm.cpu().numpy(), (pool_grad.dbm_combine(parts) + np.float32(0.5)).astype(np.float32))
-    Wb = pool_grad.bf16_round(c["W"]).astype(np.float64)
     for d in sorted({K, max(1, K // 3)}):
         dx = gs.ops.pool_mlp_backward_dx(c["grad"], n, k, c["Wt"], gs.ops.PackedMlpDxWeights(d))
         assert tuple(dx.shape) == (n * k, d)
-        assert _norm_rel(dx.cpu().numpy(), (dP.astype(np.float64) @ Wb.T)[:, :d]) <= 1e-5
+        ok, worst, rms = nu.check_gemm(dx.cpu().numpy(), *nu.gemm_reference([(dP, c["W"].T[:, :d])], "bf16"))
+        assert ok, ("B3", d, worst, rms)
+
+
+def _check_dw(dWm, X, dP):
+    """B2's dWm = X^T dP against the fp64 product of its bf16 operands, criteria (a) and (b) of oracle/numerics.py with
+    n * k products per element."""
+    ok, worst, rms = nu.check_gemm(dWm.cpu().numpy(), *nu.gemm_reference([(X.T, dP)], "bf16"))
+    assert ok, ("B2", worst, rms)
 
 
 @pytest.mark.parametrize("pool,k,K,hidden,n,by_ids", [("max", 1, 50, 128, 5888, True), ("mean", 25, 50, 128, 5000, False),
@@ -100,7 +112,7 @@ def test_b2_many_tiles_uneven_last_chunk_and_dbm_groups(pool, k, K, hidden, n, b
     dWm = torch.zeros((K, hidden), dtype=torch.float32, device="cuda")
     dbm = torch.zeros((hidden,), dtype=torch.float32, device="cuda")
     gs.ops.pool_mlp_backward_dw(c["table"], n, k, c["grad"], dWm, dbm, row_ids=c["row_ids"], row0=c["row0"], K=K)
-    assert _norm_rel(dWm.cpu().numpy(), c["X"].astype(np.float64).T @ dP.astype(np.float64)) <= 1e-5
+    _check_dw(dWm, c["X"], dP)
     assert np.array_equal(dbm.cpu().numpy(), pool_grad.dbm_combine(parts))
     # the rows of the last chunk alone: zero dP everywhere else, so a wrong last-chunk bound loses (or doubles) them
     last = np.zeros_like(dP)
@@ -113,7 +125,7 @@ def test_b2_many_tiles_uneven_last_chunk_and_dbm_groups(pool, k, K, hidden, n, b
     dbm.zero_()
     gs.ops.pool_mlp_backward_dw(c["table"], n, k, buf, dWm, dbm, row_ids=c["row_ids"], row0=c["row0"], K=K)
     assert np.abs(last).sum() > 0
-    assert _norm_rel(dWm.cpu().numpy(), c["X"].astype(np.float64).T @ last.astype(np.float64)) <= 1e-5
+    _check_dw(dWm, c["X"], last)
 
 
 def _one_hot_dp(rows, hidden):
