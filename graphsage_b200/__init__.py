@@ -7,7 +7,7 @@ All compute goes through libgraphsage_b200.so (include/graphsage_b200.h); there 
 from . import (_lib, aggregators, graph, graphed_training, inits, layers, minibatch, models, neigh_samplers, node2vec,  # noqa: F401
                ops, prediction, utils)
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator,  # noqa: F401
-                          SeqAggregator, set_default_math)
+                          SeqAggregator, TwoMaxLayerPoolingAggregator, set_default_math)
 from .graphed_training import GraphedTrainStep, make_adam_capturable  # noqa: F401
 from .layers import Dense, Layer, identity, relu  # noqa: F401
 from .models import Node2VecModel, SAGEInfo, SampleAndAggregate  # noqa: F401

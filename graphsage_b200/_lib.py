@@ -114,6 +114,8 @@ _SIGNATURES = {
                                      c_vp]),
     "gs_meanpool_mlp_fused": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,
                                       c_vp]),
+    "gs_maxpool2_mlp_fused": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp,
+                                      c_i32, c_vp, c_i64, c_vp]),
     "gs_pool_mlp_dp_bytes": (c_i64, [c_i64, c_i32, c_i32]),
     "gs_pool_mlp_backward_dp": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,
                                         c_i32, c_vp, c_vp]),

@@ -1,4 +1,5 @@
-"""MeanAggregator / GCNAggregator / MaxPoolingAggregator / MeanPoolingAggregator / SeqAggregator - the surface of
+"""MeanAggregator / GCNAggregator / MaxPoolingAggregator / MeanPoolingAggregator / TwoMaxLayerPoolingAggregator /
+SeqAggregator - the surface of
 reference graphsage/aggregators.py over the library's CUDA kernels.
 
 Two entry points per aggregator:
@@ -52,6 +53,14 @@ FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, FUSED_POOL_HIDDEN_STEP = 128, 640, 128
 
 def fused_pool_fits(k, K, hidden):
     return k <= FUSED_POOL_MAX_FANOUT and K <= FUSED_POOL_MAX_K and hidden % FUSED_POOL_HIDDEN_STEP == 0
+
+
+# K5's limits: as K4's, and the second layer's width a multiple of 256 (one CTA's slice of it)
+FUSED_POOL2_H2_STEP = 256
+
+
+def fused_pool2_fits(k, K, h1, h2):
+    return fused_pool_fits(k, K, h1) and h2 % FUSED_POOL2_H2_STEP == 0
 
 
 class _SageAggregator(Layer):
@@ -276,19 +285,25 @@ class MaxPoolingAggregator(_SageAggregator):
                               row0=s.neigh_row0, K=self.neigh_input_dim, out=out, pool=self.pool)
 
     def _pooled_parts(self, src, segments, kept=None, sites=None):
-        """The GEMM parts of the materialised form: per hop the neighbour rows (widened to fp32 from a bf16 table), with
-        training dropout the mask of sites[hop] applied to them, then the MLP and the pooling kernel.  `kept` (training)
-        receives each hop's MLP input and output."""
+        """The GEMM parts of the materialised form: per hop the neighbour rows (widened to fp32 from a bf16 table), then
+        the MLP and the pooling kernel.  With training dropout each Dense layer's input is masked first: sites[hop] is
+        the one site of a one-layer MLP, the (mlp, mlp2) pair of a two-layer one.  `kept` (training) receives each hop's
+        Dense inputs (as masked) and the last Dense's output."""
         widen = torch.is_tensor(src) and src.dtype != torch.float32
 
         def hop(i, s, out):
-            xn = _rows(src, s.neigh_ids, s.neigh_row0, s.n * s.k, widen)
-            if sites is not None:                   # out of place: layer >= 1 rows belong to the previous layer
-                xn = ops.dropout_apply(xn, sites[i])
-            h = self._mlp(xn)
+            h = _rows(src, s.neigh_ids, s.neigh_row0, s.n * s.k, widen)
+            hop_sites = None if sites is None else (sites[i],) if len(self.mlp_layers) == 1 else sites[i]
+            for j, layer in enumerate(self.mlp_layers):
+                if hop_sites is not None:           # out of place: layer >= 1 rows belong to the previous layer
+                    h = ops.dropout_apply(h, hop_sites[j])
+                if kept is not None:
+                    kept.append(h)
+                layer.math = self.math
+                h = layer(h)
             out.copy_(self._pool(h, s.n, s.k))
             if kept is not None:
-                kept.extend([xn, h])
+                kept.append(h)
         return self._summarise(src, segments, hop, widen)
 
     def aggregate_rows(self, src, segments, final=None, src_persistent=False):
@@ -317,6 +332,56 @@ class MeanPoolingAggregator(MaxPoolingAggregator):
     """act(concat_or_add(self @ Ws, mean_k(relu(neigh @ Wm + bm)) @ Wn)) - reference graphsage/aggregators.py:197-273.
     Same kernels as the max-pool aggregator with the pooling operator swapped (SURVEY section 8f row 4)."""
     pool = "mean"
+
+
+class TwoMaxLayerPoolingAggregator(MaxPoolingAggregator):
+    """act(concat_or_add(self @ Ws, max_k(relu(relu(neigh @ W1 + b1) @ W2 + b2)) @ Wn)) - aggregators.py:276-361: two
+    Dense layers (hidden 512 / 256 "small", 1024 / 512 "big") before the max.  With bf16 math the neighbour branch is K5
+    (ops.maxpool2_mlp_fused), else the materialised chain of the max-pool aggregator."""
+
+    def __init__(self, input_dim, output_dim, model_size="small", neigh_input_dim=None, dropout=0., bias=False,
+                 act=relu, name=None, concat=False, device="cuda", **kwargs):
+        _SageAggregator.__init__(self, **kwargs)
+        self.dropout = dropout
+        self.bias = bias
+        self.act = act
+        self.concat = concat
+        if neigh_input_dim is None:
+            neigh_input_dim = input_dim
+        if model_size == "small":
+            self.hidden_dim_1, self.hidden_dim_2 = 512, 256
+        elif model_size == "big":
+            self.hidden_dim_1, self.hidden_dim_2 = 1024, 512
+        else:
+            raise ValueError("model_size must be 'small' or 'big'")
+        self.hidden_dim = self.hidden_dim_2          # the pooled width (_summarise, the full-neighbourhood layer)
+        self.math = _DEFAULT_MATH[0]
+        self.mlp_layers = [Dense(input_dim=d_in, output_dim=d_out, act=relu, dropout=dropout, sparse_inputs=False,
+                                 logging=self.logging, device=device, math=self.math)
+                           for d_in, d_out in ((neigh_input_dim, self.hidden_dim_1),
+                                               (self.hidden_dim_1, self.hidden_dim_2))]
+        self.vars["neigh_weights"] = glorot([self.hidden_dim_2, output_dim], name="neigh_weights", device=device)
+        self.vars["self_weights"] = glorot([input_dim, output_dim], name="self_weights", device=device)
+        if self.bias:   # aggregators.py:325 reads self.output_dim before it is set; fixed as in MeanAggregator
+            self.vars["bias"] = zeros([output_dim * (2 if concat else 1)], name="bias", device=device)
+        self.input_dim = input_dim
+        self.output_dim = output_dim
+        self.neigh_input_dim = neigh_input_dim
+
+    def _fused_ok(self, src, segments):
+        return (self.math == ops.MATH_BF16 and torch.is_tensor(src) and not self.dropout and len(self.mlp_layers) == 2
+                and all(fused_pool2_fits(s.k, self.neigh_input_dim, self.hidden_dim_1, self.hidden_dim_2)
+                        for s in segments)
+                and all(l.act is relu and "bias" in l.vars for l in self.mlp_layers))
+
+    def _fused_hop(self, table, s, out):
+        """K5 for one hop: gather -> Dense -> Dense -> max over the fanout in one wgmma kernel (bf16 operands)."""
+        if getattr(self, "_packed_mlp", None) is None:
+            self._packed_mlp = (ops.PackedMlpWeights(), ops.PackedMlpWeights())
+        l1, l2 = (l.vars for l in self.mlp_layers)
+        ops.maxpool2_mlp_fused(table, s.n, s.k, l1["weights"], l1["bias"], self._packed_mlp[0], l2["weights"], l2["bias"],
+                               self._packed_mlp[1], row_ids=s.neigh_ids, row0=s.neigh_row0, K=self.neigh_input_dim,
+                               out=out)
 
 
 def refuse_seq_table(features):

@@ -31,7 +31,7 @@ t_slot (ops.csr_transpose(slots=True)) to find each entry's forward position.
 import torch
 
 from . import ops
-from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, _rows
+from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, TwoMaxLayerPoolingAggregator, _rows
 from .layers import act_code
 from .supervised_models import (_LayerFn, build_aggregators, check_full_neighbor_dropout, full_neighbor_site_plan,
                                 layer_params)
@@ -240,6 +240,9 @@ def refuse_full_neighbor(model, training, dropout=None):
                                   "implemented" % what)
     if not training:
         return
+    if model.aggregator_cls is TwoMaxLayerPoolingAggregator:
+        raise NotImplementedError("full-neighbourhood training is not implemented for the twomaxpool aggregator (the "
+                                  "backward through its second Dense layer has no full-neighbourhood form)")
     if getattr(model, "distributed", False):
         raise NotImplementedError("full-neighbourhood training with distributed=True is not implemented")
     if dropout is None and getattr(model, "dropout_rate", 0.):

@@ -11,7 +11,7 @@ import torch
 
 from . import ops
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
-                          refuse_seq_table)
+                          TwoMaxLayerPoolingAggregator, refuse_seq_table)
 from .layers import identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
@@ -22,8 +22,9 @@ SAGEInfo = namedtuple("SAGEInfo",
                        "output_dim"])     # the output (i.e., hidden) dimension
 
 _AGGREGATORS = {"mean": MeanAggregator, "maxpool": MaxPoolingAggregator, "gcn": GCNAggregator,
-                "meanpool": MeanPoolingAggregator, "seq": SeqAggregator}
-_SIZED_AGGREGATORS = (MaxPoolingAggregator, SeqAggregator)       # take model_size (models.py:213-226)
+                "meanpool": MeanPoolingAggregator, "seq": SeqAggregator,
+                "twomaxpool": TwoMaxLayerPoolingAggregator}    # an extension: the reference's models.py:211-222 has no branch
+_SIZED_AGGREGATORS = (MaxPoolingAggregator, SeqAggregator)       # take model_size (models.py:213-226; with its subclasses)
 
 
 def layer_segments(samples, counts, num_samples, layer):

@@ -770,13 +770,24 @@ class PackedMlpWeights(object):
         return ws
 
 
+def _check_mlp_K(W, K):
+    """The K columns the fused pooling kernels read: the packed images hold ceil(W.shape[0] / 64) K-blocks of W and the
+    kernels walk ceil(K / 64), so K must be at most W's row count and within its last K-block."""
+    if K is None:
+        return W.shape[0]
+    if not 1 <= K <= W.shape[0] or (K + 63) // 64 != (W.shape[0] + 63) // 64:
+        raise ValueError("K = %d does not match the MLP weight's %d rows (K <= rows, the same number of 64-column "
+                         "blocks)" % (K, W.shape[0]))
+    return K
+
+
 def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0, K=None, out=None, pool="max"):
     """out[g, :] = max_j relu(table[row(g, j), :K] @ W + bias) in one wgmma kernel (bf16 operands, fp32 accumulate).
     table: bfloat16 [rows, >=K] row-major with pitch % 8 == 0; W: float32 [K, hidden] (hidden % 128 == 0)."""
     require_cuda(table, W, bias, row_ids)
     if table.dtype != torch.bfloat16 or table.stride(1) != 1:
         raise TypeError("table must be row-major bfloat16")
-    K = W.shape[0] if K is None else K
+    K = _check_mlp_K(W, K)
     hidden = W.shape[1]
     if out is None:
         out = torch.empty((n_groups, hidden), dtype=torch.float32, device=table.device)
@@ -787,6 +798,30 @@ def maxpool_mlp_fused(table, n_groups, k, W, bias, packed, row_ids=None, row0=0,
     fn = lib().gs_meanpool_mlp_fused if pool == "mean" else lib().gs_maxpool_mlp_fused
     check(fn(ptr(table), table.shape[0], K, table.stride(0), ptr(row_ids), row0, n_groups, k,
              ptr(ws), ptr(bias), hidden, ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n_groups else 0, ev)
+    return out
+
+
+def maxpool2_mlp_fused(table, n_groups, k, W1, b1, packed1, W2, b2, packed2, row_ids=None, row0=0, K=None, out=None):
+    """out[g, :] = max_j relu(bf16(relu(table[row(g, j), :K] @ W1 + b1)) @ W2 + b2) in one wgmma kernel (K5; bf16
+    operands, fp32 accumulate; contract: oracle/pool2_forward.py).  table: bfloat16 [rows, >=K] row-major with
+    pitch % 8 == 0; W1: float32 [K, h1] (h1 % 128 == 0); W2: float32 [h1, h2] (h2 % 256 == 0); packed1 / packed2:
+    PackedMlpWeights, one per weight."""
+    require_cuda(table, W1, b1, W2, b2, row_ids)
+    if table.dtype != torch.bfloat16 or table.stride(1) != 1:
+        raise TypeError("table must be row-major bfloat16")
+    K = _check_mlp_K(W1, K)
+    h1, h2 = W1.shape[1], W2.shape[1]
+    if W2.shape[0] != h1:
+        raise ValueError("W2 must have h1 = %d rows (got %d)" % (h1, W2.shape[0]))
+    if out is None:
+        out = torch.empty((n_groups, h2), dtype=torch.float32, device=table.device)
+    ws1, ws2 = packed1.get(W1), packed2.get(W2)
+    if row_ids is not None:
+        row_ids = _i32(row_ids.reshape(-1), "row_ids")
+    ev = _probe("maxpool2_mlp/%d" % n_groups)
+    check(lib().gs_maxpool2_mlp_fused(ptr(table), table.shape[0], K, table.stride(0), ptr(row_ids), row0, n_groups, k,
+                                      ptr(ws1), ptr(b1), h1, ptr(ws2), ptr(b2), h2, ptr(out), out.stride(0), stream_ptr()))
     _launched(1 if n_groups else 0, ev)
     return out
 
@@ -829,7 +864,7 @@ def pool_mlp_backward_dp(table, n_groups, k, W, bias, packed, dhp, row_ids=None,
     require_cuda(table, W, bias, row_ids, dhp)
     if table.dtype != torch.bfloat16 or table.stride(1) != 1:
         raise TypeError("table must be row-major bfloat16")
-    K = W.shape[0] if K is None else K
+    K = _check_mlp_K(W, K)
     hidden = W.shape[1]
     if dhp.dtype != torch.float32 or dhp.dim() != 2 or dhp.stride(1) != 1 or tuple(dhp.shape) != (n_groups, hidden):
         raise ValueError("dhp must be a float32 [%d, %d] matrix with unit column stride" % (n_groups, hidden))

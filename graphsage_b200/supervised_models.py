@@ -20,7 +20,8 @@ import torch
 from . import ops
 from .graphed_training import GraphedTrainStep
 from .layers import act_code, identity, relu  # noqa: F401
-from .aggregators import FUSED_POOL_HIDDEN_STEP, FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, fused_pool_fits
+from .aggregators import (FUSED_POOL_HIDDEN_STEP, FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, TwoMaxLayerPoolingAggregator,
+                          fused_pool_fits)
 from .models import _SIZED_AGGREGATORS, SampleAndAggregate, layer_segments
 
 
@@ -38,9 +39,10 @@ def dropout_site_plan(kind, n_layers, head=False):
     plan = []
     if kind == "seq":                   # SeqAggregator._call applies no dropout (aggregators.py:405-449): the head only
         n_layers = 0
+    roles = {"maxpool": ("mlp",), "meanpool": ("mlp",), "twomaxpool": ("mlp", "mlp2")}.get(kind, ("neigh", "self"))
     for layer in range(n_layers):
         for hop in range(n_layers - layer):
-            plan += [(layer, hop, "mlp")] if kind in ("maxpool", "meanpool") else [(layer, hop, "neigh"), (layer, hop, "self")]
+            plan += [(layer, hop, role) for role in roles]
     return plan + ([(None, None, "head")] if head else [])
 
 
@@ -226,39 +228,59 @@ class _SummaryBranch(object):
 
 
 class _PoolAggregateRowsFn(_SummaryBranch):
-    """MaxPoolingAggregator / MeanPoolingAggregator, materialised on the fp32 kernels: gather -> Dense(relu, bias) ->
-    pool over the fanout, keeping the gathered neighbour rows and the MLP activations for pool_branch_backward.
-    sites: None, or one (seed, call, rate) per segment for the MLP input (training dropout, layers.py:107; the self rows
-    are not dropped); the kept rows are the dropped input, which is what dWm = xn^T dpre needs."""
+    """MaxPoolingAggregator / MeanPoolingAggregator / TwoMaxLayerPoolingAggregator, materialised on the fp32 kernels:
+    gather -> the chain of Dense(relu, bias) layers -> pool over the fanout, keeping per hop each Dense layer's input and
+    the last one's output.  The last Dense goes back through pool_branch_backward, the ones before it through
+    dpre = dh * [h > 0], dW = x^T dpre, db = sum dpre, dx = dpre W^T.  sites: None, or per segment the dropout site of
+    each Dense layer's input - one (seed, call, rate) with one Dense, a (mlp, mlp2) pair with two (training dropout,
+    layers.py:107; the self rows are not dropped); the kept inputs are the dropped ones, which is what dW = x^T dpre
+    needs, and a dropped zero has no gradient, so [x > 0] of the kept input is the ReLU mask."""
 
     @staticmethod
-    def apply(agg, src, segments, Ws, Wn, Wm, bm, emb=None, sites=None):
-        return _LayerFn.apply(_PoolAggregateRowsFn(agg, segments, sites), src, emb, Ws, Wn, Wm, bm)
+    def apply(agg, src, segments, Ws, Wn, *rest):
+        """rest: (weights, bias) of each Dense layer in order, then optionally emb and sites."""
+        n = 2 * len(agg.mlp_layers)
+        emb, sites = (tuple(rest[n:]) + (None, None))[:2]
+        return _LayerFn.apply(_PoolAggregateRowsFn(agg, segments, sites), src, emb, Ws, Wn, *rest[:n])
 
     def __init__(self, agg, segments, sites):
         _SummaryBranch.__init__(self, agg, segments)
         self.sites = sites
 
     def forward(self, src, kept):
-        if len(self.agg.mlp_layers) != 1 or self.agg.dropout:
-            raise NotImplementedError("training supports one MLP layer and dropout = 0")
+        if len(self.agg.mlp_layers) not in (1, 2) or self.agg.dropout:
+            raise NotImplementedError("training supports one or two MLP layers and dropout = 0")
         self.F_in = src.shape[1]
         return self.agg._pooled_parts(src, self.segments, kept, self.sites)
 
     def backward(self, xs, dxs, params, kept, cols):
-        (Wm, _), hp, dhp = params, xs[1], dxs[1]
-        dWm, dbm = torch.zeros_like(Wm), torch.zeros(Wm.shape[1], dtype=dhp.dtype, device=dhp.device)
+        hp, dhp, L = xs[1], dxs[1], len(self.agg.mlp_layers)
+        grads = []
+        for W in params[0::2]:
+            grads += [torch.zeros_like(W), torch.zeros(W.shape[1], dtype=dhp.dtype, device=dhp.device)]
         dxn_all = []
         for i, s in enumerate(self.segments):
             rows = slice(s.out_row0, s.out_row0 + s.n)
-            xn, h = kept[2 * i][:, :self.F_in], kept[2 * i + 1]
-            g_wm, g_bm, dxn = pool_branch_backward(self.agg.pool, xn, h, hp[rows], dhp[rows], Wm[:cols], s.k, cols > 0)
-            dWm += g_wm
-            dbm += g_bm
-            if dxn is not None and self.sites is not None:    # through the input mask, regenerated
-                dxn = ops.dropout_apply(dxn, self.sites[i])
-            dxn_all.append(dxn)
-        return [dWm, dbm], (self._contribs(dxs[0], dxn_all) if cols else [])
+            ins, h = list(kept[(L + 1) * i:(L + 1) * i + L]), kept[(L + 1) * i + L]
+            ins[0] = ins[0][:, :self.F_in]
+            hop_sites = None if self.sites is None else (self.sites[i],) if L == 1 else self.sites[i]
+            W = params[2 * L - 2]
+            g_w, g_b, dx = pool_branch_backward(self.agg.pool, ins[-1], h, hp[rows], dhp[rows], W[:cols] if L == 1 else W,
+                                                s.k, L > 1 or cols > 0)
+            grads[2 * L - 2] += g_w
+            grads[2 * L - 1] += g_b
+            for j in range(L - 2, -1, -1):                    # the Dense layers before the last, through their ReLU
+                if hop_sites is not None:                     # the input mask of Dense j + 1, regenerated
+                    dx = ops.dropout_apply(dx, hop_sites[j + 1])
+                dpre = dx * (ins[j + 1] > 0).to(dx.dtype)
+                grads[2 * j] += ins[j].t() @ dpre
+                grads[2 * j + 1] += dpre.sum(dim=0)
+                W = params[2 * j]
+                dx = (dpre @ (W[:cols] if j == 0 else W).t()) if (j > 0 or cols) else None
+            if dx is not None and hop_sites is not None:      # through the input mask, regenerated
+                dx = ops.dropout_apply(dx, hop_sites[0])
+            dxn_all.append(dx)
+        return grads, (self._contribs(dxs[0], dxn_all) if cols else [])
 
 
 def refuse_fused_pool(model):
@@ -366,16 +388,17 @@ class _SeqAggregateRowsFn(_SummaryBranch):
 
 def layer_params(agg):
     """The tensors a layer trains, in _LayerFn's order: the GEMM parts' weights ([weights] for GCN, else [self_weights,
-    neigh_weights]), then the branch's own - the pools' MLP weights and bias, the seq cell's kernel and bias."""
+    neigh_weights]), then the branch's own - each of the pools' Dense layers' weights and bias, the seq cell's kernel and
+    bias."""
     v = agg.vars
     if hasattr(agg, "cell"):
         cell = agg.cell.vars
         return v["self_weights"], v["neigh_weights"], cell["kernel"], cell["bias"]
     if hasattr(agg, "mlp_layers"):
-        if len(agg.mlp_layers) != 1:
+        if len(agg.mlp_layers) != 1 and not isinstance(agg, TwoMaxLayerPoolingAggregator):
             raise NotImplementedError("training supports one MLP layer")
-        mlp = agg.mlp_layers[0].vars
-        return v["self_weights"], v["neigh_weights"], mlp["weights"], mlp["bias"]
+        return (v["self_weights"], v["neigh_weights"]) + tuple(
+            t for layer in agg.mlp_layers for t in (layer.vars["weights"], layer.vars["bias"]))
     return (v["weights"],) if "weights" in v else (v["self_weights"], v["neigh_weights"])
 
 
@@ -414,8 +437,10 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     counts = [n * support[h] for h in range(L + 1)]
     src = model.features
     pool = hasattr(model.aggregators[0], "mlp_layers")
+    two = isinstance(model.aggregators[0], TwoMaxLayerPoolingAggregator)
     seq = hasattr(model.aggregators[0], "cell")
-    plan = dropout_site_plan("seq" if seq else "maxpool" if pool else "mean", L) if dropout else []
+    kind = "seq" if seq else "twomaxpool" if two else "maxpool" if pool else "mean"
+    plan = dropout_site_plan(kind, L) if dropout else []
     call = {site: model.dropout_counter + i for i, site in enumerate(plan)}
     for layer in range(L):
         hops = L - layer
@@ -425,7 +450,10 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
         sites = None
         if dropout and not seq:                              # per hop: the MLP-input site, or the (neighbour, self) pair
             key, dev = model.dropout_key, model.dropout_call_dev
-            if pool:
+            if two:                                          # the inputs of both Dense layers
+                sites = [tuple((key, call[(layer, h, role)], dropout, dev) for role in ("mlp", "mlp2"))
+                         for h in range(hops)]
+            elif pool:
                 sites = [(key, call[(layer, h, "mlp")], dropout, dev) for h in range(hops)]
             else:
                 sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
@@ -556,8 +584,9 @@ class SupervisedGraphsage(SampleAndAggregate):
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
                                                   identity_dim=identity_dim, device=device, **kwargs)
-        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool", "seq"):
-            raise NotImplementedError("training is implemented for the mean, gcn, maxpool, meanpool and seq aggregators")
+        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool", "twomaxpool", "seq"):
+            raise NotImplementedError("training is implemented for the mean, gcn, maxpool, meanpool, twomaxpool and seq "
+                                      "aggregators")
         init_dropout(self, dropout_seed, distributed, group)
         self.num_classes = num_classes
         self.sigmoid_loss = sigmoid_loss

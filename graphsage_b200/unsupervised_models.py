@@ -47,8 +47,9 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         super(UnsupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                     aggregator_type=aggregator_type, model_size=model_size,
                                                     identity_dim=identity_dim, device=device, **kwargs)
-        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool", "seq"):
-            raise NotImplementedError("training is implemented for the mean, gcn, maxpool, meanpool and seq aggregators")
+        if aggregator_type not in ("mean", "gcn", "maxpool", "meanpool", "twomaxpool", "seq"):
+            raise NotImplementedError("training is implemented for the mean, gcn, maxpool, meanpool, twomaxpool and seq "
+                                      "aggregators")
         init_dropout(self, dropout_seed, distributed, group)
         self.neg_sample_size, self.neg_sample_weights = int(neg_sample_size), float(neg_sample_weights)
         self.learning_rate, self.weight_decay = learning_rate, weight_decay

@@ -366,6 +366,20 @@ int32_t gs_meanpool_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
                               float* out, int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K5 - the two-layer max-pool aggregator's neighbour branch fused end to end (wgmma, bf16 operands, fp32 accumulate):
+ *   h1 = bf16_rne(relu(table[row(g,j), 0:K] . W1 + b1));  out[g, u] = max_{j<k} relu(h1 . W2[:, u] + b2[u])
+ *   reference graphsage/aggregators.py:276-361 (TwoMaxLayerPoolingAggregator: reshape -> Dense -> Dense -> reshape ->
+ *   reduce_max) with the gather of graphsage/models.py:299 fused in front; the gathered rows and h1 stay on chip.
+ *   Rows are addressed as in gs_maxpool_mlp_fused.  packed_w1 / packed_w2: gs_maxpool_mlp_pack of W1 fp32 [K, h1] and
+ *   of W2 fp32 [h1, h2].  b1 / b2 may be NULL (zero).  Limits: k <= 128, K <= 640, h1 % 128 == 0, h2 % 256 == 0 (else
+ *   GS_ERR_UNSUPPORTED: use gs_gather_rows + gs_sage_gemm twice + gs_segment_max).  No atomics, no allocation.
+ * --------------------------------------------------------------------------------------------- */
+int32_t gs_maxpool2_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K, int64_t pitch,
+                              const int32_t* row_ids, int64_t row0, int64_t n_groups, int32_t k,
+                              const void* packed_w1, const float* b1, int32_t h1, const void* packed_w2,
+                              const float* b2, int32_t h2, float* out, int64_t ldo, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Backward of the pooling branch through K4 (bf16 operands, fp32 accumulate; no atomics, deterministic).
  * One hop: X = the n_groups*k gathered rows (addressed as in gs_maxpool_mlp_fused), pre = X Wm, b = bias,
  * dhp [n_groups, hidden] = gradient of the pooled output.  Same limits as K4: k <= 128, K <= 640, hidden % 128 == 0
