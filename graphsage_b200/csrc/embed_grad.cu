@@ -11,7 +11,9 @@
 //   4. combine pass: the chunk where a crossing run starts adds the run's pieces in a fixed lane / chunk order.
 // No atomics anywhere: the result depends on the inputs only.
 // gs_embedding_sgd is the same machinery with the stores turned into in-place updates of the touched rows,
-// table[id] += alpha * sum (kApply); it clears nothing, so untouched rows are neither read nor written.
+// table[id] = fmaf(alpha, sum, table[id]) with one rounding (kApply); it clears nothing, so untouched rows are neither
+// read nor written.  The chunk pass's products and sums and the update are written as __fmul_rn / __fadd_rn /
+// __fmaf_rn so that no compiler contraction can change the rounding oracle/sparse_grad.py emulates.
 #define CUB_WRAPPED_NAMESPACE gs_cub
 #include <cub/device/device_radix_sort.cuh>
 
@@ -117,7 +119,7 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
 #pragma unroll
           for (int q = 0; q < kColsPerLane; ++q) {
             const int col = c0 + lane + 32 * q;
-            v[u][q] = (b + u < cnt && row != nullptr && col < d) ? sc * __ldg(row + col) : 0.f;
+            v[u][q] = (b + u < cnt && row != nullptr && col < d) ? __fmul_rn(sc, __ldg(row + col)) : 0.f;
             if constexpr (kDrop) v[u][q] = drop_col(with_call_offset(L.l[li].site, call_off[li]), pos, col, v[u][q]);
           }
         }
@@ -126,7 +128,7 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
           const int i = b + u;
           if (i >= cnt) break;
 #pragma unroll
-          for (int q = 0; q < kColsPerLane; ++q) acc[q] += v[u][q];
+          for (int q = 0; q < kColsPerLane; ++q) acc[q] = __fadd_rn(acc[q], v[u][q]);
           if ((piece_end >> i) & 1u) {
             const uint32_t key = __shfl_sync(FULL, my_key, i);
             if (key < n_rows) {
@@ -139,7 +141,7 @@ __global__ void __launch_bounds__(256) embed_chunk_kernel(Lists L, const uint32_
               for (int q = 0; q < kColsPerLane; ++q) {
                 const int col = c0 + lane + 32 * q;
                 if constexpr (kApply) {
-                  if (col < d) dst[col] = whole ? dst[col] + alpha * acc[q] : acc[q];
+                  if (col < d) dst[col] = whole ? __fmaf_rn(alpha, acc[q], dst[col]) : acc[q];
                 } else {
                   if (col < d) dst[col] = acc[q];
                 }
@@ -209,7 +211,7 @@ __global__ void __launch_bounds__(kLanes * 32) embed_combine_kernel(const uint32
 #pragma unroll
         for (int pp = 1; pp < kLanes; ++pp) r += red[pp][cl];
         if constexpr (kApply)
-          out[(int64_t)X * ldo + col] = out[(int64_t)X * ldo + col] + alpha * r;
+          out[(int64_t)X * ldo + col] = __fmaf_rn(alpha, r, out[(int64_t)X * ldo + col]);
         else
           out[(int64_t)X * ldo + col] = r;
       }

@@ -59,6 +59,8 @@ __global__ void __launch_bounds__(kRowsPerCta * 32) skipgram_rows_kernel(const _
     if (i < a.B) {
       const float* t = row_of(a.target, a.ldt, a.n_rows, a.batch1[i]);
       const float* c = row_of(a.context, a.ldc, a.n_rows, a.batch2[i]);
+      // s = fmaf(t_q, c_q, s) per lane from +0 (and z below): nvcc contracts these two loops into FFMA chains.  They
+      // are left as written because __fmaf_rn here allocates registers differently; the GPU test pins the bits.
       float s = 0.f;
       for (int q = lane; q < d; q += 32) s += col(t, q) * col(c, q);
       s = warp_sum(s);
@@ -84,10 +86,10 @@ __global__ void __launch_bounds__(kRowsPerCta * 32) skipgram_rows_kernel(const _
       }
       __syncwarp();
       for (int q = lane; q < d; q += 32) {
-        float v = g * col(c, q);
-        for (int j = 0; j < S; ++j) v += h[w][j] * col(row_of(a.context, a.ldc, a.n_rows, a.neg[j]), q);
+        float v = __fmul_rn(g, col(c, q));
+        for (int j = 0; j < S; ++j) v = __fmaf_rn(h[w][j], col(row_of(a.context, a.ldc, a.n_rows, a.neg[j]), q), v);
         a.gt[i * a.ldgt + q] = v;
-        a.gc_pos[i * a.ldgc + q] = g * col(t, q);
+        a.gc_pos[i * a.ldgc + q] = __fmul_rn(g, col(t, q));
       }
     }
     __syncthreads();
@@ -96,7 +98,7 @@ __global__ void __launch_bounds__(kRowsPerCta * 32) skipgram_rows_kernel(const _
     for (int e = threadIdx.x; e < S * width; e += blockDim.x) {
       const int j = e / width, q = e - j * width;
       float acc = first ? 0.f : part[e];
-      for (int r = 0; r < rows; ++r) acc += h[r][j] * (q < d ? col(trow[r], q) : 1.f);
+      for (int r = 0; r < rows; ++r) acc = __fmaf_rn(h[r][j], q < d ? col(trow[r], q) : 1.f, acc);
       part[e] = acc;
     }
     first = false;

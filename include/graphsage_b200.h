@@ -446,8 +446,10 @@ int32_t gs_bump_counter(uint64_t* counter_dev, uint64_t inc, void* stream);
  *   that sorted sequence into fixed chunks of 32.  Within a chunk the products scale * grad are added left to right
  *   in fp32.  A row whose contributions span several chunks gets one such partial sum per chunk (pieces q = 0, 1, ...
  *   in sorted order); piece q goes to accumulator (q / 8) % 4 of lane q % 8, each accumulator adds its pieces in
- *   ascending q, a lane adds its accumulators 0..3 in order, and the row is lane 0 + lane 1 + ... + lane 7, in order.
- *   So a long run of one id (the padding id, a hub) is split into chunks that are summed in parallel.
+ *   ascending q from +0, a lane adds its accumulators 0..3 in order, and the row is lane 0 + lane 1 + ... + lane 7, in order.
+ *   So a long run of one id (the padding id, a hub) is split into chunks that are summed in parallel.  Every product
+ *   scale * grad is rounded to fp32 before it is added (no fused multiply-add), each piece starts from +0, and every
+ *   addition is one fp32 rounding: the result is oracle/sparse_grad.py's embedding_grad_reference bit for bit.
  * workspace: device scratch of gs_embedding_grad_workspace_bytes(...) bytes (0 when there are no contributions); it
  * depends on the lists' lengths, n_rows and d only.  Limits: n_lists <= GS_MAX_EMBED_LISTS, fewer than 2^31 contributions,
  * n_rows < 2^31 - 1, ldg >= d, group >= 1.
@@ -525,7 +527,8 @@ int32_t gs_embedding_grad_dropout(const gs_embed_grad_list* lists_host, const gs
  *     table[r, 0:d] += alpha * (sum over list entries i with ids[i] == r of l.scale * l.grad[(i / l.group) * l.ldg + 0:d])
  *   for every TOUCHED row r, in place (alpha = -learning rate).  Rows no id addresses are never read or written; ids outside
  *   [0, n_rows) contribute nothing.  The row sum is formed in the summation order documented for gs_embedding_grad (same
- *   sort, chunks and combine), then added once: table[r] = table[r] + alpha * sum, fp32.  Bit-identical on every call.
+ *   sort, chunks and combine), then added once: table[r] = fmaf(alpha, sum, table[r]), one rounding.  Bit-identical on
+ *   every call.
  *   Lists, workspace (gs_embedding_grad_workspace_bytes) and limits as for gs_embedding_grad; ldt >= d.  Pass every list
  *   that touches the table in ONE call so that an id appearing in several lists is summed before the update. */
 int32_t gs_embedding_sgd(const gs_embed_grad_list* lists_host, int32_t n_lists, int64_t n_rows, int32_t d, float alpha,
@@ -543,9 +546,15 @@ int32_t gs_embedding_sgd(const gs_embed_grad_list* lists_host, int32_t n_lists, 
  *     gt[i, 0:d]     = g_i c_i + sum_j h_ij n_j      (j ascending)
  *     gc_pos[i, 0:d] = g_i t_i,   gc_pos[i, d] = g_i                       (bias gradient in column d)
  *     gc_neg[j, 0:d] = sum_i h_ij t_i,   gc_neg[j, d] = sum_i h_ij         (ldgc >= d + 1)
- *   Dot products are per-lane strided partial sums (lane l owns columns l, l + 32, ...) combined by a fixed xor butterfly.
- *   The batch reductions (loss, gc_neg) are per-CTA partial sums over the CTA's rows in ascending i, combined in CTA order
- *   by a second kernel: no atomics, bit-identical on every call.  workspace: gs_skipgram_workspace_bytes(B, S, d).
+ *   Dot products (aff, neg_aff): lane l (of 32) holds s = +0 and s = fmaf(t_q, c_q, s) for q = l, l + 32, ...; the lanes
+ *   are combined by the xor butterfly v += shfl_xor(v, o), o = 16, 8, 4, 2, 1, in fp32.  gc_pos[i, 0:d] = fp32(g_i * t_i).
+ *   gt: v = fp32(g_i * c_iq), then v = fmaf(h_ij, n_jq, v) for j ascending.  gc_neg: CTA k (grid = min(ceil(B / 8), 256))
+ *   takes the pair groups k, k + grid, ... (8 pairs each) and chains acc = fmaf(h_ij, t_iq, acc) from +0 over their rows
+ *   in ascending i; a second kernel adds the CTA partials in CTA order.  loss: each pair's softplus(-(aff_i + b_i)),
+ *   then + softplus(neg_aff_ij + nb_j) in j order; lane l (of 32) adds pairs l, l + 32, ... from +0, the butterfly
+ *   combines the lanes, then one division by fp32(B).  sigmoid(x) = 1 / (1 + expf(-x)), softplus(x) = fmaxf(x, 0) +
+ *   log1pf(expf(-|x|)).  No atomics, bit-identical on every call.  The contract and its error bounds are
+ *   oracle/sparse_grad.py's skipgram_reference.  workspace: gs_skipgram_workspace_bytes(B, S, d).
  *   Limits: 1 <= B < 2^31, 1 <= S <= GS_MAX_UNIQUE_SAMPLED, d >= 1, n_rows < 2^31. */
 int64_t gs_skipgram_workspace_bytes(int64_t B, int32_t S, int32_t d);
 int32_t gs_skipgram_grad(const float* target, int64_t ldt, const float* context, int64_t ldc, int64_t n_rows, int32_t d,

@@ -18,7 +18,8 @@ Backward of the max (TensorFlow's reduce_max gradient, as pool_branch_backward a
   (b) acc = +0; for i in transposed row j, in order: if z[j][c] == m[i][c]: acc += s[i][c];
       dz[j][c] = acc where z[j][c] > 0, else +0 (the ReLU of the Dense layer that made z).
 The last layer reads only the rows of node_ids (duplicates allowed): their gradients are scattered into a dense
-[N+1, w] gradient (ops.embedding_grad, group 1; its own summation order - match it within a tolerance) before the
+[N+1, w] gradient (ops.embedding_grad, group 1; its fixed summation order is oracle/sparse_grad.py's
+embedding_grad_reference, bit for bit - this module sums in fp64, so compare with it within a tolerance) before the
 above runs.  With identity_dim = d > 0 the layer-0 table's columns [0, d) are trained: their gradient is column [0, d) of
 the layer-0 source gradient.  Feature columns are not trainable.
 
