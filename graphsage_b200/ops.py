@@ -848,7 +848,7 @@ class PackedMlpDxWeights(PackedMlpWeights):
             raise ValueError("pool_mlp_backward_dx: cols must be in [1, %d] (the rows of Wm), got %d" % (W.shape[0], cols))
         nbytes = lib().gs_pool_mlp_dx_pack_bytes(cols, W.shape[1])
         if nbytes < 0:
-            raise ValueError("pool_mlp_backward_dx: needs 1 <= cols and hidden % 128 == 0 (cols=%d hidden=%d)"
+            raise ValueError("pool_mlp_backward_dx: needs 1 <= cols and hidden %% 128 == 0 (cols=%d hidden=%d)"
                              % (cols, W.shape[1]))
         ws = torch.empty((nbytes,), dtype=torch.uint8, device=W.device)
         Wc = W.contiguous()
@@ -870,7 +870,7 @@ def pool_mlp_backward_dp(table, n_groups, k, W, bias, packed, dhp, row_ids=None,
         raise ValueError("dhp must be a float32 [%d, %d] matrix with unit column stride" % (n_groups, hidden))
     nbytes = lib().gs_pool_mlp_dp_bytes(n_groups, k, hidden)
     if nbytes < 0:
-        raise ValueError("pool_mlp_backward_dp: needs k <= 128 and hidden % 128 == 0 (k=%d hidden=%d)" % (k, hidden))
+        raise ValueError("pool_mlp_backward_dp: needs k <= 128 and hidden %% 128 == 0 (k=%d hidden=%d)" % (k, hidden))
     grad = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=table.device)
     if row_ids is not None:
         row_ids = _i32(row_ids.reshape(-1), "row_ids")
@@ -894,7 +894,7 @@ def pool_mlp_backward_dw(table, n_groups, k, grad, dWm, dbm, row_ids=None, row0=
         raise ValueError("dWm must be a contiguous float32 [K, hidden] matrix and dbm a contiguous float32 [hidden]")
     nbytes = lib().gs_pool_mlp_dw_workspace_bytes(n_groups, k, K, hidden)
     if nbytes < 0:
-        raise ValueError("pool_mlp_backward_dw: needs k <= 128 and hidden % 128 == 0 (k=%d hidden=%d)" % (k, hidden))
+        raise ValueError("pool_mlp_backward_dw: needs k <= 128 and hidden %% 128 == 0 (k=%d hidden=%d)" % (k, hidden))
     ws = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=table.device)
     if row_ids is not None:
         row_ids = _i32(row_ids.reshape(-1), "row_ids")

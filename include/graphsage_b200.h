@@ -391,6 +391,9 @@ int32_t gs_maxpool2_mlp_fused(const void* table_bf16, int64_t n_rows, int32_t K,
  *   mean: dpre_j = (dhp / k) * [fl(pre_j + b) > 0]
  *   and writes into dp (gs_pool_mlp_dp_bytes): dP = bf16(dpre) as tile images of dP^T, then the fp32 per-(tile,
  *   column) sums of dpre (per parity of the group index: group sums in j order added in g order; then even + odd).
+ *   pre here is bit for bit the fp32 pre-activation the default K4 forward (gs_maxpool_mlp_fused /
+ *   gs_meanpool_mlp_fused without tuning keys) accumulates for the same row: the same main loop, tiles and row slots,
+ *   so dhp reaches exactly the rows whose values the forward returned (oracle/pool_backward.py).
  *   packed_weights: gs_maxpool_mlp_pack.
  * B2 gs_pool_mlp_backward_dw: dWm += X^T dP (dWm [K, hidden] fp32, ldw == hidden) and dbm += the column sums of dpre,
  *   X re-gathered from the table; both combined in a fixed order (workspace: gs_pool_mlp_dw_workspace_bytes).
