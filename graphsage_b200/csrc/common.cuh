@@ -39,6 +39,14 @@ inline int32_t launch_check(const char* what) {
 
 int sm_count();
 
+// workspace carving: every region starts on a 256-byte boundary
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+inline int32_t check_site(const gs_dropout_site& s, const char* who) {
+  GS_REQUIRE(s.rate >= 0.f && s.rate < 1.f, "%s: dropout rate %g outside [0, 1)", who, (double)s.rate);
+  return GS_OK;
+}
+
 // ---- Philox4x32-10 (contract: oracle/philox.py) --------------------------------------------
 struct u32x4 { uint32_t x, y, z, w; };
 

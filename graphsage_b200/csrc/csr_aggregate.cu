@@ -4,32 +4,16 @@
 //              mean(concat([neigh, self]), 1)  (GCN)           graphsage/aggregators.py:106-107
 //              tf.reduce_max(neigh_h, axis=1)                  graphsage/aggregators.py:182
 // with the fanout k made per row, and the plain sum GS_CSR_SUM, the backward of the means over the transposed graph
-// (SupervisedGraphsage.full_neighbor_train_step; contract in oracle/full_neighbor_grad.py).  Every output element is ONE sequential chain over the row's entries in CSR order
-// (the order of gs_gather_mean / gs_segment_max), so no work split may cut a row along its entries.  Two roles share
-// one launch of 256-thread CTAs:
-//   hub role (the first hub_blocks CTAs): rows with more than kCsrLong entries.  Work item = (chunk of 256 rows, slice of
-//     32 columns); the CTA finds the long rows of its chunk and, per row, its 8 warps load 64 entries' slices into a
-//     double-buffered shared tile while warp 0 sums the previous 64 in order.  A hub is spread over out_pitch / 32 CTAs
-//     and keeps 64 rows in flight in each, instead of one warp walking 10^5 dependent steps.
-//   short role (the rest): one warp per (row, slice of 32 * V columns), V columns per lane (float4 / 8 x bf16 loads),
-//     kUnroll entries' loads in flight before they are summed in order.
-// Hub CTAs come first in the grid, so the long rows start before the short ones fill the machine.
+// (SupervisedGraphsage.full_neighbor_train_step; contract in oracle/full_neighbor_grad.py).  Every output element is ONE
+// sequential chain over the row's entries in CSR order (the order of gs_gather_mean / gs_segment_max), run on the hub /
+// short row schedule of csr_rows.cuh; the short role reads V columns per lane (float4 / 8 x bf16 loads).
 // kDrop (gs_csr_aggregate_dropout; contract in oracle/full_neighbor_dropout.py): every entry is masked where it is
 // loaded - per entry and 4 columns one Philox call in the short role (the float4 / 8 x bf16 loads), in the hub role's
 // loading warps before the tile is written, a quad of lanes sharing its 4 columns' calls through shuffles - so warp 0's
 // ordered sum does no extra work.  The kDrop = false instantiations are the plain kernel.
-#include <algorithm>
-
-#include "common.cuh"
+#include "csr_rows.cuh"
 
 namespace gs {
-
-constexpr int kCsrThreads = 256;
-constexpr int64_t kCsrLong = 256;     // rows with more entries go to the hub role
-constexpr int kHubChunk = 256;        // rows scanned per hub work item (one per thread)
-constexpr int kHubCols = 32;          // columns per hub work item (one per lane of the summing warp)
-constexpr int kHubPerWarp = 8;        // entries each warp loads per round
-constexpr int kHubRows = kHubPerWarp * (kCsrThreads / 32);   // entries per round: 64
 
 struct CsrArgs {
   const void* src;
@@ -108,18 +92,12 @@ struct Loader<uint16_t, 8> {
   }
 };
 
-template <typename T>
-__device__ __forceinline__ float load_scalar(const CsrArgs& a, int64_t r, int c) {
-  if constexpr (sizeof(T) == 2) return bf16_bits_to_f32(__ldg(static_cast<const uint16_t*>(a.src) + r * a.pitch + c));
-  else return __ldg(static_cast<const float*>(a.src) + r * a.pitch + c);
-}
-
-// one step of the chain after its first entry (the max starts from x_0 itself, the means and the sum from +0)
-template <int OP>
-__device__ __forceinline__ float csr_step(float acc, float x) {
-  if constexpr (OP == GS_CSR_MAX) return fmaxf(acc, x);
-  else return acc + x;
-}
+template <>
+struct Loader<uint16_t, 1> {
+  static __device__ __forceinline__ void load(const CsrArgs& a, int64_t r, int c0, float (&x)[1]) {
+    x[0] = bf16_bits_to_f32(__ldg(static_cast<const uint16_t*>(a.src) + r * a.pitch + c0));
+  }
+};
 
 // the chain's end: the mean's division (after the self row for GS_CSR_MEAN_SELF); the max and the sum end as they are
 template <int OP>
@@ -184,162 +162,105 @@ __device__ __forceinline__ void quad_transpose(const u32x4& w, uint32_t (&m)[4])
   for (int u = 0; u < 4; ++u) m[u] = pick(got, (u - j) & 3);
 }
 
-// the hub role's masks of the warp's entries e0 .. e0 + kHubPerWarp - 1 of a row (cnt > kHubRows), loaded into r at
-// column c; entries past the row are computed on its last entry and multiply a loaded 0
-template <int OP>
-__device__ __forceinline__ void hub_mask(const CsrArgs& a, int64_t lo, int64_t cnt, int64_t base, int64_t e0, int c,
-                                         const DropSite& sn, const DropSite& ss, float (&r)[kHubPerWarp]) {
-  const int j = threadIdx.x & 3;
-#pragma unroll
-  for (int h = 0; h < kHubPerWarp / 4; ++h) {
-    const DropEntry mine = drop_entry<OP>(a, lo, base, min(e0 + 4 * h + j, cnt - 1));
-    uint32_t m[4];
-    quad_transpose(drop_words(mine.self ? ss : sn, mine.pos, (uint32_t)c >> 2), m);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int u = 4 * h + q;
-      const bool self = OP == GS_CSR_SUM && drop_entry<OP>(a, lo, base, min(e0 + u, cnt - 1)).self;
-      r[u] = drop_one(self ? ss : sn, m[q], r[u]);
-    }
-  }
-}
-
+// the aggregate on the csr_rows.cuh schedule: the rows of `rows` (or 0 .. n - 1), entries read from src, written up to
+// out_pitch with columns F .. out_pitch - 1 zero-filled
 template <typename T, int OP, bool kDrop>
-__device__ void hub_role(const CsrArgs& a, float (*tile)[kHubRows][kHubCols], const DropSite& sn, const DropSite& ss) {
-  __shared__ int32_t list[kHubChunk];
-  __shared__ int32_t warp_count[kCsrThreads / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t item = blockIdx.x; item < a.hub_items; item += a.hub_blocks) {
-    const int64_t chunk = item / a.hub_slices;
-    const int c = (int)(item % a.hub_slices) * kHubCols + lane;
-    // the chunk's long rows, in row order (ballot + per-warp offsets: no atomics)
-    const int64_t i0 = chunk * kHubChunk + threadIdx.x;
-    int64_t lo, cnt = 0;
-    if (i0 < a.n) csr_row(a, i0, lo, cnt);
-    const bool is_long = cnt > kCsrLong;
-    const uint32_t ballot = __ballot_sync(0xffffffffu, is_long);
-    if (lane == 0) warp_count[warp] = __popc(ballot);
-    __syncthreads();
-    int off = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kCsrThreads / 32; ++w) {
-      off += w < warp ? warp_count[w] : 0;
-      total += warp_count[w];
-    }
-    if (is_long) list[off + __popc(ballot & ((1u << lane) - 1u))] = (int32_t)threadIdx.x;
-    __syncthreads();
-    for (int q = 0; q < total; ++q) {
-      const int64_t i = chunk * kHubChunk + list[q];
-      const int64_t v = csr_row(a, i, lo, cnt);
-      const bool col_ok = c < a.F;
-      float r[kHubPerWarp];
-#pragma unroll
-      for (int u = 0; u < kHubPerWarp; ++u) {
-        const int e = warp * kHubPerWarp + u;
-        r[u] = col_ok ? load_scalar<T>(a, csr_entry(a, lo, cnt, e), c) : 0.f;     // cnt > kHubRows
-      }
-      int64_t node = 0, pbase = 0;
-      if constexpr (kDrop) {
-        node = drop_node(a, v);
-        if (OP != GS_CSR_SUM) pbase = drop_row_base(a, node, cnt);
-        hub_mask<OP>(a, lo, cnt, pbase, warp * kHubPerWarp, c, sn, ss, r);
-      }
-      float acc = 0.f;
-      int buf = 0;
-      for (int64_t base = 0; base < cnt; base += kHubRows, buf ^= 1) {
-#pragma unroll
-        for (int u = 0; u < kHubPerWarp; ++u) tile[buf][warp * kHubPerWarp + u][lane] = r[u];
-        __syncthreads();
-        const int64_t next = base + kHubRows + warp * kHubPerWarp;
-#pragma unroll
-        for (int u = 0; u < kHubPerWarp; ++u)                 // the next round's loads are in flight during the sum
-          r[u] = (col_ok && next + u < cnt) ? load_scalar<T>(a, csr_entry(a, lo, cnt, next + u), c) : 0.f;
-        if constexpr (kDrop) hub_mask<OP>(a, lo, cnt, pbase, next, c, sn, ss, r);
-        if (warp == 0) {
-          const int m = (int)min((int64_t)kHubRows, cnt - base);
-          int t = 0;
-          if (OP == GS_CSR_MAX && base == 0) acc = tile[buf][t++][lane];
-          for (; t < m; ++t) acc = csr_step<OP>(acc, tile[buf][t][lane]);
-        }
-      }
-      if (warp == 0 && c < a.out_pitch) {
-        float y = 0.f;
-        if (col_ok) {
-          float self = OP == GS_CSR_MEAN_SELF ? load_scalar<T>(a, csr_clamp(v, a.n_src_rows), c) : 0.f;
-          if constexpr (kDrop && OP == GS_CSR_MEAN_SELF) self = drop_col(ss, node, c, self);
-          y = csr_final<OP>(acc, cnt, self);
-        }
-        a.out[i * a.out_pitch + c] = y;
-      }
-      __syncthreads();      // the tiles are reused by the next row
-    }
-    __syncthreads();        // `list` and `warp_count` are rewritten by the next item
-  }
-}
+struct AggregateRows {
+  static constexpr bool kFromFirst = OP == GS_CSR_MAX;
+  static constexpr bool kEmptyIsDummy = OP != GS_CSR_SUM;   // the sum's empty row is +0 (a node nobody points to)
+  const CsrArgs& a;
+  const DropSite& sn;                                  // kDrop: the neighbour and self sites
+  const DropSite& ss;
 
-template <typename T, int V, int OP, bool kDrop>
-__device__ void short_role(const CsrArgs& a, int64_t block, const DropSite& sn, const DropSite& ss) {
-  constexpr int kUnroll = V == 8 ? 4 : 8;      // 16-byte loads in flight per lane: 4 (bf16) or 8 (fp32 float4)
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t items = a.n * a.n_slices;
-  const int64_t stride = ((int64_t)gridDim.x - a.hub_blocks) * (kCsrThreads / 32);
-  for (int64_t item = block * (kCsrThreads / 32) + warp; item < items; item += stride) {
-    const int64_t i = item / a.n_slices;
-    const int c0 = ((int)(item % a.n_slices) * 32 + lane) * V;
-    int64_t lo, cnt;
-    const int64_t v = csr_row(a, i, lo, cnt);
-    if (cnt > kCsrLong || c0 >= a.out_pitch) continue;       // a hub row (hub role), or past the row's last column
-    float acc[V];
-#pragma unroll
-    for (int q = 0; q < V; ++q) acc[q] = 0.f;
-    if (c0 < a.F) {
-      // an empty row: the dummy row alone, except for the sum, whose empty row is +0 (a node nobody points to)
-      const int64_t count = OP == GS_CSR_SUM ? cnt : cnt > 0 ? cnt : 1;
-      int64_t node = 0, pbase = 0;
-      if constexpr (kDrop) {
-        node = drop_node(a, v);
-        if (OP != GS_CSR_SUM) pbase = drop_row_base(a, node, cnt);
-      }
-      int64_t e = 0;
-      if constexpr (OP == GS_CSR_MAX) {
-        float x0[V];
-        Loader<T, V>::load(a, csr_entry(a, lo, cnt, e++), c0, x0);
-#pragma unroll
-        for (int q = 0; q < V; ++q) acc[q] = x0[q];
-      }
-      for (; e < count; e += kUnroll) {
-        float x[kUnroll][V];
-#pragma unroll
-        for (int u = 0; u < kUnroll; ++u)
-          if (e + u < count) Loader<T, V>::load(a, csr_entry(a, lo, cnt, e + u), c0, x[u]);
-#pragma unroll
-        for (int u = 0; u < kUnroll; ++u)
-          if (e + u < count) {
-            if constexpr (kDrop) {
-              const DropEntry d = drop_entry<OP>(a, lo, pbase, e + u);
-              drop_vec<V>(d.self ? ss : sn, d.pos, c0, x[u]);
-            }
-#pragma unroll
-            for (int q = 0; q < V; ++q) acc[q] = csr_step<OP>(acc[q], x[u][q]);
-          }
-      }
-      float self[V];
-#pragma unroll
-      for (int q = 0; q < V; ++q) self[q] = 0.f;
-      if (OP == GS_CSR_MEAN_SELF) Loader<T, V>::load(a, csr_clamp(v, a.n_src_rows), c0, self);
-      if constexpr (kDrop && OP == GS_CSR_MEAN_SELF) drop_vec<V>(ss, node, c0, self);
-#pragma unroll
-      for (int q = 0; q < V; ++q) acc[q] = c0 + q < a.F ? csr_final<OP>(acc[q], count, self[q]) : 0.f;
+  struct Row {
+    int64_t v, lo, cnt;
+    int64_t node = 0, pbase = 0;                       // kDrop: global node, position of entry 0 (drop_row_base)
+  };
+
+  __device__ __forceinline__ int64_t rows() const { return a.n; }
+  __device__ __forceinline__ int32_t hub_slices() const { return a.hub_slices; }
+  __device__ __forceinline__ int32_t slices() const { return a.n_slices; }
+  __device__ __forceinline__ int64_t out_cols() const { return a.out_pitch; }
+
+  __device__ __forceinline__ Row row(int64_t i) const {
+    Row r;
+    r.v = csr_row(a, i, r.lo, r.cnt);
+    return r;
+  }
+
+  __device__ __forceinline__ void begin(Row& r, int64_t, int, bool) const {
+    if constexpr (kDrop) {
+      r.node = drop_node(a, r.v);
+      if (OP != GS_CSR_SUM) r.pbase = drop_row_base(a, r.node, r.cnt);
     }
+  }
+
+  template <int W>
+  __device__ __forceinline__ void load(const Row& r, int64_t e, int c0, bool ok, float (&x)[W]) const {
+    if (ok) Loader<T, W>::load(a, csr_entry(a, r.lo, r.cnt, e), c0, x);
+  }
+
+  __device__ __forceinline__ float value(const Row& r, int64_t e, int c) const {
+    float x[1];
+    load(r, e, c, true, x);
+    return x[0];
+  }
+
+  template <int W>
+  __device__ __forceinline__ void mask(const Row& r, int64_t e, int c0, float (&x)[W]) const {
+    if constexpr (kDrop) {
+      const DropEntry d = drop_entry<OP>(a, r.lo, r.pbase, e);
+      drop_vec<W>(d.self ? ss : sn, d.pos, c0, x);
+    }
+  }
+
+  // the masks of the warp's entries e0 .. e0 + kHubPerWarp - 1 of a hub row (cnt > kHubRows) at column c; entries past
+  // the row are computed on its last entry and multiply a loaded 0
+  __device__ __forceinline__ void hub_mask(const Row& r, int64_t e0, int c, float (&x)[kHubPerWarp]) const {
+    if constexpr (kDrop) {
+      const int j = threadIdx.x & 3;
+#pragma unroll
+      for (int h = 0; h < kHubPerWarp / 4; ++h) {
+        const DropEntry mine = drop_entry<OP>(a, r.lo, r.pbase, min(e0 + 4 * h + j, r.cnt - 1));
+        uint32_t m[4];
+        quad_transpose(drop_words(mine.self ? ss : sn, mine.pos, (uint32_t)c >> 2), m);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int u = 4 * h + q;
+          const bool self = OP == GS_CSR_SUM && drop_entry<OP>(a, r.lo, r.pbase, min(e0 + u, r.cnt - 1)).self;
+          x[u] = drop_one(self ? ss : sn, m[q], x[u]);
+        }
+      }
+    }
+  }
+
+  __device__ __forceinline__ float step(float acc, float x) const {
+    if constexpr (OP == GS_CSR_MAX) return fmaxf(acc, x);
+    else return acc + x;
+  }
+
+  template <int W>
+  __device__ __forceinline__ void finish(const Row& r, int c0, int64_t count, float (&acc)[W]) const {
+    float self[W];
+#pragma unroll
+    for (int q = 0; q < W; ++q) self[q] = 0.f;
+    if (OP == GS_CSR_MEAN_SELF) Loader<T, W>::load(a, csr_clamp(r.v, a.n_src_rows), c0, self);
+    if constexpr (kDrop && OP == GS_CSR_MEAN_SELF) drop_vec<W>(ss, r.node, c0, self);
+#pragma unroll
+    for (int q = 0; q < W; ++q) acc[q] = c0 + q < a.F ? csr_final<OP>(acc[q], count, self[q]) : 0.f;
+  }
+
+  template <int W>
+  __device__ __forceinline__ void store(const Row&, int64_t i, int c0, const float (&acc)[W]) const {
     float* dst = a.out + i * a.out_pitch + c0;
-    if constexpr (V == 1) {
+    if constexpr (W == 1) {
       dst[0] = acc[0];
     } else {
 #pragma unroll
-      for (int q = 0; q < V; q += 4) *reinterpret_cast<float4*>(dst + q) = make_float4(acc[q], acc[q + 1], acc[q + 2], acc[q + 3]);
+      for (int q = 0; q < W; q += 4) *reinterpret_cast<float4*>(dst + q) = make_float4(acc[q], acc[q + 1], acc[q + 2], acc[q + 3]);
     }
   }
-}
+};
 
 template <typename T, int V, int OP, bool kDrop>
 __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __grid_constant__ CsrArgs a) {
@@ -349,8 +270,8 @@ __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __g
     sn.call += drop_call_offset(sn);
     ss.call += drop_call_offset(ss);
   }
-  if (blockIdx.x < a.hub_blocks) hub_role<T, OP, kDrop>(a, tile, sn, ss);
-  else short_role<T, V, OP, kDrop>(a, (int64_t)blockIdx.x - a.hub_blocks, sn, ss);
+  // short role: 16-byte loads in flight per lane: 4 (bf16) or 8 (fp32 float4)
+  csr_rows<V, V == 8 ? 4 : 8>(AggregateRows<T, OP, kDrop>{a, sn, ss}, tile);
 }
 
 template <typename T, int V>
@@ -415,11 +336,7 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
   }
   a.n_slices = (int32_t)((out_pitch + 32 * V - 1) / (32 * V));
   a.hub_slices = (int32_t)((out_pitch + kHubCols - 1) / kHubCols);
-  a.hub_items = (n + kHubChunk - 1) / kHubChunk * a.hub_slices;
-  a.hub_blocks = std::min<int64_t>(a.hub_items, (int64_t)sm_count() * 4);
-  const int64_t short_items = n * a.n_slices;
-  const int64_t short_blocks = std::min<int64_t>((short_items + 7) / 8, (int64_t)sm_count() * 8 * 64);
-  const unsigned blocks = (unsigned)(a.hub_blocks + short_blocks);
+  const unsigned blocks = csr_grid(n, a.hub_slices, a.n_slices, a.hub_items, a.hub_blocks);
   cudaStream_t st = (cudaStream_t)stream;
   if (drop) {
     if (dtype == GS_BF16) launch_csr_drop<uint16_t, 8>(op, blocks, a, st);
@@ -431,11 +348,6 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
   else if (V == 4) launch_csr<float, 4>(op, blocks, a, st);
   else launch_csr<float, 1>(op, blocks, a, st);
   return launch_check("csr_aggregate_kernel");
-}
-
-static int32_t check_site(const gs_dropout_site& s, const char* who) {
-  GS_REQUIRE(s.rate >= 0.f && s.rate < 1.f, "%s: dropout rate %g outside [0, 1)", who, (double)s.rate);
-  return GS_OK;
 }
 
 }  // namespace gs

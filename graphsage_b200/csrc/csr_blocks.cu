@@ -24,8 +24,6 @@ namespace gs {
 constexpr int kBlkThreads = 256;
 constexpr int kBlkWarps = kBlkThreads / 32;
 
-static size_t blk_align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct BlocksPlan {
   int64_t n_nodes = 0, cap = 0;       // N; cap = N + 2 (the flags, positions and degrees of nodes 0 .. N, plus a 0)
   int32_t levels = 0;                 // L + 1: level l < L is V_l, level L the distinct seeds
@@ -158,11 +156,11 @@ static int32_t make_blocks_plan(int64_t n_nodes, int64_t nnz, int64_t n_seeds, i
   if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceReduce::Sum (size query)");
   P.cub_bytes = std::max(std::max(scan32, scan64), reduce64);
   size_t off = 0;
-  P.off_flag = off; off += blk_align256((size_t)P.cap * 4);
-  P.off_pos = off;  off += (size_t)P.levels * blk_align256((size_t)P.cap * 4);
-  P.off_ids = off;  off += (size_t)P.levels * blk_align256((size_t)P.cap * 4);
-  P.off_deg = off;  off += blk_align256((size_t)P.cap * 8);
-  P.off_cub = off;  off += blk_align256(P.cub_bytes);
+  P.off_flag = off; off += align256((size_t)P.cap * 4);
+  P.off_pos = off;  off += (size_t)P.levels * align256((size_t)P.cap * 4);
+  P.off_ids = off;  off += (size_t)P.levels * align256((size_t)P.cap * 4);
+  P.off_deg = off;  off += align256((size_t)P.cap * 8);
+  P.off_cub = off;  off += align256(P.cub_bytes);
   P.bytes = off;
   return GS_OK;
 }
@@ -181,7 +179,7 @@ struct BlocksWs {
 static BlocksWs blocks_ws(const BlocksPlan& P, void* workspace) {
   char* ws = (char*)workspace;
   return BlocksWs{(int32_t*)(ws + P.off_flag), ws + P.off_pos, ws + P.off_ids, (int64_t*)(ws + P.off_deg),
-                  ws + P.off_cub, blk_align256((size_t)P.cap * 4)};
+                  ws + P.off_cub, align256((size_t)P.cap * 4)};
 }
 
 static unsigned blk_grid(int64_t items, int64_t per_block, int64_t max_blocks) {

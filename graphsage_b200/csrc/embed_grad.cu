@@ -227,8 +227,6 @@ struct Plan {
   size_t cub_bytes = 0, bytes = 0;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int32_t make_plan(const gs_embed_grad_list* lists, int32_t n_lists, int64_t n_rows, int32_t d, Plan& P,
                   const char* who) {
   GS_REQUIRE(n_lists >= 0 && n_lists <= GS_MAX_EMBED_LISTS, "%s: n_lists must be in [0, %d]", who,

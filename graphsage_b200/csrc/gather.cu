@@ -1128,11 +1128,6 @@ int32_t gs_segment_max(const float* x, int64_t n, int32_t k, int32_t C, int64_t 
   return gs::launch_check("segment_max_kernel");
 }
 
-static int32_t check_site(const gs_dropout_site& s, const char* who) {
-  GS_REQUIRE(s.rate >= 0.f && s.rate < 1.f, "%s: dropout rate %g outside [0, 1)", who, (double)s.rate);
-  return GS_OK;
-}
-
 int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, int64_t pitch, const gs_segment* segments_host,
                                int32_t n_segments, const gs_dropout_site* neigh_sites_host,
                                const gs_dropout_site* self_sites_host, int32_t include_self, float* out_self,
@@ -1147,8 +1142,8 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
   gs::DropTab drop;
   memset(&drop, 0, sizeof(drop));
   for (int s = 0; s < n_segments; ++s) {
-    rc = check_site(neigh_sites_host[s], "gs_gather_mean_dropout");
-    if (rc == GS_OK) rc = check_site(self_sites_host[s], "gs_gather_mean_dropout");
+    rc = gs::check_site(neigh_sites_host[s], "gs_gather_mean_dropout");
+    if (rc == GS_OK) rc = gs::check_site(self_sites_host[s], "gs_gather_mean_dropout");
     if (rc != GS_OK) return rc;
     drop.neigh[s] = gs::make_drop_site(neigh_sites_host[s]);
     drop.self[s] = gs::make_drop_site(self_sites_host[s]);
@@ -1175,7 +1170,7 @@ int32_t gs_gather_mean_dropout(const float* src, int64_t n_src_rows, int32_t F, 
 int32_t gs_dropout_apply(const float* x, int64_t ldx, int64_t rows, int32_t F, int32_t group, float scale,
                          gs_dropout_site site, int32_t accumulate, float* out, int64_t ldo, const int32_t* pos_ids,
                          void* stream) {
-  int32_t rc = check_site(site, "gs_dropout_apply");
+  int32_t rc = gs::check_site(site, "gs_dropout_apply");
   if (rc != GS_OK) return rc;
   GS_REQUIRE(rows >= 0 && F >= 0 && group >= 1, "gs_dropout_apply: bad sizes (rows=%lld F=%d group=%d)", (long long)rows, F,
              group);

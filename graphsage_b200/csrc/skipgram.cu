@@ -136,8 +136,6 @@ int64_t n_ctas(int64_t B) {
   return groups < kMaxCtas ? groups : kMaxCtas;
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 }  // namespace
 }  // namespace gs
 

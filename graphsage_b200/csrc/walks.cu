@@ -15,8 +15,6 @@ namespace gs {
 
 constexpr int kWalkThreads = 256;
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct WalkPlan {
   int64_t walks = 0;                 // n * num_walks
   size_t off_visited = 0, off_counts = 0, off_offsets = 0, off_cub = 0;
