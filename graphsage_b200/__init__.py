@@ -4,11 +4,12 @@ williamleif/GraphSAGE.  `import graphsage_b200 as graphsage` is the intended dro
 
 All compute goes through libgraphsage_b200.so (include/graphsage_b200.h); there is no CPU fallback.
 """
-from . import (_lib, aggregators, graph, graphed_training, inits, layers, minibatch, models, neigh_samplers, node2vec,  # noqa: F401
-               ops, prediction, utils)
+from . import (_lib, aggregators, graph, graphed_training, host_features, inits, layers, minibatch, models,  # noqa: F401
+               neigh_samplers, node2vec, ops, prediction, utils)
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator,  # noqa: F401
                           SeqAggregator, TwoMaxLayerPoolingAggregator, set_default_math)
 from .graphed_training import GraphedTrainStep, make_adam_capturable  # noqa: F401
+from .host_features import HostFeatures  # noqa: F401
 from .layers import Dense, Layer, identity, relu  # noqa: F401
 from .models import Node2VecModel, SAGEInfo, SampleAndAggregate  # noqa: F401
 from .neigh_samplers import CSRNeighborSampler, UniformNeighborSampler  # noqa: F401

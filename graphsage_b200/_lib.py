@@ -91,6 +91,10 @@ _SIGNATURES = {
     "gs_ipc_export": (c_i32, [c_vp, ctypes.c_char_p]),
     "gs_ipc_import": (c_i32, [ctypes.c_char_p, ctypes.POINTER(c_vp)]),
     "gs_ipc_close": (c_i32, [c_vp]),
+    "gs_host_register": (c_i32, [c_vp, c_i64, ctypes.POINTER(c_vp)]),
+    "gs_host_unregister": (c_i32, [c_vp]),
+    "gs_host_fetch": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "gs_host_translate": (c_i32, [ctypes.POINTER(ShardedTable), c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_gather_rows_f32": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp]),
     "gs_cast_rows_bf16": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp]),
     "gs_rmat_degrees": (c_i32, [c_i32, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,

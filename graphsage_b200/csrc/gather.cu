@@ -784,13 +784,15 @@ __global__ void __launch_bounds__(256) halo_claim_kernel(const __grid_constant__
   }
 }
 
+// a staged id becomes miss_row0 + miss_step * claim[id]: -(slot) - 1 for the halo locators (-1, -1), the working-set row
+// stage_row0 + slot for a host table (stage_row0, +1)
 __global__ void __launch_bounds__(256) halo_translate_kernel(const __grid_constant__ ShardTab t, const int32_t* __restrict__ ids,
                                                              int64_t n, const int32_t* __restrict__ claim,
-                                                             int32_t* __restrict__ out) {
+                                                             int32_t* __restrict__ out, int32_t miss_row0, int32_t miss_step) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int32_t id = ids[i];
     int32_t loc;
-    if (!halo_is_local(t, id, loc)) loc = -claim[id] - 1;
+    if (!halo_is_local(t, id, loc)) loc = miss_row0 + miss_step * claim[id];
     out[i] = loc;
   }
 }
@@ -1285,7 +1287,26 @@ int32_t gs_halo_translate(const gs_sharded_table* table_host, const int32_t* ids
   int64_t blocks = (n + 255) / 256;
   int64_t cap = (int64_t)gs::sm_count() * 8;
   if (blocks > cap) blocks = cap;
-  gs::halo_translate_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(sr.t, ids, n, claim, out);
+  gs::halo_translate_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(sr.t, ids, n, claim, out, -1, -1);
+  return gs::launch_check("halo_translate_kernel");
+}
+
+int32_t gs_host_translate(const gs_sharded_table* table_host, const int32_t* ids, int64_t n, const int32_t* claim,
+                          int64_t stage_row0, int32_t* out, void* stream) {
+  gs::ShardRows sr;
+  int32_t rc = fill_shard_tab(table_host, sr, 4, "gs_host_translate");
+  if (rc != GS_OK) return rc;
+  GS_REQUIRE(n >= 0, "gs_host_translate: n < 0");
+  GS_REQUIRE(table_host->remap != nullptr, "gs_host_translate: the table needs its cache_slot array as remap");
+  GS_REQUIRE(stage_row0 > table_host->zero_row && stage_row0 < 0x7fffffffLL,
+             "gs_host_translate: stage_row0 must follow the zero row and fit int32");
+  if (n == 0) return GS_OK;
+  GS_REQUIRE(ids && claim && out, "gs_host_translate: NULL pointer");
+  int64_t blocks = (n + 255) / 256;
+  int64_t cap = (int64_t)gs::sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  gs::halo_translate_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(sr.t, ids, n, claim, out,
+                                                                                 (int32_t)stage_row0, 1);
   return gs::launch_check("halo_translate_kernel");
 }
 

@@ -32,6 +32,7 @@ import torch
 
 from . import ops
 from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, TwoMaxLayerPoolingAggregator, _rows
+from .host_features import refuse_host_table
 from .layers import act_code
 from .supervised_models import (_LayerFn, build_aggregators, check_full_neighbor_dropout, full_neighbor_site_plan,
                                 layer_params)
@@ -238,6 +239,7 @@ def refuse_full_neighbor(model, training, dropout=None):
     if hasattr(model.features, "c_table"):
         raise NotImplementedError("full-neighbourhood %s with a node-partitioned (ShardedFeatures) table is not "
                                   "implemented" % what)
+    refuse_host_table(model.features, "full-neighbourhood %s (it reads the whole table)" % what)
     if not training:
         return
     if model.aggregator_cls is TwoMaxLayerPoolingAggregator:

@@ -12,6 +12,7 @@ import torch
 from . import ops
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
                           TwoMaxLayerPoolingAggregator, refuse_seq_table)
+from .host_features import HostFeatures, refuse_host_table, stage_layer0, step_rows
 from .layers import identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
@@ -47,7 +48,8 @@ class SampleAndAggregate(object):
     """The sample -> K-hop gather -> aggregate recursion of GraphSAGE (reference models.py:187-330).
 
     features : float32 CUDA tensor [N+1, F] whose LAST row is the all-zero dummy row
-               (reference supervised_train.py:133-135), or a numpy array (uploaded, dummy row NOT added).
+               (reference supervised_train.py:133-135), or a numpy array (uploaded, dummy row NOT added), or a
+               HostFeatures table in host memory (each step stages the rows it reads; see host_features.py).
     adj      : int32 CUDA tensor [N+1, max_degree] padded adjacency (reference minibatch.py:227-245).
     identity_dim : d > 0 adds a trainable [N+1, d] embedding table (`self.embeds`) in front of the features, or replaces
                them when features is None (see _init_identity_table).
@@ -78,6 +80,12 @@ class SampleAndAggregate(object):
             self.features = features
             self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
             return
+        if isinstance(features, HostFeatures):           # rows in host memory, staged per step into a working set
+            self.features = features
+            self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
+            if self.batch_size is not None:
+                features.reserve(step_rows(self.batch_size, layer_infos))
+            return
         if not torch.is_tensor(features):
             features = torch.as_tensor(features, dtype=torch.float32)
         dt = torch.bfloat16 if features.dtype == torch.bfloat16 else torch.float32   # bf16 tables are kept (config 3)
@@ -103,6 +111,7 @@ class SampleAndAggregate(object):
         from .inits import glorot
         if hasattr(features, "c_table"):
             raise NotImplementedError("identity_dim > 0 with a node-partitioned feature table is not implemented")
+        refuse_host_table(features, "identity_dim > 0 (the embeddings are trained in a device table beside the features)")
         if features is not None:
             if torch.is_tensor(features) and features.dtype == torch.bfloat16:
                 raise NotImplementedError("identity_dim > 0 with a bfloat16 feature table is not implemented")
@@ -189,15 +198,17 @@ class SampleAndAggregate(object):
             return self._aggregate_materialised(samples, feats, dims, num_samples, support_sizes, batch_size,
                                                 aggregators, concat), aggregators
         counts = [batch_size * support_sizes[h] for h in range(L + 1)]
-        src = feats
+        src, samples, persistent = stage_layer0(feats, samples)
         for layer in range(L):
             src = aggregators[layer].aggregate_rows(src, layer_segments(samples, counts, num_samples, layer),
-                                                    final=_final if layer == L - 1 else None, src_persistent=(layer == 0))
+                                                    final=_final if layer == L - 1 else None,
+                                                    src_persistent=(layer == 0 and persistent))
         return src[:counts[0]], aggregators
 
     def _aggregate_materialised(self, samples, feats, dims, num_samples, support_sizes, batch_size, aggregators,
                                 concat):
         """The reference's literal recursion (hidden[h] materialised); used when dropout > 0."""
+        feats, samples, _ = stage_layer0(feats, samples)
         hidden = [ops.gather_rows(feats, s) for s in samples]                    # models.py:299
         L = len(num_samples)
         for layer in range(L):
@@ -399,6 +410,9 @@ class PipelinedForward(object):
     """
 
     def __init__(self, model, batch_size, normalize=True, depth=2):
+        # the runners overlap on their streams, but a host table has one working set: a step would restage it under the
+        # layer 0 of the step before
+        refuse_host_table(model.features, "PipelinedForward")
         dev = model.device
         self.model, self.depth = model, int(depth)
         self.runners = [GraphedForward(model, batch_size, normalize, first_step=r, step_stride=self.depth)

@@ -334,6 +334,40 @@ def translate_ids(table, ids):
     return out
 
 
+def host_register(t):
+    """Page-lock a contiguous CPU tensor once and map it for the device (gs_host_register); returns its device alias."""
+    import ctypes
+    if t.is_cuda or not t.is_contiguous():
+        raise ValueError("host_register needs a contiguous CPU tensor")
+    alias = ctypes.c_void_p()
+    check(lib().gs_host_register(t.data_ptr(), t.numel() * t.element_size(), ctypes.byref(alias)))
+    return alias.value
+
+
+def host_unregister(t):
+    check(lib().gs_host_unregister(t.data_ptr()))
+
+
+def host_fetch(host_alias, row_bytes, stage_ids, count, staging):
+    """staging[i] = row stage_ids[i] of the mapped host table, i < *count (gs_host_fetch); staging rows are row_bytes
+    apart, the table's pitch.  capacity = stage_ids.numel(); the launch does not read *count on the host."""
+    capacity = stage_ids.numel()
+    ev = _probe("host_fetch")
+    check(lib().gs_host_fetch(host_alias, int(row_bytes), ptr(stage_ids), ptr(count), capacity, ptr(staging),
+                              stream_ptr()))
+    _launched(1 if capacity else 0, ev)
+
+
+def host_translate(table, ids, claim, stage_row0, out=None):
+    """ids -> working-set rows of a host table (gs_host_translate): the cache slot, the zero row, or stage_row0 + slot."""
+    ids = _i32(ids.reshape(-1), "ids")
+    if out is None:
+        out = torch.empty_like(ids)
+    check(lib().gs_host_translate(table, ptr(ids), ids.numel(), ptr(claim), int(stage_row0), ptr(out), stream_ptr()))
+    _launched(1 if ids.numel() else 0)
+    return out
+
+
 def _shard_prepare(src, segments):
     """Row addressing for a gather over a parallel.ShardedFeatures: returns (segments, ids_are_locators, staging)."""
     F = src.shape[1]

@@ -68,28 +68,39 @@ def default_cache_rows(n_nodes, world):
     return (int(n_nodes) + 3) // 4 if world > 1 else 0
 
 
-def hot_remote_rows(adj, n_nodes, world, rank, n_rows, row_start=None):
-    """The `n_rows` REMOTE nodes this rank's batches will read most, by the access probabilities the padded table
-    implies for seeds owned by `rank` (owner-computes): hop-1 nodes are the entries of the own rows' adjacency rows,
-    hop-2 nodes the entries of THEIR rows; a node's score is its expected number of reads per seed (hop 1 + hop 2,
-    fanout-weighted 10 and 250).  Returns sorted int64 ids (possibly fewer than n_rows)."""
-    if n_rows <= 0 or world <= 1:
-        return np.zeros(0, dtype=np.int64)
+def expected_reads(adj, n_nodes, lo, hi):
+    """Expected reads of every node [n_nodes] per seed drawn from [lo, hi), by the access probabilities the padded table
+    implies: hop-1 nodes are the entries of the seeds' adjacency rows, hop-2 nodes the entries of THEIR rows; a node's
+    score is hop 1 + hop 2, fanout-weighted 10 and 250.  float64."""
     adj = np.asarray(adj)
     md = adj.shape[1]
-    rs = uniform_bounds(n_nodes, world) if row_start is None else list(row_start)
-    lo, hi = rs[rank], rs[rank + 1]
     p1 = np.bincount(adj[lo:hi].reshape(-1), minlength=n_nodes + 1).astype(np.float64)
     p1 /= max(p1.sum(), 1.0)                                  # P(a hop-1 draw lands on u)
     nz = np.nonzero(p1[:n_nodes])[0]
     p2 = np.bincount(adj[nz].reshape(-1), weights=np.repeat(p1[nz] / md, md), minlength=n_nodes + 1)
-    score = (10.0 * p1 + 250.0 * p2)[:n_nodes]
-    score[lo:hi] = -1.0                                       # own rows need no replica
+    return (10.0 * p1 + 250.0 * p2)[:n_nodes]
+
+
+def top_scored(score, n_rows):
+    """The (at most) n_rows ids of highest positive score, sorted int64."""
     n_rows = int(min(n_rows, int((score > 0).sum())))
-    if n_rows == 0:
+    if n_rows <= 0:
         return np.zeros(0, dtype=np.int64)
     hot = np.argpartition(-score, n_rows - 1)[:n_rows]
     return np.sort(hot).astype(np.int64)
+
+
+def hot_remote_rows(adj, n_nodes, world, rank, n_rows, row_start=None):
+    """The `n_rows` REMOTE nodes this rank's batches will read most, by the access probabilities the padded table
+    implies for seeds owned by `rank` (owner-computes): expected_reads over the own rows.  Returns sorted int64 ids
+    (possibly fewer than n_rows)."""
+    if n_rows <= 0 or world <= 1:
+        return np.zeros(0, dtype=np.int64)
+    rs = uniform_bounds(n_nodes, world) if row_start is None else list(row_start)
+    lo, hi = rs[rank], rs[rank + 1]
+    score = expected_reads(adj, n_nodes, lo, hi)
+    score[lo:hi] = -1.0                                       # own rows need no replica
+    return top_scored(score, n_rows)
 
 
 def locality_order(comm):
@@ -129,24 +140,34 @@ def route_seeds(seeds, n_nodes, group=None, row_start=None):
     return out
 
 
-def hot_remote_rows_csr(indices, n_nodes, world, rank, n_rows, row_start=None, chunk=1 << 27):
-    """Replica choice for a graph held as CSR on the device (no padded table): the `n_rows` remote nodes with the highest
-    in-degree - under uniform neighbour sampling a node is read in proportion to how many adjacency lists contain it.
-    `indices` is the CSR column array (CUDA int32); returns sorted int64 ids on the host."""
-    if n_rows <= 0 or world <= 1:
-        return np.zeros(0, dtype=np.int64)
-    rs = uniform_bounds(n_nodes, world) if row_start is None else list(row_start)
-    lo, hi = rs[rank], rs[rank + 1]
+def in_degrees(indices, n_nodes, chunk=1 << 27):
+    """How many adjacency lists hold each node (int64 [n_nodes] on indices' device), counted in chunks of the CSR column
+    array; under uniform neighbour sampling a node is read in proportion to it."""
     cnt = torch.zeros((n_nodes,), dtype=torch.int64, device=indices.device)
     for i in range(0, indices.numel(), chunk):
         part = indices[i:i + chunk].long()
         cnt += torch.bincount(part.clamp_(0, n_nodes - 1), minlength=n_nodes)
         del part
-    cnt[lo:hi] = -1
-    n_rows = int(min(n_rows, n_nodes - (hi - lo)))
-    hot = torch.topk(cnt, n_rows, sorted=False).indices
+    return cnt
+
+
+def top_counted(cnt, n_rows):
+    """The (at most) n_rows ids of highest positive count (cnt: int64 tensor), sorted int64 on the host."""
+    hot = torch.topk(cnt, int(n_rows), sorted=False).indices
     hot = hot[cnt[hot] > 0]
     return np.sort(hot.cpu().numpy()).astype(np.int64)
+
+
+def hot_remote_rows_csr(indices, n_nodes, world, rank, n_rows, row_start=None, chunk=1 << 27):
+    """Replica choice for a graph held as CSR on the device (no padded table): the `n_rows` remote nodes with the highest
+    in-degree (in_degrees).  `indices` is the CSR column array (CUDA int32); returns sorted int64 ids on the host."""
+    if n_rows <= 0 or world <= 1:
+        return np.zeros(0, dtype=np.int64)
+    rs = uniform_bounds(n_nodes, world) if row_start is None else list(row_start)
+    lo, hi = rs[rank], rs[rank + 1]
+    cnt = in_degrees(indices, n_nodes, chunk)
+    cnt[lo:hi] = -1
+    return top_counted(cnt, min(n_rows, n_nodes - (hi - lo)))
 
 
 def broadcast_parameters(params, src=0, group=None):

@@ -19,6 +19,7 @@ import torch
 
 from . import ops
 from .graphed_training import GraphedTrainStep
+from .host_features import refuse_host_table, stage_layer0
 from .layers import act_code, identity, relu  # noqa: F401
 from .aggregators import (FUSED_POOL_HIDDEN_STEP, FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, TwoMaxLayerPoolingAggregator,
                           fused_pool_fits)
@@ -435,7 +436,8 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
     num_samples = [info.num_samples for info in model.layer_infos]
     L = len(num_samples)
     counts = [n * support[h] for h in range(L + 1)]
-    src = model.features
+    # a host table's layer-0 source is this step's working set, rewritten by the next stage: never the cached bf16 cast
+    src, samples, persistent = stage_layer0(model.features, samples)
     pool = hasattr(model.aggregators[0], "mlp_layers")
     two = isinstance(model.aggregators[0], TwoMaxLayerPoolingAggregator)
     seq = hasattr(model.aggregators[0], "cell")
@@ -459,7 +461,7 @@ def differentiable_outputs(model, batch, normalize=True, dropout=0.):
                 sites = [((key, call[(layer, h, "neigh")], dropout, dev), (key, call[(layer, h, "self")], dropout, dev))
                          for h in range(hops)]
         src = train_layer(model.aggregators[layer], src, layer_segments(samples, counts, num_samples, layer), emb, sites,
-                          fused, layer == 0)
+                          fused, layer == 0 and persistent)
     model.dropout_counter += len(plan)
     out = src[:counts[0]]
     if normalize:
@@ -529,6 +531,11 @@ def embedding_parameters(model):
     return [model.embeds] if getattr(model, "embeds", None) is not None else []
 
 
+def refuse_distributed_host_table(features, distributed):
+    if distributed:
+        refuse_host_table(features, "distributed=True")
+
+
 def refuse_distributed_embeddings(identity_dim, distributed):
     if identity_dim > 0 and distributed:
         raise NotImplementedError("identity_dim > 0 with distributed=True is not implemented (the [N+1, d] table would "
@@ -581,6 +588,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         uses dropout_seed + rank.  fused_pool: train the maxpool / meanpool branch through the fused bf16 kernels
         (_FusedPoolAggregateRowsFn) instead of the materialised fp32 path."""
         refuse_distributed_embeddings(identity_dim, distributed)
+        refuse_distributed_host_table(features, distributed)
         super(SupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                   aggregator_type=aggregator_type, model_size=model_size,
                                                   identity_dim=identity_dim, device=device, **kwargs)

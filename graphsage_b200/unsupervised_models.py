@@ -11,11 +11,12 @@ import torch
 
 from . import ops
 from .graphed_training import GraphedTrainStep
+from .host_features import HostFeatures
 from .models import SampleAndAggregate
 from .prediction import BipartiteEdgePredLayer, mrr_from_affinities
 from .supervised_models import (aggregator_parameters, build_aggregators, check_full_neighbor_dropout, clipped_step,
                                 differentiable_outputs, embedding_parameters, init_dropout, refuse_distributed_embeddings,
-                                refuse_fused_pool, weight_decay_term)
+                                refuse_distributed_host_table, refuse_fused_pool, weight_decay_term)
 
 
 class UnigramNegativeSampler(object):
@@ -44,6 +45,7 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         uses dropout_seed + rank.  fused_pool: train the maxpool / meanpool branch through the fused bf16 kernels (see
         SupervisedGraphsage)."""
         refuse_distributed_embeddings(identity_dim, distributed)
+        refuse_distributed_host_table(features, distributed)
         super(UnsupervisedGraphsage, self).__init__(placeholders, features, adj, degrees, layer_infos, concat=concat,
                                                     aggregator_type=aggregator_type, model_size=model_size,
                                                     identity_dim=identity_dim, device=device, **kwargs)
@@ -57,6 +59,10 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         self.aggregators = build_aggregators(self)
         self.fused_pool = bool(fused_pool)
         refuse_fused_pool(self)
+        if self.fused_pool and isinstance(features, HostFeatures) and features.dtype == torch.bfloat16:
+            # K4's backward reads the bf16 working set itself, and the negatives' pass restages it before the backward
+            raise NotImplementedError("fused_pool=True in the unsupervised model with a bfloat16 host-memory "
+                                      "(HostFeatures) table is not implemented")
         dim_mult = 2 if self.concat else 1
         self.link_pred_layer = BipartiteEdgePredLayer(dim_mult * self.dims[-1], dim_mult * self.dims[-1], placeholders,
                                                       neg_sample_weights=self.neg_sample_weights, bilinear_weights=False,

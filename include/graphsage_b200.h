@@ -236,6 +236,30 @@ int32_t gs_ipc_export(const void* dev_ptr, uint8_t* handle64_out_host);
 int32_t gs_ipc_import(const uint8_t* handle64_host, void** dev_ptr_out);
 int32_t gs_ipc_close(void* dev_ptr);
 
+/* ---------------------------------------------------------------------------------------------
+ * Feature table in host memory (graphsage_b200.HostFeatures).  The [N+1, pitch] rows stay in page-locked host memory
+ * that the device addresses directly; per step the rows the batch reads are staged into a device "working set"
+ *   [C cached rows | 1 zero row | S staging rows]     (one contiguous table, the host table's pitch and dtype)
+ * and layer 0 runs on it with translated ids.  The hit test is the halo one with a single shard: describe the working
+ * set as a gs_sharded_table with n_shards = 1, row_start = {0, N}, base[0] = the working set, zero_row = C and
+ * remap = cache_slot (device int32 [N+1]: the working-set row of a cached id, -1 otherwise).  Per step:
+ *   gs_halo_begin  ->  gs_halo_claim per id list (every distinct uncached id in [0, N) takes the next staging slot)
+ *   ->  gs_host_fetch (rows stage_ids[0 .. *count) from the host table into the staging rows)
+ *   ->  gs_host_translate per id list.
+ * No step reads *count on the host: every launch size follows from the batch shape, so the sequence is capturable. */
+/* Page-lock host_ptr[0 .. bytes) once, mapped into the device address space; *dev_alias_out is the address the kernels
+ * read it through.  gs_host_unregister undoes it (the memory itself stays the caller's). */
+int32_t gs_host_register(void* host_ptr, int64_t bytes, void** dev_alias_out);
+int32_t gs_host_unregister(void* host_ptr);
+/* staging[i] = host_alias[stage_ids[i]] for i in [0, min(*count, capacity)): whole rows of row_bytes (a multiple of 16)
+ * over the host link with 16-byte loads, several rows in flight per warp.  The grid does not depend on *count. */
+int32_t gs_host_fetch(const void* host_alias, int64_t row_bytes, const int32_t* stage_ids, const int32_t* count,
+                      int64_t capacity, void* staging, void* stream);
+/* gs_halo_translate with non-negative rows: out[i] = the working-set row of ids[i] - remap[id] for a cached id, zero_row
+ * for an id outside [0, N), stage_row0 + claim[id] for a staged one. */
+int32_t gs_host_translate(const gs_sharded_table* table_host, const int32_t* ids, int64_t n, const int32_t* claim,
+                          int64_t stage_row0, int32_t* out, void* stream);
+
 /* embedding_lookup (models.py:299) with the result widened to fp32: out[i, 0:F] = (float)feats[ids ? ids[i] : row0 + i, 0:F],
  * columns F..out_pitch-1 zeroed.  feats is GS_BF16 or GS_F32.  The bf16 max-pool path uses it for the SELF rows, which
  * meet the fp32 self_weights contraction (aggregators.py:185). */
