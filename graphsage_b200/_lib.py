@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgraphsage_b200.so")
 
 ABI_VERSION = 2          # GS_ABI_VERSION of include/graphsage_b200.h this binding was written against
-GS_F32, GS_BF16, GS_F64 = 0, 1, 2
+GS_F32, GS_BF16, GS_F64, GS_I8ROW = 0, 1, 2, 3
 ACT_NONE, ACT_RELU = 0, 1
 COMBINE_ADD, COMBINE_CONCAT = 0, 1
 MATH_FP32_SIMT, MATH_TF32X3, MATH_TF32, MATH_BF16 = 0, 1, 2, 3
@@ -97,6 +97,8 @@ _SIGNATURES = {
     "gs_host_translate": (c_i32, [ctypes.POINTER(ShardedTable), c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_gather_rows_f32": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp]),
     "gs_cast_rows_bf16": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp]),
+    "gs_i8row_pitch": (c_i64, [c_i32]),
+    "gs_quantize_rows_i8": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp]),
     "gs_rmat_degrees": (c_i32, [c_i32, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                 ctypes.c_double, c_u64, c_u64, c_u64, c_u64, c_vp, c_vp]),
     "gs_rmat_fill": (c_i32, [c_i32, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u64, c_u64,
@@ -112,6 +114,8 @@ _SIGNATURES = {
                                   c_vp, c_i64, c_vp, c_vp]),
     "gs_sage_layer_small": (c_i32, [c_vp, c_i64, c_i32, c_i64, ctypes.POINTER(Segment), c_i32, ctypes.POINTER(GemmPart),
                                     c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_i64, c_vp, c_u64, c_vp]),
+    "gs_sage_layer_small_i8": (c_i32, [c_vp, c_i64, c_i32, c_i64, ctypes.POINTER(Segment), c_i32, ctypes.POINTER(GemmPart),
+                                       c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_i64, c_vp, c_u64, c_vp]),
     "gs_maxpool_mlp_workspace_bytes": (c_i64, [c_i32, c_i32]),
     "gs_maxpool_mlp_pack": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "gs_maxpool_mlp_fused": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64,

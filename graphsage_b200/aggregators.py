@@ -91,7 +91,7 @@ class _SageAggregator(Layer):
     def _small_layer(self, src, segments, parts, combine, include_self, final):
         """Whole layer in one launch when it is small (last layers: B rows).  Returns None if not applicable."""
         code, post = act_code(self.act)
-        if (len(segments) != 1 or not torch.is_tensor(src) or post is not None or self.dropout
+        if (len(segments) != 1 or not (torch.is_tensor(src) or isinstance(src, ops.I8Rows)) or post is not None or self.dropout
                 or segments[0].out_row0 + segments[0].n > ops.SMALL_LAYER_MAX_ROWS or src.shape[1] > 2048
                 or any(K != src.shape[1] for (_, K, _) in parts)
                 or (sum(B.shape[1] for (_, _, B) in parts) if combine == ops.COMBINE_CONCAT else parts[0][2].shape[1]) > 1024):
@@ -285,11 +285,11 @@ class MaxPoolingAggregator(_SageAggregator):
                               row0=s.neigh_row0, K=self.neigh_input_dim, out=out, pool=self.pool)
 
     def _pooled_parts(self, src, segments, kept=None, sites=None):
-        """The GEMM parts of the materialised form: per hop the neighbour rows (widened to fp32 from a bf16 table), then
+        """The GEMM parts of the materialised form: per hop the neighbour rows (widened to fp32 from a bf16 or int8 table), then
         the MLP and the pooling kernel.  With training dropout each Dense layer's input is masked first: sites[hop] is
         the one site of a one-layer MLP, the (mlp, mlp2) pair of a two-layer one.  `kept` (training) receives each hop's
         Dense inputs (as masked) and the last Dense's output."""
-        widen = torch.is_tensor(src) and src.dtype != torch.float32
+        widen = (torch.is_tensor(src) or isinstance(src, ops.I8Rows)) and src.dtype != torch.float32
 
         def hop(i, s, out):
             h = _rows(src, s.neigh_ids, s.neigh_row0, s.n * s.k, widen)

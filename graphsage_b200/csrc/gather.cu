@@ -408,16 +408,51 @@ __global__ void __launch_bounds__(192, 3) gather_mean_tma2_kernel(const __grid_c
 }
 
 // ------------------------------------------------------------------------------------------
-// gather + mean over a BFLOAT16 table (BASELINE.md's 160.9 MB bf16 gather yardstick): the structure of
-// gather_mean_tma2_kernel - whole rows (1,216 B at F = 602) fetched by cp.async.bulk in groups of kGroupRows through a
-// two-buffer ring - with the rows widened to fp32 as they are summed (fp32 accumulate, j order, like the fp32 kernel), so
-// the result equals the fp32 kernel's on the bf16-rounded table.  A thread owns 8 columns (one 128-bit shared load).
+// gather + mean over a NARROW row table: the structure of gather_mean_tma2_kernel - whole rows fetched by cp.async.bulk in
+// groups of kGroupRows through a two-buffer ring - with the rows widened to fp32 as they are summed (fp32 accumulate, j
+// order, self row last, like the fp32 kernel), so the result equals the fp32 kernel's on the widened table.  A thread owns
+// 8 columns.  Fmt is the row format: Fmt::T the table's element type (pitch counts them), Fmt::load the widening of a
+// thread's 8 columns of one staged row.
+//   Bf16Cols : bfloat16 rows (BASELINE.md's 160.9 MB bf16 gather yardstick; 1,216 B at F = 602), one 128-bit shared load.
+//   I8RowCols: GS_I8ROW rows (608 B at F = 602): 8 int8 values (two 32-bit shared loads) times the row's fp32 scale, read
+//              from the staged row itself - deq = fl(float(q) * s), never contracted into the sum.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(192) gather_mean_bf16_tma2_kernel(const uint16_t* __restrict__ src, int64_t n_src_rows, int F,
-                                                                    int64_t pitch, const __grid_constant__ SegTable tab,
-                                                                    int include_self, float* __restrict__ out_self,
-                                                                    float* __restrict__ out_mean, int64_t out_pitch,
-                                                                    int row_bytes) {
+struct Bf16Cols {
+  using T = uint16_t;
+  __device__ static __forceinline__ void load(const uint4* row, int c, int /*F*/, float (&v)[8]) {
+    const uint4 u = row[c];
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      v[2 * e] = __uint_as_float(w[e] << 16);
+      v[2 * e + 1] = __uint_as_float(w[e] & 0xffff0000u);
+    }
+  }
+};
+
+__device__ __forceinline__ float i8row_scale(const unsigned char* row, int F) {
+  return *reinterpret_cast<const float*>(row + ((F + 3) & ~3));
+}
+
+struct I8RowCols {
+  using T = uint8_t;
+  __device__ static __forceinline__ void load(const uint4* row, int c, int F, float (&v)[8]) {
+    const unsigned char* b = reinterpret_cast<const unsigned char*>(row);
+    const float s = i8row_scale(b, F);
+    const char4 lo = reinterpret_cast<const char4*>(b)[2 * c], hi = reinterpret_cast<const char4*>(b)[2 * c + 1];
+    v[0] = __fmul_rn((float)lo.x, s); v[1] = __fmul_rn((float)lo.y, s); v[2] = __fmul_rn((float)lo.z, s);
+    v[3] = __fmul_rn((float)lo.w, s); v[4] = __fmul_rn((float)hi.x, s); v[5] = __fmul_rn((float)hi.y, s);
+    v[6] = __fmul_rn((float)hi.z, s); v[7] = __fmul_rn((float)hi.w, s);
+  }
+};
+
+template <class Fmt>
+__global__ void __launch_bounds__(192) gather_mean_narrow_tma2_kernel(const typename Fmt::T* __restrict__ src,
+                                                                      int64_t n_src_rows, int F, int64_t pitch,
+                                                                      const __grid_constant__ SegTable tab,
+                                                                      int include_self, float* __restrict__ out_self,
+                                                                      float* __restrict__ out_mean, int64_t out_pitch,
+                                                                      int row_bytes) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t bar[2];
   if (threadIdx.x == 0) {
@@ -454,14 +489,6 @@ __global__ void __launch_bounds__(192) gather_mean_bf16_tma2_kernel(const uint16
     if (first + cnt >= rows_total) { r_issue += gridDim.x; g_issue = 0; } else { ++g_issue; }
     return true;
   };
-  auto widen = [](uint4 u, float (&v)[8]) {
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      v[2 * e] = __uint_as_float(w[e] << 16);
-      v[2 * e + 1] = __uint_as_float(w[e] & 0xffff0000u);
-    }
-  };
   uint32_t phase[2] = {0u, 0u};
   int buf = 0;
   bool have = issue(0);
@@ -487,7 +514,7 @@ __global__ void __launch_bounds__(192) gather_mean_bf16_tma2_kernel(const uint16
     if (c < ncol8 && c * 8 < F) {
       for (int j = 0; j < nn; ++j) {
         float v[8];
-        widen(rows[j * row_u4 + c], v);
+        Fmt::load(rows + j * row_u4, c, F, v);
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc[e] += v[e];
       }
@@ -499,7 +526,7 @@ __global__ void __launch_bounds__(192) gather_mean_bf16_tma2_kernel(const uint16
 #pragma unroll
         for (int e = 0; e < 8; ++e) { a[e] = 0.f; sv[e] = 0.f; }
         if (c * 8 < F) {
-          widen(rows[(cnt - 1) * row_u4 + c], sv);
+          Fmt::load(rows + (cnt - 1) * row_u4, c, F, sv);
           const float div = (float)(k + (include_self ? 1 : 0));
 #pragma unroll
           for (int e = 0; e < 8; ++e) {
@@ -628,6 +655,56 @@ __global__ void __launch_bounds__(256) gather_rows_bf16_to_f32_vec_kernel(const 
       }
       op[2 * c] = make_float4(v[0], v[1], v[2], v[3]);
       op[2 * c + 1] = make_float4(v[4], v[5], v[6], v[7]);
+    }
+  }
+}
+
+// rows of a GS_I8ROW table widened to fp32: out[i, c] = fl(float(q_c) * s) of row ids[i] (or row0 + i), pad columns zeroed -
+// the values every int8 reader produces.  One warp per row; pitch in bytes.
+__global__ void __launch_bounds__(256) gather_rows_i8row_to_f32_kernel(const uint8_t* __restrict__ src, int64_t n_rows, int F,
+                                                                       int64_t pitch, const int32_t* __restrict__ ids,
+                                                                       int64_t row0, int64_t n, float* __restrict__ out,
+                                                                       int64_t out_pitch) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t i = warp; i < n; i += nwarps) {
+    const uint8_t* row = src + clamp_row(ids ? (int64_t)ids[i] : row0 + i, n_rows) * pitch;
+    const float s = i8row_scale(row, F);
+    for (int c = lane; c < (int)out_pitch; c += 32)
+      out[i * out_pitch + c] = c < F ? __fmul_rn((float)(int8_t)row[c], s) : 0.f;
+  }
+}
+
+// fp32 rows -> GS_I8ROW rows (contract: include/graphsage_b200.h, oracle/int8_rows.py).  One warp per row: the absmax by a
+// shuffle reduction (exact), s = fl(a / 127), q_c = clamp(rint(fl(x_c / s)), -127, 127) - IEEE division and round half to
+// even, so numpy restates every byte - then the row is written whole, padding and scale included.
+__global__ void __launch_bounds__(256) quantize_rows_i8_kernel(const float* __restrict__ x, int64_t n, int F, int64_t ldx,
+                                                               uint8_t* __restrict__ out, int64_t out_pitch) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int p4 = (F + 3) & ~3;
+  for (int64_t i = warp; i < n; i += nwarps) {
+    const float* xr = x + i * ldx;
+    float a = 0.f;
+    for (int c = lane; c < F; c += 32) a = fmaxf(a, fabsf(xr[c]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    const float s = __fdiv_rn(a, 127.f);
+    const uint32_t sbits = __float_as_uint(s);
+    uint8_t* orow = out + i * out_pitch;
+    for (int c = lane; c < (int)out_pitch; c += 32) {
+      uint32_t b = 0u;
+      if (c < F) {
+        if (s != 0.f) {
+          const float t = fminf(fmaxf(rintf(__fdiv_rn(xr[c], s)), -127.f), 127.f);
+          b = (uint32_t)(int32_t)t & 0xffu;
+        }
+      } else if (c >= p4 && c < p4 + 4) {
+        b = (sbits >> (8 * (c - p4))) & 0xffu;              // the scale, little-endian
+      }
+      orow[c] = (uint8_t)b;
     }
   }
 }
@@ -920,6 +997,31 @@ static int32_t launch_gather_tma2(const Rows& rows_of, int F, const SegTable& ta
                                                                                  drop ? *drop : no_drop);
   return launch_check("gather_mean_tma2_kernel");
 }
+
+// launch of the narrow-row gather (bf16 or int8 rows of row_bytes, 16-byte multiples; out_pitch / 8 <= 192 threads)
+template <class Fmt>
+static int32_t launch_gather_narrow(const typename Fmt::T* src, int64_t n_src_rows, int F, int64_t pitch, const SegTable& tab,
+                                    int include_self, void* out_self, void* out_mean, int64_t out_pitch, int row_bytes,
+                                    cudaStream_t st) {
+  const int32_t rc_attr = ensure_dyn_smem((const void*)gather_mean_narrow_tma2_kernel<Fmt>, 200 * 1024);
+  if (rc_attr != GS_OK) return rc_attr;
+  const size_t smem2 = (size_t)2 * kGroupRows * row_bytes;
+  const int ncol8 = (int)(out_pitch / 8);
+  int threads = ((ncol8 + 31) / 32) * 32;
+  if (threads < 32) threads = 32;
+  GS_REQUIRE(threads <= 192, "gs_gather_mean: out_pitch too wide for a narrow-row table");
+  int per_sm = (int)((224 * 1024) / (smem2 + 1024));
+  if (per_sm < 1) per_sm = 1;
+  int lim = tuning("gather_ctas_per_sm", 8);
+  if (per_sm > lim) per_sm = lim;
+  int64_t blocks = tab.total_rows;
+  int64_t cap = (int64_t)sm_count() * per_sm;
+  if (blocks > cap) blocks = cap;
+  gather_mean_narrow_tma2_kernel<Fmt><<<(unsigned)blocks, threads, smem2, st>>>(src, n_src_rows, F, pitch, tab, include_self,
+                                                                                (float*)out_self, (float*)out_mean, out_pitch,
+                                                                                row_bytes);
+  return launch_check("gather_mean_narrow_tma2_kernel");
+}
 }  // namespace gs
 
 // copies the caller's segments into `tab`, checks each one and sums total_rows; raises *kmax (if given) to the largest fanout
@@ -981,7 +1083,8 @@ int32_t gs_gather_rows(const void* feats, int32_t dtype, int64_t n_rows, int32_t
 int32_t gs_gather_mean(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
                        const gs_segment* segments_host, int32_t n_segments, int32_t include_self, void* out_self,
                        void* out_mean, int64_t out_pitch, void* stream) {
-  GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16, "gs_gather_mean: dtype %d (GS_F32 or GS_BF16)", dtype);
+  GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16 || dtype == GS_I8ROW, "gs_gather_mean: dtype %d (GS_F32, GS_BF16 or GS_I8ROW)",
+             dtype);
   GS_REQUIRE(n_segments >= 0 && n_segments <= GS_MAX_SEGMENTS, "gs_gather_mean: n_segments=%d (max %d)", n_segments,
              GS_MAX_SEGMENTS);
   GS_REQUIRE(segments_host || n_segments == 0, "gs_gather_mean: segments_host is NULL");
@@ -1001,25 +1104,20 @@ int32_t gs_gather_mean(const void* src, int32_t dtype, int64_t n_src_rows, int32
       gs::set_error("gs_gather_mean(GS_BF16): needs 16-byte aligned rows (pitch %% 8 == 0), out_pitch %% 8 == 0 and F <= 1536");
       return GS_ERR_UNSUPPORTED;
     }
-    const int32_t rc_attr = gs::ensure_dyn_smem((const void*)gs::gather_mean_bf16_tma2_kernel, 200 * 1024);
-    if (rc_attr != GS_OK) return rc_attr;
-    const int row_bytes = (int)(f8 * 2);
-    const size_t smem2 = (size_t)2 * gs::kGroupRows * row_bytes;
-    const int ncol8 = (int)(out_pitch / 8);
-    int threads = ((ncol8 + 31) / 32) * 32;
-    if (threads < 32) threads = 32;
-    GS_REQUIRE(threads <= 192, "gs_gather_mean(GS_BF16): out_pitch too wide");
-    int per_sm = (int)((224 * 1024) / (smem2 + 1024));
-    if (per_sm < 1) per_sm = 1;
-    int lim = gs::tuning("gather_ctas_per_sm", 8);
-    if (per_sm > lim) per_sm = lim;
-    int64_t blocks = tab.total_rows;
-    int64_t cap = (int64_t)gs::sm_count() * per_sm;
-    if (blocks > cap) blocks = cap;
-    gs::gather_mean_bf16_tma2_kernel<<<(unsigned)blocks, threads, smem2, st>>>((const uint16_t*)src, n_src_rows, F, pitch, tab,
-                                                                              include_self, (float*)out_self, (float*)out_mean,
-                                                                              out_pitch, row_bytes);
-    return gs::launch_check("gather_mean_bf16_tma2_kernel");
+    return gs::launch_gather_narrow<gs::Bf16Cols>((const uint16_t*)src, n_src_rows, F, pitch, tab, include_self, out_self,
+                                                  out_mean, out_pitch, (int)(f8 * 2), st);
+  }
+  if (dtype == GS_I8ROW) {
+    // int8 rows with their scale: whole pitch-byte rows by bulk copy, dequantised in registers (pitch counts bytes)
+    const int64_t rb = gs_i8row_pitch(F);
+    if (!(gs::aligned16(src) && gs::aligned16(out_mean) && (!out_self || gs::aligned16(out_self)) && pitch % 16 == 0 &&
+          rb <= pitch && out_pitch % 8 == 0 && out_pitch <= 1536)) {
+      gs::set_error("gs_gather_mean(GS_I8ROW): needs 16-byte aligned rows of pitch %% 16 == 0 and >= gs_i8row_pitch(F), "
+                    "out_pitch %% 8 == 0 and <= 1536");
+      return GS_ERR_UNSUPPORTED;
+    }
+    return gs::launch_gather_narrow<gs::I8RowCols>((const uint8_t*)src, n_src_rows, F, pitch, tab, include_self, out_self,
+                                                   out_mean, out_pitch, (int)rb, st);
   }
   const float* fsrc = (const float*)src;
   const bool vec_ok = gs::aligned16(src) && gs::aligned16(out_mean) && (!out_self || gs::aligned16(out_self)) &&
@@ -1078,11 +1176,18 @@ int32_t gs_gather_rows_f32(const void* feats, int32_t dtype, int64_t n_rows, int
   GS_REQUIRE(n >= 0 && F >= 0, "gs_gather_rows_f32: negative size");
   if (n == 0 || out_pitch == 0) return GS_OK;
   GS_REQUIRE(feats && out, "gs_gather_rows_f32: NULL pointer");
-  GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16, "gs_gather_rows_f32: dtype %d", dtype);
+  GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16 || dtype == GS_I8ROW, "gs_gather_rows_f32: dtype %d", dtype);
   GS_REQUIRE(n_rows > 0 && pitch >= F && out_pitch >= F, "gs_gather_rows_f32: pitch < F");
   int64_t blocks = (n + 7) / 8;
   int64_t cap = (int64_t)gs::sm_count() * 8;
   if (blocks > cap) blocks = cap;
+  if (dtype == GS_I8ROW) {
+    GS_REQUIRE(pitch >= gs_i8row_pitch(F) && gs::aligned16(feats) && pitch % 16 == 0,
+               "gs_gather_rows_f32(GS_I8ROW): needs 16-byte aligned rows of pitch %% 16 == 0 and >= gs_i8row_pitch(F)");
+    gs::gather_rows_i8row_to_f32_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+        (const uint8_t*)feats, n_rows, F, pitch, ids, row0, n, out, out_pitch);
+    return gs::launch_check("gather_rows_i8row_to_f32_kernel");
+  }
   if (dtype == GS_F32)
     gs::gather_rows_to_f32_kernel<float><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
         (const float*)feats, n_rows, F, pitch, ids, row0, n, out, out_pitch);
@@ -1093,6 +1198,28 @@ int32_t gs_gather_rows_f32(const void* feats, int32_t dtype, int64_t n_rows, int
     gs::gather_rows_to_f32_kernel<uint16_t><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
         (const uint16_t*)feats, n_rows, F, pitch, ids, row0, n, out, out_pitch);
   return gs::launch_check("gather_rows_to_f32_kernel");
+}
+
+int64_t gs_i8row_pitch(int32_t F) {
+  if (F < 1) return 0;
+  const int64_t p4 = ((int64_t)F + 3) / 4 * 4;
+  return (p4 + 4 + 15) / 16 * 16;
+}
+
+int32_t gs_quantize_rows_i8(const float* x, int64_t n, int32_t F, int64_t ldx, void* out, int64_t out_pitch_bytes,
+                            void* stream) {
+  GS_REQUIRE(n >= 0 && F >= 1 && ldx >= F, "gs_quantize_rows_i8: bad sizes (n=%lld F=%d ldx=%lld)", (long long)n, F,
+             (long long)ldx);
+  GS_REQUIRE(out_pitch_bytes >= gs_i8row_pitch(F) && out_pitch_bytes % 16 == 0,
+             "gs_quantize_rows_i8: out_pitch_bytes must be a multiple of 16 and >= gs_i8row_pitch(F) = %lld",
+             (long long)gs_i8row_pitch(F));
+  if (n == 0) return GS_OK;
+  GS_REQUIRE(x && out, "gs_quantize_rows_i8: NULL pointer");
+  int64_t blocks = (n + 7) / 8;
+  int64_t cap = (int64_t)gs::sm_count() * 8;
+  if (blocks > cap) blocks = cap;
+  gs::quantize_rows_i8_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, n, F, ldx, (uint8_t*)out, out_pitch_bytes);
+  return gs::launch_check("quantize_rows_i8_kernel");
 }
 
 int32_t gs_cast_rows_bf16(const float* x, int64_t n, int32_t F, int64_t ldx, void* out_bf16, int64_t out_pitch,

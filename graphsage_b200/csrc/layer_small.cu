@@ -26,12 +26,27 @@ struct LsParams {
   uint64_t* counter_dev;
   uint64_t counter_inc;
   int32_t vec;          // everything 16-byte friendly: 128-bit loads in both phases
+  const uint8_t* src_i8;  // GS_I8ROW table (gs_sage_layer_small_i8; pitch in bytes), else NULL
 };
 
 __device__ __forceinline__ int64_t ls_clamp(int64_t id, int64_t n) { return (id < 0 || id >= n) ? n - 1 : id; }
 
+// element c of source row `row`: the fp32 value, or (kI8) the dequantised fl(float(q_c) * s) of an int8 row
+template <bool kI8>
+__device__ __forceinline__ float ls_load(const LsParams& prm, int64_t row, int c) {
+  if constexpr (kI8) {
+    const uint8_t* r = prm.src_i8 + row * prm.pitch;
+    return __fmul_rn((float)(int8_t)r[c], *reinterpret_cast<const float*>(r + ((prm.F + 3) & ~3)));
+  } else {
+    return prm.src[row * prm.pitch + c];
+  }
+}
+
 // Latency is the enemy here (one CTA per SM, a few rows each): every load batch is made of
 // independent loads (LS_ROWS rows x 5 neighbours in phase 1, 8 weight rows x K-slices in phase 2).
+// kI8: the source is a GS_I8ROW table, read by the scalar phase 1 (its per-column sums are those of the vector one);
+// phase 2 follows prm.vec as for the fp32 table
+template <bool kI8>
 __global__ void __launch_bounds__(LS_THREADS) sage_layer_small_kernel(const __grid_constant__ LsParams prm) {
   extern __shared__ float sm[];     // xs[LS_ROWS][F] | xm[LS_ROWS][F] | part[nslices][LS_ROWS][ncolp] | red[LS_ROWS][16]
   const int F = prm.F;
@@ -41,7 +56,7 @@ __global__ void __launch_bounds__(LS_THREADS) sage_layer_small_kernel(const __gr
   const int k = sg.k;
   const int64_t row0 = (int64_t)blockIdx.x * LS_ROWS;
   // ---- phase 1: self rows and fanout means into shared memory
-  if (prm.vec) {
+  if (!kI8 && prm.vec) {
     // thread = (row, float4 column); neighbours in independent batches of 5 x 128-bit loads
     const int f4 = F >> 2;
     for (int p = threadIdx.x; p < f4 * LS_ROWS; p += LS_THREADS) {
@@ -82,7 +97,7 @@ __global__ void __launch_bounds__(LS_THREADS) sage_layer_small_kernel(const __gr
       sv[r] = 0.f;
       if (i < sg.n) {
         const int64_t srow = ls_clamp(sg.self_ids ? (int64_t)sg.self_ids[i] : sg.self_row0 + i, prm.n_src_rows);
-        sv[r] = prm.src[srow * prm.pitch + c];
+        sv[r] = ls_load<kI8>(prm, srow, c);
       }
     }
     for (int j0 = 0; j0 < k; j0 += 5) {
@@ -96,7 +111,7 @@ __global__ void __launch_bounds__(LS_THREADS) sage_layer_small_kernel(const __gr
           if (i < sg.n && j0 + u < k) {
             const int64_t nr = ls_clamp(sg.neigh_ids ? (int64_t)sg.neigh_ids[i * k + j0 + u] : sg.neigh_row0 + i * k + j0 + u,
                                         prm.n_src_rows);
-            v[r][u] = prm.src[nr * prm.pitch + c];
+            v[r][u] = ls_load<kI8>(prm, nr, c);
           }
         }
       }
@@ -261,14 +276,16 @@ __global__ void __launch_bounds__(LS_THREADS) sage_layer_small_kernel(const __gr
 
 }  // namespace gs
 
-extern "C" int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int32_t F, int64_t pitch,
-                                       const gs_segment* segment_host, int32_t include_self,
-                                       const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
-                                       int32_t act, int32_t l2_normalize, float* out, int64_t ldo, uint64_t* counter_dev,
-                                       uint64_t counter_inc, void* stream) {
+static int32_t sage_layer_small(const void* src, bool i8, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                const gs_segment* segment_host, int32_t include_self, const gs_gemm_part* parts_host,
+                                int32_t n_parts, int32_t combine, const float* bias, int32_t act, int32_t l2_normalize, float* out,
+                                int64_t ldo, uint64_t* counter_dev, uint64_t counter_inc, void* stream) {
   GS_REQUIRE(src && segment_host && parts_host && out, "gs_sage_layer_small: NULL pointer");
   GS_REQUIRE(n_parts == 1 || n_parts == 2, "gs_sage_layer_small: n_parts=%d", n_parts);
   GS_REQUIRE(F >= 1 && F <= 2048 && pitch >= F && n_src_rows > 0, "gs_sage_layer_small: F=%d (max 2048) / pitch", F);
+  if (i8)
+    GS_REQUIRE(pitch % 16 == 0 && pitch >= gs_i8row_pitch(F) && (reinterpret_cast<uintptr_t>(src) & 15u) == 0,
+               "gs_sage_layer_small_i8: needs 16-byte aligned rows of pitch %% 16 == 0 and >= gs_i8row_pitch(F)");
   GS_REQUIRE(segment_host->k >= 1 && segment_host->n >= 0, "gs_sage_layer_small: bad segment");
   GS_REQUIRE(combine == GS_COMBINE_ADD || combine == GS_COMBINE_CONCAT, "gs_sage_layer_small: combine=%d", combine);
   GS_REQUIRE(act == GS_ACT_NONE || act == GS_ACT_RELU, "gs_sage_layer_small: act=%d", act);
@@ -285,11 +302,14 @@ extern "C" int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int
   ntot = parts_host[0].N + ((n_parts == 2 && combine == GS_COMBINE_CONCAT) ? parts_host[1].N : 0);
   GS_REQUIRE(ntot <= 1024 && ldo >= ntot, "gs_sage_layer_small: output width %d (max 1024) / ldo", ntot);
   if (segment_host->n == 0) return GS_OK;
-  prm.src = src; prm.n_src_rows = n_src_rows; prm.pitch = pitch; prm.F = F;
+  prm.src = i8 ? nullptr : (const float*)src; prm.src_i8 = i8 ? (const uint8_t*)src : nullptr;
+  prm.n_src_rows = n_src_rows; prm.pitch = pitch; prm.F = F;
   prm.seg = *segment_host; prm.include_self = include_self;
   prm.n_parts = n_parts; prm.combine = combine; prm.bias = bias; prm.act = act; prm.l2norm = l2_normalize;
   prm.out = out; prm.ldo = ldo; prm.counter_dev = counter_dev; prm.counter_inc = counter_inc;
-  bool vec = (F % 4 == 0) && (pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(src) & 15u) == 0) && (ntot % 4 == 0) &&
+  // an int8 table stands for its dequantised fp32 twin with an aligned pitch that is a multiple of 4 floats, so only the
+  // conditions that do not depend on the source layout decide here
+  bool vec = (F % 4 == 0) && (i8 || ((pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(src) & 15u) == 0))) && (ntot % 4 == 0) &&
              (parts_host[0].N % 4 == 0);
   for (int i = 0; i < n_parts; ++i)
     vec = vec && (parts_host[i].ldb % 4 == 0) && ((reinterpret_cast<uintptr_t>(parts_host[i].B) & 15u) == 0);
@@ -300,11 +320,33 @@ extern "C" int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int
                           : (ncolp <= gs::LS_THREADS ? gs::LS_THREADS / ncolp : 1);
   const size_t smem = (size_t)(2 * gs::LS_ROWS * F + nslices * gs::LS_ROWS * ncolp + gs::LS_ROWS * 16) * sizeof(float);
   GS_REQUIRE(smem <= 200 * 1024, "gs_sage_layer_small: needs %zu bytes of shared memory", smem);
+  const void* kernel = i8 ? (const void*)gs::sage_layer_small_kernel<true> : (const void*)gs::sage_layer_small_kernel<false>;
   {
-    const int32_t rc_attr = gs::ensure_dyn_smem((const void*)gs::sage_layer_small_kernel, 200 * 1024);
+    const int32_t rc_attr = gs::ensure_dyn_smem(kernel, 200 * 1024);
     if (rc_attr != GS_OK) return rc_attr;
   }
   unsigned blocks = (unsigned)((segment_host->n + gs::LS_ROWS - 1) / gs::LS_ROWS);
-  gs::sage_layer_small_kernel<<<blocks, gs::LS_THREADS, smem, (cudaStream_t)stream>>>(prm);
+  if (i8)
+    gs::sage_layer_small_kernel<true><<<blocks, gs::LS_THREADS, smem, (cudaStream_t)stream>>>(prm);
+  else
+    gs::sage_layer_small_kernel<false><<<blocks, gs::LS_THREADS, smem, (cudaStream_t)stream>>>(prm);
   return gs::launch_check("sage_layer_small_kernel");
+}
+
+extern "C" int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                       const gs_segment* segment_host, int32_t include_self,
+                                       const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
+                                       int32_t act, int32_t l2_normalize, float* out, int64_t ldo, uint64_t* counter_dev,
+                                       uint64_t counter_inc, void* stream) {
+  return sage_layer_small(src, false, n_src_rows, F, pitch, segment_host, include_self, parts_host, n_parts, combine, bias, act,
+                          l2_normalize, out, ldo, counter_dev, counter_inc, stream);
+}
+
+extern "C" int32_t gs_sage_layer_small_i8(const void* src, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                          const gs_segment* segment_host, int32_t include_self,
+                                          const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine, const float* bias,
+                                          int32_t act, int32_t l2_normalize, float* out, int64_t ldo, uint64_t* counter_dev,
+                                          uint64_t counter_inc, void* stream) {
+  return sage_layer_small(src, true, n_src_rows, F, pitch, segment_host, include_self, parts_host, n_parts, combine, bias, act,
+                          l2_normalize, out, ldo, counter_dev, counter_inc, stream);
 }

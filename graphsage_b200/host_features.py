@@ -58,11 +58,13 @@ def _check_cache_ids(cache_ids, n_nodes):
 
 
 class HostFeatures(object):
-    """A [N+1, F] float32 or bfloat16 feature table in page-locked host memory, usable wherever SampleAndAggregate,
+    """A [N+1, F] float32, bfloat16 or int8 feature table in page-locked host memory, usable wherever SampleAndAggregate,
     SupervisedGraphsage and UnsupervisedGraphsage take `features`.
 
     table     : CPU tensor or numpy array [N+1, F]; its last row is the all-zero dummy row, as for a device table.  It is
-                copied once into a host buffer of pitch ops.pad_cols(F) (16-byte rows), which is pinned and mapped.
+                copied once into a host buffer of pitch ops.pad_cols(F) (16-byte rows), which is pinned and mapped.  Or an
+                Int8Features table whose rows are on the CPU: its byte rows (scale included) are pinned in place, staged
+                whole, and layer 0 reads the working set as an int8 table.
     cache_ids : sorted, unique int64 ids in [0, N) whose rows are copied into device memory once and served from there
                 (hot_rows picks them); None caches nothing.
     device    : the GPU the working set lives on (default: the current one).
@@ -72,25 +74,33 @@ class HostFeatures(object):
     the pinned memory."""
 
     def __init__(self, table, cache_ids=None, device=None):
-        t = table if torch.is_tensor(table) else torch.from_numpy(np.asarray(table))
-        if t.is_cuda:
-            raise ValueError("HostFeatures takes a host (CPU) table; a CUDA table is used as features directly")
-        if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < 1:
-            raise ValueError("the table must be a 2-D [N+1, F] array with F >= 1")
-        if t.dtype not in (torch.float32, torch.bfloat16):
-            raise TypeError("the table must be float32 or bfloat16 (got %s)" % t.dtype)
-        if bool((t[-1] != 0).any()):
-            raise ValueError("the table's last row is the dummy row and must be all zero")
-        self.n_nodes, F = int(t.shape[0]) - 1, int(t.shape[1])
+        if isinstance(table, ops.I8Rows):            # Int8Features: rows of bytes, each holding its scale
+            if table.rows.is_cuda:
+                raise ValueError("HostFeatures takes a host (CPU) table; a CUDA Int8Features table is used as features "
+                                 "directly")
+            self.n_nodes, F = int(table.shape[0]) - 1, int(table.shape[1])
+            self.dtype, self.host = torch.int8, table.rows.contiguous()
+            self.pitch = self.row_bytes = self.host.shape[1]
+        else:
+            t = table if torch.is_tensor(table) else torch.from_numpy(np.asarray(table))
+            if t.is_cuda:
+                raise ValueError("HostFeatures takes a host (CPU) table; a CUDA table is used as features directly")
+            if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < 1:
+                raise ValueError("the table must be a 2-D [N+1, F] array with F >= 1")
+            if t.dtype not in (torch.float32, torch.bfloat16):
+                raise TypeError("the table must be float32 or bfloat16 (got %s)" % t.dtype)
+            if bool((t[-1] != 0).any()):
+                raise ValueError("the table's last row is the dummy row and must be all zero")
+            self.n_nodes, F = int(t.shape[0]) - 1, int(t.shape[1])
+            self.dtype = t.dtype
+            self.pitch = ops.pad_cols(F)
+            self.row_bytes = self.pitch * t.element_size()
+            self.host = torch.zeros((self.n_nodes + 1, self.pitch), dtype=self.dtype)
+            self.host[:, :F] = t
         ids = _check_cache_ids(cache_ids, self.n_nodes)
         self.shape = (self.n_nodes + 1, F)
-        self.dtype = t.dtype
-        self.pitch = ops.pad_cols(F)
-        self.row_bytes = self.pitch * t.element_size()
         self.cache_ids = ids
         self.n_cached = len(ids)
-        self.host = torch.zeros((self.n_nodes + 1, self.pitch), dtype=self.dtype)
-        self.host[:, :F] = t
         self._alias = None
         self._alias = ops.host_register(self.host)            # pinned once; every step's fetch reads through it
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -98,7 +108,7 @@ class HostFeatures(object):
         self.cache_slot = torch.full((self.n_nodes + 1,), -1, dtype=torch.int32, device=dev)
         self.claim = torch.empty((self.n_nodes + 1,), dtype=torch.int32, device=dev)
         self.count = torch.zeros((1,), dtype=torch.int32, device=dev)
-        self.ws = torch.zeros((C + 1, self.pitch), dtype=self.dtype, device=dev)
+        self.ws = torch.zeros((C + 1, self.pitch), dtype=self.host.dtype, device=dev)
         self.capacity, self._captured, self._retired = 0, False, []
         if C:
             cid = torch.from_numpy(ids.astype(np.int32)).to(dev)
@@ -115,7 +125,7 @@ class HostFeatures(object):
             raise RuntimeError("HostFeatures: the working set must grow to %d staging rows inside a CUDA-graph capture; "
                                "run the batch shape once before capturing it" % rows)
         head = self.n_cached + 1
-        ws = torch.empty((head + rows, self.pitch), dtype=self.dtype, device=self.device)
+        ws = torch.empty((head + rows, self.pitch), dtype=self.ws.dtype, device=self.device)
         ws[:head].copy_(self.ws[:head])
         if self._captured:
             self._retired.append(self.ws)      # a captured graph still addresses the old buffer: keep it alive
@@ -132,7 +142,8 @@ class HostFeatures(object):
         return t
 
     def stage(self, samples):
-        """One step's layer-0 source: (working set [C + 1 + capacity, F] view, the id lists translated to its rows).
+        """One step's layer-0 source: (working set [C + 1 + capacity, F] view - an ops.I8Rows over it for int8 rows -, the id
+        lists translated to its rows).
         samples: the step's int32 device id lists (SampleAndAggregate.sample); all of them are read by layer 0."""
         lists = [ops._i32(s.reshape(-1), "samples") for s in samples]
         S = sum(t.numel() for t in lists)
@@ -149,6 +160,8 @@ class HostFeatures(object):
         head = self.n_cached + 1
         ops.host_fetch(self._alias, self.row_bytes, stage_ids[:S], self.count, self.ws[head:])
         out = [ops.host_translate(tab, t, self.claim, head) for t in lists]
+        if self.dtype == torch.int8:
+            return ops.I8Rows(self.ws, self.shape[1]), out
         return self.ws[:, :self.shape[1]], out
 
     def close(self):

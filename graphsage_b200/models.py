@@ -13,6 +13,7 @@ from . import ops
 from .aggregators import (GCNAggregator, MaxPoolingAggregator, MeanAggregator, MeanPoolingAggregator, SeqAggregator,
                           TwoMaxLayerPoolingAggregator, refuse_seq_table)
 from .host_features import HostFeatures, refuse_host_table, stage_layer0, step_rows
+from .int8_features import Int8Features, refuse_int8_table
 from .layers import identity, relu  # noqa: F401
 
 # reference graphsage/models.py:180-185
@@ -49,7 +50,8 @@ class SampleAndAggregate(object):
 
     features : float32 CUDA tensor [N+1, F] whose LAST row is the all-zero dummy row
                (reference supervised_train.py:133-135), or a numpy array (uploaded, dummy row NOT added), or a
-               HostFeatures table in host memory (each step stages the rows it reads; see host_features.py).
+               HostFeatures table in host memory (each step stages the rows it reads; see host_features.py), or an
+               Int8Features table on the device (int8 rows with a per-row scale; see int8_features.py).
     adj      : int32 CUDA tensor [N+1, max_degree] padded adjacency (reference minibatch.py:227-245).
     identity_dim : d > 0 adds a trainable [N+1, d] embedding table (`self.embeds`) in front of the features, or replaces
                them when features is None (see _init_identity_table).
@@ -77,6 +79,13 @@ class SampleAndAggregate(object):
             self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, 0, device)
             return
         if hasattr(features, "c_table"):                 # parallel.ShardedFeatures: node-partitioned table
+            self.features = features
+            self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
+            return
+        if isinstance(features, Int8Features):           # int8 rows: layer 0 reads them dequantised
+            if not features.rows.is_cuda:
+                raise ValueError("an Int8Features table in host memory is used through HostFeatures(table, cache_ids); "
+                                 "build it with device='cuda' to keep its rows on the GPU")
             self.features = features
             self._finish_init(placeholders, adj, degrees, layer_infos, concat, model_size, identity_dim, device)
             return
@@ -112,6 +121,7 @@ class SampleAndAggregate(object):
         if hasattr(features, "c_table"):
             raise NotImplementedError("identity_dim > 0 with a node-partitioned feature table is not implemented")
         refuse_host_table(features, "identity_dim > 0 (the embeddings are trained in a device table beside the features)")
+        refuse_int8_table(features, "identity_dim > 0")
         if features is not None:
             if torch.is_tensor(features) and features.dtype == torch.bfloat16:
                 raise NotImplementedError("identity_dim > 0 with a bfloat16 feature table is not implemented")

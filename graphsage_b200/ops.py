@@ -191,6 +191,54 @@ def random_walks(indptr, indices, starts, num_walks, walk_len, seed, counter=0, 
     return out
 
 
+def i8row_pitch(f):
+    """Bytes per row of a GS_I8ROW table of f features (gs_i8row_pitch): round_up(round_up(f, 4) + 4, 16)."""
+    return ((int(f) + 3) // 4 * 4 + 4 + 15) // 16 * 16
+
+
+class I8Rows(object):
+    """A GS_I8ROW table as the kernels read it (row format: include/graphsage_b200.h): `rows`, a uint8 tensor [n, pitch]
+    of int8 values with each row's fp32 scale inside the row, and F features.  It stands where an fp32 [n, F] table
+    would: shape (n, F), dtype torch.int8.  gather_mean, gather_rows_f32 and sage_layer_small read it as the dequantised
+    fp32 table and give that table's bits."""
+    dtype = torch.int8
+
+    def __init__(self, rows, F):
+        if rows.dtype != torch.uint8 or rows.dim() != 2 or rows.stride(1) != 1 or rows.stride(0) % 16 \
+                or rows.shape[1] < i8row_pitch(F):
+            raise ValueError("int8 rows must be a row-major uint8 [n, >= %d] tensor with a pitch of 16-byte multiples"
+                             % i8row_pitch(F))
+        self.rows, self.shape = rows, torch.Size((rows.shape[0], int(F)))
+
+    @property
+    def device(self):
+        return self.rows.device
+
+
+def _table(src):
+    """(pointer, dtype code, rows, pitch) of a row-major source table: pitch in elements, or in bytes for I8Rows."""
+    if isinstance(src, I8Rows):
+        require_cuda(src.rows)
+        return ptr(src.rows), _lib.GS_I8ROW, src.rows.shape[0], src.rows.stride(0)
+    return ptr(src), _dtype_code(src), src.shape[0], src.stride(0)
+
+
+def quantize_rows_i8(x, out=None):
+    """fp32 [n, F] CUDA rows -> GS_I8ROW rows, uint8 [n, i8row_pitch(F)] (gs_quantize_rows_i8; contract
+    oracle/int8_rows.py).  The caller refuses non-finite values."""
+    require_cuda(x, out)
+    if x.dtype != torch.float32 or x.dim() != 2 or x.stride(1) != 1 or x.shape[1] < 1:
+        raise ValueError("x must be a row-major float32 [n, F >= 1] matrix")
+    n, F = x.shape
+    if out is None:
+        out = torch.empty((n, i8row_pitch(F)), dtype=torch.uint8, device=x.device)
+    if out.dtype != torch.uint8 or out.dim() != 2 or out.stride(1) != 1 or out.shape[0] < n or out.shape[1] != out.stride(0):
+        raise ValueError("out must be a contiguous uint8 [>= n, pitch] matrix")
+    check(lib().gs_quantize_rows_i8(ptr(x), n, F, x.stride(0), ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n else 0)
+    return out
+
+
 def _dtype_code(t):
     if t.dtype == torch.float32:
         return _lib.GS_F32
@@ -225,10 +273,13 @@ def gather_rows(feats, ids, out=None):
 
 def gather_rows_f32(feats, ids=None, row0=0, n=None, out=None):
     """embedding_lookup widened to fp32 (reference graphsage/models.py:299): rows ids[i] (or row0 + i) of a bf16 / fp32
-    table into an fp32 [n, pad_cols(F)] buffer (returned as its [:, :F] view); pad columns are zeroed."""
-    require_cuda(feats, ids, out)
-    if feats.dim() != 2 or feats.stride(1) != 1:
-        raise ValueError("features must be a row-major 2-D tensor")
+    table, or of an I8Rows table (dequantised), into an fp32 [n, pad_cols(F)] buffer (returned as its [:, :F] view); pad
+    columns are zeroed."""
+    require_cuda(ids, out)
+    if not isinstance(feats, I8Rows):
+        require_cuda(feats)
+        if feats.dim() != 2 or feats.stride(1) != 1:
+            raise ValueError("features must be a row-major 2-D tensor")
     F = feats.shape[1]
     if ids is not None:
         ids = _i32(ids.reshape(-1), "ids")
@@ -239,8 +290,8 @@ def gather_rows_f32(feats, ids=None, row0=0, n=None, out=None):
         out = torch.empty((n, pad_cols(F)), dtype=torch.float32, device=feats.device)[:, :F]
     if out.dtype != torch.float32 or out.stride(1) != 1 or out.shape[0] < n:
         raise ValueError("out must be a row-major float32 matrix with >= n rows")
-    check(lib().gs_gather_rows_f32(ptr(feats), _dtype_code(feats), feats.shape[0], F, feats.stride(0), ptr(ids), int(row0), n,
-                                   ptr(out), out.stride(0), stream_ptr()))
+    src, code, n_rows, pitch = _table(feats)
+    check(lib().gs_gather_rows_f32(src, code, n_rows, F, pitch, ptr(ids), int(row0), n, ptr(out), out.stride(0), stream_ptr()))
     _launched(1 if n else 0)
     return out
 
@@ -299,12 +350,14 @@ def _check_out(t, rows, out_pitch, name):
 def gather_mean(src, segments, include_self=False, want_self=True, out_pitch=None, out_mean=None, out_self=None):
     """Fused embedding_lookup + reduce_mean over the fanout (models.py:299 + aggregators.py:48 / :106-107).
     segments: list of Seg; returns (out_self or None, out_mean), each [rows, out_pitch].
-    `src` is a float32 [rows, F] CUDA tensor, or a parallel.ShardedFeatures (node-partitioned table)."""
+    `src` is a float32 (or bfloat16) [rows, F] CUDA tensor, an I8Rows table (the means of its dequantised rows), or a
+    parallel.ShardedFeatures (node-partitioned table)."""
     if hasattr(src, "c_table"):
         return _gather_mean_sharded(src, segments, include_self, want_self, out_pitch, out_mean, out_self)
-    require_cuda(src)
-    if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
-        raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
+    if not isinstance(src, I8Rows):
+        require_cuda(src)
+        if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
+            raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
     F = src.shape[1]
     if out_pitch is None:
         out_pitch = pad_cols(F)
@@ -317,7 +370,8 @@ def gather_mean(src, segments, include_self=False, want_self=True, out_pitch=Non
         out_self = torch.empty((rows, out_pitch), dtype=torch.float32, device=src.device)
     arr = (Segment * max(len(segments), 1))(*[s.c_struct() for s in segments])
     ev = _probe("gather_mean/%d" % rows)
-    check(lib().gs_gather_mean(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), arr, len(segments),
+    table, code, n_rows, pitch = _table(src)
+    check(lib().gs_gather_mean(table, code, n_rows, F, pitch, arr, len(segments),
                                int(bool(include_self)), ptr(out_self) if want_self else 0, ptr(out_mean), out_pitch,
                                stream_ptr()))
     _launched(1 if rows else 0, ev)
@@ -761,19 +815,24 @@ SMALL_LAYER_MAX_ROWS = 2048
 def sage_layer_small(src, seg, parts, combine=COMBINE_ADD, include_self=False, bias=None, act=ACT_NONE,
                      l2_normalize=False, counter_dev=None, counter_inc=0):
     """One whole aggregator layer (fanout mean -> matmuls -> add|concat -> bias -> act -> optional row
-    l2-normalise) for a small number of rows in ONE launch, exact fp32.  parts: [(None, K, B)] with K == src width."""
-    require_cuda(src, bias, counter_dev)
-    if src.dtype != torch.float32 or src.stride(1) != 1:
-        raise ValueError("src must be row-major float32")
+    l2-normalise) for a small number of rows in ONE launch, exact fp32.  parts: [(None, K, B)] with K == src width.
+    src: a float32 CUDA table, or an I8Rows table (gs_sage_layer_small_i8: the bits of the dequantised table)."""
+    require_cuda(bias, counter_dev)
+    i8 = isinstance(src, I8Rows)
+    if not i8:
+        require_cuda(src)
+        if src.dtype != torch.float32 or src.stride(1) != 1:
+            raise ValueError("src must be row-major float32")
     _, arr, keep = _gemm_parts([(None, K, B) for (_, K, B) in parts])
     ntot = sum(p[2].shape[1] for p in parts) if (combine == COMBINE_CONCAT) else parts[0][2].shape[1]
     rows = seg.out_row0 + seg.n
     out = torch.empty((rows, ntot), dtype=torch.float32, device=src.device)
     cseg = seg.c_struct()
     ev = _probe("sage_layer_small/%d" % rows)
-    check(lib().gs_sage_layer_small(ptr(src), src.shape[0], src.shape[1], src.stride(0), cseg, int(bool(include_self)),
-                                    arr, len(parts), combine, ptr(bias), act, int(bool(l2_normalize)), ptr(out),
-                                    out.stride(0), ptr(counter_dev), int(counter_inc), stream_ptr()))
+    table, _, n_rows, pitch = _table(src)
+    fn = lib().gs_sage_layer_small_i8 if i8 else lib().gs_sage_layer_small
+    check(fn(table, n_rows, src.shape[1], pitch, cseg, int(bool(include_self)), arr, len(parts), combine, ptr(bias), act,
+             int(bool(l2_normalize)), ptr(out), out.stride(0), ptr(counter_dev), int(counter_inc), stream_ptr()))
     _launched(1 if seg.n else 0, ev)
     return out
 

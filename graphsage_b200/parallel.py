@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from ._lib import ShardedTable, check, lib
-from .ops import pad_cols
+from .ops import I8Rows, pad_cols
 
 
 def rows_per_shard(n_nodes, world):
@@ -243,6 +243,9 @@ class ShardedFeatures(object):
         lo, hi = self.row_start[self.rank], self.row_start[self.rank + 1]
         n_local = hi - lo
         self.lo, self.hi, self.n_local = lo, hi, n_local
+        if isinstance(local_rows, I8Rows) or isinstance(replica_rows, I8Rows):
+            raise NotImplementedError("a node-partitioned (ShardedFeatures) table of int8 (Int8Features) rows is not "
+                                      "implemented")
         if local_rows is None:
             # big shards are produced on the device: the caller fills self.local[:n_local, :F] itself (then fill_replicas())
             if not n_features:

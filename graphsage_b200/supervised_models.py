@@ -20,6 +20,7 @@ import torch
 from . import ops
 from .graphed_training import GraphedTrainStep
 from .host_features import refuse_host_table, stage_layer0
+from .int8_features import refuse_int8_table
 from .layers import act_code, identity, relu  # noqa: F401
 from .aggregators import (FUSED_POOL_HIDDEN_STEP, FUSED_POOL_MAX_FANOUT, FUSED_POOL_MAX_K, TwoMaxLayerPoolingAggregator,
                           fused_pool_fits)
@@ -290,6 +291,7 @@ def refuse_fused_pool(model):
         return
     if not hasattr(model.aggregators[0], "mlp_layers"):
         raise NotImplementedError("fused_pool=True applies to the maxpool and meanpool aggregators only")
+    refuse_int8_table(model.features, "fused_pool=True")
     if hasattr(model.features, "c_table"):
         raise NotImplementedError("fused_pool=True with a node-partitioned (ShardedFeatures) table is not implemented")
     if model.dropout_rate:
@@ -534,6 +536,7 @@ def embedding_parameters(model):
 def refuse_distributed_host_table(features, distributed):
     if distributed:
         refuse_host_table(features, "distributed=True")
+        refuse_int8_table(features, "distributed=True")
 
 
 def refuse_distributed_embeddings(identity_dim, distributed):

@@ -35,7 +35,25 @@ typedef enum {
   GS_ERR_UNSUPPORTED = -3
 } gs_status;
 
-typedef enum { GS_F32 = 0, GS_BF16 = 1, GS_F64 = 2 } gs_dtype;   /* GS_F64: gs_sgd_fit's X only */
+typedef enum { GS_F32 = 0, GS_BF16 = 1, GS_F64 = 2, GS_I8ROW = 3 } gs_dtype;   /* GS_F64: gs_sgd_fit's X only */
+
+/* GS_I8ROW - an int8 feature table with one fp32 scale per row (graphsage_b200.Int8Features; numpy restatement in
+ * oracle/int8_rows.py).  Each row is a byte array of `pitch` bytes, the scale stored inside it, so routines that copy rows
+ * by bytes (gs_host_fetch, bulk row copies) move int8 rows unchanged:
+ *   bytes [0, F)           q_c   int8
+ *   bytes [F, P4)          zero                      P4 = round_up(F, 4)
+ *   bytes [P4, P4 + 4)     s     fp32, little-endian
+ *   bytes [P4 + 4, pitch)  zero                      pitch = gs_i8row_pitch(F) = round_up(P4 + 4, 16)
+ * Quantise (gs_quantize_rows_i8): a = max_c |x_c|, s = fl(a / 127); if s == 0 every q_c = 0 (an all-zero row - the dummy
+ * row N - has s = 0 and zero bytes), else q_c = clamp(rint_half_even(fl(x_c / s)), -127, 127).  Non-finite input is the
+ * caller's to refuse.  Dequantise: deq_c = fl(float(q_c) * s), one fp32 rounding.  Every kernel that reads GS_I8ROW rows
+ * (gs_gather_mean, gs_gather_rows_f32, gs_sage_layer_small_i8) sees exactly deq and from there computes what its fp32
+ * form computes on the table deq: the same bits.  Where such a call takes a `pitch`, it counts bytes. */
+int64_t gs_i8row_pitch(int32_t F);
+/* fp32 rows x [n, F] (row stride ldx floats) -> GS_I8ROW rows out [n, out_pitch_bytes] (out_pitch_bytes % 16 == 0 and
+ * >= gs_i8row_pitch(F); bytes past the row are zeroed).  One warp per row. */
+int32_t gs_quantize_rows_i8(const float* x, int64_t n, int32_t F, int64_t ldx, void* out, int64_t out_pitch_bytes,
+                            void* stream);
 typedef enum { GS_ACT_NONE = 0, GS_ACT_RELU = 1 } gs_act;
 /* how the neighbour part and the self part are combined */
 typedef enum {
@@ -158,7 +176,9 @@ int32_t gs_gather_rows(const void* feats, int32_t dtype, int64_t n_rows, int32_t
  *   out_self[r] = self row (only if out_self != NULL)
  * src is [n_src_rows, F] with `pitch`; F columns are produced, columns F..out_pitch-1 are zeroed.
  * dtype GS_F32, or GS_BF16: a bfloat16 table (rows 16-byte multiples: pitch % 8 == 0, out_pitch % 8 == 0) summed in fp32 -
- * the outputs stay fp32 and equal the fp32 kernel's on the bf16-rounded table (half the gathered bytes).
+ * the outputs stay fp32 and equal the fp32 kernel's on the bf16-rounded table (half the gathered bytes); or GS_I8ROW
+ * (pitch in bytes, % 16 == 0, >= gs_i8row_pitch(F); out_pitch % 8 == 0 and <= 1536): whole rows by bulk copy, dequantised
+ * in registers - the fp32 kernel's outputs on the dequantised table (a quarter of the fp32 bytes).
  * --------------------------------------------------------------------------------------------- */
 #define GS_MAX_SEGMENTS 4
 typedef struct {
@@ -261,8 +281,9 @@ int32_t gs_host_translate(const gs_sharded_table* table_host, const int32_t* ids
                           int64_t stage_row0, int32_t* out, void* stream);
 
 /* embedding_lookup (models.py:299) with the result widened to fp32: out[i, 0:F] = (float)feats[ids ? ids[i] : row0 + i, 0:F],
- * columns F..out_pitch-1 zeroed.  feats is GS_BF16 or GS_F32.  The bf16 max-pool path uses it for the SELF rows, which
- * meet the fp32 self_weights contraction (aggregators.py:185). */
+ * columns F..out_pitch-1 zeroed.  feats is GS_BF16, GS_F32 or GS_I8ROW (pitch in bytes; the dequantised values).  The bf16
+ * max-pool path uses it for the SELF rows, which meet the fp32 self_weights contraction (aggregators.py:185); over an int8
+ * table the pooling aggregators read their neighbour and self rows through it. */
 int32_t gs_gather_rows_f32(const void* feats, int32_t dtype, int64_t n_rows, int32_t F, int64_t pitch,
                            const int32_t* ids, int64_t row0, int64_t n, float* out, int64_t out_pitch,
                            void* stream);
@@ -364,6 +385,15 @@ int32_t gs_sage_layer_small(const float* src, int64_t n_src_rows, int32_t F, int
                             const float* bias, int32_t act, int32_t l2_normalize,
                             float* out, int64_t ldo, uint64_t* counter_dev, uint64_t counter_inc,
                             void* stream);
+/* gs_sage_layer_small over a GS_I8ROW table (pitch in bytes, % 16 == 0, >= gs_i8row_pitch(F); 16-byte aligned): the bits
+ * gs_sage_layer_small gives on the dequantised table held with a 16-byte-aligned pitch that is a multiple of 4 floats (the
+ * layout SampleAndAggregate keeps fp32 tables in).  The one-layer model of <= 2,048 rows runs layer 0 here. */
+int32_t gs_sage_layer_small_i8(const void* src, int64_t n_src_rows, int32_t F, int64_t pitch,
+                               const gs_segment* segment_host, int32_t include_self,
+                               const gs_gemm_part* parts_host, int32_t n_parts, int32_t combine,
+                               const float* bias, int32_t act, int32_t l2_normalize,
+                               float* out, int64_t ldo, uint64_t* counter_dev, uint64_t counter_inc,
+                               void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * K4 - the max-pool aggregator's neighbour branch fused end to end on the tensor cores (wgmma, bf16 operands, fp32

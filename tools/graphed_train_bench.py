@@ -59,6 +59,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--math", default=os.environ.get("GS_MATH", "tf32x3"))
     ap.add_argument("--only", default="sup_mean,sup_maxpool,unsup_mean,n2v")
+    ap.add_argument("--table", choices=["fp32", "bf16", "int8"], default="fp32",
+                    help="the feature table the graphsage models read: fp32, bf16, or int8 rows with a per-row scale")
     args = ap.parse_args()
     if args.steps < 1 or args.rounds < 1 or args.warmup < 0:
         ap.error("--steps and --rounds must be >= 1, --warmup >= 0")
@@ -79,15 +81,17 @@ def main():
         table = torch.zeros((N_NODES + 1, ops.pad_cols(F)), dtype=torch.float32, device=dev)
         table[:, :F] = torch.from_numpy(g["features"]).to(dev)
         adj_dev = torch.from_numpy(g["adj"]).to(dev)
+        features = {"fp32": lambda: table[:, :F], "bf16": lambda: table.to(torch.bfloat16)[:, :F],
+                    "int8": lambda: gs.Int8Features(table[:, :F])}[args.table]()
 
     def sage(kind, supervised):
         gs.inits.manual_seed(1)
         sampler = gs.UniformNeighborSampler(adj_dev, seed=123)
         infos = [gs.SAGEInfo("node", sampler, FANOUT[0], DIM), gs.SAGEInfo("node", sampler, FANOUT[1], DIM)]
         if supervised:
-            return gs.SupervisedGraphsage(N_CLASSES, {"batch_size": BATCH, "dropout": 0.}, table[:, :F], adj_dev, None, infos,
+            return gs.SupervisedGraphsage(N_CLASSES, {"batch_size": BATCH, "dropout": 0.}, features, adj_dev, None, infos,
                                           concat=True, aggregator_type=kind, sigmoid_loss=False, learning_rate=0.01, device=dev)
-        return gs.UnsupervisedGraphsage({"batch_size": BATCH, "dropout": 0.}, table[:, :F], adj_dev, g["deg"][:N_NODES], infos,
+        return gs.UnsupervisedGraphsage({"batch_size": BATCH, "dropout": 0.}, features, adj_dev, g["deg"][:N_NODES], infos,
                                         concat=True, aggregator_type=kind, neg_sample_size=NEG, learning_rate=1e-5, device=dev)
 
     def sage_inputs(supervised):
@@ -131,7 +135,7 @@ def main():
         del eager, graphed, step
         torch.cuda.empty_cache()
 
-    print(json.dumps({"metric": "training_step_ms", "card": _card(), "math": args.math, "steps": args.steps,
+    print(json.dumps({"metric": "training_step_ms", "card": _card(), "math": args.math, "table": args.table, "steps": args.steps,
                       "warmup": args.warmup, "batch": BATCH, "fanout": FANOUT, "dim": DIM, "results": results,
                       "higher_is_better": False,
                       "note": "per round: --steps eager train_step calls, then --steps replays of graphed_train_step, on the "

@@ -56,6 +56,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--fractions", default="0,0.1,0.25,0.5,1")
     ap.add_argument("--math", default=os.environ.get("GS_MATH", "tf32x3"))
+    ap.add_argument("--table", choices=["fp32", "int8"], default="fp32",
+                    help="int8: an Int8Features table (int8 rows with a per-row scale), on the host and on the device")
     args = ap.parse_args()
     if args.steps < 1 or args.rounds < 1 or args.warmup < 0:
         ap.error("--steps and --rounds must be >= 1, --warmup >= 0")
@@ -91,8 +93,14 @@ def main():
     rows_per_step = BATCH * (1 + FANOUT[1] + FANOUT[1] * FANOUT[0])
     results = {}
     for frac in [float(x) for x in args.fractions.split(",")]:
-        hf = gs.HostFeatures(torch.from_numpy(feats), cache_ids=hot_rows(g["adj"], int(round(frac * N_NODES))))
-        host_m, dev_m = model(hf), model(table[:, :F])
+        cache = hot_rows(g["adj"], int(round(frac * N_NODES)))
+        if args.table == "int8":
+            hf = gs.HostFeatures(gs.Int8Features(feats), cache_ids=cache)
+            dev_table = gs.Int8Features(table[:, :F])
+        else:
+            hf = gs.HostFeatures(torch.from_numpy(feats), cache_ids=cache)
+            dev_table = table[:, :F]
+        host_m, dev_m = model(hf), model(dev_table)
         for x in inputs[:args.warmup]:
             host_m.train_step(*x)
             dev_m.train_step(*x)
@@ -113,7 +121,7 @@ def main():
             ops.PROBE = None
         same = bool(torch.equal(host_m.train_step(*timed[0]), dev_m.train_step(*timed[0])))
         # control: a second device-table model through the same steps - are two device-table runs bit-identical here?
-        twin = model(table[:, :F])
+        twin = model(dev_table)
         for x in inputs[:args.warmup] + timed * (args.rounds + 1) + timed[:1]:
             twin.train_step(*x)
         same_twin = bool(torch.equal(twin.train_step(*timed[0]), dev_m.train_step(*timed[0])))
@@ -129,13 +137,14 @@ def main():
             "staged_rows_per_step": rows, "sampled_rows_per_step": rows_per_step,
             "fetch_ms": f_ms, "host_link_GBps": rows * hf.row_bytes / (f_ms * 1e-3) / 1e9,
             "same_loss_as_device_table": same, "device_table_twice_same_loss": same_twin}
+        row_bytes = hf.row_bytes
         hf.close()
         del host_m, dev_m, hf
         torch.cuda.empty_cache()
 
     print(json.dumps({"metric": "host_table_training_step_ms", "card": card, "math": args.math, "steps": args.steps,
                       "warmup": args.warmup, "batch": BATCH, "fanout": FANOUT, "dim": DIM, "features": F,
-                      "row_bytes": ops.pad_cols(F) * 4, "results": results, "higher_is_better": False}))
+                      "table": args.table, "row_bytes": row_bytes, "results": results, "higher_is_better": False}))
 
 
 if __name__ == "__main__":
