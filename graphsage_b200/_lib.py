@@ -52,6 +52,7 @@ MAX_UNIQUE_SAMPLED = 1024          # GS_MAX_UNIQUE_SAMPLED
 UNIQUE_DRAW_BUDGET = 1 << 20       # GS_UNIQUE_DRAW_BUDGET
 WALK_MAX_WALKS = 1 << 20           # GS_WALK_MAX_WALKS
 WALK_MAX_LEN = 33                  # GS_WALK_MAX_LEN
+WALK_PQ_MIN, WALK_PQ_MAX = 1e-4, 1e4   # GS_WALK_PQ_MIN, GS_WALK_PQ_MAX
 MAX_BLOCK_LAYERS = 8               # GS_MAX_BLOCK_LAYERS
 
 
@@ -161,6 +162,10 @@ _SIGNATURES = {
     "gs_random_walks_workspace_bytes": (c_i64, [c_i64, c_i32, c_i32]),
     "gs_random_walks": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_random_walks_emit": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp]),
+    "gs_csr_sort_rows_workspace_bytes": (c_i64, [c_i64, c_i64]),
+    "gs_csr_sort_rows": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    "gs_random_walks_biased": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, ctypes.c_double, ctypes.c_double,
+                                       c_u64, c_u64, c_i64, c_vp, c_i64, c_vp, c_vp]),
     "gs_csr_aggregate": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp]),
     "gs_csr_aggregate_dropout": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32,
                                          DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),

@@ -142,6 +142,7 @@ constexpr uint32_t kStreamUnigram = 0x20000000u;
 constexpr uint32_t kStreamBuild = 0x10000000u;
 constexpr uint32_t kStreamUnigramUnique = 0x30000000u;
 constexpr uint32_t kStreamWalk = 0x50000000u;
+constexpr uint32_t kStreamWalkBiased = 0x60000000u;  // 2^28 words: ((w * 32 + move) << 3) + call
 
 // ---- PTX wrappers (mbarrier / bulk copy) ---------------------------------------------------
 #ifdef __CUDACC__

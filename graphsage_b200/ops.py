@@ -1,6 +1,7 @@
 """Functional wrappers: torch CUDA tensors in, torch CUDA tensors out, all work done by
 libgraphsage_b200.so on the current CUDA stream.  torch only owns memory and streams here."""
 import collections
+import math
 
 import torch
 
@@ -157,14 +158,48 @@ def sample_csr(indptr, indices, ids, k, seed, counter, replace_if_short=True, pa
     return out
 
 
-def random_walks(indptr, indices, starts, num_walks, walk_len, seed, counter=0, start_offset=0):
+def check_walk_bias(p, q):
+    """node2vec's return and in-out parameters: finite and in [WALK_PQ_MIN, WALK_PQ_MAX] (ValueError otherwise)."""
+    for name, v in (("p", p), ("q", q)):
+        v = float(v)
+        if not (math.isfinite(v) and _lib.WALK_PQ_MIN <= v <= _lib.WALK_PQ_MAX):
+            raise ValueError("%s must be finite and in [%g, %g] (got %r)" % (name, _lib.WALK_PQ_MIN, _lib.WALK_PQ_MAX, v))
+
+
+def csr_sort_rows(indptr, indices):
+    """A copy of indices sorted ascending within each CSR row (gs_csr_sort_rows): the membership-test input of the
+    biased walk.  Entries outside every row keep their values.  Start-up work, no host synchronisation."""
+    require_cuda(indptr, indices)
+    if indptr.dtype != torch.int64:
+        raise TypeError("indptr must be int64")
+    indptr, indices = indptr.contiguous(), _i32(indices, "indices")
+    n_nodes, nnz = indptr.numel() - 1, indices.numel()
+    nbytes = lib().gs_csr_sort_rows_workspace_bytes(n_nodes, nnz)
+    if nbytes < 0:
+        check(-1)
+    out = torch.empty_like(indices)
+    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=indices.device)
+    ev = _probe("csr_sort_rows/%d" % nnz)
+    check(lib().gs_csr_sort_rows(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(out), ptr(ws), nbytes,
+                                 stream_ptr()))
+    _launched(1 if nnz and n_nodes else 0, ev)
+    return out
+
+
+def random_walks(indptr, indices, starts, num_walks, walk_len, seed, counter=0, start_offset=0, p=1.0, q=1.0,
+                 sorted_indices=None):
     """Co-occurrence pairs of uniform random walks (gs_random_walks; reference graphsage/utils.py:77-92): num_walks walks
     of walk_len - 1 steps from every start, (starts[t], visited id) for every visited id other than the start, ordered
     by start, walk and step.  Contract: oracle/walks.py (start_offset is the global position of starts[0], so chunks
     with the right offsets give the pairs of one call).  Returns an int32 CUDA tensor [P, 2].
+    p, q: node2vec's return and in-out parameters (gs_random_walks_biased, contract oracle/biased_walks.py), finite and
+    in [1e-4, 1e4]; p == q == 1 is the uniform walk above.  Otherwise the walk needs each row sorted for its membership
+    test: sorted_indices = csr_sort_rows(indptr, indices), built here when not given (pass it to reuse it over calls).
     P is read back to size the output: one device-to-host copy (and so a synchronisation) per call - start-up work,
     not meant for capture."""
-    require_cuda(indptr, indices, starts)
+    check_walk_bias(p, q)
+    biased = not (float(p) == 1.0 and float(q) == 1.0)
+    require_cuda(indptr, indices, starts, sorted_indices if biased else None)
     if indptr.dtype != torch.int64:
         raise TypeError("indptr must be int64")
     indptr, indices, starts = indptr.contiguous(), _i32(indices, "indices"), _i32(starts.reshape(-1), "starts")
@@ -182,9 +217,20 @@ def random_walks(indptr, indices, starts, num_walks, walk_len, seed, counter=0, 
     dev = starts.device
     ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev)
     n_pairs = torch.empty((1,), dtype=torch.int64, device=dev)
-    ev = _probe("random_walks/%d" % (n * num_walks))
-    check(lib().gs_random_walks(ptr(indptr), ptr(indices), indptr.numel() - 1, ptr(starts), n, num_walks, walk_len,
-                                seed & _U64, counter & _U64, start_offset, ptr(ws), nbytes, ptr(n_pairs), stream_ptr()))
+    if biased:
+        if sorted_indices is None:
+            sorted_indices = csr_sort_rows(indptr, indices)
+        sorted_indices = _i32(sorted_indices, "sorted_indices")
+        if sorted_indices.numel() != indices.numel():
+            raise ValueError("sorted_indices has %d entries, indices %d" % (sorted_indices.numel(), indices.numel()))
+    ev = _probe(("random_walks_biased/%d" if biased else "random_walks/%d") % (n * num_walks))
+    if biased:
+        check(lib().gs_random_walks_biased(ptr(indptr), ptr(indices), ptr(sorted_indices), indptr.numel() - 1,
+                                           ptr(starts), n, num_walks, walk_len, float(p), float(q), seed & _U64,
+                                           counter & _U64, start_offset, ptr(ws), nbytes, ptr(n_pairs), stream_ptr()))
+    else:
+        check(lib().gs_random_walks(ptr(indptr), ptr(indices), indptr.numel() - 1, ptr(starts), n, num_walks, walk_len,
+                                    seed & _U64, counter & _U64, start_offset, ptr(ws), nbytes, ptr(n_pairs), stream_ptr()))
     out = torch.empty((int(n_pairs.item()), 2), dtype=torch.int32, device=dev)
     check(lib().gs_random_walks_emit(ptr(starts), n, num_walks, walk_len, ptr(ws), nbytes, ptr(out), stream_ptr()))
     _launched(3 if n else 0, ev)                  # walk, emit (+ CUB's scan passes)

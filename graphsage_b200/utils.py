@@ -96,11 +96,13 @@ def run_random_walks(G, nodes, num_walks=N_WALKS, rng=None):
 WALK_CHUNK = 1 << 16  # starts per device call of run_random_walks_device: bounds the device memory a call needs
 
 
-def run_random_walks_device(G, nodes, num_walks=N_WALKS, seed=123, device=None, counter=0):
+def run_random_walks_device(G, nodes, num_walks=N_WALKS, seed=123, device=None, counter=0, p=1.0, q=1.0):
     """run_random_walks on the GPU (ops.random_walks, contract oracle/walks.py): the same list of (node, context) tuples
     of node names, with the reference's loop and WALK_LEN, drawn from the seeded Philox stream instead of `random`.
     Row k of the CSR is G.neighbors(node) in order, so neighbour k is what rng.choice's index k would pick.  The starts
-    are walked in chunks of WALK_CHUNK, each copied back before the next, so the pairs need not fit in device memory."""
+    are walked in chunks of WALK_CHUNK, each copied back before the next, so the pairs need not fit in device memory.
+    p, q: node2vec's return and in-out parameters (contract oracle/biased_walks.py); p == q == 1 is the uniform walk.
+    The rows are sorted for the biased walk once per call, not per chunk."""
     import torch
 
     from . import ops
@@ -112,10 +114,14 @@ def run_random_walks_device(G, nodes, num_walks=N_WALKS, seed=123, device=None, 
     indptr = torch.from_numpy(csr["indptr"]).to(dev)
     indices = torch.from_numpy(csr["indices"]).to(dev)
     starts = np.array([pos[n] for n in nodes], dtype=np.int32)
+    ops.check_walk_bias(p, q)
+    biased = not (float(p) == 1.0 and float(q) == 1.0)
+    sorted_indices = ops.csr_sort_rows(indptr, indices) if biased else None
     pairs = []
     for c0 in range(0, len(starts), WALK_CHUNK):
         chunk = torch.from_numpy(starts[c0:c0 + WALK_CHUNK]).to(dev)
-        idx = ops.random_walks(indptr, indices, chunk, num_walks, WALK_LEN, seed, counter, start_offset=c0).cpu().numpy()
+        idx = ops.random_walks(indptr, indices, chunk, num_walks, WALK_LEN, seed, counter, start_offset=c0, p=p, q=q,
+                               sorted_indices=sorted_indices).cpu().numpy()
         pairs += [(names[a], names[b]) for a, b in idx.tolist()]
     return pairs
 
@@ -126,20 +132,53 @@ def format_walks(pairs):
     return "\n".join([str(p[0]) + "\t" + str(p[1]) for p in pairs])
 
 
+USAGE = "usage: python -m graphsage_b200.utils <graph_file> <out_file> [--p P] [--q Q]"
+
+
+def _parse_main_args(argv):
+    """(graph_file, out_file, bias): bias is {} without --p / --q, else {"p": P, "q": Q} (the one not given is 1)."""
+    files, bias, k = [], {}, 0
+    while k < len(argv):
+        a = argv[k]
+        name, eq, val = a.partition("=")
+        if name in ("--p", "--q"):
+            if not eq:
+                if k + 1 >= len(argv):
+                    raise SystemExit(USAGE)
+                val, k = argv[k + 1], k + 1
+            try:
+                bias[name[2:]] = float(val)
+            except ValueError:
+                raise SystemExit("%s: %s must be a number (got %r)" % (USAGE, name, val))
+        else:
+            files.append(a)
+        k += 1
+    if len(files) != 2:
+        raise SystemExit(USAGE)
+    if bias:
+        bias = {"p": bias.get("p", 1.0), "q": bias.get("q", 1.0)}
+        from . import ops
+        try:
+            ops.check_walk_bias(bias["p"], bias["q"])
+        except ValueError as e:
+            raise SystemExit("%s: %s" % (USAGE, e))
+    return files[0], files[1], bias
+
+
 def main(argv=None, walker=None):
-    """`python -m graphsage_b200.utils <graph_file> <out_file>` (reference utils.py:94-104): the walks file of the train
-    subgraph (nodes that are neither val nor test), 50 walks of WALK_LEN per node, seed 123 and counter 0.
-    walker(G, nodes) -> pairs replaces run_random_walks_device (tests supply pairs without a device)."""
+    """`python -m graphsage_b200.utils <graph_file> <out_file> [--p P] [--q Q]` (reference utils.py:94-104): the walks
+    file of the train subgraph (nodes that are neither val nor test), 50 walks of WALK_LEN per node, seed 123 and
+    counter 0.  --p / --q make them node2vec's biased walks (either one alone leaves the other at 1).
+    walker(G, nodes) -> pairs replaces run_random_walks_device (tests supply pairs without a device); with --p / --q it
+    is called as walker(G, nodes, p=P, q=Q)."""
     import sys
     argv = sys.argv[1:] if argv is None else list(argv)
-    if len(argv) != 2:
-        raise SystemExit("usage: python -m graphsage_b200.utils <graph_file> <out_file>")
-    graph_file, out_file = argv
+    graph_file, out_file, bias = _parse_main_args(argv)
     with open(graph_file) as fp:
         G = node_link_graph(json.load(fp))
     nodes = [n for n in G.nodes() if not G.node[n]["val"] and not G.node[n]["test"]]
     G = G.subgraph(nodes)
-    pairs = (run_random_walks_device if walker is None else walker)(G, nodes)
+    pairs = (run_random_walks_device if walker is None else walker)(G, nodes, **bias)
     with open(out_file, "w") as fp:
         fp.write(format_walks(pairs))
     return pairs

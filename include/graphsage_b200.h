@@ -716,6 +716,45 @@ int32_t gs_random_walks_emit(const int32_t* starts, int64_t n, int32_t num_walks
                              int64_t workspace_bytes, int32_t* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * node2vec's second-order (p, q) walk (Grover & Leskovec, KDD'16) by rejection sampling.  Contract:
+ * oracle/biased_walks.py.  Every rule of gs_random_walks above holds - start excluded, L positions, the L-th move unused,
+ * a start of degree 0 emits nothing, a sink or out-of-range id ends the walk, pair order, start_offset - and the same
+ * workspace (gs_random_walks_workspace_bytes) and gs_random_walks_emit follow it.  Only the next node changes: from
+ * current node v, reached from t, every CSR entry x of v's row (duplicates once each) is a candidate of class
+ *     return  x == t                                    a = 1/p
+ *     in      x != t, x an entry of t's row (t -> x)    a = 1
+ *     out     otherwise                                 a = 1/q
+ *   with float64 thr_c = 2^32 if a_c == max(a) else floor(a_c / max(a) * 2^32): the chain moves to entry x with
+ *   probability thr_x / sum over v's entries of thr.  GS_WALK_PQ_MIN <= p, q <= GS_WALK_PQ_MAX (finite), so thr_c >= 1.
+ *   Move 0 (no t) takes entry mulhi32(word 0 of call 0, deg): uniform and always accepted.
+ *   Move s >= 1: attempts a = 0 .. GS_WALK_BIASED_ATTEMPTS - 1: candidate entry mulhi32(cand_a, deg) of v's row in its
+ *   given order, accepted iff (uint64)acc_a < thr_class(x).  If all reject: u = w0 | w1 << 32, target =
+ *   floor(u * S / 2^64) (S = sum of thr over the row), and the first entry whose inclusive prefix sum of thr exceeds it.
+ *   Words: philox4x32_10(ctr = (counter_lo, counter_hi, i, 0x60000000 + ((w * 32 + s) << 3) + call), key = seed); calls
+ *   0..6 carry attempts 2 call and 2 call + 1 as (cand, acc, cand, acc); call 7's words 0, 1 are u.  w < 2^20 and s < 32,
+ *   so the stream is exactly [0x60000000, 0x70000000): no other kStream* base lies in it, and the uniform walk's words
+ *   end below 0x50800000.
+ *   p == q == 1 runs gs_random_walks (sorted_indices unused, may be NULL): the uniform walk's pairs, byte for byte.
+ * gs_csr_sort_rows - sorted_indices int32 [nnz] = indices sorted ascending (signed) within each row
+ *   [indptr[i], indptr[i+1]); entries outside every row are copied unchanged.  The membership test "x in t's row" is a
+ *   binary search in t's sorted row; the candidates still come from `indices`' own order.  Start-up work: a device copy
+ *   and a CUB segmented sort, no host synchronisation.  Rows must lie in [0, nnz); n_nodes, nnz < 2^31 - 1.
+ *   workspace: gs_csr_sort_rows_workspace_bytes(...) bytes (0 when nnz or n_nodes is 0); -1 outside the limits.
+ * gs_random_walks_biased - one thread per walk, no atomics and no host synchronisation; writes P to *n_pairs as
+ *   gs_random_walks does.  sorted_indices: gs_csr_sort_rows of (indptr, indices).
+ * --------------------------------------------------------------------------------------------- */
+#define GS_WALK_PQ_MIN 1e-4
+#define GS_WALK_PQ_MAX 1e4
+#define GS_WALK_BIASED_ATTEMPTS 14
+int64_t gs_csr_sort_rows_workspace_bytes(int64_t n_nodes, int64_t nnz);
+int32_t gs_csr_sort_rows(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                         int32_t* sorted_indices, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t gs_random_walks_biased(const int64_t* indptr, const int32_t* indices, const int32_t* sorted_indices,
+                               int64_t n_nodes, const int32_t* starts, int64_t n, int32_t num_walks, int32_t walk_len,
+                               double p, double q, uint64_t seed, uint64_t counter, int64_t start_offset, void* workspace,
+                               int64_t workspace_bytes, int64_t* n_pairs, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Full-neighbourhood reduction over CSR rows (layer-wise inference, SampleAndAggregate.full_neighbor_embeddings): the
  * fixed-fanout reductions of gs_gather_mean / gs_segment_max (aggregators.py:48, 106-107, 182) with k made per row.
  * Contract: oracle/full_neighbor.py.  Output row i is for node v = rows ? rows[i] : i; its entries are
