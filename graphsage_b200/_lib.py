@@ -54,6 +54,7 @@ WALK_MAX_WALKS = 1 << 20           # GS_WALK_MAX_WALKS
 WALK_MAX_LEN = 33                  # GS_WALK_MAX_LEN
 WALK_PQ_MIN, WALK_PQ_MAX = 1e-4, 1e4   # GS_WALK_PQ_MIN, GS_WALK_PQ_MAX
 MAX_BLOCK_LAYERS = 8               # GS_MAX_BLOCK_LAYERS
+MAX_FANOUT = 256                   # GS_MAX_FANOUT
 
 
 class EmbedGradList(ctypes.Structure):
@@ -178,6 +179,13 @@ _SIGNATURES = {
     "gs_csr_blocks_fill": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, ctypes.POINTER(c_i64),
                                    ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
                                    c_vp]),
+    "gs_csr_sampled_blocks_plan": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64, c_u64,
+                                           c_vp, c_i64, c_vp, c_vp]),
+    "gs_csr_sampled_blocks_fill": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64, c_u64,
+                                           c_vp, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
+                                           ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), c_vp]),
+    "gs_csr_sample_rows_workspace_bytes": (c_i64, [c_i64, c_i64]),
+    "gs_csr_sample_rows": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_u64, c_u64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp]),
 }
 
 _lib = None

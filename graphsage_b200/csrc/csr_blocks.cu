@@ -11,6 +11,15 @@
 //                       at their local positions, zero elsewhere, CUB exclusive scan), indices (one warp per local row,
 //                       entries in CSR order relabelled through pos_l) and rows.
 // Integer work only and no atomics: two calls give the same bytes.
+//
+// Sampled blocks (gs_csr_sampled_blocks_plan / _fill, gs_csr_sample_rows; contract in oracle/sampled_blocks.py): the same
+// kernels, instantiated with kSample = true, read S_l(v) - at most k_l entries of v's row, drawn without replacement by
+// Floyd's algorithm - instead of the whole row.  One warp per node: the draws u_i are spread over the lanes (lane i % 32,
+// slot i / 32), the k held positions too; each of Floyd's k steps broadcasts u_i, tests membership with one ballot and
+// stores the taken position at its owner.  The fill ranks the held positions (each lane counts the smaller ones over the
+// warp) to write them in ascending order.  The plan and the fill recompute the same draws; nothing is stored between
+// them.  A hub row is never walked: with d > k a warp touches only the k drawn entries.  kSample = false is the code
+// above, instruction for instruction (the draw arguments are appended and unused).
 #include <algorithm>
 
 #include "common.cuh"
@@ -23,6 +32,69 @@ namespace gs {
 
 constexpr int kBlkThreads = 256;
 constexpr int kBlkWarps = kBlkThreads / 32;
+
+constexpr int kMaxFanout = GS_MAX_FANOUT;
+constexpr int kSlots = kMaxFanout / 32;   // held positions per lane
+
+// the draws of one sampled layer: S_l(v) takes min(d, k) entries; u_i = word 0 of
+// philox4x32_10((i, v, call, kStreamSampledBlocks | layer), key = seed)
+struct SampleArgs {
+  uint32_t k0, k1, call, tag;
+  int32_t k;
+};
+
+static SampleArgs make_sample_args(int32_t k, uint64_t seed, uint64_t call, int32_t layer) {
+  return SampleArgs{(uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)call, kStreamSampledBlocks | (uint32_t)layer, k};
+}
+
+// Floyd's sample of k of the d > k positions of node v's row, in draw order: position i of the sample sits in slot i / 32
+// of lane i % 32; unused slots hold INT32_MAX.  Step i: j = d - k + i, t = mulhi(u_i, j + 1); t unless already held, else j.
+__device__ __forceinline__ void floyd_sample(const SampleArgs& sa, int64_t v, int64_t d, int lane,
+                                             int32_t (&held)[kSlots]) {
+  const int k = sa.k;
+  uint32_t u[kSlots];
+#pragma unroll
+  for (int s = 0; s < kSlots; ++s) {
+    held[s] = INT32_MAX;
+    u[s] = 0;
+    const int i = s * 32 + lane;
+    if (s * 32 < k && i < k) u[s] = philox4x32_10(u32x4{(uint32_t)i, (uint32_t)v, sa.call, sa.tag}, sa.k0, sa.k1).x;
+  }
+  for (int i = 0; i < k; ++i) {
+    const int slot = i >> 5, owner = i & 31;
+    uint32_t mine = 0;
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s)
+      if (s == slot) mine = u[s];
+    const uint32_t ui = __shfl_sync(0xffffffffu, mine, owner);
+    const int64_t j = d - k + i;
+    const int32_t t = (int32_t)(((uint64_t)ui * (uint64_t)(j + 1)) >> 32);
+    bool hit = false;
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s)
+      if (s * 32 < k) hit |= held[s] == t;
+    const int32_t take = __any_sync(0xffffffffu, hit) ? (int32_t)j : t;
+#pragma unroll
+    for (int s = 0; s < kSlots; ++s)
+      if (s == slot && lane == owner) held[s] = take;
+  }
+}
+
+// rank[s] = the number of held positions below held[s] (they are distinct): the slot's place in ascending order
+__device__ __forceinline__ void warp_ranks(const int32_t (&held)[kSlots], int k, int32_t (&rank)[kSlots]) {
+#pragma unroll
+  for (int s = 0; s < kSlots; ++s) rank[s] = 0;
+#pragma unroll
+  for (int s2 = 0; s2 < kSlots; ++s2) {
+    if (s2 * 32 >= k) break;
+    for (int src = 0; src < 32; ++src) {
+      const int32_t x = __shfl_sync(0xffffffffu, held[s2], src);
+#pragma unroll
+      for (int s = 0; s < kSlots; ++s)
+        if (s * 32 < k) rank[s] += x < held[s];
+    }
+  }
+}
 
 struct BlocksPlan {
   int64_t n_nodes = 0, cap = 0;       // N; cap = N + 2 (the flags, positions and degrees of nodes 0 .. N, plus a 0)
@@ -47,13 +119,16 @@ __device__ __forceinline__ int64_t blk_node(const int32_t* __restrict__ seeds, c
 }
 
 // one warp per node of the previous level (count: *count_dev, or n when count_dev is NULL): flag the node and, with
-// expand, its row's clamped entries; the dummy N too with expand.  Stores of 1 only: the order of racing stores is moot.
+// expand, its row's clamped entries (kSample: those of S_l(v)); the dummy N too with expand.  Stores of 1 only: the order
+// of racing stores is moot.
+template <bool kSample>
 __global__ void __launch_bounds__(kBlkThreads) blk_mark_kernel(const int64_t* __restrict__ indptr,
                                                                const int32_t* __restrict__ indices, int64_t n_nodes,
                                                                const int32_t* __restrict__ seeds,
                                                                const int32_t* __restrict__ ids,
                                                                const int32_t* __restrict__ count_dev, int64_t n,
-                                                               int32_t expand, int32_t* __restrict__ flag) {
+                                                               int32_t expand, int32_t* __restrict__ flag,
+                                                               SampleArgs sa) {
   const int lane = threadIdx.x & 31;
   const int64_t count = count_dev ? (int64_t)*count_dev : n;
   const int64_t warps = (int64_t)gridDim.x * kBlkWarps;
@@ -64,6 +139,14 @@ __global__ void __launch_bounds__(kBlkThreads) blk_mark_kernel(const int64_t* __
     if (!expand || v >= n_nodes) continue;
     int64_t lo, cnt;
     blk_row(indptr, v, lo, cnt);
+    if (kSample && cnt > sa.k) {
+      int32_t held[kSlots];
+      floyd_sample(sa, v, cnt, lane, held);
+#pragma unroll
+      for (int s = 0; s < kSlots; ++s)
+        if (held[s] != INT32_MAX) flag[blk_clamp(indices[lo + held[s]], n_nodes)] = 1;
+      continue;
+    }
     for (int64_t e = lane; e < cnt; e += 32) flag[blk_clamp(indices[lo + e], n_nodes)] = 1;
   }
 }
@@ -75,11 +158,14 @@ __global__ void __launch_bounds__(kBlkThreads) blk_compact_kernel(const int32_t*
   if (v <= n_nodes && pos[v + 1] != pos[v]) ids[pos[v]] = (int32_t)v;
 }
 
-// deg[i] = the raw degree of the i-th node of V_{l+1} (0 for the dummy), for i < cap (0 past |V_{l+1}|)
+// deg[i] = the raw degree of the i-th node of V_{l+1} (kSample: min(degree, k); 0 for the dummy), for i < cap (0 past
+// |V_{l+1}|)
+template <bool kSample>
 __global__ void __launch_bounds__(kBlkThreads) blk_member_degree_kernel(const int64_t* __restrict__ indptr,
                                                                         int64_t n_nodes, const int32_t* __restrict__ ids,
                                                                         const int32_t* __restrict__ count_dev,
-                                                                        int64_t cap, int64_t* __restrict__ deg) {
+                                                                        int64_t cap, int64_t* __restrict__ deg,
+                                                                        SampleArgs sa) {
   const int64_t count = *count_dev;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (int64_t)gridDim.x * blockDim.x) {
     int64_t c = 0;
@@ -87,42 +173,78 @@ __global__ void __launch_bounds__(kBlkThreads) blk_member_degree_kernel(const in
       int64_t lo;
       blk_row(indptr, ids[i], lo, c);
     }
-    deg[i] = c;
+    deg[i] = kSample ? min(c, (int64_t)sa.k) : c;
   }
 }
 
 // counts[2l] = |V_l| (from its position map)
 __global__ void blk_size_kernel(const int32_t* __restrict__ pos_end, int64_t* __restrict__ count) { *count = *pos_end; }
 
-// deg[p] for the n_local - 1 CSR rows of a block: V_l[p]'s raw degree when it is in V_{l+1} (member: next_pos steps at
-// it), else 0; deg[n_local - 1] = 0 so the exclusive scan's last element is the entry count
+// deg[p] for the n_local - 1 CSR rows of a block: V_l[p]'s raw degree (kSample: min(degree, k)) when it is in V_{l+1}
+// (member: next_pos steps at it), else 0; deg[n_local - 1] = 0 so the exclusive scan's last element is the entry count.
+// kSample with ids == NULL: row p is node p and every row is a member (gs_csr_sample_rows, S_l over all nodes).
+template <bool kSample>
 __global__ void __launch_bounds__(kBlkThreads) blk_local_degree_kernel(const int64_t* __restrict__ indptr,
                                                                        int64_t n_nodes, const int32_t* __restrict__ ids,
                                                                        const int32_t* __restrict__ next_pos,
-                                                                       int64_t n_local, int64_t* __restrict__ deg) {
+                                                                       int64_t n_local, int64_t* __restrict__ deg,
+                                                                       SampleArgs sa) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n_local) return;
   int64_t c = 0;
+  if (kSample && ids == nullptr) {
+    if (p < n_local - 1) {
+      int64_t lo;
+      blk_row(indptr, p, lo, c);
+    }
+    deg[p] = min(c, (int64_t)sa.k);
+    return;
+  }
   const int64_t v = ids[p];
   if (p < n_local - 1 && v < n_nodes && next_pos[v + 1] != next_pos[v]) {
     int64_t lo;
     blk_row(indptr, v, lo, c);
   }
-  deg[p] = c;
+  deg[p] = kSample ? min(c, (int64_t)sa.k) : c;
 }
 
-// one warp per local row: its raw entries, clamped, relabelled through pos, in CSR order
+// one warp per local row: its raw entries, clamped, relabelled through pos, in CSR order.  kSample: the entries of
+// S_l(v) (a row with more than k entries: Floyd's draws again, written in ascending position order); ids == NULL: row p
+// is node p; pos == NULL: the entries are copied as they are (gs_csr_sample_rows)
+template <bool kSample>
 __global__ void __launch_bounds__(kBlkThreads) blk_fill_kernel(const int64_t* __restrict__ indptr,
                                                                const int32_t* __restrict__ indices, int64_t n_nodes,
                                                                const int32_t* __restrict__ ids,
                                                                const int32_t* __restrict__ pos,
                                                                const int64_t* __restrict__ b_indptr, int64_t n_rows,
-                                                               int32_t* __restrict__ b_indices) {
+                                                               int32_t* __restrict__ b_indices, SampleArgs sa) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = (int64_t)gridDim.x * kBlkWarps;
   for (int64_t p = (int64_t)blockIdx.x * kBlkWarps + (threadIdx.x >> 5); p < n_rows; p += warps) {
     const int64_t at = b_indptr[p], cnt = b_indptr[p + 1] - at;
     if (cnt == 0) continue;
+    if (kSample) {
+      const int64_t v = ids ? (int64_t)ids[p] : p;
+      int64_t lo, d;
+      blk_row(indptr, v, lo, d);
+      if (d > cnt) {                                   // cnt = k < d: the sample, ascending
+        int32_t held[kSlots], rank[kSlots];
+        floyd_sample(sa, v, d, lane, held);
+        warp_ranks(held, sa.k, rank);
+#pragma unroll
+        for (int s = 0; s < kSlots; ++s) {
+          if (held[s] == INT32_MAX) continue;
+          const int32_t x = indices[lo + held[s]];
+          b_indices[at + rank[s]] = pos ? pos[blk_clamp(x, n_nodes)] : x;
+        }
+      } else {
+        for (int64_t e = lane; e < cnt; e += 32) {
+          const int32_t x = indices[lo + e];
+          b_indices[at + e] = pos ? pos[blk_clamp(x, n_nodes)] : x;
+        }
+      }
+      continue;
+    }
     const int64_t lo = indptr[ids[p]];
     for (int64_t e = lane; e < cnt; e += 32) b_indices[at + e] = pos[blk_clamp(indices[lo + e], n_nodes)];
   }
@@ -186,6 +308,132 @@ static unsigned blk_grid(int64_t items, int64_t per_block, int64_t max_blocks) {
   return (unsigned)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, max_blocks));
 }
 
+static int32_t check_fanouts(const int32_t* fanouts, int32_t n_layers, int64_t nnz, const char* who) {
+  GS_REQUIRE(fanouts != nullptr, "%s: NULL fanouts", who);
+  GS_REQUIRE(nnz <= INT32_MAX, "%s: sampled rows need nnz < 2^31 (got %lld)", who, (long long)nnz);
+  for (int l = 0; l < n_layers; ++l)
+    GS_REQUIRE(fanouts[l] >= 1 && fanouts[l] <= kMaxFanout, "%s: fanout %d of layer %d outside [1, %d]", who, fanouts[l], l,
+               kMaxFanout);
+  return GS_OK;
+}
+
+// gs_csr_blocks_plan, or with fanouts (host, one per layer) gs_csr_sampled_blocks_plan
+static int32_t blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts, uint64_t seed,
+                           uint64_t call, void* workspace, int64_t workspace_bytes, int64_t* counts_dev, void* stream,
+                           const char* who) {
+  BlocksPlan P;
+  int32_t rc = make_blocks_plan(n_nodes, nnz, n_seeds, n_layers, P, who);
+  if (rc != GS_OK) return rc;
+  GS_REQUIRE(indptr && counts_dev && (nnz == 0 || indices) && (n_seeds == 0 || seeds), "%s: NULL pointer", who);
+  GS_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)P.bytes, "%s: workspace of %lld bytes, %lld needed", who,
+             (long long)workspace_bytes, (long long)P.bytes);
+  if (fanouts && (rc = check_fanouts(fanouts, n_layers, nnz, who)) != GS_OK) return rc;
+  auto mark = fanouts ? blk_mark_kernel<true> : blk_mark_kernel<false>;
+  auto member_degree = fanouts ? blk_member_degree_kernel<true> : blk_member_degree_kernel<false>;
+  cudaStream_t st = (cudaStream_t)stream;
+  const BlocksWs W = blocks_ws(P, workspace);
+  const int64_t max_warp_blocks = (int64_t)sm_count() * 16;
+  const unsigned node_blocks = blk_grid(P.cap, kBlkThreads, INT32_MAX);
+  for (int l = n_layers; l >= 0; --l) {
+    const bool seed_level = l == n_layers;             // level L: the distinct seeds, rows not expanded
+    const int32_t* prev_ids = seed_level ? nullptr : W.ids(l + 1);
+    const int32_t* prev_count = seed_level ? nullptr : W.pos(l + 1) + (P.cap - 1);
+    const int64_t prev_cap = seed_level ? n_seeds : P.cap - 1;
+    const SampleArgs sa = fanouts && !seed_level ? make_sample_args(fanouts[l], seed, call, l) : SampleArgs{};
+    GS_CUDA(cudaMemsetAsync(W.flag, 0, (size_t)P.cap * 4, st));
+    mark<<<blk_grid(prev_cap, kBlkWarps, max_warp_blocks), kBlkThreads, 0, st>>>(
+        indptr, indices, n_nodes, seed_level ? seeds : nullptr, prev_ids, prev_count, n_seeds, seed_level ? 0 : 1,
+        W.flag, sa);
+    rc = launch_check("blk_mark_kernel");
+    if (rc != GS_OK) return rc;
+    size_t cub_bytes = P.cub_bytes;
+    cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(W.cub, cub_bytes, (const int32_t*)W.flag, W.pos(l), (int)P.cap,
+                                                          st);
+    if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
+    blk_compact_kernel<<<node_blocks, kBlkThreads, 0, st>>>(W.pos(l), n_nodes, W.ids(l));
+    rc = launch_check("blk_compact_kernel");
+    if (rc != GS_OK) return rc;
+    if (seed_level) continue;
+    blk_size_kernel<<<1, 1, 0, st>>>(W.pos(l) + (P.cap - 1), counts_dev + 2 * l);
+    rc = launch_check("blk_size_kernel");
+    if (rc != GS_OK) return rc;
+    // the entry count of block l: the degrees (sampled: min(degree, k_l)) of V_{l+1}'s (distinct) nodes
+    member_degree<<<blk_grid(P.cap, kBlkThreads, (int64_t)sm_count() * 8), kBlkThreads, 0, st>>>(
+        indptr, n_nodes, W.ids(l + 1), W.pos(l + 1) + (P.cap - 1), P.cap, W.deg, sa);
+    rc = launch_check("blk_member_degree_kernel");
+    if (rc != GS_OK) return rc;
+    cub_bytes = P.cub_bytes;
+    e = gs_cub::cub::DeviceReduce::Sum(W.cub, cub_bytes, (const int64_t*)W.deg, counts_dev + 2 * l + 1, (int)P.cap, st);
+    if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceReduce::Sum");
+  }
+  return GS_OK;
+}
+
+// gs_csr_blocks_fill, or with fanouts gs_csr_sampled_blocks_fill
+static int32_t blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts, uint64_t seed,
+                           uint64_t call, void* workspace, int64_t workspace_bytes, const int64_t* counts,
+                           int32_t* const* src_ids, int64_t* const* b_indptr, int32_t* const* b_indices,
+                           int32_t* const* b_rows, void* stream, const char* who) {
+  BlocksPlan P;
+  int32_t rc = make_blocks_plan(n_nodes, nnz, n_seeds, n_layers, P, who);
+  if (rc != GS_OK) return rc;
+  GS_REQUIRE(indptr && counts && src_ids && b_indptr && b_indices && b_rows && (nnz == 0 || indices) &&
+                 (n_seeds == 0 || seeds),
+             "%s: NULL pointer", who);
+  GS_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)P.bytes, "%s: workspace of %lld bytes, %lld needed", who,
+             (long long)workspace_bytes, (long long)P.bytes);
+  if (fanouts && (rc = check_fanouts(fanouts, n_layers, nnz, who)) != GS_OK) return rc;
+  auto local_degree = fanouts ? blk_local_degree_kernel<true> : blk_local_degree_kernel<false>;
+  auto fill = fanouts ? blk_fill_kernel<true> : blk_fill_kernel<false>;
+  cudaStream_t st = (cudaStream_t)stream;
+  const BlocksWs W = blocks_ws(P, workspace);
+  const int64_t max_warp_blocks = (int64_t)sm_count() * 16;
+  for (int l = 0; l < n_layers; ++l) {
+    const int64_t n_local = counts[2 * l], entries = counts[2 * l + 1];
+    const bool last = l == n_layers - 1;
+    const int64_t n_out = last ? n_seeds : counts[2 * l + 2];
+    const SampleArgs sa = fanouts ? make_sample_args(fanouts[l], seed, call, l) : SampleArgs{};
+    GS_REQUIRE(n_local >= 1 && n_local <= n_nodes + 1 && entries >= 0 && n_out >= 0, "%s: bad counts for block %d", who,
+               l);
+    GS_REQUIRE(src_ids[l] && b_indptr[l] && (entries == 0 || b_indices[l]) && (n_out == 0 || b_rows[l]),
+               "%s: NULL output of block %d", who, l);
+    GS_CUDA(cudaMemcpyAsync(src_ids[l], W.ids(l), (size_t)n_local * 4, cudaMemcpyDeviceToDevice, st));
+    local_degree<<<blk_grid(n_local, kBlkThreads, INT32_MAX), kBlkThreads, 0, st>>>(indptr, n_nodes, W.ids(l),
+                                                                                    W.pos(l + 1), n_local, W.deg, sa);
+    rc = launch_check("blk_local_degree_kernel");
+    if (rc != GS_OK) return rc;
+    size_t cub_bytes = P.cub_bytes;
+    cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(W.cub, cub_bytes, (const int64_t*)W.deg, b_indptr[l],
+                                                          (int)n_local, st);
+    if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
+    if (entries > 0) {
+      fill<<<blk_grid(n_local - 1, kBlkWarps, max_warp_blocks), kBlkThreads, 0, st>>>(
+          indptr, indices, n_nodes, W.ids(l), W.pos(l), b_indptr[l], n_local - 1, b_indices[l], sa);
+      rc = launch_check("blk_fill_kernel");
+      if (rc != GS_OK) return rc;
+    }
+    if (n_out > 0) {
+      blk_rows_kernel<<<blk_grid(n_out, kBlkThreads, INT32_MAX), kBlkThreads, 0, st>>>(
+          last ? seeds : nullptr, W.ids(l + 1), n_out, n_nodes, W.pos(l), b_rows[l]);
+      rc = launch_check("blk_rows_kernel");
+      if (rc != GS_OK) return rc;
+    }
+  }
+  return GS_OK;
+}
+
+static int32_t sample_rows_plan(int64_t n_nodes, int64_t nnz, size_t& cub_bytes, size_t& bytes, const char* who) {
+  GS_REQUIRE(n_nodes >= 0 && n_nodes < 0x7fffffffLL - 2, "%s: n_nodes must be in [0, 2^31 - 3)", who);
+  GS_REQUIRE(nnz >= 0 && nnz <= INT32_MAX, "%s: sampled rows need 0 <= nnz < 2^31", who);
+  cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (const int64_t*)nullptr, (int64_t*)nullptr,
+                                                        (int)(n_nodes + 1));
+  if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceScan::ExclusiveSum (size query)");
+  bytes = align256((size_t)(n_nodes + 1) * 8) + align256(cub_bytes);
+  return GS_OK;
+}
+
 }  // namespace gs
 
 extern "C" {
@@ -199,98 +447,72 @@ int64_t gs_csr_blocks_workspace_bytes(int64_t n_nodes, int64_t nnz, int64_t n_se
 int32_t gs_csr_blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
                            const int32_t* seeds, int64_t n_seeds, int32_t n_layers, void* workspace,
                            int64_t workspace_bytes, int64_t* counts_dev, void* stream) {
-  const char* who = "gs_csr_blocks_plan";
-  gs::BlocksPlan P;
-  int32_t rc = gs::make_blocks_plan(n_nodes, nnz, n_seeds, n_layers, P, who);
-  if (rc != GS_OK) return rc;
-  GS_REQUIRE(indptr && counts_dev && (nnz == 0 || indices) && (n_seeds == 0 || seeds), "%s: NULL pointer", who);
-  GS_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)P.bytes, "%s: workspace of %lld bytes, %lld needed", who,
-             (long long)workspace_bytes, (long long)P.bytes);
-  cudaStream_t st = (cudaStream_t)stream;
-  const gs::BlocksWs W = gs::blocks_ws(P, workspace);
-  const int64_t max_warp_blocks = (int64_t)gs::sm_count() * 16;
-  const unsigned node_blocks = gs::blk_grid(P.cap, gs::kBlkThreads, INT32_MAX);
-  for (int l = n_layers; l >= 0; --l) {
-    const bool seed_level = l == n_layers;             // level L: the distinct seeds, rows not expanded
-    const int32_t* prev_ids = seed_level ? nullptr : W.ids(l + 1);
-    const int32_t* prev_count = seed_level ? nullptr : W.pos(l + 1) + (P.cap - 1);
-    const int64_t prev_cap = seed_level ? n_seeds : P.cap - 1;
-    GS_CUDA(cudaMemsetAsync(W.flag, 0, (size_t)P.cap * 4, st));
-    gs::blk_mark_kernel<<<gs::blk_grid(prev_cap, gs::kBlkWarps, max_warp_blocks), gs::kBlkThreads, 0, st>>>(
-        indptr, indices, n_nodes, seed_level ? seeds : nullptr, prev_ids, prev_count, n_seeds, seed_level ? 0 : 1,
-        W.flag);
-    rc = gs::launch_check("blk_mark_kernel");
-    if (rc != GS_OK) return rc;
-    size_t cub_bytes = P.cub_bytes;
-    cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(W.cub, cub_bytes, (const int32_t*)W.flag, W.pos(l), (int)P.cap,
-                                                          st);
-    if (e != cudaSuccess) return gs::cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
-    gs::blk_compact_kernel<<<node_blocks, gs::kBlkThreads, 0, st>>>(W.pos(l), n_nodes, W.ids(l));
-    rc = gs::launch_check("blk_compact_kernel");
-    if (rc != GS_OK) return rc;
-    if (seed_level) continue;
-    gs::blk_size_kernel<<<1, 1, 0, st>>>(W.pos(l) + (P.cap - 1), counts_dev + 2 * l);
-    rc = gs::launch_check("blk_size_kernel");
-    if (rc != GS_OK) return rc;
-    // the entry count of block l: the degrees of V_{l+1}'s (distinct) nodes
-    gs::blk_member_degree_kernel<<<gs::blk_grid(P.cap, gs::kBlkThreads, (int64_t)gs::sm_count() * 8), gs::kBlkThreads, 0,
-                                   st>>>(indptr, n_nodes, W.ids(l + 1), W.pos(l + 1) + (P.cap - 1), P.cap, W.deg);
-    rc = gs::launch_check("blk_member_degree_kernel");
-    if (rc != GS_OK) return rc;
-    cub_bytes = P.cub_bytes;
-    e = gs_cub::cub::DeviceReduce::Sum(W.cub, cub_bytes, (const int64_t*)W.deg, counts_dev + 2 * l + 1, (int)P.cap, st);
-    if (e != cudaSuccess) return gs::cuda_fail(e, "cub::DeviceReduce::Sum");
-  }
-  return GS_OK;
+  return gs::blocks_plan(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, nullptr, 0, 0, workspace,
+                         workspace_bytes, counts_dev, stream, "gs_csr_blocks_plan");
 }
 
 int32_t gs_csr_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
                            const int32_t* seeds, int64_t n_seeds, int32_t n_layers, void* workspace,
                            int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
                            int64_t* const* b_indptr, int32_t* const* b_indices, int32_t* const* b_rows, void* stream) {
-  const char* who = "gs_csr_blocks_fill";
-  gs::BlocksPlan P;
-  int32_t rc = gs::make_blocks_plan(n_nodes, nnz, n_seeds, n_layers, P, who);
+  return gs::blocks_fill(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, nullptr, 0, 0, workspace,
+                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, stream, "gs_csr_blocks_fill");
+}
+
+int32_t gs_csr_sampled_blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                   const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts,
+                                   uint64_t seed, uint64_t call, void* workspace, int64_t workspace_bytes,
+                                   int64_t* counts_dev, void* stream) {
+  const char* who = "gs_csr_sampled_blocks_plan";
+  GS_REQUIRE(fanouts != nullptr, "%s: NULL fanouts", who);
+  return gs::blocks_plan(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, fanouts, seed, call, workspace,
+                         workspace_bytes, counts_dev, stream, who);
+}
+
+int32_t gs_csr_sampled_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                   const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts,
+                                   uint64_t seed, uint64_t call, void* workspace, int64_t workspace_bytes,
+                                   const int64_t* counts, int32_t* const* src_ids, int64_t* const* b_indptr,
+                                   int32_t* const* b_indices, int32_t* const* b_rows, void* stream) {
+  const char* who = "gs_csr_sampled_blocks_fill";
+  GS_REQUIRE(fanouts != nullptr, "%s: NULL fanouts", who);
+  return gs::blocks_fill(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, fanouts, seed, call, workspace,
+                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, stream, who);
+}
+
+int64_t gs_csr_sample_rows_workspace_bytes(int64_t n_nodes, int64_t nnz) {
+  size_t cub_bytes = 0, bytes = 0;
+  if (gs::sample_rows_plan(n_nodes, nnz, cub_bytes, bytes, "gs_csr_sample_rows_workspace_bytes") != GS_OK) return -1;
+  return (int64_t)bytes;
+}
+
+int32_t gs_csr_sample_rows(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t k,
+                           uint64_t seed, uint64_t call, int32_t layer, void* workspace, int64_t workspace_bytes,
+                           int64_t* out_indptr, int32_t* out_indices, void* stream) {
+  const char* who = "gs_csr_sample_rows";
+  size_t cub_bytes = 0, bytes = 0;
+  int32_t rc = gs::sample_rows_plan(n_nodes, nnz, cub_bytes, bytes, who);
   if (rc != GS_OK) return rc;
-  GS_REQUIRE(indptr && counts && src_ids && b_indptr && b_indices && b_rows && (nnz == 0 || indices) &&
-                 (n_seeds == 0 || seeds),
-             "%s: NULL pointer", who);
-  GS_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)P.bytes, "%s: workspace of %lld bytes, %lld needed", who,
-             (long long)workspace_bytes, (long long)P.bytes);
+  GS_REQUIRE(k >= 1 && k <= gs::kMaxFanout, "%s: fanout %d outside [1, %d]", who, k, gs::kMaxFanout);
+  GS_REQUIRE(layer >= 0 && layer < GS_MAX_BLOCK_LAYERS, "%s: layer %d outside [0, %d)", who, layer, GS_MAX_BLOCK_LAYERS);
+  GS_REQUIRE(indptr && out_indptr && (nnz == 0 || indices), "%s: NULL pointer", who);
+  GS_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)bytes, "%s: workspace of %lld bytes, %lld needed", who,
+             (long long)workspace_bytes, (long long)bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  const gs::BlocksWs W = gs::blocks_ws(P, workspace);
-  const int64_t max_warp_blocks = (int64_t)gs::sm_count() * 16;
-  for (int l = 0; l < n_layers; ++l) {
-    const int64_t n_local = counts[2 * l], entries = counts[2 * l + 1];
-    const bool last = l == n_layers - 1;
-    const int64_t n_out = last ? n_seeds : counts[2 * l + 2];
-    GS_REQUIRE(n_local >= 1 && n_local <= n_nodes + 1 && entries >= 0 && n_out >= 0, "%s: bad counts for block %d", who,
-               l);
-    GS_REQUIRE(src_ids[l] && b_indptr[l] && (entries == 0 || b_indices[l]) && (n_out == 0 || b_rows[l]),
-               "%s: NULL output of block %d", who, l);
-    GS_CUDA(cudaMemcpyAsync(src_ids[l], W.ids(l), (size_t)n_local * 4, cudaMemcpyDeviceToDevice, st));
-    gs::blk_local_degree_kernel<<<gs::blk_grid(n_local, gs::kBlkThreads, INT32_MAX), gs::kBlkThreads, 0, st>>>(
-        indptr, n_nodes, W.ids(l), W.pos(l + 1), n_local, W.deg);
-    rc = gs::launch_check("blk_local_degree_kernel");
-    if (rc != GS_OK) return rc;
-    size_t cub_bytes = P.cub_bytes;
-    cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(W.cub, cub_bytes, (const int64_t*)W.deg, b_indptr[l],
-                                                          (int)n_local, st);
-    if (e != cudaSuccess) return gs::cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
-    if (entries > 0) {
-      gs::blk_fill_kernel<<<gs::blk_grid(n_local - 1, gs::kBlkWarps, max_warp_blocks), gs::kBlkThreads, 0, st>>>(
-          indptr, indices, n_nodes, W.ids(l), W.pos(l), b_indptr[l], n_local - 1, b_indices[l]);
-      rc = gs::launch_check("blk_fill_kernel");
-      if (rc != GS_OK) return rc;
-    }
-    if (n_out > 0) {
-      gs::blk_rows_kernel<<<gs::blk_grid(n_out, gs::kBlkThreads, INT32_MAX), gs::kBlkThreads, 0, st>>>(
-          last ? seeds : nullptr, W.ids(l + 1), n_out, n_nodes, W.pos(l), b_rows[l]);
-      rc = gs::launch_check("blk_rows_kernel");
-      if (rc != GS_OK) return rc;
-    }
-  }
-  return GS_OK;
+  int64_t* deg = (int64_t*)workspace;
+  void* cub = (char*)workspace + gs::align256((size_t)(n_nodes + 1) * 8);
+  const gs::SampleArgs sa = gs::make_sample_args(k, seed, call, layer);
+  gs::blk_local_degree_kernel<true><<<gs::blk_grid(n_nodes + 1, gs::kBlkThreads, INT32_MAX), gs::kBlkThreads, 0, st>>>(
+      indptr, n_nodes, nullptr, nullptr, n_nodes + 1, deg, sa);
+  rc = gs::launch_check("blk_local_degree_kernel");
+  if (rc != GS_OK) return rc;
+  cudaError_t e = gs_cub::cub::DeviceScan::ExclusiveSum(cub, cub_bytes, (const int64_t*)deg, out_indptr,
+                                                        (int)(n_nodes + 1), st);
+  if (e != cudaSuccess) return gs::cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
+  if (out_indices == nullptr || n_nodes == 0) return GS_OK;
+  gs::blk_fill_kernel<true><<<gs::blk_grid(n_nodes, gs::kBlkWarps, (int64_t)gs::sm_count() * 16), gs::kBlkThreads, 0,
+                              st>>>(indptr, indices, n_nodes, nullptr, nullptr, out_indptr, n_nodes, out_indices, sa);
+  return gs::launch_check("blk_fill_kernel");
 }
 
 }  // extern "C"

@@ -21,6 +21,12 @@ reads the global table: the means through the global CSR with rows = V_1, the po
 ops.TableRows), reduced through block 0.  Same bits as the whole-graph pass for the seeds; every buffer is block-sized.
 The blocks and their transposes are built per call, not cached.
 
+Sampled minibatches (sampled_minibatch_*; contract: oracle/sampled_blocks.py) run the same layers over blocks whose rows
+keep at most k_l sampled entries (ops.csr_blocks with fanouts).  Layer 0 cannot reduce the global table through the
+global CSR, since its rows are sampled: the means reduce block 0 over V_0's rows (gathered by id, widened to fp32), the
+pools' MLP reads V_0's rows by id as before; the self rows are V_1's table rows by id in both.  Everything else is the
+minibatch path.  The draws are keyed by the model's neigh_sampler (seed, counter); one block set advances the counter by 1.
+
 Training dropout (dropout=p > 0; contract: oracle/full_neighbor_dropout.py) masks by global identities: per CSR entry for
 the means' neighbour branch (gs_csr_aggregate_dropout, the entry's global CSR position), per node for the mean's self
 rows, GCN's own row and the pools' MLP input (ops.dropout_apply by id).  Each graph carries the position map of its
@@ -101,9 +107,11 @@ class _FullLayer(object):
     ids), the pools' MLP on V_0's rows; everything after the MLP, and the whole backward, is in the graph's (block 0's)
     local space."""
 
-    def __init__(self, agg, graph, rows, src_ids=None, table_csr=None):
+    def __init__(self, agg, graph, rows, src_ids=None, table_csr=None, self_ids=None):
+        """self_ids (a sampled block 0, with src_ids and no table_csr): V_1's global ids - the self rows are read from the
+        table by id, and the reductions run over the block itself, the means' on V_0's gathered rows."""
         self.agg, self.graph, self.rows = agg, graph, rows
-        self.src_ids, self.table_csr = src_ids, table_csr
+        self.src_ids, self.table_csr, self.self_ids = src_ids, table_csr, self_ids
         self.sites = None                       # training dropout: {"neigh", "self"} or {"mlp"} -> (seed, call, rate)
         self.gcn = isinstance(agg, GCNAggregator)
         self.pool = isinstance(agg, MaxPoolingAggregator)
@@ -128,12 +136,17 @@ class _FullLayer(object):
         agg, g, rows = self.agg, self.graph, self.rows
         self.table = h if self.src_ids is not None else None
         indptr, indices, h_rows = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows)
+        hn, n_rows = h, h_rows                  # the means' reduction source and its rows
+        if self.self_ids is not None:           # a sampled block 0: self rows by global id, reductions in the block
+            h_rows = self.self_ids
+            if not self.pool:
+                hn = ops.gather_rows_f32(h, self.src_ids)
         s = self.sites
         # the means' masks: the table CSR is the global one (positions by node id), else the graph's own map
         tgraph = FullNeighborGraph(indptr, indices) if self.table_csr is not None else g
         drop = {} if s is None or self.pool else {"dropout": (s["neigh"], s["self"], tgraph.pos_map)}
         if self.gcn:
-            m = ops.csr_aggregate(h, indptr, indices, "mean_self", rows=h_rows, **drop)
+            m = ops.csr_aggregate(hn, indptr, indices, "mean_self", rows=n_rows, **drop)
             return [(m, agg.neigh_input_dim, agg.vars["weights"])]
         widen = h.dtype != torch.float32
         n = h.shape[0] if h_rows is None else h_rows.numel()
@@ -141,7 +154,7 @@ class _FullLayer(object):
         if not self.pool:
             if s is not None:                                        # the self rows by node id, after widening
                 hs = ops.dropout_apply(hs, s["self"], pos_ids=tgraph.node_ids(h_rows), out=None if hs is h else hs)
-            m = ops.csr_aggregate(h, indptr, indices, "mean", rows=h_rows, **drop)
+            m = ops.csr_aggregate(hn, indptr, indices, "mean", rows=n_rows, **drop)
             return [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
         if self.src_ids is None:
             x = z = _rows(h, None, 0, h.shape[0], True) if widen else h
@@ -281,31 +294,65 @@ def _inputs(model, indptr, indices, node_ids):
     return indptr, indices, ids
 
 
-def minibatch_layers(aggregators, indptr, indices, ids):
-    """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped)."""
+def minibatch_layers(aggregators, indptr, indices, ids, draw=None):
+    """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped); draw =
+    (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead."""
     L = len(aggregators)
-    blocks = ops.csr_blocks(indptr, indices, ids, L)
+    if draw is None:
+        blocks = ops.csr_blocks(indptr, indices, ids, L)
+    else:
+        fanouts, seed, call = draw
+        blocks = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call)
     layers = []
     for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
         graph = FullNeighborGraph(b.indptr, b.indices, pos_map=(indptr, b.src_ids, indices.numel()))
         if layer == 0:
             v1 = blocks[1].src_ids if L > 1 else ids
-            layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
+            if draw is not None:
+                layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, self_ids=v1))
+            else:
+                layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
         else:
             layers.append(_FullLayer(agg, graph, b.rows))
     return layers
 
 
-def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None):
+def refuse_sampled(model, training):
+    """The NotImplementedErrors of the sampled-block entry points: refuse_full_neighbor's, CUDA-graph capture and, when
+    training, a model with dropout_rate > 0."""
+    if training and getattr(model, "dropout_rate", 0.):
+        raise NotImplementedError("sampled-block training with dropout > 0 is not implemented (the per-edge masks are "
+                                  "keyed by global CSR positions, and a sampled block entry does not keep its position)")
+    refuse_full_neighbor(model, training)
+    refuse_capture("a sampled-block minibatch (it reads the block sizes back)")
+
+
+def sampled_draw(model):
+    """(fanouts, seed, call) of one sampled block set - block l takes layer_infos[l].num_samples, the draws are keyed by
+    the neigh_sampler's seed at its counter - and advances that counter by 1."""
+    sampler = model.layer_infos[0].neigh_sampler
+    fanouts = ops.check_fanouts([info.num_samples for info in model.layer_infos], len(model.layer_infos))
+    call = int(sampler.counter)
+    sampler.counter = call + 1
+    return fanouts, int(sampler.seed), call
+
+
+def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False):
     """The checked layers of one call: over the receptive-field blocks of node_ids (minibatch; reads the block sizes
-    back once), else over the whole CSR - the model's cached FullNeighborGraph when training, an uncached one otherwise
-    (inference builds no transposes, and must not evict the ones a training CSR has cached)."""
-    refuse_full_neighbor(model, training, dropout)
+    back once; sampled: over sampled blocks), else over the whole CSR - the model's cached FullNeighborGraph when
+    training, an uncached one otherwise (inference builds no transposes, and must not evict the ones a training CSR has
+    cached)."""
+    if sampled:
+        refuse_sampled(model, training)
+    else:
+        refuse_full_neighbor(model, training, dropout)
     if minibatch:
         refuse_capture("a full-neighbourhood minibatch (it reads the block sizes back)")
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
     if model.aggregators is None:
         model.aggregators = build_aggregators(model)
+    if sampled:
+        return minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model))
     if minibatch:
         return minibatch_layers(model.aggregators, indptr, indices, ids)
     graph = full_neighbor_graph(model, indptr, indices) if training else FullNeighborGraph(indptr, indices)
@@ -313,23 +360,28 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None)
     return [_FullLayer(agg, graph, ids if layer == L - 1 else None) for layer, agg in enumerate(model.aggregators)]
 
 
-def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False):
-    """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings), without autograd."""
+def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False, sampled=False):
+    """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings; sampled:
+    sampled_minibatch_embeddings), without autograd."""
     h = model.features
     with torch.no_grad():
-        for fl in _layers(model, indptr, indices, node_ids, False, minibatch):
+        for fl in _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled):
             h = fl.agg._finish(fl.forward(h, None), fl.agg._combine())
         if normalize:
             h = ops.l2_normalize_rows_(h.contiguous())
     return h
 
 
-def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False, dropout=None):
-    """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch) with an autograd graph over the
+def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False, dropout=None,
+                          sampled=False):
+    """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch, sampled) with an autograd graph over the
     aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
-    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them."""
+    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them (not with
+    sampled)."""
     p = check_full_neighbor_dropout(dropout)
-    layers = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p)
+    if sampled and p:
+        raise NotImplementedError("sampled-block training with dropout > 0 is not implemented")
+    layers = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled)
     if p:
         pool = isinstance(layers[0].agg, MaxPoolingAggregator)
         plan = full_neighbor_site_plan("maxpool" if pool else "mean", len(layers))

@@ -275,6 +275,17 @@ class SampleAndAggregate(object):
         from .full_neighbor_training import full_neighbor_embeddings
         return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True)
 
+    def sampled_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True):
+        """Embeddings of node_ids over SAMPLED receptive-field blocks (contract: oracle/sampled_blocks.py): block l keeps
+        at most layer_infos[l].num_samples entries of each row of the full CSR, drawn without replacement (Floyd's
+        algorithm, Philox keyed by layer_infos[0].neigh_sampler's seed at its counter, which advances by 1), and every
+        distinct node of a block is computed once per layer - GraphSAGE's minibatch over sampled blocks, against
+        forward()'s one tree per seed over the padded table.  With every fanout >= the largest degree it is
+        full_neighbor_minibatch_embeddings, bit for bit.  Reads the block sizes back once per call, so it cannot be
+        captured in a CUDA graph.  Same refusals as full_neighbor_embeddings."""
+        from .full_neighbor_training import full_neighbor_embeddings
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, sampled=True)
+
     def _csr_input(self, t, dtype, name):
         """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""
         if not torch.is_tensor(t):

@@ -697,13 +697,33 @@ def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out
 CsrBlock = collections.namedtuple("CsrBlock", ["src_ids", "indptr", "indices", "rows"])   # one layer of csr_blocks
 
 
-def csr_blocks(indptr, indices, seeds, n_layers):
+def check_fanouts(fanouts, n_layers):
+    """fanouts as a list of n_layers ints in [1, MAX_FANOUT] (ValueError otherwise)."""
+    fan = [int(k) for k in fanouts]
+    if len(fan) != int(n_layers):
+        raise ValueError("fanouts must have one entry per layer (%d, got %d)" % (n_layers, len(fan)))
+    for k in fan:
+        if not 1 <= k <= _lib.MAX_FANOUT:
+            raise ValueError("a fanout must be in [1, %d] (got %d)" % (_lib.MAX_FANOUT, k))
+    return fan
+
+
+def _sampled_csr_args(nnz):
+    if nnz > 2**31 - 1:
+        raise ValueError("sampled rows need fewer than 2^31 CSR entries (got %d)" % nnz)
+
+
+def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0):
     """The receptive field of `seeds` over n_layers layers of whole neighbourhoods (gs_csr_blocks_plan / _fill; contract
     in oracle/full_neighbor_blocks.py): a list, index l = layer l, of CsrBlock(src_ids int32 V_l, indptr int64 [|V_l|],
     indices int32, rows int32).  A block is a CSR over |V_l| - 1 local nodes whose last local row is the dummy, so
     csr_aggregate(table of V_l's rows, indptr, indices, rows=rows) gives the whole-graph layer's rows of the next level.
     Built on the device; the 2L sizes are read back once to allocate the outputs - one device-to-host copy (and so a
-    synchronisation) per call, not meant for capture."""
+    synchronisation) per call, not meant for capture.
+    fanouts: None (whole rows), or one fanout per layer, each in [1, MAX_FANOUT]: block l is then built over S_l, at
+    most fanouts[l] entries of each row drawn without replacement by Floyd's algorithm from Philox words keyed by `seed`
+    at counter word `call` (gs_csr_sampled_blocks_plan / _fill; contract in oracle/sampled_blocks.py).  The same
+    (seed, call) gives the same bytes."""
     require_cuda(indptr, indices, seeds)
     if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
         raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
@@ -712,6 +732,10 @@ def csr_blocks(indptr, indices, seeds, n_layers):
     if not 1 <= L <= _lib.MAX_BLOCK_LAYERS:
         raise ValueError("n_layers must be in [1, %d] (got %d)" % (_lib.MAX_BLOCK_LAYERS, L))
     n_nodes, nnz, n = indptr.numel() - 1, indices.numel(), seeds.numel()
+    if fanouts is not None:
+        fan = (_lib.c_i32 * L)(*check_fanouts(fanouts, L))
+        _sampled_csr_args(nnz)
+        draw = (fan, int(seed) & _U64, int(call) & _U64)
     nbytes = lib().gs_csr_blocks_workspace_bytes(n_nodes, nnz, n, L)
     if nbytes < 0:
         check(-1)
@@ -719,8 +743,11 @@ def csr_blocks(indptr, indices, seeds, n_layers):
     ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
     counts = torch.empty((2 * L,), dtype=torch.int64, device=dev)
     ev = _probe("csr_blocks/%d" % n)
-    check(lib().gs_csr_blocks_plan(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L,
-                                   ptr(ws), nbytes, ptr(counts), stream_ptr()))
+    head = (ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L)
+    if fanouts is None:
+        check(lib().gs_csr_blocks_plan(*head, ptr(ws), nbytes, ptr(counts), stream_ptr()))
+    else:
+        check(lib().gs_csr_sampled_blocks_plan(*head, *draw, ptr(ws), nbytes, ptr(counts), stream_ptr()))
     sizes = [int(x) for x in counts.tolist()]                # the one device-to-host read
     out_rows = [sizes[2 * l + 2] for l in range(L - 1)] + [n]
     blocks = [CsrBlock(torch.empty((sizes[2 * l],), dtype=torch.int32, device=dev),
@@ -728,10 +755,42 @@ def csr_blocks(indptr, indices, seeds, n_layers):
                        torch.empty((sizes[2 * l + 1],), dtype=torch.int32, device=dev),
                        torch.empty((out_rows[l],), dtype=torch.int32, device=dev)) for l in range(L)]
     arrs = [(_lib.c_vp * L)(*[ptr(b[k]) if b[k].numel() else 0 for b in blocks]) for k in range(4)]
-    check(lib().gs_csr_blocks_fill(ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L,
-                                   ptr(ws), nbytes, (_lib.c_i64 * (2 * L))(*sizes), *arrs, stream_ptr()))
+    sz = (_lib.c_i64 * (2 * L))(*sizes)
+    if fanouts is None:
+        check(lib().gs_csr_blocks_fill(*head, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
+    else:
+        check(lib().gs_csr_sampled_blocks_fill(*head, *draw, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
     _launched(6 * L + 4, ev)           # plan: mark, compact, size, degrees per level; fill: degrees, fill, rows (+ CUB)
     return blocks
+
+
+def sample_csr_rows(indptr, indices, k, seed, call, layer):
+    """S_layer over every node (gs_csr_sample_rows; contract in oracle/sampled_blocks.py): (indptr int64 [N + 1], indices
+    int32), row v holding min(d, k) entries of v's row - all of them in CSR order when d <= k, else Floyd's k draws in
+    ascending position order - with the entries' values as stored (not clamped).  The draws are the ones
+    csr_blocks(..., fanouts, seed, call) makes for its block `layer`.  Reads the entry count back once."""
+    indptr, indices = _csr_args(indptr, indices)
+    k, layer = int(k), int(layer)
+    if not 1 <= k <= _lib.MAX_FANOUT:
+        raise ValueError("a fanout must be in [1, %d] (got %d)" % (_lib.MAX_FANOUT, k))
+    if not 0 <= layer < _lib.MAX_BLOCK_LAYERS:
+        raise ValueError("layer must be in [0, %d) (got %d)" % (_lib.MAX_BLOCK_LAYERS, layer))
+    n_nodes, nnz = indptr.numel() - 1, indices.numel()
+    _sampled_csr_args(nnz)
+    nbytes = lib().gs_csr_sample_rows_workspace_bytes(n_nodes, nnz)
+    if nbytes < 0:
+        check(-1)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=indptr.device)
+    out_indptr = torch.empty((n_nodes + 1,), dtype=torch.int64, device=indptr.device)
+    args = (ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, k, int(seed) & _U64, int(call) & _U64, layer, ptr(ws),
+            nbytes, ptr(out_indptr))
+    check(lib().gs_csr_sample_rows(*args, 0, stream_ptr()))
+    total = int(out_indptr[-1].item())                       # the one device-to-host read
+    out_indices = torch.empty((total,), dtype=torch.int32, device=indptr.device)
+    if total:
+        check(lib().gs_csr_sample_rows(*args, ptr(out_indices), stream_ptr()))
+    _launched(4 if total else 2)
+    return out_indptr, out_indices
 
 
 class TableRows(object):

@@ -725,6 +725,24 @@ class SupervisedGraphsage(SampleAndAggregate):
         +-5.  Returns the detached loss."""
         return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
 
+    def sampled_minibatch_outputs(self, indptr, indices, node_ids):
+        """outputs() over sampled receptive-field blocks (SampleAndAggregate.sampled_minibatch_embeddings; contract:
+        oracle/sampled_blocks.py), with an autograd graph over the aggregator weights and (identity_dim > 0) the node
+        embeddings.  One block set per call: the sampler's counter advances by 1.  Refused (NotImplementedError): what
+        full_neighbor_outputs refuses, CUDA-graph capture, and a model with dropout_rate > 0 (the per-edge masks name
+        global CSR positions, which a sampled block entry does not keep)."""
+        from .full_neighbor_training import full_neighbor_outputs
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True)
+
+    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels):
+        """loss() over sampled_minibatch_outputs: the same head, cross-entropy and weight decay."""
+        return self._logits_loss(self._node_pred(self.sampled_minibatch_outputs(indptr, indices, node_ids)), labels)
+
+    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels):
+        """One Adam step on sampled_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the detached
+        loss."""
+        return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels))
+
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on
         full_neighbor_embeddings(indptr, indices, node_ids) - deterministic, no sampling, no dropout."""

@@ -867,6 +867,39 @@ int32_t gs_csr_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_
                            int64_t* const* indptr_out, int32_t* const* indices_out, int32_t* const* rows_out,
                            void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Sampled receptive-field blocks (sampled_minibatch_*): the blocks above built over S_l, a per-layer sample of each row.
+ * Contract: oracle/sampled_blocks.py.  S_l(v) for node v < N with d = the raw row length and k = fanouts[l] (1 <= k <=
+ * GS_MAX_FANOUT): every entry in CSR order when d <= k; else the k entry positions of Floyd's algorithm - for i = 0 .. k-1:
+ * j = d - k + i, t = (u_i * (j + 1)) >> 32, take t unless already taken, else j - sorted ascending.  Positions, not ids:
+ * a repeated id is drawn as separate entries.  u_i = word 0 of Philox4x32-10(counter = (i, v, call mod 2^32,
+ * 0x70000000 | l), key = seed).  The draw of t is biased by at most j / 2^32.
+ * gs_csr_sampled_blocks_plan / _fill - gs_csr_blocks_plan / _fill with V_l = sorted-unique(V_{l+1}, the clamped entries
+ *   of S_l over V_{l+1}'s nodes, N) and block l's member rows holding S_l(v); the same workspace
+ *   (gs_csr_blocks_workspace_bytes), layout and rules.  The plan and the fill draw the same words again (nothing is
+ *   stored between them).  fanouts: HOST int32 [n_layers], block l uses fanouts[l]; nnz < 2^31.  Block entries:
+ *   sum over V_{l+1} of min(d, k_l).  Integer work only, no atomics: two calls with the same (seed, call) give the same
+ *   bytes.
+ * gs_csr_sample_rows - S_layer over every node as a CSR: out_indptr int64 [N + 1] (exclusive scan of min(d, k)), and, when
+ *   out_indices is not NULL, out_indices int32 [out_indptr[N]] = the sampled entries as stored in `indices` (not
+ *   clamped).  Call it with out_indices NULL, read out_indptr[N], then again with the array.  workspace:
+ *   gs_csr_sample_rows_workspace_bytes(...) bytes; 0 <= layer < GS_MAX_BLOCK_LAYERS.
+ * --------------------------------------------------------------------------------------------- */
+#define GS_MAX_FANOUT 256
+int32_t gs_csr_sampled_blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                   const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts,
+                                   uint64_t seed, uint64_t call, void* workspace, int64_t workspace_bytes,
+                                   int64_t* counts_dev, void* stream);
+int32_t gs_csr_sampled_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                   const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts,
+                                   uint64_t seed, uint64_t call, void* workspace, int64_t workspace_bytes,
+                                   const int64_t* counts, int32_t* const* src_ids, int64_t* const* indptr_out,
+                                   int32_t* const* indices_out, int32_t* const* rows_out, void* stream);
+int64_t gs_csr_sample_rows_workspace_bytes(int64_t n_nodes, int64_t nnz);
+int32_t gs_csr_sample_rows(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t k,
+                           uint64_t seed, uint64_t call, int32_t layer, void* workspace, int64_t workspace_bytes,
+                           int64_t* out_indptr, int32_t* out_indices /* may be NULL */, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
