@@ -61,12 +61,19 @@ def perm_prefix(seed, counter, max_deg, k):
     return p[:k].copy()
 
 
-def sample_padded(adj, ids, k, seed, counter, col_perm=None):
-    """out[i, j] = adj[ids[i], pi[j]]; adj int32 [N+1, MD], ids int32 [n] -> int32 [n, k]."""
-    adj = np.asarray(adj)
+def clamp_rows(ids, n_rows):
+    """ids outside [0, n_rows) read the table's last row, the dummy row n_rows - 1 (int64)."""
     ids = np.asarray(ids).astype(np.int64)
+    return np.where((ids < 0) | (ids >= n_rows), n_rows - 1, ids)
+
+
+def sample_padded(adj, ids, k, seed, counter, col_perm=None):
+    """out[i, j] = adj[ids[i], pi[j]]; adj int32 [N+1, MD], ids int32 [n] -> int32 [n, k].  An id outside [0, N+1)
+    reads the dummy row N (clamp_rows)."""
+    adj = np.asarray(adj)
+    ids = clamp_rows(ids, adj.shape[0])
     pi = perm_prefix(seed, counter, adj.shape[1], k) if col_perm is None else np.asarray(col_perm)[:k]
-    return adj[ids][:, pi].astype(np.int32).reshape(len(ids), k)
+    return adj[ids[:, None], np.asarray(pi, dtype=np.int64)[None, :]].astype(np.int32).reshape(len(ids), k)
 
 
 def sample_csr(indptr, indices, ids, k, seed, counter, replace_if_short=True, pad_id=-1):
