@@ -170,6 +170,8 @@ _SIGNATURES = {
     "gs_csr_aggregate": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp]),
     "gs_csr_aggregate_dropout": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32,
                                          DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "gs_csr_aggregate_dropout_offsets": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32,
+                                                 DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp]),
     "gs_csr_transpose_workspace_bytes": (c_i64, [c_i64, c_i64, c_i32]),
     "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gs_csr_max_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64,
@@ -184,6 +186,10 @@ _SIGNATURES = {
     "gs_csr_sampled_blocks_fill": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64, c_u64,
                                            c_vp, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
                                            ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), c_vp]),
+    "gs_csr_sampled_blocks_fill_offsets": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64,
+                                                   c_u64, c_vp, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_vp),
+                                                   ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
+                                                   ctypes.POINTER(c_vp), c_vp]),
     "gs_csr_sample_rows_workspace_bytes": (c_i64, [c_i64, c_i64]),
     "gs_csr_sample_rows": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_u64, c_u64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp]),
 }

@@ -11,6 +11,10 @@
 // loaded - per entry and 4 columns one Philox call in the short role (the float4 / 8 x bf16 loads), in the hub role's
 // loading warps before the tile is written, a quad of lanes sharing its 4 columns' calls through shuffles - so warp 0's
 // ordered sum does no extra work.  The kDrop = false instantiations are the plain kernel.
+// kOff (gs_csr_aggregate_dropout_offsets; contract in oracle/sampled_blocks_dropout.py): a sampled block's row keeps
+// only some entries of its node's raw row, so entry e is masked at pos_indptr[g] + pos_off[lo + e] (its offset in the raw
+// row) instead of + e; the implicit dummy entry of an empty row keeps pos_nnz + g.  The means only: the transposed sum
+// of a sampled block reads t_slot already mapped through the offsets.
 #include "csr_rows.cuh"
 
 namespace gs {
@@ -37,6 +41,7 @@ struct CsrArgs {
   const int32_t* pos_ids;
   int64_t pos_nnz;
   const int32_t* t_slot;
+  const int32_t* pos_off;    // kOff only: each entry's offset in its node's raw CSR row
 };
 
 __device__ __forceinline__ int64_t csr_clamp(int64_t id, int64_t n_rows) { return (id < 0 || id >= n_rows) ? n_rows - 1 : id; }
@@ -164,7 +169,7 @@ __device__ __forceinline__ void quad_transpose(const u32x4& w, uint32_t (&m)[4])
 
 // the aggregate on the csr_rows.cuh schedule: the rows of `rows` (or 0 .. n - 1), entries read from src, written up to
 // out_pitch with columns F .. out_pitch - 1 zero-filled
-template <typename T, int OP, bool kDrop>
+template <typename T, int OP, bool kDrop, bool kOff = false>
 struct AggregateRows {
   static constexpr bool kFromFirst = OP == GS_CSR_MAX;
   static constexpr bool kEmptyIsDummy = OP != GS_CSR_SUM;   // the sum's empty row is +0 (a node nobody points to)
@@ -206,10 +211,17 @@ struct AggregateRows {
     return x[0];
   }
 
+  // site and position of entry e of row r (kOff: entry 0's position plus the entry's raw-row offset; an empty row's
+  // one entry is its dummy, at pbase itself)
+  __device__ __forceinline__ DropEntry entry(const Row& r, int64_t e) const {
+    if constexpr (kOff) return {r.pbase + (r.cnt > 0 ? (int64_t)__ldg(a.pos_off + r.lo + e) : 0), false};
+    else return drop_entry<OP>(a, r.lo, r.pbase, e);
+  }
+
   template <int W>
   __device__ __forceinline__ void mask(const Row& r, int64_t e, int c0, float (&x)[W]) const {
     if constexpr (kDrop) {
-      const DropEntry d = drop_entry<OP>(a, r.lo, r.pbase, e);
+      const DropEntry d = entry(r, e);
       drop_vec<W>(d.self ? ss : sn, d.pos, c0, x);
     }
   }
@@ -221,7 +233,7 @@ struct AggregateRows {
       const int j = threadIdx.x & 3;
 #pragma unroll
       for (int h = 0; h < kHubPerWarp / 4; ++h) {
-        const DropEntry mine = drop_entry<OP>(a, r.lo, r.pbase, min(e0 + 4 * h + j, r.cnt - 1));
+        const DropEntry mine = entry(r, min(e0 + 4 * h + j, r.cnt - 1));
         uint32_t m[4];
         quad_transpose(drop_words(mine.self ? ss : sn, mine.pos, (uint32_t)c >> 2), m);
 #pragma unroll
@@ -262,7 +274,7 @@ struct AggregateRows {
   }
 };
 
-template <typename T, int V, int OP, bool kDrop>
+template <typename T, int V, int OP, bool kDrop, bool kOff = false>
 __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __grid_constant__ CsrArgs a) {
   __shared__ __align__(16) float tile[2][kHubRows][kHubCols];
   DropSite sn = a.neigh, ss = a.self;
@@ -271,7 +283,7 @@ __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __g
     ss.call += drop_call_offset(ss);
   }
   // short role: 16-byte loads in flight per lane: 4 (bf16) or 8 (fp32 float4)
-  csr_rows<V, V == 8 ? 4 : 8>(AggregateRows<T, OP, kDrop>{a, sn, ss}, tile);
+  csr_rows<V, V == 8 ? 4 : 8>(AggregateRows<T, OP, kDrop, kOff>{a, sn, ss}, tile);
 }
 
 template <typename T, int V>
@@ -282,12 +294,12 @@ static void launch_csr(int32_t op, unsigned blocks, const CsrArgs& a, cudaStream
   else if constexpr (sizeof(T) == 4) csr_aggregate_kernel<T, V, GS_CSR_SUM, false><<<blocks, kCsrThreads, 0, st>>>(a);
 }
 
-// the masked instantiations: the means, and the sum over fp32 sources
-template <typename T, int V>
+// the masked instantiations: the means, and the sum over fp32 sources; with per-entry offsets (kOff), the means only
+template <typename T, int V, bool kOff>
 static void launch_csr_drop(int32_t op, unsigned blocks, const CsrArgs& a, cudaStream_t st) {
-  if (op == GS_CSR_MEAN) csr_aggregate_kernel<T, V, GS_CSR_MEAN, true><<<blocks, kCsrThreads, 0, st>>>(a);
-  else if (op == GS_CSR_MEAN_SELF) csr_aggregate_kernel<T, V, GS_CSR_MEAN_SELF, true><<<blocks, kCsrThreads, 0, st>>>(a);
-  else if constexpr (sizeof(T) == 4) csr_aggregate_kernel<T, V, GS_CSR_SUM, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  if (op == GS_CSR_MEAN) csr_aggregate_kernel<T, V, GS_CSR_MEAN, true, kOff><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if (op == GS_CSR_MEAN_SELF) csr_aggregate_kernel<T, V, GS_CSR_MEAN_SELF, true, kOff><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if constexpr (sizeof(T) == 4 && !kOff) csr_aggregate_kernel<T, V, GS_CSR_SUM, true><<<blocks, kCsrThreads, 0, st>>>(a);
 }
 
 struct CsrDrop {
@@ -296,6 +308,7 @@ struct CsrDrop {
   const int32_t* pos_ids;
   int64_t pos_nnz;
   const int32_t* t_slot;
+  const int32_t* pos_off;
 };
 
 static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
@@ -324,7 +337,7 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
   memset(&a.neigh, 0, sizeof(a.neigh));
   memset(&a.self, 0, sizeof(a.self));
   a.pos_indptr = nullptr;
-  a.pos_ids = a.t_slot = nullptr;
+  a.pos_ids = a.t_slot = a.pos_off = nullptr;
   a.pos_nnz = 0;
   if (drop) {
     a.neigh = make_drop_site(drop->neigh);
@@ -333,15 +346,22 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
     a.pos_ids = drop->pos_ids;
     a.pos_nnz = drop->pos_nnz;
     a.t_slot = drop->t_slot;
+    a.pos_off = drop->pos_off;
   }
   a.n_slices = (int32_t)((out_pitch + 32 * V - 1) / (32 * V));
   a.hub_slices = (int32_t)((out_pitch + kHubCols - 1) / kHubCols);
   const unsigned blocks = csr_grid(n, a.hub_slices, a.n_slices, a.hub_items, a.hub_blocks);
   cudaStream_t st = (cudaStream_t)stream;
+  if (drop && drop->pos_off) {
+    if (dtype == GS_BF16) launch_csr_drop<uint16_t, 8, true>(op, blocks, a, st);
+    else if (V == 4) launch_csr_drop<float, 4, true>(op, blocks, a, st);
+    else launch_csr_drop<float, 1, true>(op, blocks, a, st);
+    return launch_check("csr_aggregate_kernel<drop, offsets>");
+  }
   if (drop) {
-    if (dtype == GS_BF16) launch_csr_drop<uint16_t, 8>(op, blocks, a, st);
-    else if (V == 4) launch_csr_drop<float, 4>(op, blocks, a, st);
-    else launch_csr_drop<float, 1>(op, blocks, a, st);
+    if (dtype == GS_BF16) launch_csr_drop<uint16_t, 8, false>(op, blocks, a, st);
+    else if (V == 4) launch_csr_drop<float, 4, false>(op, blocks, a, st);
+    else launch_csr_drop<float, 1, false>(op, blocks, a, st);
     return launch_check("csr_aggregate_kernel<drop>");
   }
   if (dtype == GS_BF16) launch_csr<uint16_t, 8>(op, blocks, a, st);
@@ -361,6 +381,35 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
                            nullptr, "gs_csr_aggregate");
 }
 
+}  // extern "C"
+
+namespace gs {
+
+// gs_csr_aggregate_dropout, or with pos_off (the means only) gs_csr_aggregate_dropout_offsets
+static int32_t csr_aggregate_dropout(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                     const int64_t* indptr, const int32_t* indices, const int32_t* t_slot,
+                                     int64_t n_nodes, const int32_t* rows, int64_t n, int32_t op,
+                                     gs_dropout_site neigh_site, gs_dropout_site self_site, const int64_t* pos_indptr,
+                                     const int32_t* pos_ids, int64_t pos_nnz, const int32_t* pos_off, float* out,
+                                     int64_t out_pitch, void* stream, const char* who) {
+  int32_t rc = check_site(neigh_site, who);
+  if (rc == GS_OK) rc = check_site(self_site, who);
+  if (rc != GS_OK) return rc;
+  GS_REQUIRE(pos_nnz >= 0, "%s: pos_nnz < 0", who);
+  if (neigh_site.rate == 0.f && self_site.rate == 0.f)      // every mask keeps and divides by 1: the plain kernel
+    return csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
+                         nullptr, who);
+  GS_REQUIRE(n == 0 || pos_indptr, "%s: NULL pos_indptr", who);
+  GS_REQUIRE(op != GS_CSR_SUM || n == 0 || t_slot, "%s: GS_CSR_SUM needs t_slot", who);
+  const CsrDrop drop{neigh_site, self_site, pos_indptr, pos_ids, pos_nnz, op == GS_CSR_SUM ? t_slot : nullptr, pos_off};
+  return csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
+                       &drop, who);
+}
+
+}  // namespace gs
+
+extern "C" {
+
 int32_t gs_csr_aggregate_dropout(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
                                  const int64_t* indptr, const int32_t* indices, const int32_t* t_slot, int64_t n_nodes,
                                  const int32_t* rows, int64_t n, int32_t op, gs_dropout_site neigh_site,
@@ -369,18 +418,24 @@ int32_t gs_csr_aggregate_dropout(const void* src, int32_t dtype, int64_t n_src_r
   const char* who = "gs_csr_aggregate_dropout";
   GS_REQUIRE(op == GS_CSR_MEAN || op == GS_CSR_MEAN_SELF || op == GS_CSR_SUM, "%s: op must be GS_CSR_MEAN, "
              "GS_CSR_MEAN_SELF or GS_CSR_SUM (got %d)", who, (int)op);
-  int32_t rc = gs::check_site(neigh_site, who);
-  if (rc == GS_OK) rc = gs::check_site(self_site, who);
-  if (rc != GS_OK) return rc;
-  GS_REQUIRE(pos_nnz >= 0, "%s: pos_nnz < 0", who);
-  if (neigh_site.rate == 0.f && self_site.rate == 0.f)      // every mask keeps and divides by 1: the plain kernel
-    return gs::csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
-                             nullptr, who);
-  GS_REQUIRE(n == 0 || pos_indptr, "%s: NULL pos_indptr", who);
-  GS_REQUIRE(op != GS_CSR_SUM || n == 0 || t_slot, "%s: GS_CSR_SUM needs t_slot", who);
-  const gs::CsrDrop drop{neigh_site, self_site, pos_indptr, pos_ids, pos_nnz, op == GS_CSR_SUM ? t_slot : nullptr};
-  return gs::csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
-                           &drop, who);
+  return gs::csr_aggregate_dropout(src, dtype, n_src_rows, F, pitch, indptr, indices, t_slot, n_nodes, rows, n, op,
+                                   neigh_site, self_site, pos_indptr, pos_ids, pos_nnz, nullptr, out, out_pitch, stream,
+                                   who);
+}
+
+int32_t gs_csr_aggregate_dropout_offsets(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                         const int64_t* indptr, const int32_t* indices, int64_t n_nodes,
+                                         const int32_t* rows, int64_t n, int32_t op, gs_dropout_site neigh_site,
+                                         gs_dropout_site self_site, const int64_t* pos_indptr, const int32_t* pos_ids,
+                                         int64_t pos_nnz, const int32_t* pos_off, float* out, int64_t out_pitch,
+                                         void* stream) {
+  const char* who = "gs_csr_aggregate_dropout_offsets";
+  GS_REQUIRE(op == GS_CSR_MEAN || op == GS_CSR_MEAN_SELF, "%s: op must be GS_CSR_MEAN or GS_CSR_MEAN_SELF (got %d)",
+             who, (int)op);
+  GS_REQUIRE(n == 0 || pos_off, "%s: NULL pos_off", who);
+  return gs::csr_aggregate_dropout(src, dtype, n_src_rows, F, pitch, indptr, indices, nullptr, n_nodes, rows, n, op,
+                                   neigh_site, self_site, pos_indptr, pos_ids, pos_nnz, pos_off, out, out_pitch, stream,
+                                   who);
 }
 
 }  // extern "C"

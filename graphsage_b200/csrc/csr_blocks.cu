@@ -20,6 +20,9 @@
 // warp) to write them in ascending order.  The plan and the fill recompute the same draws; nothing is stored between
 // them.  A hub row is never walked: with d > k a warp touches only the k drawn entries.  kSample = false is the code
 // above, instruction for instruction (the draw arguments are appended and unused).
+// gs_csr_sampled_blocks_fill_offsets runs the fill with kOff = true: where it writes an entry it also writes the entry's
+// offset in its node's raw row (the held Floyd position, or e), which the training masks name it by
+// (oracle/sampled_blocks_dropout.py).  No other kernel changes, and the other arrays are the same bytes.
 #include <algorithm>
 
 #include "common.cuh"
@@ -210,14 +213,16 @@ __global__ void __launch_bounds__(kBlkThreads) blk_local_degree_kernel(const int
 
 // one warp per local row: its raw entries, clamped, relabelled through pos, in CSR order.  kSample: the entries of
 // S_l(v) (a row with more than k entries: Floyd's draws again, written in ascending position order); ids == NULL: row p
-// is node p; pos == NULL: the entries are copied as they are (gs_csr_sample_rows)
-template <bool kSample>
+// is node p; pos == NULL: the entries are copied as they are (gs_csr_sample_rows).  kOff (kSample only): b_off[at + .]
+// = the entry's offset in v's raw row, beside b_indices
+template <bool kSample, bool kOff = false>
 __global__ void __launch_bounds__(kBlkThreads) blk_fill_kernel(const int64_t* __restrict__ indptr,
                                                                const int32_t* __restrict__ indices, int64_t n_nodes,
                                                                const int32_t* __restrict__ ids,
                                                                const int32_t* __restrict__ pos,
                                                                const int64_t* __restrict__ b_indptr, int64_t n_rows,
-                                                               int32_t* __restrict__ b_indices, SampleArgs sa) {
+                                                               int32_t* __restrict__ b_indices, SampleArgs sa,
+                                                               int32_t* __restrict__ b_off = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t warps = (int64_t)gridDim.x * kBlkWarps;
   for (int64_t p = (int64_t)blockIdx.x * kBlkWarps + (threadIdx.x >> 5); p < n_rows; p += warps) {
@@ -236,11 +241,13 @@ __global__ void __launch_bounds__(kBlkThreads) blk_fill_kernel(const int64_t* __
           if (held[s] == INT32_MAX) continue;
           const int32_t x = indices[lo + held[s]];
           b_indices[at + rank[s]] = pos ? pos[blk_clamp(x, n_nodes)] : x;
+          if (kOff) b_off[at + rank[s]] = held[s];
         }
       } else {
         for (int64_t e = lane; e < cnt; e += 32) {
           const int32_t x = indices[lo + e];
           b_indices[at + e] = pos ? pos[blk_clamp(x, n_nodes)] : x;
+          if (kOff) b_off[at + e] = (int32_t)e;
         }
       }
       continue;
@@ -370,12 +377,12 @@ static int32_t blocks_plan(const int64_t* indptr, const int32_t* indices, int64_
   return GS_OK;
 }
 
-// gs_csr_blocks_fill, or with fanouts gs_csr_sampled_blocks_fill
+// gs_csr_blocks_fill, or with fanouts gs_csr_sampled_blocks_fill (and with b_off, _fill_offsets)
 static int32_t blocks_fill(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
                            const int32_t* seeds, int64_t n_seeds, int32_t n_layers, const int32_t* fanouts, uint64_t seed,
                            uint64_t call, void* workspace, int64_t workspace_bytes, const int64_t* counts,
                            int32_t* const* src_ids, int64_t* const* b_indptr, int32_t* const* b_indices,
-                           int32_t* const* b_rows, void* stream, const char* who) {
+                           int32_t* const* b_rows, int32_t* const* b_off, void* stream, const char* who) {
   BlocksPlan P;
   int32_t rc = make_blocks_plan(n_nodes, nnz, n_seeds, n_layers, P, who);
   if (rc != GS_OK) return rc;
@@ -386,7 +393,7 @@ static int32_t blocks_fill(const int64_t* indptr, const int32_t* indices, int64_
              (long long)workspace_bytes, (long long)P.bytes);
   if (fanouts && (rc = check_fanouts(fanouts, n_layers, nnz, who)) != GS_OK) return rc;
   auto local_degree = fanouts ? blk_local_degree_kernel<true> : blk_local_degree_kernel<false>;
-  auto fill = fanouts ? blk_fill_kernel<true> : blk_fill_kernel<false>;
+  auto fill = b_off ? blk_fill_kernel<true, true> : fanouts ? blk_fill_kernel<true> : blk_fill_kernel<false>;
   cudaStream_t st = (cudaStream_t)stream;
   const BlocksWs W = blocks_ws(P, workspace);
   const int64_t max_warp_blocks = (int64_t)sm_count() * 16;
@@ -397,7 +404,8 @@ static int32_t blocks_fill(const int64_t* indptr, const int32_t* indices, int64_
     const SampleArgs sa = fanouts ? make_sample_args(fanouts[l], seed, call, l) : SampleArgs{};
     GS_REQUIRE(n_local >= 1 && n_local <= n_nodes + 1 && entries >= 0 && n_out >= 0, "%s: bad counts for block %d", who,
                l);
-    GS_REQUIRE(src_ids[l] && b_indptr[l] && (entries == 0 || b_indices[l]) && (n_out == 0 || b_rows[l]),
+    GS_REQUIRE(src_ids[l] && b_indptr[l] && (entries == 0 || (b_indices[l] && (!b_off || b_off[l]))) &&
+                   (n_out == 0 || b_rows[l]),
                "%s: NULL output of block %d", who, l);
     GS_CUDA(cudaMemcpyAsync(src_ids[l], W.ids(l), (size_t)n_local * 4, cudaMemcpyDeviceToDevice, st));
     local_degree<<<blk_grid(n_local, kBlkThreads, INT32_MAX), kBlkThreads, 0, st>>>(indptr, n_nodes, W.ids(l),
@@ -410,7 +418,8 @@ static int32_t blocks_fill(const int64_t* indptr, const int32_t* indices, int64_
     if (e != cudaSuccess) return cuda_fail(e, "cub::DeviceScan::ExclusiveSum");
     if (entries > 0) {
       fill<<<blk_grid(n_local - 1, kBlkWarps, max_warp_blocks), kBlkThreads, 0, st>>>(
-          indptr, indices, n_nodes, W.ids(l), W.pos(l), b_indptr[l], n_local - 1, b_indices[l], sa);
+          indptr, indices, n_nodes, W.ids(l), W.pos(l), b_indptr[l], n_local - 1, b_indices[l], sa,
+          b_off ? b_off[l] : nullptr);
       rc = launch_check("blk_fill_kernel");
       if (rc != GS_OK) return rc;
     }
@@ -456,7 +465,8 @@ int32_t gs_csr_blocks_fill(const int64_t* indptr, const int32_t* indices, int64_
                            int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
                            int64_t* const* b_indptr, int32_t* const* b_indices, int32_t* const* b_rows, void* stream) {
   return gs::blocks_fill(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, nullptr, 0, 0, workspace,
-                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, stream, "gs_csr_blocks_fill");
+                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, nullptr, stream,
+                         "gs_csr_blocks_fill");
 }
 
 int32_t gs_csr_sampled_blocks_plan(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
@@ -477,7 +487,19 @@ int32_t gs_csr_sampled_blocks_fill(const int64_t* indptr, const int32_t* indices
   const char* who = "gs_csr_sampled_blocks_fill";
   GS_REQUIRE(fanouts != nullptr, "%s: NULL fanouts", who);
   return gs::blocks_fill(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, fanouts, seed, call, workspace,
-                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, stream, who);
+                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, nullptr, stream, who);
+}
+
+int32_t gs_csr_sampled_blocks_fill_offsets(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers,
+                                           const int32_t* fanouts, uint64_t seed, uint64_t call, void* workspace,
+                                           int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
+                                           int64_t* const* b_indptr, int32_t* const* b_indices, int32_t* const* b_rows,
+                                           int32_t* const* b_off, void* stream) {
+  const char* who = "gs_csr_sampled_blocks_fill_offsets";
+  GS_REQUIRE(fanouts != nullptr && b_off != nullptr, "%s: NULL fanouts or offsets", who);
+  return gs::blocks_fill(indptr, indices, n_nodes, nnz, seeds, n_seeds, n_layers, fanouts, seed, call, workspace,
+                         workspace_bytes, counts, src_ids, b_indptr, b_indices, b_rows, b_off, stream, who);
 }
 
 int64_t gs_csr_sample_rows_workspace_bytes(int64_t n_nodes, int64_t nnz) {

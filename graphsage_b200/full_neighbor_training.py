@@ -32,7 +32,11 @@ the means' neighbour branch (gs_csr_aggregate_dropout, the entry's global CSR po
 rows, GCN's own row and the pools' MLP input (ops.dropout_apply by id).  Each graph carries the position map of its
 kernels - (indptr, None, nnz) for the whole graph, (global indptr, src_ids, global nnz) for a block - so a block masks every
 element as the whole-graph pass does.  The backward regenerates every mask: the transposed sum reads the transpose's
-t_slot (ops.csr_transpose(slots=True)) to find each entry's forward position.
+t_slot (ops.csr_transpose(slots=True)) to find each entry's forward position.  A sampled block (contract:
+oracle/sampled_blocks_dropout.py) keeps only some entries of each raw row, so its map carries a fourth element, each
+entry's offset in its raw row (ops.csr_blocks(..., entry_offsets=True)): the forward masks entry j at pos_indptr[g] +
+offset, and the backward maps t_slot through the offsets (ops.csr_slots_to_offsets) before the same transposed sum.  A
+sampled entry is then masked as the same edge is in the whole-graph pass.
 """
 import torch
 
@@ -50,8 +54,8 @@ class FullNeighborGraph(object):
     _version of both); the tensors themselves are held, so their memory cannot be reused by a different CSR while cached."""
 
     def __init__(self, indptr, indices, pos_map=None):
-        """pos_map: (pos_indptr, pos_ids or None, pos_nnz), how the masks name this CSR's rows and entries globally
-        (default: the CSR is the global one)."""
+        """pos_map: (pos_indptr, pos_ids or None, pos_nnz[, pos_off]), how the masks name this CSR's rows and entries
+        globally (default: the CSR is the global one); pos_off: a sampled block's per-entry raw-row offsets."""
         self.indptr, self.indices = indptr, indices
         self.pos_map = pos_map if pos_map is not None else (indptr, None, indices.numel())
         self.key = FullNeighborGraph.key_of(indptr, indices)
@@ -90,7 +94,10 @@ class FullNeighborGraph(object):
             t_indptr, t_indices = self.transpose(with_self)
             return ops.csr_aggregate(gp, t_indptr, t_indices, "sum")
         t_indptr, t_indices, t_slot = self.transpose(with_self, slots=True)
-        return ops.csr_aggregate(gp, t_indptr, t_indices, "sum", dropout=(sites[0], sites[1], self.pos_map), t_slot=t_slot)
+        if len(self.pos_map) == 4:                   # a sampled block: slots in the block row -> offsets in the raw row
+            t_slot = ops.csr_slots_to_offsets(t_slot, t_indices, self.indptr, self.pos_map[3])
+        return ops.csr_aggregate(gp, t_indptr, t_indices, "sum", dropout=(sites[0], sites[1], self.pos_map[:3]),
+                                 t_slot=t_slot)
 
     def node_ids(self, rows):
         """The global node ids of local rows (None: every row) for the per-node masks; None when they are the rows."""
@@ -153,7 +160,9 @@ class _FullLayer(object):
         hs = _rows(h, h_rows, 0, n, widen) if (widen or h_rows is not None) else h
         if not self.pool:
             if s is not None:                                        # the self rows by node id, after widening
-                hs = ops.dropout_apply(hs, s["self"], pos_ids=tgraph.node_ids(h_rows), out=None if hs is h else hs)
+                # a sampled block 0 reads them by global id (self_ids), which are their positions
+                ids = h_rows if self.self_ids is not None else tgraph.node_ids(h_rows)
+                hs = ops.dropout_apply(hs, s["self"], pos_ids=ids, out=None if hs is h else hs)
             m = ops.csr_aggregate(hn, indptr, indices, "mean", rows=n_rows, **drop)
             return [(hs, agg.input_dim, agg.vars["self_weights"]), (m, agg.neigh_input_dim, agg.vars["neigh_weights"])]
         if self.src_ids is None:
@@ -294,18 +303,25 @@ def _inputs(model, indptr, indices, node_ids):
     return indptr, indices, ids
 
 
-def minibatch_layers(aggregators, indptr, indices, ids, draw=None):
+def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0.):
     """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped); draw =
-    (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead."""
+    (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead, and with
+    dropout = p > 0 each block's position map also carries its entries' raw-row offsets."""
     L = len(aggregators)
+    offsets = [None] * L
     if draw is None:
         blocks = ops.csr_blocks(indptr, indices, ids, L)
     else:
         fanouts, seed, call = draw
-        blocks = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call)
+        if dropout:
+            blocks, offsets = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call,
+                                             entry_offsets=True)
+        else:
+            blocks = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call)
     layers = []
     for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
-        graph = FullNeighborGraph(b.indptr, b.indices, pos_map=(indptr, b.src_ids, indices.numel()))
+        pos_map = (indptr, b.src_ids, indices.numel()) + ((offsets[layer],) if offsets[layer] is not None else ())
+        graph = FullNeighborGraph(b.indptr, b.indices, pos_map=pos_map)
         if layer == 0:
             v1 = blocks[1].src_ids if L > 1 else ids
             if draw is not None:
@@ -317,13 +333,14 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None):
     return layers
 
 
-def refuse_sampled(model, training):
+def refuse_sampled(model, training, dropout=None):
     """The NotImplementedErrors of the sampled-block entry points: refuse_full_neighbor's, CUDA-graph capture and, when
-    training, a model with dropout_rate > 0."""
-    if training and getattr(model, "dropout_rate", 0.):
-        raise NotImplementedError("sampled-block training with dropout > 0 is not implemented (the per-edge masks are "
-                                  "keyed by global CSR positions, and a sampled block entry does not keep its position)")
-    refuse_full_neighbor(model, training)
+    training, dropout=None on a model with dropout_rate > 0."""
+    if training and dropout is None and getattr(model, "dropout_rate", 0.):
+        raise NotImplementedError("sampled-block training with dropout > 0 needs the rate passed explicitly - pass "
+                                  "dropout=model.dropout_rate for the per-edge masks keyed by global CSR positions "
+                                  "(oracle/sampled_blocks_dropout.py)")
+    refuse_full_neighbor(model, training, dropout)
     refuse_capture("a sampled-block minibatch (it reads the block sizes back)")
 
 
@@ -343,7 +360,7 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None,
     training, an uncached one otherwise (inference builds no transposes, and must not evict the ones a training CSR has
     cached)."""
     if sampled:
-        refuse_sampled(model, training)
+        refuse_sampled(model, training, dropout)
     else:
         refuse_full_neighbor(model, training, dropout)
     if minibatch:
@@ -352,7 +369,7 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None,
     if model.aggregators is None:
         model.aggregators = build_aggregators(model)
     if sampled:
-        return minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model))
+        return minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model), dropout=dropout)
     if minibatch:
         return minibatch_layers(model.aggregators, indptr, indices, ids)
     graph = full_neighbor_graph(model, indptr, indices) if training else FullNeighborGraph(indptr, indices)
@@ -376,11 +393,8 @@ def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, mini
                           sampled=False):
     """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch, sampled) with an autograd graph over the
     aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
-    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them (not with
-    sampled)."""
+    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them."""
     p = check_full_neighbor_dropout(dropout)
-    if sampled and p:
-        raise NotImplementedError("sampled-block training with dropout > 0 is not implemented")
     layers = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled)
     if p:
         pool = isinstance(layers[0].agg, MaxPoolingAggregator)

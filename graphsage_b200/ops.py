@@ -571,7 +571,11 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
     [n, pad_cols(F)] buffer (or of `out`, whose extra columns are zeroed).
     dropout: None, or (neighbour site, self site, (pos_indptr, pos_ids or None, pos_nnz)) - full-neighbourhood training
     dropout (gs_csr_aggregate_dropout; contract in oracle/full_neighbor_dropout.py) for ops "mean", "mean_self" and "sum";
-    "sum" then also takes t_slot, the slots of csr_transpose(..., slots=True)."""
+    "sum" then also takes t_slot, the slots of csr_transpose(..., slots=True).  The position map may carry a fourth
+    element, pos_off: a sampled block's per-entry offsets (csr_blocks(..., entry_offsets=True); int32, one per entry of
+    `indices`) - entry j of node v's row is then masked at pos_indptr[g(v)] + pos_off[indptr[v] + j]
+    (gs_csr_aggregate_dropout_offsets; contract in oracle/sampled_blocks_dropout.py), ops "mean" and "mean_self" only; the
+    backward "sum" takes csr_slots_to_offsets' t_slot and a three-element map instead."""
     require_cuda(src, indptr, indices, rows, out)
     if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
         raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
@@ -587,7 +591,8 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
         raise ValueError("op 'sum' needs one CSR row per source row: indptr of %d entries for %d source rows (got %d) - "
                          "the layout of csr_transpose" % (src.shape[0] + 1, src.shape[0], indptr.numel()))
     indptr, indices = indptr.contiguous(), _i32(indices.reshape(-1), "indices")
-    if indices.numel() == 0:
+    entries = indices.numel()
+    if entries == 0:
         indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
     n_nodes = indptr.numel() - 1
     if rows is not None:
@@ -598,7 +603,11 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
     if out.dtype != torch.float32 or out.dim() != 2 or out.stride(1) != 1 or out.shape[0] < n:
         raise ValueError("out must be a row-major float32 [>= %d, .] CUDA matrix" % n)
     if dropout is not None:
-        neigh, self_site, (pos_indptr, pos_ids, pos_nnz) = dropout
+        neigh, self_site, pos_map = dropout
+        if len(pos_map) not in (3, 4):
+            raise ValueError("the position map is (pos_indptr, pos_ids, pos_nnz[, pos_off])")
+        pos_indptr, pos_ids, pos_nnz = pos_map[:3]
+        pos_off = pos_map[3] if len(pos_map) == 4 else None
         if op == "max":
             raise ValueError("dropout applies to the ops 'mean', 'mean_self' and 'sum'")
         if op == "sum" and (t_slot is None or t_slot.dtype != torch.int32 or t_slot.numel() < indices.numel()):
@@ -611,6 +620,9 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
             need = n_nodes if op == "sum" else n_nodes + 1         # the sum's CSR has a row per source row already
             if pos_ids.numel() < need:
                 raise ValueError("pos_ids needs one id per local row: %d, got %d" % (need, pos_ids.numel()))
+        if pos_off is not None:
+            return _csr_aggregate_dropout_offsets(src, indptr, indices, entries, n_nodes, rows, n, op, out, neigh,
+                                                  self_site, pos_indptr, pos_ids, pos_nnz, pos_off)
         ev = _probe("csr_aggregate_dropout/%d" % n)
         check(lib().gs_csr_aggregate_dropout(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), ptr(indptr),
                                              ptr(indices), ptr(t_slot) if op == "sum" else 0, n_nodes, ptr(rows), n,
@@ -624,6 +636,43 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
                                  n_nodes, ptr(rows), n, CSR_OPS[op], ptr(out), out.stride(0), stream_ptr()))
     _launched(1 if n else 0, ev)
     return out[:n, :F]
+
+
+def _csr_aggregate_dropout_offsets(src, indptr, indices, entries, n_nodes, rows, n, op, out, neigh, self_site, pos_indptr,
+                                   pos_ids, pos_nnz, pos_off):
+    """csr_aggregate's masked mean over a sampled block, its entries named by their raw-row offsets."""
+    if op not in ("mean", "mean_self"):
+        raise ValueError("per-entry offsets apply to the ops 'mean' and 'mean_self' (the backward 'sum' takes "
+                         "csr_slots_to_offsets' t_slot)")
+    require_cuda(pos_off)
+    if not isinstance(pos_off, torch.Tensor) or pos_off.dtype != torch.int32 or pos_off.dim() != 1:
+        raise TypeError("pos_off must be a 1-D int32 tensor")
+    if pos_off.numel() < entries:
+        raise ValueError("pos_off needs one offset per CSR entry: %d, got %d" % (entries, pos_off.numel()))
+    pos_off = pos_off.contiguous() if pos_off.numel() else torch.zeros((1,), dtype=torch.int32, device=indptr.device)
+    ev = _probe("csr_aggregate_dropout_offsets/%d" % n)
+    check(lib().gs_csr_aggregate_dropout_offsets(ptr(src), _dtype_code(src), src.shape[0], src.shape[1], src.stride(0),
+                                                 ptr(indptr), ptr(indices), n_nodes, ptr(rows), n, CSR_OPS[op],
+                                                 dropout_site(neigh), dropout_site(self_site),
+                                                 ptr(pos_indptr.contiguous()), ptr(pos_ids), int(pos_nnz), ptr(pos_off),
+                                                 ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return out[:n, :src.shape[1]]
+
+
+def csr_slots_to_offsets(t_slot, t_indices, indptr, pos_off):
+    """The slots of csr_transpose(indptr, indices, slots=True) over a sampled block, mapped to raw-row offsets: t_slot' =
+    pos_off[indptr[i] + t_slot] for i = t_indices[.] where t_slot >= 0, -1 and -2 kept - the positions the forward of
+    csr_aggregate(..., dropout=(.., .., (pos_indptr, pos_ids, pos_nnz, pos_off))) masked each entry at, so the backward
+    "sum" regenerates them with a three-element map.  Two gathers over the transposed entries; the entries past the
+    transpose's count (unspecified) are clamped into range and stay unspecified.  int32 [len(t_slot)]."""
+    require_cuda(t_slot, t_indices, indptr, pos_off)
+    if pos_off.numel() == 0:                         # no forward entry: every slot is -1 or -2
+        return t_slot
+    s = t_slot.long()
+    i = t_indices.long().clamp(0, indptr.numel() - 1)
+    at = (indptr.index_select(0, i) + s).clamp(0, pos_off.numel() - 1)
+    return torch.where(s >= 0, pos_off.index_select(0, at), s).to(torch.int32)
 
 
 def _csr_args(indptr, indices):
@@ -713,7 +762,7 @@ def _sampled_csr_args(nnz):
         raise ValueError("sampled rows need fewer than 2^31 CSR entries (got %d)" % nnz)
 
 
-def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0):
+def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, entry_offsets=False):
     """The receptive field of `seeds` over n_layers layers of whole neighbourhoods (gs_csr_blocks_plan / _fill; contract
     in oracle/full_neighbor_blocks.py): a list, index l = layer l, of CsrBlock(src_ids int32 V_l, indptr int64 [|V_l|],
     indices int32, rows int32).  A block is a CSR over |V_l| - 1 local nodes whose last local row is the dummy, so
@@ -723,7 +772,12 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0):
     fanouts: None (whole rows), or one fanout per layer, each in [1, MAX_FANOUT]: block l is then built over S_l, at
     most fanouts[l] entries of each row drawn without replacement by Floyd's algorithm from Philox words keyed by `seed`
     at counter word `call` (gs_csr_sampled_blocks_plan / _fill; contract in oracle/sampled_blocks.py).  The same
-    (seed, call) gives the same bytes."""
+    (seed, call) gives the same bytes.
+    entry_offsets (with fanouts): return (blocks, offsets), offsets[l] int32 [entries of block l] aligned with block l's
+    indices - each entry's offset in its node's raw CSR row, which training dropout masks it by
+    (gs_csr_sampled_blocks_fill_offsets; contract in oracle/sampled_blocks_dropout.py).  The blocks are the same bytes."""
+    if entry_offsets and fanouts is None:
+        raise ValueError("entry_offsets needs fanouts (a whole-neighbourhood block entry is its raw row's entry)")
     require_cuda(indptr, indices, seeds)
     if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
         raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
@@ -758,10 +812,14 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0):
     sz = (_lib.c_i64 * (2 * L))(*sizes)
     if fanouts is None:
         check(lib().gs_csr_blocks_fill(*head, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
+    elif entry_offsets:
+        offsets = [torch.empty((sizes[2 * l + 1],), dtype=torch.int32, device=dev) for l in range(L)]
+        off_arr = (_lib.c_vp * L)(*[ptr(o) if o.numel() else 0 for o in offsets])
+        check(lib().gs_csr_sampled_blocks_fill_offsets(*head, *draw, ptr(ws), nbytes, sz, *arrs, off_arr, stream_ptr()))
     else:
         check(lib().gs_csr_sampled_blocks_fill(*head, *draw, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
     _launched(6 * L + 4, ev)           # plan: mark, compact, size, degrees per level; fill: degrees, fill, rows (+ CUB)
-    return blocks
+    return (blocks, offsets) if entry_offsets else blocks
 
 
 def sample_csr_rows(indptr, indices, k, seed, call, layer):

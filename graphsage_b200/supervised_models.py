@@ -725,23 +725,28 @@ class SupervisedGraphsage(SampleAndAggregate):
         +-5.  Returns the detached loss."""
         return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
 
-    def sampled_minibatch_outputs(self, indptr, indices, node_ids):
+    def sampled_minibatch_outputs(self, indptr, indices, node_ids, dropout=None):
         """outputs() over sampled receptive-field blocks (SampleAndAggregate.sampled_minibatch_embeddings; contract:
         oracle/sampled_blocks.py), with an autograd graph over the aggregator weights and (identity_dim > 0) the node
-        embeddings.  One block set per call: the sampler's counter advances by 1.  Refused (NotImplementedError): what
-        full_neighbor_outputs refuses, CUDA-graph capture, and a model with dropout_rate > 0 (the per-edge masks name
-        global CSR positions, which a sampled block entry does not keep)."""
+        embeddings.  One block set per call: the sampler's counter advances by 1.  dropout: None (no masks), or a
+        training rate p in [0, 1) - callers pass dropout=model.dropout_rate: the full-neighbourhood masks, a sampled
+        entry masked as the same CSR entry is in the whole-graph pass (contract: oracle/sampled_blocks_dropout.py), sites
+        numbered from dropout_counter; p = 0 gives the bits of dropout=None.  Refused (NotImplementedError): what
+        full_neighbor_outputs refuses, CUDA-graph capture, and dropout=None on a model whose dropout_rate > 0."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True, dropout=dropout)
 
-    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels):
-        """loss() over sampled_minibatch_outputs: the same head, cross-entropy and weight decay."""
-        return self._logits_loss(self._node_pred(self.sampled_minibatch_outputs(indptr, indices, node_ids)), labels)
+    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None):
+        """loss() over sampled_minibatch_outputs: the same head, cross-entropy and weight decay.  dropout: as
+        sampled_minibatch_outputs; p > 0 also drops the head input (row r of node_ids at position r)."""
+        check_full_neighbor_dropout(dropout)
+        out = self.sampled_minibatch_outputs(indptr, indices, node_ids, dropout=dropout)
+        return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels):
+    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None):
         """One Adam step on sampled_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the detached
         loss."""
-        return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels))
+        return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
 
     def full_neighbor_predict(self, indptr, indices, node_ids):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on

@@ -797,6 +797,20 @@ int32_t gs_csr_aggregate_dropout(const void* src, int32_t dtype, int64_t n_src_r
                                  const int32_t* pos_ids /* may be NULL */, int64_t pos_nnz, float* out, int64_t out_pitch,
                                  void* stream);
 
+/* gs_csr_aggregate_dropout over a sampled block (gs_csr_sampled_blocks_fill_offsets; contract:
+ * oracle/sampled_blocks_dropout.py), op GS_CSR_MEAN or GS_CSR_MEAN_SELF: entry j of a row of node v is masked at
+ * pos_indptr[g(v)] + pos_off[indptr[v] + j] - its offset in g(v)'s raw CSR row - instead of + j, so a sampled entry is
+ * masked as the same global entry is in the whole-graph pass.  pos_off: int32, one per entry of `indices`; not read for
+ * an empty row, whose implicit dummy entry stays at pos_nnz + g(v).  Everything else, and both rates 0, as above.  The
+ * backward sum over a sampled block runs through gs_csr_aggregate_dropout's GS_CSR_SUM with t_slot mapped through the
+ * offsets (t_slot' = pos_off[indptr[i] + t_slot] where t_slot >= 0). */
+int32_t gs_csr_aggregate_dropout_offsets(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                         const int64_t* indptr, const int32_t* indices, int64_t n_nodes,
+                                         const int32_t* rows /* may be NULL */, int64_t n, int32_t op,
+                                         gs_dropout_site neigh_site, gs_dropout_site self_site, const int64_t* pos_indptr,
+                                         const int32_t* pos_ids /* may be NULL */, int64_t pos_nnz,
+                                         const int32_t* pos_off, float* out, int64_t out_pitch, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Backward of the full-neighbourhood reductions (SupervisedGraphsage.full_neighbor_train_step).  Contract:
  * oracle/full_neighbor_grad.py.  Nodes 0 .. N-1 have CSR rows; the dummy node N closes every [N+1, .] table.
@@ -895,6 +909,16 @@ int32_t gs_csr_sampled_blocks_fill(const int64_t* indptr, const int32_t* indices
                                    uint64_t seed, uint64_t call, void* workspace, int64_t workspace_bytes,
                                    const int64_t* counts, int32_t* const* src_ids, int64_t* const* indptr_out,
                                    int32_t* const* indices_out, int32_t* const* rows_out, void* stream);
+/* gs_csr_sampled_blocks_fill that also writes, per block, offsets_out[l] int32 [entries of block l] aligned with
+ * indices_out[l]: each entry's offset q in its node's raw CSR row - the sorted Floyd position when d > k_l, the entry's
+ * own index j when d <= k_l - which gs_csr_aggregate_dropout_offsets masks by.  The same kernels; the other four arrays
+ * are the bytes of gs_csr_sampled_blocks_fill. */
+int32_t gs_csr_sampled_blocks_fill_offsets(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz,
+                                           const int32_t* seeds, int64_t n_seeds, int32_t n_layers,
+                                           const int32_t* fanouts, uint64_t seed, uint64_t call, void* workspace,
+                                           int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
+                                           int64_t* const* indptr_out, int32_t* const* indices_out,
+                                           int32_t* const* rows_out, int32_t* const* offsets_out, void* stream);
 int64_t gs_csr_sample_rows_workspace_bytes(int64_t n_nodes, int64_t nnz);
 int32_t gs_csr_sample_rows(const int64_t* indptr, const int32_t* indices, int64_t n_nodes, int64_t nnz, int32_t k,
                            uint64_t seed, uint64_t call, int32_t layer, void* workspace, int64_t workspace_bytes,

@@ -1,7 +1,7 @@
 """Time minibatch training over sampled blocks (SupervisedGraphsage.sampled_minibatch_train_step) on the GPU, against
 the sampled tree path (train_step, graphed_train_step) and the whole-neighbourhood blocks on the same ids.
 
-    python tools/sampled_blocks_bench.py [--iters 10] [--rounds 2] [--out sampled_blocks_bench.json]
+    python tools/sampled_blocks_bench.py [--iters 10] [--rounds 2] [--out sampled_blocks_bench.json] [--dropout P]
 
 Graph: community_graph_csr(232,965, mean_deg=50) - Reddit's node count, hub-heavy - with 602 random fp32 features.
 Model: 2 layers, concat, width 128 per half, tf32x3 combine GEMMs, 41 classes, layer_infos fanouts (25, 10) as the
@@ -15,6 +15,8 @@ random node ids.  Per case, after one warm-up of each step:
   step_ms           sampled_minibatch_train_step end to end (--iters steps, CUDA events), peak_MB above the resident set;
   tree_step_ms      train_step;  graphed_step_ms  graphed_train_step's replays;
   full_step_ms      full_neighbor_minibatch_train_step ("oom" if it does not fit).
+With --dropout P only the sampled step is timed, at dropout=0 and dropout=P alternately (step_ms_p0, step_ms_p, and
+their peak_MB), for the cost of the training masks (oracle/sampled_blocks_dropout.py) on this path.
 Everything is measured --rounds times in one process; the card name and power limit are read in the same command."""
 import argparse
 import json
@@ -124,11 +126,28 @@ def measure(kind, features, adj, indptr, indices, ids, labels, iters):
     return res
 
 
+def measure_dropout(kind, features, adj, indptr, indices, ids, labels, iters, p):
+    """sampled_minibatch_train_step at dropout 0 and p, alternating, after a warm-up of each."""
+    m = build_model(kind, features, adj)
+    res = {"aggregator": kind, "batch": int(ids.numel()), "fanouts": list(FANOUTS), "dropout": p}
+    for rate in (0., p):
+        m.sampled_minibatch_train_step(indptr, indices, ids, labels, dropout=rate)
+    for rep in range(2):
+        for rate, key in ((0., "p0"), (p, "p")):
+            ms, mb = timed_steps(lambda: m.sampled_minibatch_train_step(indptr, indices, ids, labels, dropout=rate),
+                                 iters)
+            res.setdefault("step_ms_" + key, []).append(ms)
+            res.setdefault("peak_MB_" + key, []).append(mb)
+    torch.cuda.empty_cache()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--out", default="sampled_blocks_bench.json")
+    ap.add_argument("--dropout", type=float, default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "the benchmark needs a CUDA device"
     gs._lib.lib()
@@ -150,7 +169,11 @@ def main():
             ids = torch.from_numpy(rs.choice(n, BATCH, replace=False).astype(np.int32)).cuda()
             labels = torch.zeros((BATCH, C), device="cuda")
             labels[torch.arange(BATCH, device="cuda"), torch.from_numpy(rs.randint(0, C, BATCH)).cuda()] = 1.0
-            out = dict(round=r, **measure(kind, features, adj, indptr, indices, ids, labels, a.iters))
+            if a.dropout is not None:
+                out = dict(round=r, **measure_dropout(kind, features, adj, indptr, indices, ids, labels, a.iters,
+                                                      a.dropout))
+            else:
+                out = dict(round=r, **measure(kind, features, adj, indptr, indices, ids, labels, a.iters))
             print(json.dumps(out), flush=True)
             res["rounds"][r].append(out)
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
