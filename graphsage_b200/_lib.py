@@ -97,6 +97,7 @@ _SIGNATURES = {
     "gs_host_unregister": (c_i32, [c_vp]),
     "gs_host_fetch": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "gs_host_translate": (c_i32, [ctypes.POINTER(ShardedTable), c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
+    "gs_host_gather_rows_f32": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "gs_gather_rows_f32": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp]),
     "gs_cast_rows_bf16": (c_i32, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp]),
     "gs_i8row_pitch": (c_i64, [c_i32]),

@@ -26,6 +26,10 @@ keep at most k_l sampled entries (ops.csr_blocks with fanouts).  Layer 0 cannot 
 global CSR, since its rows are sampled: the means reduce block 0 over V_0's rows (gathered by id, widened to fp32), the
 pools' MLP reads V_0's rows by id as before; the self rows are V_1's table rows by id in both.  Everything else is the
 minibatch path.  The draws are keyed by the model's neigh_sampler (seed, counter); one block set advances the counter by 1.
+Over a host (HostFeatures) or int8 (Int8Features) table, layer 0 runs in block-local space instead, as every layer >= 1
+does: X0 = V_0's rows as fp32 (HostFeatures.gather_rows_f32: cache or host link in one pass; ops.gather_rows_f32 for a
+device int8 table), then _FullLayer(agg, block 0, block 0's rows = V_1's positions in V_0) over X0.  Its operands are the
+fp32 values the device table's layer 0 reads, in the same order and layout, so the bits are the same; only V_0 is read.
 
 Training dropout (dropout=p > 0; contract: oracle/full_neighbor_dropout.py) masks by global identities: per CSR entry for
 the means' neighbour branch (gs_csr_aggregate_dropout, the entry's global CSR position), per node for the mean's self
@@ -42,11 +46,11 @@ import torch
 
 from . import ops
 from .aggregators import GCNAggregator, MaxPoolingAggregator, SeqAggregator, TwoMaxLayerPoolingAggregator, _rows
-from .host_features import refuse_host_table
-from .int8_features import refuse_int8_table
+from .host_features import HostFeatures, refuse_host_table
+from .int8_features import is_int8_table, refuse_int8_table
 from .layers import act_code
 from .supervised_models import (_LayerFn, build_aggregators, check_full_neighbor_dropout, full_neighbor_site_plan,
-                                layer_params)
+                                layer_params, refuse_dropout_table)
 
 
 class FullNeighborGraph(object):
@@ -114,11 +118,14 @@ class _FullLayer(object):
     ids), the pools' MLP on V_0's rows; everything after the MLP, and the whole backward, is in the graph's (block 0's)
     local space."""
 
-    def __init__(self, agg, graph, rows, src_ids=None, table_csr=None, self_ids=None):
+    def __init__(self, agg, graph, rows, src_ids=None, table_csr=None, self_ids=None, x0_dtype=None):
         """self_ids (a sampled block 0, with src_ids and no table_csr): V_1's global ids - the self rows are read from the
-        table by id, and the reductions run over the block itself, the means' on V_0's gathered rows."""
+        table by id, and the reductions run over the block itself, the means' on V_0's gathered rows.
+        x0_dtype (a sampled block 0 in block-local space, no src_ids): the source is X0, V_0's rows of a table of this
+        dtype read as fp32 for this call only - the self rows are laid out as that table's own layer 0 lays them out
+        (widened rows padded), and X0 may be masked in place."""
         self.agg, self.graph, self.rows = agg, graph, rows
-        self.src_ids, self.table_csr, self.self_ids = src_ids, table_csr, self_ids
+        self.src_ids, self.table_csr, self.self_ids, self.x0_dtype = src_ids, table_csr, self_ids, x0_dtype
         self.sites = None                       # training dropout: {"neigh", "self"} or {"mlp"} -> (seed, call, rate)
         self.gcn = isinstance(agg, GCNAggregator)
         self.pool = isinstance(agg, MaxPoolingAggregator)
@@ -157,7 +164,8 @@ class _FullLayer(object):
             return [(m, agg.neigh_input_dim, agg.vars["weights"])]
         widen = h.dtype != torch.float32
         n = h.shape[0] if h_rows is None else h_rows.numel()
-        hs = _rows(h, h_rows, 0, n, widen) if (widen or h_rows is not None) else h
+        wself = widen if self.x0_dtype is None else self.x0_dtype != torch.float32
+        hs = _rows(h, h_rows, 0, n, wself) if (wself or h_rows is not None) else h
         if not self.pool:
             if s is not None:                                        # the self rows by node id, after widening
                 # a sampled block 0 reads them by global id (self_ids), which are their positions
@@ -172,7 +180,9 @@ class _FullLayer(object):
         else:                                                        # V_0's rows read by id: no gathered copy
             x, z = None, ops.TableRows(h, [(self.src_ids, 0)], self.src_ids.numel())
         if s is not None:                                            # the MLP input, once per node, by node id
-            x = z = ops.dropout_apply(x, s["mlp"], pos_ids=g.node_ids(None), out=None if x is h else x)
+            # X0 is this call's own buffer: masked in place, as the table path masks its gathered copy
+            own = x is not h or self.x0_dtype is not None
+            x = z = ops.dropout_apply(x, s["mlp"], pos_ids=g.node_ids(None), out=x if own else None)
         for dense in agg.mlp_layers:                 # Dense without its dropout (layers.py:104-116), once per node
             code, post = act_code(dense.act)
             if getattr(dense, "_packed", None) is None:
@@ -252,9 +262,10 @@ def refuse_capture(what):
         raise NotImplementedError("%s cannot be captured in a CUDA graph" % what)
 
 
-def refuse_full_neighbor(model, training, dropout=None):
+def refuse_full_neighbor(model, training, dropout=None, tables=True):
     """The NotImplementedErrors of the full-neighbourhood entry points; training adds those of the training paths.
-    dropout: the training call's explicit rate (None: the model's dropout_rate must be 0)."""
+    dropout: the training call's explicit rate (None: the model's dropout_rate must be 0).  tables=False leaves out the
+    host- and int8-table refusals (the sampled blocks read V_0's rows only)."""
     what = "training" if training else "inference"
     if model.aggregator_cls is SeqAggregator:
         raise NotImplementedError("full-neighbourhood %s is not implemented for the seq aggregator (its neighbour "
@@ -262,8 +273,9 @@ def refuse_full_neighbor(model, training, dropout=None):
     if hasattr(model.features, "c_table"):
         raise NotImplementedError("full-neighbourhood %s with a node-partitioned (ShardedFeatures) table is not "
                                   "implemented" % what)
-    refuse_host_table(model.features, "full-neighbourhood %s (it reads the whole table)" % what)
-    refuse_int8_table(model.features, "full-neighbourhood %s" % what)
+    if tables:
+        refuse_host_table(model.features, "full-neighbourhood %s (it reads the whole table)" % what)
+        refuse_int8_table(model.features, "full-neighbourhood %s" % what)
     if not training:
         return
     if model.aggregator_cls is TwoMaxLayerPoolingAggregator:
@@ -303,10 +315,11 @@ def _inputs(model, indptr, indices, node_ids):
     return indptr, indices, ids
 
 
-def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0.):
+def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x0_dtype=None):
     """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped); draw =
     (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead, and with
-    dropout = p > 0 each block's position map also carries its entries' raw-row offsets."""
+    dropout = p > 0 each block's position map also carries its entries' raw-row offsets.  x0_dtype (sampled): layer 0
+    runs in block-local space over X0, V_0's fp32 rows of a table of that dtype (sampled_layer0_rows)."""
     L = len(aggregators)
     offsets = [None] * L
     if draw is None:
@@ -324,7 +337,9 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0.):
         graph = FullNeighborGraph(b.indptr, b.indices, pos_map=pos_map)
         if layer == 0:
             v1 = blocks[1].src_ids if L > 1 else ids
-            if draw is not None:
+            if draw is not None and x0_dtype is not None:
+                layers.append(_FullLayer(agg, graph, b.rows, x0_dtype=x0_dtype))
+            elif draw is not None:
                 layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, self_ids=v1))
             else:
                 layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
@@ -334,14 +349,32 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0.):
 
 
 def refuse_sampled(model, training, dropout=None):
-    """The NotImplementedErrors of the sampled-block entry points: refuse_full_neighbor's, CUDA-graph capture and, when
-    training, dropout=None on a model with dropout_rate > 0."""
+    """The NotImplementedErrors of the sampled-block entry points: refuse_full_neighbor's but its host- and int8-table
+    ones, CUDA-graph capture and, when training, dropout=None on a model with dropout_rate > 0 and dropout = p > 0 on an
+    int8 table."""
     if training and dropout is None and getattr(model, "dropout_rate", 0.):
         raise NotImplementedError("sampled-block training with dropout > 0 needs the rate passed explicitly - pass "
                                   "dropout=model.dropout_rate for the per-edge masks keyed by global CSR positions "
                                   "(oracle/sampled_blocks_dropout.py)")
-    refuse_full_neighbor(model, training, dropout)
+    refuse_full_neighbor(model, training, dropout, tables=False)
+    if training and dropout and is_int8_table(model.features):
+        refuse_dropout_table(model.features)
     refuse_capture("a sampled-block minibatch (it reads the block sizes back)")
+
+
+def reads_v0_rows(features):
+    """Whether a sampled block set's layer 0 runs over X0, V_0's rows as fp32: a host table (only V_0 crosses the link)
+    or an int8 table (V_0 dequantised once).  fp32 and bf16 device tables are read by id in place."""
+    return isinstance(features, HostFeatures) or is_int8_table(features)
+
+
+def sampled_layer0_rows(features, src_ids):
+    """X0: the rows src_ids (V_0) of a host or int8 table as an fp32 [|V_0|, pad_cols(F)] buffer's [:, :F] view, the
+    layout ops.gather_rows_f32 gives - HostFeatures.gather_rows_f32 for a host table, ops.gather_rows_f32 for a device
+    int8 one."""
+    if isinstance(features, HostFeatures):
+        return features.gather_rows_f32(src_ids)
+    return ops.gather_rows_f32(features, src_ids)
 
 
 def sampled_draw(model):
@@ -355,10 +388,11 @@ def sampled_draw(model):
 
 
 def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False):
-    """The checked layers of one call: over the receptive-field blocks of node_ids (minibatch; reads the block sizes
-    back once; sampled: over sampled blocks), else over the whole CSR - the model's cached FullNeighborGraph when
-    training, an uncached one otherwise (inference builds no transposes, and must not evict the ones a training CSR has
-    cached)."""
+    """(the checked layers of one call, layer 0's source): over the receptive-field blocks of node_ids (minibatch; reads
+    the block sizes back once; sampled: over sampled blocks), else over the whole CSR - the model's cached
+    FullNeighborGraph when training, an uncached one otherwise (inference builds no transposes, and must not evict the
+    ones a training CSR has cached).  The source is the model's table, or X0 for sampled blocks over a host or int8
+    table."""
     if sampled:
         refuse_sampled(model, training, dropout)
     else:
@@ -368,21 +402,26 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None,
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
     if model.aggregators is None:
         model.aggregators = build_aggregators(model)
+    h = model.features
     if sampled:
-        return minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model), dropout=dropout)
+        x0 = reads_v0_rows(h)
+        layers = minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model), dropout=dropout,
+                                  x0_dtype=h.dtype if x0 else None)
+        # |V_0| is known from the block build's size read: X0 is sized without another
+        return layers, (sampled_layer0_rows(h, layers[0].graph.pos_map[1]) if x0 else h)
     if minibatch:
-        return minibatch_layers(model.aggregators, indptr, indices, ids)
+        return minibatch_layers(model.aggregators, indptr, indices, ids), h
     graph = full_neighbor_graph(model, indptr, indices) if training else FullNeighborGraph(indptr, indices)
     L = len(model.aggregators)
-    return [_FullLayer(agg, graph, ids if layer == L - 1 else None) for layer, agg in enumerate(model.aggregators)]
+    return [_FullLayer(agg, graph, ids if layer == L - 1 else None) for layer, agg in enumerate(model.aggregators)], h
 
 
 def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False, sampled=False):
     """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings; sampled:
     sampled_minibatch_embeddings), without autograd."""
-    h = model.features
     with torch.no_grad():
-        for fl in _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled):
+        layers, h = _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled)
+        for fl in layers:
             h = fl.agg._finish(fl.forward(h, None), fl.agg._combine())
         if normalize:
             h = ops.l2_normalize_rows_(h.contiguous())
@@ -395,7 +434,7 @@ def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, mini
     aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
     sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them."""
     p = check_full_neighbor_dropout(dropout)
-    layers = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled)
+    layers, h = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled)
     if p:
         pool = isinstance(layers[0].agg, MaxPoolingAggregator)
         plan = full_neighbor_site_plan("maxpool" if pool else "mean", len(layers))
@@ -403,7 +442,6 @@ def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, mini
             layers[layer].sites = layers[layer].sites or {}
             layers[layer].sites[role] = (model.dropout_key, model.dropout_counter + i, p)
         model.dropout_counter += len(plan)
-    h = model.features
     for layer, fl in enumerate(layers):
         emb = getattr(model, "embeds", None) if layer == 0 else None
         h = _LayerFn.apply(fl, h, emb, *layer_params(fl.agg))

@@ -17,6 +17,10 @@ with the count on the device, no host synchronisation and launch sizes fixed by 
 capturable in a CUDA graph.  The hot rows (`cache_ids`, see hot_rows) are copied into the working set once and never
 cross the link again.  Nothing downstream can tell where a row came from: outputs, losses and gradients are the bits the
 same model computes on the table held on the device.
+
+The sampled-block entry points (sampled_minibatch_*) stage nothing: their layer 0 reads only V_0, the sorted, unique
+source ids of block 0, and needs them as fp32 rows, so gather_rows_f32 loads them in one pass (gs_host_gather_rows_f32:
+cached rows from the working set's head, the rest over the link) straight into the fp32 operand.
 """
 import ctypes
 
@@ -163,6 +167,13 @@ class HostFeatures(object):
         if self.dtype == torch.int8:
             return ops.I8Rows(self.ws, self.shape[1]), out
         return self.ws[:, :self.shape[1]], out
+
+    def gather_rows_f32(self, ids):
+        """Rows `ids` (int32 device ids) widened to fp32 in one pass (gs_host_gather_rows_f32): cached rows from the
+        working set, ids outside [0, N) as the zero row, the rest over the host link - no staging, no claim.  The layer-0
+        rows of a sampled block set (V_0); the fp32 [n, pad_cols(F)] buffer's [:, :F] view, the bits ops.gather_rows_f32
+        gives on the same table held on the device."""
+        return ops.host_gather_rows_f32(self._alias, self.ws, self.cache_slot, self.n_nodes, self.shape[1], ids)
 
     def close(self):
         """Unpin the host rows and drop the device buffers (the object is unusable afterwards)."""

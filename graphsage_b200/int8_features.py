@@ -29,7 +29,8 @@ class Int8Features(ops.I8Rows):
 
     .rows is the uint8 [N+1, pitch] byte table, .shape == (N+1, F), .dtype == torch.int8; dequantize() gives the fp32
     table every kernel reads.  Not supported (NotImplementedError): fused_pool=True, the seq aggregator, training dropout,
-    identity_dim > 0, node-partitioned tables and distributed=True, and the full-neighbourhood passes."""
+    identity_dim > 0, node-partitioned tables and distributed=True, and the whole-graph and whole-neighbourhood passes
+    (the sampled-block entry points, sampled_minibatch_*, take it)."""
 
     def __init__(self, table, device=None):
         t = table if torch.is_tensor(table) else torch.from_numpy(np.asarray(table))

@@ -282,7 +282,9 @@ class SampleAndAggregate(object):
         distinct node of a block is computed once per layer - GraphSAGE's minibatch over sampled blocks, against
         forward()'s one tree per seed over the padded table.  With every fanout >= the largest degree it is
         full_neighbor_minibatch_embeddings, bit for bit.  Reads the block sizes back once per call, so it cannot be
-        captured in a CUDA graph.  Same refusals as full_neighbor_embeddings."""
+        captured in a CUDA graph.  Same refusals as full_neighbor_embeddings, except that a host-memory (HostFeatures) or
+        int8 (Int8Features) table is taken: layer 0 then reads only V_0's rows, as fp32, and gives the bits of the device
+        table (fp32 / bf16 twin, or the int8 table and its dequantize())."""
         from .full_neighbor_training import full_neighbor_embeddings
         return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, sampled=True)
 

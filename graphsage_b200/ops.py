@@ -458,6 +458,26 @@ def host_fetch(host_alias, row_bytes, stage_ids, count, staging):
     _launched(1 if capacity else 0, ev)
 
 
+def host_gather_rows_f32(host_alias, cache, cache_slot, n_nodes, F, ids, out=None):
+    """Rows ids[i] of a mapped host table widened to fp32 (gs_host_gather_rows_f32): from `cache` (a device table of the
+    host rows' dtype and pitch - a uint8 byte table for int8 rows) where cache_slot[id] >= 0, the zero row for an id
+    outside [0, n_nodes), else over the host link.  Returns an fp32 [n, pad_cols(F)] buffer's [:, :F] view, pad columns
+    zeroed (the layout of gather_rows_f32)."""
+    require_cuda(cache, cache_slot, ids, out)
+    ids = _i32(ids.reshape(-1), "ids")
+    n = ids.numel()
+    if out is None:
+        out = torch.empty((n, pad_cols(F)), dtype=torch.float32, device=ids.device)[:, :F]
+    if out.dtype != torch.float32 or out.stride(1) != 1 or out.shape[0] < n:
+        raise ValueError("out must be a row-major float32 matrix with >= n rows")
+    code = _lib.GS_I8ROW if cache.dtype == torch.uint8 else _dtype_code(cache)
+    ev = _probe("host_gather_rows_f32")
+    check(lib().gs_host_gather_rows_f32(host_alias, ptr(cache), ptr(_i32(cache_slot, "cache_slot")), code, int(n_nodes),
+                                        int(F), cache.stride(0), ptr(ids), n, ptr(out), out.stride(0), stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return out
+
+
 def host_translate(table, ids, claim, stage_row0, out=None):
     """ids -> working-set rows of a host table (gs_host_translate): the cache slot, the zero row, or stage_row0 + slot."""
     ids = _i32(ids.reshape(-1), "ids")

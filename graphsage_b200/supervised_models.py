@@ -732,7 +732,8 @@ class SupervisedGraphsage(SampleAndAggregate):
         training rate p in [0, 1) - callers pass dropout=model.dropout_rate: the full-neighbourhood masks, a sampled
         entry masked as the same CSR entry is in the whole-graph pass (contract: oracle/sampled_blocks_dropout.py), sites
         numbered from dropout_counter; p = 0 gives the bits of dropout=None.  Refused (NotImplementedError): what
-        full_neighbor_outputs refuses, CUDA-graph capture, and dropout=None on a model whose dropout_rate > 0."""
+        full_neighbor_outputs refuses but host-memory and int8 tables (taken here: see sampled_minibatch_embeddings),
+        CUDA-graph capture, dropout=None on a model whose dropout_rate > 0, and dropout = p > 0 on an int8 table."""
         from .full_neighbor_training import full_neighbor_outputs
         return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True, dropout=dropout)
 

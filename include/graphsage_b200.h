@@ -279,6 +279,18 @@ int32_t gs_host_fetch(const void* host_alias, int64_t row_bytes, const int32_t* 
  * for an id outside [0, N), stage_row0 + claim[id] for a staged one. */
 int32_t gs_host_translate(const gs_sharded_table* table_host, const int32_t* ids, int64_t n, const int32_t* claim,
                           int64_t stage_row0, int32_t* out, void* stream);
+/* The sampled blocks' layer-0 load (no working set, no claim): out[i, 0:F) = the row of ids[i] widened to fp32, columns
+ * F..out_pitch-1 zeroed, for i < n.  The row is cache[cache_slot[id]] when cache_slot[id] >= 0 (the working set's cached
+ * rows), the zero row for an id outside [0, n_nodes) - the dummy id N included; no host read is made for it - and else
+ * host_alias[id] over the host link (gs_host_register).  dtype GS_F32 / GS_BF16 (pitch in elements; bf16 widened
+ * exactly) or GS_I8ROW (pitch in bytes; deq_c = fl(float(q_c) * s), the scale read from the row), the same pitch for
+ * host and cache rows: 16-byte multiples at 16-byte aligned addresses.  out: 16-byte aligned, out_pitch % 4 == 0 and
+ * >= F (and <= gs_i8row_pitch(F) for GS_I8ROW).  Duplicate ids are allowed; no atomics, no allocation, no host
+ * synchronisation; a capped grid keeps several rows' loads in flight per warp, as gs_host_fetch does.  int8 rows with
+ * F <= 4092 are read as whole-row copies read them, one warp per row, the scale taken from the row's own unit. */
+int32_t gs_host_gather_rows_f32(const void* host_alias, const void* cache, const int32_t* cache_slot, int32_t dtype,
+                                int64_t n_nodes, int32_t F, int64_t pitch, const int32_t* ids, int64_t n, float* out,
+                                int64_t out_pitch, void* stream);
 
 /* embedding_lookup (models.py:299) with the result widened to fp32: out[i, 0:F] = (float)feats[ids ? ids[i] : row0 + i, 0:F],
  * columns F..out_pitch-1 zeroed.  feats is GS_BF16, GS_F32 or GS_I8ROW (pitch in bytes; the dequantised values).  The bf16
