@@ -173,10 +173,14 @@ _SIGNATURES = {
                                          DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "gs_csr_aggregate_dropout_offsets": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32,
                                                  DropoutSite, DropoutSite, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    "gs_csr_aggregate_weighted": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp,
+                                          c_i64, c_vp]),
     "gs_csr_transpose_workspace_bytes": (c_i64, [c_i64, c_i64, c_i32]),
     "gs_csr_transpose": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gs_csr_max_backward": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64,
                                     c_vp, c_i64, c_vp]),
+    "gs_csr_max_backward_weighted": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                             c_i64, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "gs_csr_blocks_workspace_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i32]),
     "gs_csr_blocks_plan": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp]),
     "gs_csr_blocks_fill": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, c_vp, c_i64, ctypes.POINTER(c_i64),

@@ -15,6 +15,12 @@
 // only some entries of its node's raw row, so entry e is masked at pos_indptr[g] + pos_off[lo + e] (its offset in the raw
 // row) instead of + e; the implicit dummy entry of an empty row keeps pos_nnz + g.  The means only: the transposed sum
 // of a sampled block reads t_slot already mapped through the offsets.
+// kW (gs_csr_aggregate_weighted; contract in oracle/weighted.py): entry e's term is fl(weight[lo + e] * x), rounded to
+// fp32 before it joins the chain (__fmul_rn: never contracted into the sum), 1 for an empty row's dummy entry.  The short
+// role loads the weight beside the entry's index and columns (weight()) and scales where the term is consumed (scale()),
+// so all kUnroll entries' loads stay in flight; the hub role's loading warps scale their terms in hub_mask(), after the
+// round's loads are issued and before the tile is written, so warp 0's ordered sum is unchanged.  All four ops; the
+// sum's weights are aligned with its own (transposed) indices.
 #include "csr_rows.cuh"
 
 namespace gs {
@@ -42,6 +48,7 @@ struct CsrArgs {
   int64_t pos_nnz;
   const int32_t* t_slot;
   const int32_t* pos_off;    // kOff only: each entry's offset in its node's raw CSR row
+  const float* weight;       // kW only: one weight per entry of indices
 };
 
 __device__ __forceinline__ int64_t csr_clamp(int64_t id, int64_t n_rows) { return (id < 0 || id >= n_rows) ? n_rows - 1 : id; }
@@ -169,7 +176,7 @@ __device__ __forceinline__ void quad_transpose(const u32x4& w, uint32_t (&m)[4])
 
 // the aggregate on the csr_rows.cuh schedule: the rows of `rows` (or 0 .. n - 1), entries read from src, written up to
 // out_pitch with columns F .. out_pitch - 1 zero-filled
-template <typename T, int OP, bool kDrop, bool kOff = false>
+template <typename T, int OP, bool kDrop, bool kOff = false, bool kW = false>
 struct AggregateRows {
   static constexpr bool kFromFirst = OP == GS_CSR_MAX;
   static constexpr bool kEmptyIsDummy = OP != GS_CSR_SUM;   // the sum's empty row is +0 (a node nobody points to)
@@ -205,6 +212,20 @@ struct AggregateRows {
     if (ok) Loader<T, W>::load(a, csr_entry(a, r.lo, r.cnt, e), c0, x);
   }
 
+  // kW: entry e's weight (an empty row's one entry is its dummy, of weight 1), and its scaling of the loaded columns
+  __device__ __forceinline__ float weight(const Row& r, int64_t e, bool ok) const {
+    if constexpr (kW) return (ok && r.cnt > 0) ? __ldg(a.weight + r.lo + e) : 1.f;
+    else return 1.f;
+  }
+
+  template <int W>
+  __device__ __forceinline__ void scale(float w, float (&x)[W]) const {
+    if constexpr (kW) {
+#pragma unroll
+      for (int q = 0; q < W; ++q) x[q] = __fmul_rn(w, x[q]);
+    }
+  }
+
   __device__ __forceinline__ float value(const Row& r, int64_t e, int c) const {
     float x[1];
     load(r, e, c, true, x);
@@ -226,9 +247,16 @@ struct AggregateRows {
     }
   }
 
-  // the masks of the warp's entries e0 .. e0 + kHubPerWarp - 1 of a hub row (cnt > kHubRows) at column c; entries past
-  // the row are computed on its last entry and multiply a loaded 0
+  // the masks (kDrop) or weights (kW) of the warp's entries e0 .. e0 + kHubPerWarp - 1 of a hub row (cnt > kHubRows) at
+  // column c; entries past the row are computed on its last entry and multiply a loaded 0
   __device__ __forceinline__ void hub_mask(const Row& r, int64_t e0, int c, float (&x)[kHubPerWarp]) const {
+    if constexpr (kW) {
+      float w[kHubPerWarp];
+#pragma unroll
+      for (int u = 0; u < kHubPerWarp; ++u) w[u] = __ldg(a.weight + r.lo + min(e0 + u, r.cnt - 1));
+#pragma unroll
+      for (int u = 0; u < kHubPerWarp; ++u) x[u] = __fmul_rn(w[u], x[u]);
+    }
     if constexpr (kDrop) {
       const int j = threadIdx.x & 3;
 #pragma unroll
@@ -274,7 +302,7 @@ struct AggregateRows {
   }
 };
 
-template <typename T, int V, int OP, bool kDrop, bool kOff = false>
+template <typename T, int V, int OP, bool kDrop, bool kOff = false, bool kW = false>
 __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __grid_constant__ CsrArgs a) {
   __shared__ __align__(16) float tile[2][kHubRows][kHubCols];
   DropSite sn = a.neigh, ss = a.self;
@@ -283,7 +311,7 @@ __global__ void __launch_bounds__(kCsrThreads, 3) csr_aggregate_kernel(const __g
     ss.call += drop_call_offset(ss);
   }
   // short role: 16-byte loads in flight per lane: 4 (bf16) or 8 (fp32 float4)
-  csr_rows<V, V == 8 ? 4 : 8>(AggregateRows<T, OP, kDrop, kOff>{a, sn, ss}, tile);
+  csr_rows<V, V == 8 ? 4 : 8>(AggregateRows<T, OP, kDrop, kOff, kW>{a, sn, ss}, tile);
 }
 
 template <typename T, int V>
@@ -292,6 +320,15 @@ static void launch_csr(int32_t op, unsigned blocks, const CsrArgs& a, cudaStream
   else if (op == GS_CSR_MEAN_SELF) csr_aggregate_kernel<T, V, GS_CSR_MEAN_SELF, false><<<blocks, kCsrThreads, 0, st>>>(a);
   else if (op == GS_CSR_MAX) csr_aggregate_kernel<T, V, GS_CSR_MAX, false><<<blocks, kCsrThreads, 0, st>>>(a);
   else if constexpr (sizeof(T) == 4) csr_aggregate_kernel<T, V, GS_CSR_SUM, false><<<blocks, kCsrThreads, 0, st>>>(a);
+}
+
+// the weighted instantiations: every op, the sum over fp32 sources only
+template <typename T, int V>
+static void launch_csr_weighted(int32_t op, unsigned blocks, const CsrArgs& a, cudaStream_t st) {
+  if (op == GS_CSR_MEAN) csr_aggregate_kernel<T, V, GS_CSR_MEAN, false, false, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if (op == GS_CSR_MEAN_SELF) csr_aggregate_kernel<T, V, GS_CSR_MEAN_SELF, false, false, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if (op == GS_CSR_MAX) csr_aggregate_kernel<T, V, GS_CSR_MAX, false, false, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  else if constexpr (sizeof(T) == 4) csr_aggregate_kernel<T, V, GS_CSR_SUM, false, false, true><<<blocks, kCsrThreads, 0, st>>>(a);
 }
 
 // the masked instantiations: the means, and the sum over fp32 sources; with per-entry offsets (kOff), the means only
@@ -313,7 +350,8 @@ struct CsrDrop {
 
 static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
                              const int64_t* indptr, const int32_t* indices, int64_t n_nodes, const int32_t* rows, int64_t n,
-                             int32_t op, float* out, int64_t out_pitch, void* stream, const CsrDrop* drop, const char* who) {
+                             int32_t op, float* out, int64_t out_pitch, void* stream, const CsrDrop* drop, const char* who,
+                             const float* weight = nullptr) {
   GS_REQUIRE(op == GS_CSR_MEAN || op == GS_CSR_MEAN_SELF || op == GS_CSR_MAX || op == GS_CSR_SUM, "%s: unknown op %d", who,
              (int)op);
   GS_REQUIRE(dtype == GS_F32 || dtype == GS_BF16, "%s: dtype must be GS_F32 or GS_BF16", who);
@@ -339,6 +377,7 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
   a.pos_indptr = nullptr;
   a.pos_ids = a.t_slot = a.pos_off = nullptr;
   a.pos_nnz = 0;
+  a.weight = weight;
   if (drop) {
     a.neigh = make_drop_site(drop->neigh);
     a.self = make_drop_site(drop->self);
@@ -352,6 +391,12 @@ static int32_t csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows,
   a.hub_slices = (int32_t)((out_pitch + kHubCols - 1) / kHubCols);
   const unsigned blocks = csr_grid(n, a.hub_slices, a.n_slices, a.hub_items, a.hub_blocks);
   cudaStream_t st = (cudaStream_t)stream;
+  if (weight) {
+    if (dtype == GS_BF16) launch_csr_weighted<uint16_t, 8>(op, blocks, a, st);
+    else if (V == 4) launch_csr_weighted<float, 4>(op, blocks, a, st);
+    else launch_csr_weighted<float, 1>(op, blocks, a, st);
+    return launch_check("csr_aggregate_kernel<weighted>");
+  }
   if (drop && drop->pos_off) {
     if (dtype == GS_BF16) launch_csr_drop<uint16_t, 8, true>(op, blocks, a, st);
     else if (V == 4) launch_csr_drop<float, 4, true>(op, blocks, a, st);
@@ -379,6 +424,17 @@ int32_t gs_csr_aggregate(const void* src, int32_t dtype, int64_t n_src_rows, int
                          int64_t out_pitch, void* stream) {
   return gs::csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
                            nullptr, "gs_csr_aggregate");
+}
+
+int32_t gs_csr_aggregate_weighted(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                  const int64_t* indptr, const int32_t* indices, const float* weight, int64_t n_nodes,
+                                  const int32_t* rows, int64_t n, int32_t op, float* out, int64_t out_pitch,
+                                  void* stream) {
+  const char* who = "gs_csr_aggregate_weighted";
+  GS_REQUIRE(weight || n == 0 || n_nodes == 0, "%s: NULL weight", who);
+  // with no node, every row reduces over the dummy entry alone (weight 1): the plain kernel
+  return gs::csr_aggregate(src, dtype, n_src_rows, F, pitch, indptr, indices, n_nodes, rows, n, op, out, out_pitch, stream,
+                           nullptr, who, n_nodes == 0 ? nullptr : weight);
 }
 
 }  // extern "C"

@@ -8,6 +8,9 @@
 //   gs_csr_max_backward  TensorFlow's reduce_max gradient over whole CSR rows in two launches of one kernel template:
 //                        (a) per forward row, the tie count and the scale s = dm / count; (b) per transposed row, the
 //                        masked sum of s, then the ReLU mask of the Dense layer.
+//                        kW (gs_csr_max_backward_weighted; oracle/weighted.py): m = max fl(w_e * z_e), so (a) counts the
+//                        entries with fl(w_e * z_e) == m (forward weights, 1 for the dummy entry) and (b) adds fl(w * s)
+//                        where fl(w * z_j) == m (w: the transposed entry's forward weight).
 // Each output element of (a) and (b) is ONE sequential chain over its row's entries in order, run on the hub / short row
 // schedule of csr_rows.cuh; the hub rows here include the in-degree hubs of the transpose.
 #include "csr_rows.cuh"
@@ -160,10 +163,11 @@ struct BwdArgs {
   int64_t n_nodes;            // N; the phase has N + 1 rows
   int32_t slices;             // ceil(F / 32)
   int64_t hub_items, hub_blocks;
+  const float* w;             // kW only: one weight per entry of the phase's indices
 };
 
 // the max backward on the csr_rows.cuh schedule: the N + 1 rows of the phase, one column per lane, written up to F
-template <int PHASE>
+template <int PHASE, bool kW = false>
 struct MaxBackwardRows {
   static constexpr bool kFromFirst = false;
   static constexpr bool kEmptyIsDummy = false;     // row() already gives (a)'s empty rows their {N} entry
@@ -213,8 +217,14 @@ struct MaxBackwardRows {
   }
 
   // the term entry e adds: (a) 1 for a tie with the max; (b) s[k][c] where z[j][c] attains the max of forward row k
+  // kW: the weighted term of (a), fl(w_e * z[k][c]) against m, and the routing of (b), fl(w_e * s) where fl(w_e * z) == m
   __device__ __forceinline__ float value(const Row& r, int64_t e, int c) const {
     const int64_t k = entry(r, e);
+    if constexpr (kW) {
+      const float w = (PHASE == 0 && r.dummy) ? 1.f : __ldg(a.w + r.lo + e);
+      if (PHASE == 0) return __fmul_rn(w, __ldg(a.z + k * a.ldz + c)) == r.rv ? 1.f : 0.f;
+      return __ldg(a.m + k * a.ldm + c) == __fmul_rn(w, r.rv) ? __fmul_rn(w, __ldg(a.s + k * a.lds + c)) : 0.f;
+    }
     if (PHASE == 0) return __ldg(a.z + k * a.ldz + c) == r.rv ? 1.f : 0.f;
     return __ldg(a.m + k * a.ldm + c) == r.rv ? __ldg(a.s + k * a.lds + c) : 0.f;
   }
@@ -223,6 +233,8 @@ struct MaxBackwardRows {
     x[0] = ok ? value(r, e, c) : 0.f;
   }
   __device__ __forceinline__ void mask(const Row&, int64_t, int, float (&)[1]) const {}
+  __device__ __forceinline__ float weight(const Row&, int64_t, bool) const { return 1.f; }
+  __device__ __forceinline__ void scale(float, float (&)[1]) const {}
   __device__ __forceinline__ void hub_mask(const Row&, int64_t, int, float (&)[kHubPerWarp]) const {}
   __device__ __forceinline__ float step(float acc, float x) const { return acc + x; }
   __device__ __forceinline__ void finish(const Row&, int, int64_t, float (&)[1]) const {}
@@ -233,10 +245,34 @@ struct MaxBackwardRows {
   }
 };
 
-template <int PHASE>
+template <int PHASE, bool kW = false>
 __global__ void __launch_bounds__(kCsrThreads, 3) csr_max_backward_kernel(const __grid_constant__ BwdArgs a) {
   __shared__ __align__(16) float tile[2][kHubRows][kHubCols];
-  csr_rows<1, 8>(MaxBackwardRows<PHASE>{a}, tile);
+  csr_rows<1, 8>(MaxBackwardRows<PHASE, kW>{a}, tile);
+}
+
+// gs_csr_max_backward, or with weights (w forward, t_w transposed) gs_csr_max_backward_weighted
+static int32_t csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm, int64_t lddm,
+                                int32_t F, const int64_t* indptr, const int32_t* indices, const float* w,
+                                const int64_t* t_indptr, const int32_t* t_indices, const float* t_w, int64_t n_nodes,
+                                float* s, int64_t lds, float* dz, int64_t lddz, void* stream, const char* who) {
+  GS_REQUIRE(F >= 1 && n_nodes >= 0 && ldz >= F && ldm >= F && lddm >= F && lds >= F && lddz >= F, "%s: bad sizes", who);
+  GS_REQUIRE(z && m && dm && s && dz && t_indptr && t_indices && (n_nodes == 0 || (indptr && indices)),
+             "%s: NULL pointer", who);
+  BwdArgs a{z, ldz, m, ldm, dm, lddm, s, lds, dz, lddz, F, indptr, indices, n_nodes, 0, 0, 0, w};
+  a.slices = (F + kHubCols - 1) / kHubCols;
+  const unsigned blocks = csr_grid(n_nodes + 1, a.slices, a.slices, a.hub_items, a.hub_blocks);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (t_w) csr_max_backward_kernel<0, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  else csr_max_backward_kernel<0><<<blocks, kCsrThreads, 0, st>>>(a);         // (a) tie counts -> s
+  int32_t rc = launch_check("csr_max_backward_kernel<0>");
+  if (rc != GS_OK) return rc;
+  a.indptr = t_indptr;
+  a.indices = t_indices;
+  a.w = t_w;
+  if (t_w) csr_max_backward_kernel<1, true><<<blocks, kCsrThreads, 0, st>>>(a);
+  else csr_max_backward_kernel<1><<<blocks, kCsrThreads, 0, st>>>(a);         // (b) masked sums over the transpose -> dz
+  return launch_check("csr_max_backward_kernel<1>");
 }
 
 }  // namespace gs
@@ -301,21 +337,19 @@ int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t
                             int32_t F, const int64_t* indptr, const int32_t* indices, const int64_t* t_indptr,
                             const int32_t* t_indices, int64_t n_nodes, float* s, int64_t lds, float* dz, int64_t lddz,
                             void* stream) {
-  const char* who = "gs_csr_max_backward";
-  GS_REQUIRE(F >= 1 && n_nodes >= 0 && ldz >= F && ldm >= F && lddm >= F && lds >= F && lddz >= F, "%s: bad sizes", who);
-  GS_REQUIRE(z && m && dm && s && dz && t_indptr && t_indices && (n_nodes == 0 || (indptr && indices)),
-             "%s: NULL pointer", who);
-  gs::BwdArgs a{z, ldz, m, ldm, dm, lddm, s, lds, dz, lddz, F, indptr, indices, n_nodes, 0, 0, 0};
-  a.slices = (F + gs::kHubCols - 1) / gs::kHubCols;
-  const unsigned blocks = gs::csr_grid(n_nodes + 1, a.slices, a.slices, a.hub_items, a.hub_blocks);
-  cudaStream_t st = (cudaStream_t)stream;
-  gs::csr_max_backward_kernel<0><<<blocks, gs::kCsrThreads, 0, st>>>(a);       // (a) tie counts -> s
-  int32_t rc = gs::launch_check("csr_max_backward_kernel<0>");
-  if (rc != GS_OK) return rc;
-  a.indptr = t_indptr;
-  a.indices = t_indices;
-  gs::csr_max_backward_kernel<1><<<blocks, gs::kCsrThreads, 0, st>>>(a);       // (b) masked sums over the transpose -> dz
-  return gs::launch_check("csr_max_backward_kernel<1>");
+  return gs::csr_max_backward(z, ldz, m, ldm, dm, lddm, F, indptr, indices, nullptr, t_indptr, t_indices, nullptr, n_nodes,
+                              s, lds, dz, lddz, stream, "gs_csr_max_backward");
+}
+
+int32_t gs_csr_max_backward_weighted(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm,
+                                     int64_t lddm, int32_t F, const int64_t* indptr, const int32_t* indices,
+                                     const float* weight, const int64_t* t_indptr, const int32_t* t_indices,
+                                     const float* t_weight, int64_t n_nodes, float* s, int64_t lds, float* dz,
+                                     int64_t lddz, void* stream) {
+  const char* who = "gs_csr_max_backward_weighted";
+  GS_REQUIRE(t_weight && (n_nodes == 0 || weight), "%s: NULL weight or t_weight", who);
+  return gs::csr_max_backward(z, ldz, m, ldm, dm, lddm, F, indptr, indices, weight, t_indptr, t_indices, t_weight,
+                              n_nodes, s, lds, dz, lddz, stream, who);
 }
 
 }  // extern "C"

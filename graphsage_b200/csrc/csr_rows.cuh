@@ -14,9 +14,10 @@
 // from +0), kEmptyIsDummy (the short role reduces an empty row over one entry, the dummy row), the launch's rows(),
 // hub_slices(), slices() and out_cols() (the columns written), row(i) (row i's entry range: Row::cnt entries), begin()
 // (row state read before the entries; col_ok: c < F), value() (the term an entry adds at one column, hub role), load()
-// and mask() (an entry's W columns, ok: inside the row; the loads, then what is applied before the sum), hub_mask()
-// (applied to the hub role's kHubPerWarp terms), step(), finish() (the chain's end on columns c0 .. c0 + W - 1 < F) and
-// store().
+// and mask() (an entry's W columns, ok: inside the row; the loads, then what is applied before the sum), weight() and
+// scale() (an entry's scale, loaded beside its columns, applied after mask() where the term is consumed - so no load
+// waits on another; 1 and nothing where a kernel has no scale), hub_mask() (applied to the hub role's kHubPerWarp
+// terms), step(), finish() (the chain's end on columns c0 .. c0 + W - 1 < F) and store().
 #pragma once
 #include <algorithm>
 
@@ -128,19 +129,24 @@ __device__ void csr_short_role(const P& p, int64_t block) {
       int64_t e = 0;
       if constexpr (P::kFromFirst) {
         float x0[V];
-        p.load(r, e++, c0, true, x0);
+        p.load(r, e, c0, true, x0);
+        p.scale(p.weight(r, e++, true), x0);
 #pragma unroll
         for (int q = 0; q < V; ++q) acc[q] = x0[q];
       }
       for (; e < count; e += kUnroll) {
         float x[kUnroll][V];
+        float wt[kUnroll];
 #pragma unroll
-        for (int u = 0; u < kUnroll; ++u)
+        for (int u = 0; u < kUnroll; ++u) {
           p.load(r, e + u, c0, e + u < count, x[u]);
+          wt[u] = p.weight(r, e + u, e + u < count);
+        }
 #pragma unroll
         for (int u = 0; u < kUnroll; ++u)
           if (e + u < count) {
             p.mask(r, e + u, c0, x[u]);
+            p.scale(wt[u], x[u]);
 #pragma unroll
             for (int q = 0; q < V; ++q) acc[q] = p.step(acc[q], x[u][q]);
           }

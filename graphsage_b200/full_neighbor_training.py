@@ -41,7 +41,16 @@ oracle/sampled_blocks_dropout.py) keeps only some entries of each raw row, so it
 entry's offset in its raw row (ops.csr_blocks(..., entry_offsets=True)): the forward masks entry j at pos_indptr[g] +
 offset, and the backward maps t_slot through the offsets (ops.csr_slots_to_offsets) before the same transposed sum.  A
 sampled entry is then masked as the same edge is in the whole-graph pass.
+
+Edge weights (edge_weight=w, fp32, one per CSR entry; contract: oracle/weighted.py) scale each message before the
+reduction: every reduction runs gs_csr_aggregate_weighted with its graph's per-entry weights, the means' backward sums
+fl(w * g / count) over the transpose with each transposed entry's forward weight (ops.csr_transpose_weights, cached on
+the FullNeighborGraph beside the transposes), and the max-pool backward splits ties on the weighted values
+(ops.csr_max_backward with weights).  A block's entries carry the weights of the raw entries they copy
+(ops.csr_block_weights, built per call); layer 0 of a whole-neighbourhood minibatch reads the global CSR, so it takes w.
+Not with training dropout p > 0.
 """
+import numpy as np
 import torch
 
 from . import ops
@@ -57,18 +66,20 @@ class FullNeighborGraph(object):
     """The transposes and divisors of one CSR, built on first use.  `key` identifies the CSR tensors (data_ptr, numel,
     _version of both); the tensors themselves are held, so their memory cannot be reused by a different CSR while cached."""
 
-    def __init__(self, indptr, indices, pos_map=None):
+    def __init__(self, indptr, indices, pos_map=None, weights=None):
         """pos_map: (pos_indptr, pos_ids or None, pos_nnz[, pos_off]), how the masks name this CSR's rows and entries
-        globally (default: the CSR is the global one); pos_off: a sampled block's per-entry raw-row offsets."""
-        self.indptr, self.indices = indptr, indices
+        globally (default: the CSR is the global one); pos_off: a sampled block's per-entry raw-row offsets.  weights:
+        None, or fp32 [len(indices)], the edge weights of this CSR's entries (part of the key)."""
+        self.indptr, self.indices, self.weights = indptr, indices, weights
         self.pos_map = pos_map if pos_map is not None else (indptr, None, indices.numel())
-        self.key = FullNeighborGraph.key_of(indptr, indices)
+        self.key = FullNeighborGraph.key_of(indptr, indices, weights)
         self.n_rows = indptr.numel()                 # N + 1
-        self._t, self._counts = {}, {}
+        self._t, self._counts, self._tw = {}, {}, {}
 
     @staticmethod
-    def key_of(indptr, indices):
-        return tuple((t.data_ptr(), t.numel(), t._version) for t in (indptr, indices))
+    def key_of(indptr, indices, weights=None):
+        ts = (indptr, indices) if weights is None else (indptr, indices, weights)
+        return tuple((t.data_ptr(), t.numel(), t._version) for t in ts)
 
     def transpose(self, with_self, slots=False):
         """(t_indptr, t_indices), or with slots (t_indptr, t_indices, t_slot); a slotted transpose serves both."""
@@ -82,6 +93,13 @@ class FullNeighborGraph(object):
             self._t[with_self] = ops.csr_transpose(self.indptr, self.indices, with_self=with_self)
         return self._t[with_self]
 
+    def t_weights(self, with_self):
+        """The edge weights of transpose(with_self)'s entries, aligned with its t_indices (ops.csr_transpose_weights)."""
+        if with_self not in self._tw:
+            _, t_indices, t_slot = self.transpose(with_self, slots=True)
+            self._tw[with_self] = ops.csr_transpose_weights(self.weights, self.indptr, t_indices, t_slot)
+        return self._tw[with_self]
+
     def counts(self, with_self):
         """The forward's divisors for the N + 1 effective rows (max(degree, 1), + 1 for GCN), fp32 [N + 1, 1]."""
         if with_self not in self._counts:
@@ -94,6 +112,9 @@ class FullNeighborGraph(object):
         """d(source) of the mean over the effective rows for their gradient g [N + 1, w]: sum of g / count over the
         transposed rows; sites = (neighbour, self): the forward's masks, regenerated through t_slot."""
         gp = (g / self.counts(with_self)).contiguous()
+        if self.weights is not None:                 # no dropout with weights
+            t_indptr, t_indices = self.transpose(with_self, slots=True)[:2]
+            return ops.csr_aggregate(gp, t_indptr, t_indices, "sum", weights=self.t_weights(with_self))
         if sites is None:
             t_indptr, t_indices = self.transpose(with_self)
             return ops.csr_aggregate(gp, t_indptr, t_indices, "sum")
@@ -119,7 +140,8 @@ class _FullLayer(object):
     local space."""
 
     def __init__(self, agg, graph, rows, src_ids=None, table_csr=None, self_ids=None, x0_dtype=None):
-        """self_ids (a sampled block 0, with src_ids and no table_csr): V_1's global ids - the self rows are read from the
+        """table_csr: (global indptr, global indices, V_1's global ids, global edge weights or None).
+        self_ids (a sampled block 0, with src_ids and no table_csr): V_1's global ids - the self rows are read from the
         table by id, and the reductions run over the block itself, the means' on V_0's gathered rows.
         x0_dtype (a sampled block 0 in block-local space, no src_ids): the source is X0, V_0's rows of a table of this
         dtype read as fp32 for this call only - the self rows are laid out as that table's own layer 0 lays them out
@@ -149,7 +171,8 @@ class _FullLayer(object):
         besides the parts."""
         agg, g, rows = self.agg, self.graph, self.rows
         self.table = h if self.src_ids is not None else None
-        indptr, indices, h_rows = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows)
+        indptr, indices, h_rows, w = self.table_csr if self.table_csr is not None else (g.indptr, g.indices, rows,
+                                                                                        g.weights)
         hn, n_rows = h, h_rows                  # the means' reduction source and its rows
         if self.self_ids is not None:           # a sampled block 0: self rows by global id, reductions in the block
             h_rows = self.self_ids
@@ -159,6 +182,8 @@ class _FullLayer(object):
         # the means' masks: the table CSR is the global one (positions by node id), else the graph's own map
         tgraph = FullNeighborGraph(indptr, indices) if self.table_csr is not None else g
         drop = {} if s is None or self.pool else {"dropout": (s["neigh"], s["self"], tgraph.pos_map)}
+        if w is not None:                            # the edge weights of the means' CSR (no dropout with them)
+            drop = {"weights": w}
         if self.gcn:
             m = ops.csr_aggregate(hn, indptr, indices, "mean_self", rows=n_rows, **drop)
             return [(m, agg.neigh_input_dim, agg.vars["weights"])]
@@ -191,12 +216,13 @@ class _FullLayer(object):
                               math=agg.math, packed=dense._packed)
             z = post(z) if post else z
         op = "max" if agg.pool == "max" else "mean"
+        gw = {} if g.weights is None else {"weights": g.weights}
         if kept is not None and op == "max" and rows is not None:
             # training: the backward needs every row's max - the same chains, then the rows
-            p_all = ops.csr_aggregate(z, g.indptr, g.indices, "max")
+            p_all = ops.csr_aggregate(z, g.indptr, g.indices, "max", **gw)
             p = p_all.index_select(0, rows)
         else:
-            p = p_all = ops.csr_aggregate(z, g.indptr, g.indices, op, rows=rows)
+            p = p_all = ops.csr_aggregate(z, g.indptr, g.indices, op, rows=rows, **gw)
         if kept is not None:
             kept.extend([x, z, p_all])
         return [(hs, agg.input_dim, agg.vars["self_weights"]), (p, agg.hidden_dim, agg.vars["neigh_weights"])]
@@ -219,7 +245,11 @@ class _FullLayer(object):
         (Wm, _), (x, z, p_all), dp = params, kept, dxs[1]
         if x is None:                                # the MLP read V_0's rows by id: gather them for dWm
             x = ops.gather_rows_f32(self.table, self.src_ids)
-        if self.agg.pool == "max":
+        if self.agg.pool == "max" and g.weights is not None:
+            t_indptr, t_indices = g.transpose(False, slots=True)[:2]
+            dzp = ops.csr_max_backward(z, p_all, dp, g.indptr, g.indices, t_indptr, t_indices, weights=g.weights,
+                                       t_weights=g.t_weights(False))
+        elif self.agg.pool == "max":
             t_indptr, t_indices = self.graph.transpose(False)
             dzp = ops.csr_max_backward(z, p_all, dp, self.graph.indptr, self.graph.indices, t_indptr, t_indices)
         else:
@@ -291,12 +321,40 @@ def refuse_full_neighbor(model, training, dropout=None, tables=True):
     refuse_capture("a full-neighbourhood training step")
 
 
-def full_neighbor_graph(model, indptr, indices):
-    """The model's cached FullNeighborGraph for this CSR (rebuilt when the CSR tensors change)."""
+def full_neighbor_graph(model, indptr, indices, weights=None):
+    """The model's cached FullNeighborGraph for this CSR and edge weights (rebuilt when the tensors change)."""
     g = getattr(model, "_full_neighbor_graph", None)
-    if g is None or g.key != FullNeighborGraph.key_of(indptr, indices):
-        g = model._full_neighbor_graph = FullNeighborGraph(indptr, indices)
+    if g is None or g.key != FullNeighborGraph.key_of(indptr, indices, weights):
+        g = model._full_neighbor_graph = FullNeighborGraph(indptr, indices, weights=weights)
     return g
+
+
+def refuse_weighted_dropout(edge_weight, dropout):
+    """edge_weight together with training dropout p > 0 is not implemented."""
+    if edge_weight is not None and dropout:
+        raise NotImplementedError("edge_weight with training dropout > 0 is not implemented (pass dropout=None or 0, "
+                                  "or no edge_weight)")
+
+
+def edge_weights(model, edge_weight, indices):
+    """edge_weight as a 1-D fp32 tensor on the model's device, one weight per entry of indices: numpy arrays are
+    uploaded, tensors must already be there (TypeError: not float32; ValueError: wrong length or device).  No check of
+    the values: that would synchronise with the host."""
+    if edge_weight is None:
+        return None
+    if not torch.is_tensor(edge_weight):
+        arr = np.asarray(edge_weight)
+        if arr.dtype != np.float32:
+            raise TypeError("edge_weight must be float32 (got %s)" % arr.dtype)
+        edge_weight = torch.as_tensor(arr, device=model.device)
+    if edge_weight.dtype != torch.float32:
+        raise TypeError("edge_weight must be float32 (got %s)" % edge_weight.dtype)
+    if edge_weight.device != indices.device:
+        raise ValueError("edge_weight must be on the model's device %s (got %s)" % (indices.device, edge_weight.device))
+    if edge_weight.dim() != 1 or edge_weight.numel() != indices.numel():
+        raise ValueError("edge_weight needs one weight per CSR entry: shape (%d,), got %s"
+                         % (indices.numel(), tuple(edge_weight.shape)))
+    return edge_weight.contiguous()
 
 
 def _inputs(model, indptr, indices, node_ids):
@@ -315,18 +373,19 @@ def _inputs(model, indptr, indices, node_ids):
     return indptr, indices, ids
 
 
-def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x0_dtype=None):
+def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x0_dtype=None, weights=None):
     """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped); draw =
     (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead, and with
     dropout = p > 0 each block's position map also carries its entries' raw-row offsets.  x0_dtype (sampled): layer 0
-    runs in block-local space over X0, V_0's fp32 rows of a table of that dtype (sampled_layer0_rows)."""
+    runs in block-local space over X0, V_0's fp32 rows of a table of that dtype (sampled_layer0_rows).  weights: the
+    global edge weights; each block then carries those of the raw entries it copies (ops.csr_block_weights)."""
     L = len(aggregators)
     offsets = [None] * L
     if draw is None:
         blocks = ops.csr_blocks(indptr, indices, ids, L)
     else:
         fanouts, seed, call = draw
-        if dropout:
+        if dropout or weights is not None:
             blocks, offsets = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call,
                                              entry_offsets=True)
         else:
@@ -334,7 +393,8 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x
     layers = []
     for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
         pos_map = (indptr, b.src_ids, indices.numel()) + ((offsets[layer],) if offsets[layer] is not None else ())
-        graph = FullNeighborGraph(b.indptr, b.indices, pos_map=pos_map)
+        bw = None if weights is None else ops.csr_block_weights(weights, indptr, b, offsets[layer])
+        graph = FullNeighborGraph(b.indptr, b.indices, pos_map=pos_map, weights=bw)
         if layer == 0:
             v1 = blocks[1].src_ids if L > 1 else ids
             if draw is not None and x0_dtype is not None:
@@ -342,7 +402,8 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x
             elif draw is not None:
                 layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, self_ids=v1))
             else:
-                layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids, table_csr=(indptr, indices, v1)))
+                layers.append(_FullLayer(agg, graph, b.rows, src_ids=b.src_ids,
+                                         table_csr=(indptr, indices, v1, weights)))
         else:
             layers.append(_FullLayer(agg, graph, b.rows))
     return layers
@@ -387,40 +448,44 @@ def sampled_draw(model):
     return fanouts, int(sampler.seed), call
 
 
-def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False):
+def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False, edge_weight=None):
     """(the checked layers of one call, layer 0's source): over the receptive-field blocks of node_ids (minibatch; reads
     the block sizes back once; sampled: over sampled blocks), else over the whole CSR - the model's cached
     FullNeighborGraph when training, an uncached one otherwise (inference builds no transposes, and must not evict the
     ones a training CSR has cached).  The source is the model's table, or X0 for sampled blocks over a host or int8
-    table."""
+    table.  edge_weight: None, or one fp32 weight per CSR entry (edge_weights)."""
     if sampled:
         refuse_sampled(model, training, dropout)
     else:
         refuse_full_neighbor(model, training, dropout)
+    refuse_weighted_dropout(edge_weight, dropout)
     if minibatch:
         refuse_capture("a full-neighbourhood minibatch (it reads the block sizes back)")
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
+    w = edge_weights(model, edge_weight, indices)
     if model.aggregators is None:
         model.aggregators = build_aggregators(model)
     h = model.features
     if sampled:
         x0 = reads_v0_rows(h)
         layers = minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model), dropout=dropout,
-                                  x0_dtype=h.dtype if x0 else None)
+                                  x0_dtype=h.dtype if x0 else None, weights=w)
         # |V_0| is known from the block build's size read: X0 is sized without another
         return layers, (sampled_layer0_rows(h, layers[0].graph.pos_map[1]) if x0 else h)
     if minibatch:
-        return minibatch_layers(model.aggregators, indptr, indices, ids), h
-    graph = full_neighbor_graph(model, indptr, indices) if training else FullNeighborGraph(indptr, indices)
+        return minibatch_layers(model.aggregators, indptr, indices, ids, weights=w), h
+    graph = (full_neighbor_graph(model, indptr, indices, w) if training else
+             FullNeighborGraph(indptr, indices, weights=w))
     L = len(model.aggregators)
     return [_FullLayer(agg, graph, ids if layer == L - 1 else None) for layer, agg in enumerate(model.aggregators)], h
 
 
-def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False, sampled=False):
+def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False, sampled=False,
+                             edge_weight=None):
     """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings; sampled:
     sampled_minibatch_embeddings), without autograd."""
     with torch.no_grad():
-        layers, h = _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled)
+        layers, h = _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled, edge_weight=edge_weight)
         for fl in layers:
             h = fl.agg._finish(fl.forward(h, None), fl.agg._combine())
         if normalize:
@@ -429,12 +494,14 @@ def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=Tr
 
 
 def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False, dropout=None,
-                          sampled=False):
+                          sampled=False, edge_weight=None):
     """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch, sampled) with an autograd graph over the
     aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
-    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them."""
+    sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them.  edge_weight: the
+    CSR's per-entry weights (oracle/weighted.py)."""
     p = check_full_neighbor_dropout(dropout)
-    layers, h = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled)
+    layers, h = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled,
+                        edge_weight=edge_weight)
     if p:
         pool = isinstance(layers[0].agg, MaxPoolingAggregator)
         plan = full_neighbor_site_plan("maxpool" if pool else "mean", len(layers))

@@ -254,28 +254,31 @@ class SampleAndAggregate(object):
                 fp.write("\n".join(str(int(x)) for x in ids.tolist()))
         return emb
 
-    def full_neighbor_embeddings(self, indptr, indices, node_ids=None, normalize=True):
+    def full_neighbor_embeddings(self, indptr, indices, node_ids=None, normalize=True, edge_weight=None):
         """Deterministic embeddings over WHOLE neighbourhoods, layer by layer (contract: oracle/full_neighbor.py): layer l
         computes every node's row of h^{l+1} once - the last layer only the rows of `node_ids` (default: all N nodes) -
         from its CSR row (indptr int64 [N+1], indices int32; an empty row uses the dummy node N, as the padded table does).
         The neighbour reductions are gs_csr_aggregate, the combine the aggregator's own GEMM (_finish); the pooling
         aggregators run their MLP once per node.  No sampling and no dropout: two calls give the same bits.  Returns fp32
         [len(node_ids), out_w], l2-normalised like forward().  Peak memory: two fp32 [N+1, width] layer buffers, plus the
-        pools' [N+1, hidden] MLP output."""
+        pools' [N+1, hidden] MLP output.  edge_weight: None, or the CSR's edge weights - fp32, one per entry of indices
+        (numpy, or a tensor on the model's device) - each message scaled by its edge's weight before the reduction, the
+        divisors unchanged (gs_csr_aggregate_weighted; contract: oracle/weighted.py)."""
         from .full_neighbor_training import full_neighbor_embeddings
-        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize)
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, edge_weight=edge_weight)
 
-    def full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True):
+    def full_neighbor_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True, edge_weight=None):
         """full_neighbor_embeddings(indptr, indices, node_ids, normalize) - torch.equal to it - computed over the
         receptive field of node_ids only (contract: oracle/full_neighbor_blocks.py): ops.csr_blocks builds, on the
         device, one block per layer holding the nodes that layer must compute, and each layer runs over its block.  Cost
         and memory follow the blocks, not the graph: use it when node_ids' receptive field is a small part of the graph
         (serving, evaluating a split in batches).  Reads the block sizes back once per call (a synchronisation), so it
-        cannot be captured in a CUDA graph.  Same refusals as full_neighbor_embeddings."""
+        cannot be captured in a CUDA graph.  Same refusals and edge_weight as full_neighbor_embeddings: each block entry
+        carries its raw CSR entry's weight."""
         from .full_neighbor_training import full_neighbor_embeddings
-        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True)
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, edge_weight=edge_weight)
 
-    def sampled_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True):
+    def sampled_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True, edge_weight=None):
         """Embeddings of node_ids over SAMPLED receptive-field blocks (contract: oracle/sampled_blocks.py): block l keeps
         at most layer_infos[l].num_samples entries of each row of the full CSR, drawn without replacement (Floyd's
         algorithm, Philox keyed by layer_infos[0].neigh_sampler's seed at its counter, which advances by 1), and every
@@ -284,9 +287,11 @@ class SampleAndAggregate(object):
         full_neighbor_minibatch_embeddings, bit for bit.  Reads the block sizes back once per call, so it cannot be
         captured in a CUDA graph.  Same refusals as full_neighbor_embeddings, except that a host-memory (HostFeatures) or
         int8 (Int8Features) table is taken: layer 0 then reads only V_0's rows, as fp32, and gives the bits of the device
-        table (fp32 / bf16 twin, or the int8 table and its dequantize())."""
+        table (fp32 / bf16 twin, or the int8 table and its dequantize()).  edge_weight: as full_neighbor_embeddings, each
+        sampled entry carrying its raw CSR entry's weight (the draws stay uniform)."""
         from .full_neighbor_training import full_neighbor_embeddings
-        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, sampled=True)
+        return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, sampled=True,
+                                        edge_weight=edge_weight)
 
     def _csr_input(self, t, dtype, name):
         """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""

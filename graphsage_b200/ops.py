@@ -579,7 +579,18 @@ def segment_max(x, n, k):
 CSR_OPS = {"mean": _lib.CSR_MEAN, "mean_self": _lib.CSR_MEAN_SELF, "max": _lib.CSR_MAX, "sum": _lib.CSR_SUM}
 
 
-def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t_slot=None):
+def _csr_weights(weights, entries, name="weights"):
+    """weights as a 1-D fp32 CUDA tensor of `entries` values (one per CSR entry), a 1-element stand-in when there are
+    none."""
+    if not isinstance(weights, torch.Tensor) or weights.dtype != torch.float32 or weights.dim() != 1:
+        raise TypeError("%s must be a 1-D float32 tensor" % name)
+    require_cuda(weights)
+    if weights.numel() != entries:
+        raise ValueError("%s needs one weight per CSR entry: %d, got %d" % (name, entries, weights.numel()))
+    return weights.contiguous() if entries else torch.ones((1,), dtype=torch.float32, device=weights.device)
+
+
+def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t_slot=None, weights=None):
     """The reduction of each node's whole CSR row (gs_csr_aggregate; contract in oracle/full_neighbor.py): output row i is
     for node v = rows[i] - or, without rows, for every node 0 .. N-1 and then the dummy node N (N = len(indptr) - 1: the
     [N+1, .] layout of the tables it reads) - over the source rows indices[indptr[v] .. indptr[v+1]) in CSR order - op "mean", "mean_self"
@@ -595,7 +606,10 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
     element, pos_off: a sampled block's per-entry offsets (csr_blocks(..., entry_offsets=True); int32, one per entry of
     `indices`) - entry j of node v's row is then masked at pos_indptr[g(v)] + pos_off[indptr[v] + j]
     (gs_csr_aggregate_dropout_offsets; contract in oracle/sampled_blocks_dropout.py), ops "mean" and "mean_self" only; the
-    backward "sum" takes csr_slots_to_offsets' t_slot and a three-element map instead."""
+    backward "sum" takes csr_slots_to_offsets' t_slot and a three-element map instead.
+    weights: None, or fp32 [len(indices)], one weight per entry (gs_csr_aggregate_weighted; contract in
+    oracle/weighted.py), every op: entry j adds fl(w_j * x_j); an empty row's dummy entry weighs 1; the divisors stay the
+    counts.  "sum" reads weights aligned with its own (transposed) indices - csr_transpose_weights'.  Not with dropout."""
     require_cuda(src, indptr, indices, rows, out)
     if src.dtype not in (torch.float32, torch.bfloat16) or src.dim() != 2 or src.stride(1) != 1:
         raise ValueError("src must be a row-major float32 (or bfloat16) 2-D tensor")
@@ -612,6 +626,10 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
                          "the layout of csr_transpose" % (src.shape[0] + 1, src.shape[0], indptr.numel()))
     indptr, indices = indptr.contiguous(), _i32(indices.reshape(-1), "indices")
     entries = indices.numel()
+    if weights is not None:
+        if dropout is not None:
+            raise ValueError("csr_aggregate takes weights or dropout, not both")
+        weights = _csr_weights(weights, entries)
     if entries == 0:
         indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
     n_nodes = indptr.numel() - 1
@@ -649,6 +667,13 @@ def csr_aggregate(src, indptr, indices, op, rows=None, out=None, dropout=None, t
                                              CSR_OPS[op], dropout_site(neigh), dropout_site(self_site),
                                              ptr(pos_indptr.contiguous()), ptr(pos_ids), int(pos_nnz), ptr(out),
                                              out.stride(0), stream_ptr()))
+        _launched(1 if n else 0, ev)
+        return out[:n, :F]
+    if weights is not None:
+        ev = _probe("csr_aggregate_weighted/%d" % n)
+        check(lib().gs_csr_aggregate_weighted(ptr(src), _dtype_code(src), src.shape[0], F, src.stride(0), ptr(indptr),
+                                              ptr(indices), ptr(weights), n_nodes, ptr(rows), n, CSR_OPS[op], ptr(out),
+                                              out.stride(0), stream_ptr()))
         _launched(1 if n else 0, ev)
         return out[:n, :F]
     ev = _probe("csr_aggregate/%d" % n)
@@ -695,6 +720,37 @@ def csr_slots_to_offsets(t_slot, t_indices, indptr, pos_off):
     return torch.where(s >= 0, pos_off.index_select(0, at), s).to(torch.int32)
 
 
+def csr_transpose_weights(weights, indptr, t_indices, t_slot):
+    """The forward weights of csr_transpose(indptr, indices, slots=True)'s entries, aligned with t_indices:
+    weights[indptr[i] + t_slot] for i = t_indices[.] where t_slot >= 0, 1 for the implicit {N} entry (-1) and the
+    with_self entry (-2) - what csr_aggregate(op="sum", weights=...) and csr_max_backward(t_weights=...) read.  Two
+    gathers; the entries past the transpose's count are clamped into range and stay unspecified.  fp32 [len(t_slot)]."""
+    require_cuda(weights, indptr, t_indices, t_slot)
+    one = torch.ones((), dtype=torch.float32, device=t_slot.device)
+    if weights.numel() == 0:                         # no forward entry: every slot is -1 or -2
+        return one.expand(t_slot.numel()).contiguous()
+    s = t_slot.long()
+    i = t_indices.long().clamp(0, indptr.numel() - 1)
+    at = (indptr.index_select(0, i) + s).clamp(0, weights.numel() - 1)
+    return torch.where(s >= 0, weights.index_select(0, at), one)
+
+
+def csr_block_weights(weights, indptr, block, offsets=None):
+    """The per-entry weights of a block of csr_blocks(indptr, indices, ...), aligned with block.indices: the weight of the
+    raw-CSR entry each block entry copies - weights[indptr[src_ids[u]] + j] for entry j of local row u, or, with offsets
+    (a sampled block's csr_blocks(..., entry_offsets=True)), weights[indptr[src_ids[u]] + offsets[e]].  Gathers only, no
+    host synchronisation.  fp32 [len(block.indices)]."""
+    require_cuda(weights, indptr)
+    E = block.indices.numel()
+    if E == 0:
+        return torch.zeros((0,), dtype=torch.float32, device=weights.device)
+    e = torch.arange(E, dtype=torch.int64, device=weights.device)
+    u = torch.searchsorted(block.indptr, e, right=True) - 1          # the local row of each entry
+    off = e - block.indptr.index_select(0, u) if offsets is None else offsets.long()
+    g = block.src_ids.long().index_select(0, u)
+    return weights.index_select(0, indptr.index_select(0, g) + off)
+
+
 def _csr_args(indptr, indices):
     require_cuda(indptr, indices)
     if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
@@ -727,12 +783,17 @@ def csr_transpose(indptr, indices, with_self=False, slots=False):
     return (t_indptr, t_indices, t_slot) if slots else (t_indptr, t_indices)
 
 
-def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out=None):
+def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out=None, weights=None, t_weights=None):
     """The gradient of m = csr_aggregate(z, indptr, indices, "max") over all N + 1 rows, through the ReLU that made z
     (gs_csr_max_backward; oracle/full_neighbor_grad.py): s = dm / tie count per (row, column), then per node j the sum, in
     transposed order, of s[i] over the rows i that read j where z[j] attains m[i]; +0 where z[j] <= 0.  z, m, dm: fp32
     [N + 1, F] CUDA matrices with unit column stride; (t_indptr, t_indices) = csr_transpose(indptr, indices).  s: optional
-    [N + 1, >= F] scratch (the scale of phase (a), kept for inspection).  Returns fp32 [N + 1, F]."""
+    [N + 1, >= F] scratch (the scale of phase (a), kept for inspection).  Returns fp32 [N + 1, F].
+    weights, t_weights: both None, or the gradient of m = csr_aggregate(z, ..., "max", weights=weights)
+    (gs_csr_max_backward_weighted; oracle/weighted.py): ties counted on fl(w * z), routed as fl(w * s); t_weights =
+    csr_transpose_weights(weights, indptr, t_indices, t_slot), aligned with t_indices."""
+    if (weights is None) != (t_weights is None):
+        raise ValueError("csr_max_backward takes both weights and t_weights, or neither")
     indptr, indices = _csr_args(indptr, indices)
     t_indptr, t_indices = _csr_args(t_indptr, t_indices)
     rows = indptr.numel()
@@ -753,8 +814,19 @@ def csr_max_backward(z, m, dm, indptr, indices, t_indptr, t_indices, s=None, out
         _fp32_table(t, name, F)
         if t.shape[0] != rows:
             raise ValueError("%s must have N + 1 = %d rows" % (name, rows))
+    if weights is not None:
+        weights = _csr_weights(weights, indices.numel())
+        t_weights = _csr_weights(t_weights, t_indices.numel(), "t_weights")
     if indices.numel() == 0:
         indices = torch.zeros((1,), dtype=torch.int32, device=indptr.device)
+    if weights is not None:
+        ev = _probe("csr_max_backward_weighted/%d" % rows)
+        check(lib().gs_csr_max_backward_weighted(ptr(z), z.stride(0), ptr(m), m.stride(0), ptr(dm), dm.stride(0), F,
+                                                 ptr(indptr), ptr(indices), ptr(weights), ptr(t_indptr), ptr(t_indices),
+                                                 ptr(t_weights), rows - 1, ptr(s), s.stride(0), ptr(out), out.stride(0),
+                                                 stream_ptr()))
+        _launched(2, ev)
+        return out[:, :F]
     ev = _probe("csr_max_backward/%d" % rows)
     check(lib().gs_csr_max_backward(ptr(z), z.stride(0), ptr(m), m.stride(0), ptr(dm), dm.stride(0), F, ptr(indptr),
                                     ptr(indices), ptr(t_indptr), ptr(t_indices), rows - 1, ptr(s), s.stride(0), ptr(out),

@@ -671,7 +671,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         with torch.no_grad():
             return self._predictions(self.logits(batch))
 
-    def full_neighbor_outputs(self, indptr, indices, node_ids, dropout=None):
+    def full_neighbor_outputs(self, indptr, indices, node_ids, dropout=None, edge_weight=None):
         """outputs() over whole neighbourhoods: full_neighbor_embeddings(indptr, indices, node_ids) - the same bits -
         with an autograd graph over the aggregator weights and (identity_dim > 0) the node embeddings, for any head to
         compose (contract: oracle/full_neighbor_grad.py).  The CSR's transposes are built on first use and cached on the
@@ -680,9 +680,10 @@ class SupervisedGraphsage(SampleAndAggregate):
         (one per CSR entry and per node, keyed by global ids: oracle/full_neighbor_dropout.py), not the sampled one, so
         they are applied only when asked for; p = 0 gives the bits of dropout=None.  Refused (NotImplementedError): the
         seq aggregator, ShardedFeatures, distributed=True, CUDA-graph capture, and dropout=None on a model whose
-        dropout_rate > 0."""
+        dropout_rate > 0.  edge_weight: as full_neighbor_embeddings (weighted messages, oracle/weighted.py); the
+        transposes' weights are cached with the transposes, keyed by the weight tensor too.  Refused with dropout p > 0."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids, dropout=dropout)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight)
 
     def _full_neighbor_logits(self, out, dropout):
         """The head on full-neighbourhood outputs; with p > 0 its input is dropped at the site after the layers'."""
@@ -692,40 +693,44 @@ class SupervisedGraphsage(SampleAndAggregate):
             self.dropout_counter += 1
         return self._node_pred(out)
 
-    def full_neighbor_loss(self, indptr, indices, node_ids, labels, dropout=None):
+    def full_neighbor_loss(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """loss() on full_neighbor_outputs: the same head, cross-entropy and weight decay, over the rows of node_ids.
         dropout: as full_neighbor_outputs; p > 0 also drops the head input (row r of node_ids at position r)."""
         check_full_neighbor_dropout(dropout)
-        out = self.full_neighbor_outputs(indptr, indices, node_ids, dropout=dropout)
+        out = self.full_neighbor_outputs(indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight)
         return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def full_neighbor_train_step(self, indptr, indices, node_ids, labels, dropout=None):
+    def full_neighbor_train_step(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """One deterministic full-batch Adam step: every node of node_ids over its whole neighbourhood (no sampling;
         dropout as full_neighbor_loss), gradients clipped to +-5 as in train_step.  Returns the detached loss; no host
         synchronisation."""
-        return clipped_step(self, self.full_neighbor_loss(indptr, indices, node_ids, labels, dropout=dropout))
+        return clipped_step(self, self.full_neighbor_loss(indptr, indices, node_ids, labels, dropout=dropout,
+                                                          edge_weight=edge_weight))
 
-    def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids, dropout=None):
+    def full_neighbor_minibatch_outputs(self, indptr, indices, node_ids, dropout=None, edge_weight=None):
         """full_neighbor_outputs over the receptive field of node_ids only: the same values, bit for bit, with per-layer
         blocks built on the device by ops.csr_blocks (contract: oracle/full_neighbor_blocks.py) and their transposes built
         per call, not cached.  Cost and memory follow the blocks, not the graph: the minibatch form of exact-neighbourhood
         training.  Reads the block sizes back once per call.  dropout and refusals as full_neighbor_outputs: the masks are
-        keyed by global ids, so the rows equal the whole-graph pass's from the same counter."""
+        keyed by global ids, so the rows equal the whole-graph pass's from the same counter.  edge_weight: as
+        full_neighbor_outputs, each block entry carrying its raw CSR entry's weight (built per call)."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, dropout=dropout)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, dropout=dropout,
+                                     edge_weight=edge_weight)
 
-    def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None):
+    def full_neighbor_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """full_neighbor_loss over full_neighbor_minibatch_outputs: the same head, cross-entropy and weight decay."""
         check_full_neighbor_dropout(dropout)
-        out = self.full_neighbor_minibatch_outputs(indptr, indices, node_ids, dropout=dropout)
+        out = self.full_neighbor_minibatch_outputs(indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight)
         return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None):
+    def full_neighbor_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """full_neighbor_train_step for a minibatch: one Adam step on full_neighbor_minibatch_loss, gradients clipped to
         +-5.  Returns the detached loss."""
-        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
+        return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout,
+                                                                    edge_weight=edge_weight))
 
-    def sampled_minibatch_outputs(self, indptr, indices, node_ids, dropout=None):
+    def sampled_minibatch_outputs(self, indptr, indices, node_ids, dropout=None, edge_weight=None):
         """outputs() over sampled receptive-field blocks (SampleAndAggregate.sampled_minibatch_embeddings; contract:
         oracle/sampled_blocks.py), with an autograd graph over the aggregator weights and (identity_dim > 0) the node
         embeddings.  One block set per call: the sampler's counter advances by 1.  dropout: None (no masks), or a
@@ -733,27 +738,33 @@ class SupervisedGraphsage(SampleAndAggregate):
         entry masked as the same CSR entry is in the whole-graph pass (contract: oracle/sampled_blocks_dropout.py), sites
         numbered from dropout_counter; p = 0 gives the bits of dropout=None.  Refused (NotImplementedError): what
         full_neighbor_outputs refuses but host-memory and int8 tables (taken here: see sampled_minibatch_embeddings),
-        CUDA-graph capture, dropout=None on a model whose dropout_rate > 0, and dropout = p > 0 on an int8 table."""
+        CUDA-graph capture, dropout=None on a model whose dropout_rate > 0, and dropout = p > 0 on an int8 table.
+        edge_weight: as full_neighbor_outputs, each sampled entry carrying its raw CSR entry's weight; refused with
+        dropout p > 0."""
         from .full_neighbor_training import full_neighbor_outputs
-        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True, dropout=dropout)
+        return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True, dropout=dropout,
+                                     edge_weight=edge_weight)
 
-    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None):
+    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """loss() over sampled_minibatch_outputs: the same head, cross-entropy and weight decay.  dropout: as
         sampled_minibatch_outputs; p > 0 also drops the head input (row r of node_ids at position r)."""
         check_full_neighbor_dropout(dropout)
-        out = self.sampled_minibatch_outputs(indptr, indices, node_ids, dropout=dropout)
+        out = self.sampled_minibatch_outputs(indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight)
         return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None):
+    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
         """One Adam step on sampled_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the detached
         loss."""
-        return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout))
+        return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout,
+                                                              edge_weight=edge_weight))
 
-    def full_neighbor_predict(self, indptr, indices, node_ids):
+    def full_neighbor_predict(self, indptr, indices, node_ids, edge_weight=None):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on
-        full_neighbor_embeddings(indptr, indices, node_ids) - deterministic, no sampling, no dropout."""
+        full_neighbor_embeddings(indptr, indices, node_ids, edge_weight=edge_weight) - deterministic, no sampling, no
+        dropout."""
         with torch.no_grad():
-            return self._predictions(self._node_pred(self.full_neighbor_embeddings(indptr, indices, node_ids)))
+            return self._predictions(self._node_pred(self.full_neighbor_embeddings(indptr, indices, node_ids,
+                                                                                   edge_weight=edge_weight)))
 
     def last_predictions(self):
         """model.preds of the last loss() / train_step() call (supervised_models.py:120-126): the predictions from that

@@ -823,6 +823,20 @@ int32_t gs_csr_aggregate_dropout_offsets(const void* src, int32_t dtype, int64_t
                                          const int32_t* pos_ids /* may be NULL */, int64_t pos_nnz,
                                          const int32_t* pos_off, float* out, int64_t out_pitch, void* stream);
 
+/* gs_csr_aggregate over weighted edges (contract: oracle/weighted.py), every op: weight is fp32, one value per entry of
+ * `indices` (data, no gradient; any finite value).  Entry j's term is fl(weight[indptr[v] + j] * x_j) - the product rounded
+ * to fp32 before it joins the chain, never contracted into it - and the chain, its order and its divisor (count, not the
+ * weights' sum) are gs_csr_aggregate's: mean (Σ fl(w x)) / count, GCN the same sum plus the node's own row (weight 1)
+ * over count + 1, max max fl(w x).  The implicit dummy entry of an empty row, or of a v outside [0, n_nodes), weighs 1, so
+ * all-one weights give gs_csr_aggregate's bits.  GS_CSR_SUM (fp32) reads weights aligned with its own (transposed)
+ * indices: the backward of the weighted means is the sum of fl(w * g / count) over the transposed rows, each transposed
+ * entry carrying its forward entry's weight (1 for slots -1 and -2).  No allocation, no atomics, no host
+ * synchronisation. */
+int32_t gs_csr_aggregate_weighted(const void* src, int32_t dtype, int64_t n_src_rows, int32_t F, int64_t pitch,
+                                  const int64_t* indptr, const int32_t* indices, const float* weight, int64_t n_nodes,
+                                  const int32_t* rows /* may be NULL */, int64_t n, int32_t op, float* out,
+                                  int64_t out_pitch, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Backward of the full-neighbourhood reductions (SupervisedGraphsage.full_neighbor_train_step).  Contract:
  * oracle/full_neighbor_grad.py.  Nodes 0 .. N-1 have CSR rows; the dummy node N closes every [N+1, .] table.
@@ -864,6 +878,17 @@ int32_t gs_csr_max_backward(const float* z, int64_t ldz, const float* m, int64_t
                             int32_t F, const int64_t* indptr, const int32_t* indices, const int64_t* t_indptr,
                             const int32_t* t_indices, int64_t n_nodes, float* s, int64_t lds, float* dz, int64_t lddz,
                             void* stream);
+/* gs_csr_max_backward of m = GS_CSR_MAX over weighted edges (gs_csr_aggregate_weighted; oracle/weighted.py): weight is
+ * aligned with `indices` (the forward's; the dummy entry of an empty row and the dummy row weigh 1), t_weight with
+ * t_indices (t_weight[k] = weight[indptr[t_indices[k]] + t_slot[k]] for t_slot >= 0, else 1).
+ *   (a) cnt = #{entries e of row i : fl(w_e * z[e][c]) == m[i][c]}, s[i][c] = dm[i][c] / (float)cnt;
+ *   (b) acc = +0; for i in transposed row j, in order, with that entry's weight w: if fl(w * z[j][c]) == m[i][c],
+ *       acc += fl(w * s[i][c]); dz[j][c] = z[j][c] > 0 ? acc : +0. */
+int32_t gs_csr_max_backward_weighted(const float* z, int64_t ldz, const float* m, int64_t ldm, const float* dm,
+                                     int64_t lddm, int32_t F, const int64_t* indptr, const int32_t* indices,
+                                     const float* weight, const int64_t* t_indptr, const int32_t* t_indices,
+                                     const float* t_weight, int64_t n_nodes, float* s, int64_t lds, float* dz,
+                                     int64_t lddz, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Receptive-field blocks of a minibatch over whole neighbourhoods (full_neighbor_minibatch_*).  Contract:
