@@ -197,6 +197,17 @@ _SIGNATURES = {
                                                    ctypes.POINTER(c_vp), c_vp]),
     "gs_csr_sample_rows_workspace_bytes": (c_i64, [c_i64, c_i64]),
     "gs_csr_sample_rows": (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_u64, c_u64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "gs_csr_weighted_blocks_plan": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64,
+                                            c_u64, c_vp, c_i64, c_vp, c_vp]),
+    "gs_csr_weighted_blocks_fill": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32, ctypes.POINTER(c_i32), c_u64,
+                                            c_u64, c_vp, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_vp),
+                                            ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), c_vp]),
+    "gs_csr_weighted_blocks_fill_offsets": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i32,
+                                                    ctypes.POINTER(c_i32), c_u64, c_u64, c_vp, c_i64, ctypes.POINTER(c_i64),
+                                                    ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), ctypes.POINTER(c_vp),
+                                                    ctypes.POINTER(c_vp), ctypes.POINTER(c_vp), c_vp]),
+    "gs_csr_sample_rows_weighted": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, c_u64, c_u64, c_i32, c_vp, c_i64, c_vp,
+                                            c_vp, c_vp]),
 }
 
 _lib = None

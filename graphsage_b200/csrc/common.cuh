@@ -144,6 +144,8 @@ constexpr uint32_t kStreamUnigramUnique = 0x30000000u;
 constexpr uint32_t kStreamWalk = 0x50000000u;
 constexpr uint32_t kStreamWalkBiased = 0x60000000u;  // 2^28 words: ((w * 32 + move) << 3) + call
 constexpr uint32_t kStreamSampledBlocks = 0x70000000u;  // GS_MAX_BLOCK_LAYERS words: | layer (counter (i, v, call, .))
+// weighted blocks: [0x80000000, 0x80000008), | layer (counter (j >> 1, v, call, .)); past every range above
+constexpr uint32_t kStreamWeightedBlocks = 0x80000000u;
 
 // ---- PTX wrappers (mbarrier / bulk copy) ---------------------------------------------------
 #ifdef __CUDACC__

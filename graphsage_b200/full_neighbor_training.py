@@ -49,6 +49,11 @@ the FullNeighborGraph beside the transposes), and the max-pool backward splits t
 (ops.csr_max_backward with weights).  A block's entries carry the weights of the raw entries they copy
 (ops.csr_block_weights, built per call); layer 0 of a whole-neighbourhood minibatch reads the global CSR, so it takes w.
 Not with training dropout p > 0.
+
+Weighted draws (sample_weight=w, fp32, one per CSR entry; contract: oracle/weighted_sampling.py) change only how the
+sampled blocks choose their entries: ops.csr_blocks(..., sample_weights=w) keeps at most k_l of each row's entries with
+w > 0, drawn in proportion to w.  The blocks have the uniform blocks' layout and offsets, so every layer, mask, edge
+weight and table above runs on them unchanged.
 """
 import numpy as np
 import torch
@@ -336,24 +341,24 @@ def refuse_weighted_dropout(edge_weight, dropout):
                                   "or no edge_weight)")
 
 
-def edge_weights(model, edge_weight, indices):
+def edge_weights(model, edge_weight, indices, name="edge_weight"):
     """edge_weight as a 1-D fp32 tensor on the model's device, one weight per entry of indices: numpy arrays are
     uploaded, tensors must already be there (TypeError: not float32; ValueError: wrong length or device).  No check of
-    the values: that would synchronise with the host."""
+    the values: that would synchronise with the host.  name: the keyword the errors name (sample_weight too)."""
     if edge_weight is None:
         return None
     if not torch.is_tensor(edge_weight):
         arr = np.asarray(edge_weight)
         if arr.dtype != np.float32:
-            raise TypeError("edge_weight must be float32 (got %s)" % arr.dtype)
+            raise TypeError("%s must be float32 (got %s)" % (name, arr.dtype))
         edge_weight = torch.as_tensor(arr, device=model.device)
     if edge_weight.dtype != torch.float32:
-        raise TypeError("edge_weight must be float32 (got %s)" % edge_weight.dtype)
+        raise TypeError("%s must be float32 (got %s)" % (name, edge_weight.dtype))
     if edge_weight.device != indices.device:
-        raise ValueError("edge_weight must be on the model's device %s (got %s)" % (indices.device, edge_weight.device))
+        raise ValueError("%s must be on the model's device %s (got %s)" % (name, indices.device, edge_weight.device))
     if edge_weight.dim() != 1 or edge_weight.numel() != indices.numel():
-        raise ValueError("edge_weight needs one weight per CSR entry: shape (%d,), got %s"
-                         % (indices.numel(), tuple(edge_weight.shape)))
+        raise ValueError("%s needs one weight per CSR entry: shape (%d,), got %s"
+                         % (name, indices.numel(), tuple(edge_weight.shape)))
     return edge_weight.contiguous()
 
 
@@ -375,7 +380,8 @@ def _inputs(model, indptr, indices, node_ids):
 
 def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x0_dtype=None, weights=None):
     """One _FullLayer per aggregator over the blocks of ops.csr_blocks(indptr, indices, ids, L) (ids clamped); draw =
-    (fanouts, seed, call): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call) instead, and with
+    (fanouts, seed, call[, sample weights]): over the sampled blocks of ops.csr_blocks(..., fanouts, seed, call,
+    sample_weights=) instead (a None or absent fourth element: uniform draws), and with
     dropout = p > 0 each block's position map also carries its entries' raw-row offsets.  x0_dtype (sampled): layer 0
     runs in block-local space over X0, V_0's fp32 rows of a table of that dtype (sampled_layer0_rows).  weights: the
     global edge weights; each block then carries those of the raw entries it copies (ops.csr_block_weights)."""
@@ -384,12 +390,13 @@ def minibatch_layers(aggregators, indptr, indices, ids, draw=None, dropout=0., x
     if draw is None:
         blocks = ops.csr_blocks(indptr, indices, ids, L)
     else:
-        fanouts, seed, call = draw
+        fanouts, seed, call = draw[:3]
+        sw = {} if len(draw) < 4 or draw[3] is None else {"sample_weights": draw[3]}
         if dropout or weights is not None:
             blocks, offsets = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call,
-                                             entry_offsets=True)
+                                             entry_offsets=True, **sw)
         else:
-            blocks = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call)
+            blocks = ops.csr_blocks(indptr, indices, ids, L, fanouts=fanouts, seed=seed, call=call, **sw)
     layers = []
     for layer, (agg, b) in enumerate(zip(aggregators, blocks)):
         pos_map = (indptr, b.src_ids, indices.numel()) + ((offsets[layer],) if offsets[layer] is not None else ())
@@ -448,12 +455,14 @@ def sampled_draw(model):
     return fanouts, int(sampler.seed), call
 
 
-def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False, edge_weight=None):
+def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None, sampled=False, edge_weight=None,
+            sample_weight=None):
     """(the checked layers of one call, layer 0's source): over the receptive-field blocks of node_ids (minibatch; reads
     the block sizes back once; sampled: over sampled blocks), else over the whole CSR - the model's cached
     FullNeighborGraph when training, an uncached one otherwise (inference builds no transposes, and must not evict the
     ones a training CSR has cached).  The source is the model's table, or X0 for sampled blocks over a host or int8
-    table.  edge_weight: None, or one fp32 weight per CSR entry (edge_weights)."""
+    table.  edge_weight: None, or one fp32 weight per CSR entry (edge_weights).  sample_weight (sampled only): None, or
+    one fp32 weight per CSR entry that the sampled blocks draw in proportion to."""
     if sampled:
         refuse_sampled(model, training, dropout)
     else:
@@ -463,13 +472,14 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None,
         refuse_capture("a full-neighbourhood minibatch (it reads the block sizes back)")
     indptr, indices, ids = _inputs(model, indptr, indices, node_ids)
     w = edge_weights(model, edge_weight, indices)
+    sw = edge_weights(model, sample_weight, indices, "sample_weight")
     if model.aggregators is None:
         model.aggregators = build_aggregators(model)
     h = model.features
     if sampled:
         x0 = reads_v0_rows(h)
-        layers = minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model), dropout=dropout,
-                                  x0_dtype=h.dtype if x0 else None, weights=w)
+        layers = minibatch_layers(model.aggregators, indptr, indices, ids, draw=sampled_draw(model) + (sw,),
+                                  dropout=dropout, x0_dtype=h.dtype if x0 else None, weights=w)
         # |V_0| is known from the block build's size read: X0 is sized without another
         return layers, (sampled_layer0_rows(h, layers[0].graph.pos_map[1]) if x0 else h)
     if minibatch:
@@ -481,11 +491,12 @@ def _layers(model, indptr, indices, node_ids, training, minibatch, dropout=None,
 
 
 def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=True, minibatch=False, sampled=False,
-                             edge_weight=None):
+                             edge_weight=None, sample_weight=None):
     """SampleAndAggregate.full_neighbor_embeddings (minibatch: full_neighbor_minibatch_embeddings; sampled:
     sampled_minibatch_embeddings), without autograd."""
     with torch.no_grad():
-        layers, h = _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled, edge_weight=edge_weight)
+        layers, h = _layers(model, indptr, indices, node_ids, False, minibatch, sampled=sampled, edge_weight=edge_weight,
+                            sample_weight=sample_weight)
         for fl in layers:
             h = fl.agg._finish(fl.forward(h, None), fl.agg._combine())
         if normalize:
@@ -494,14 +505,15 @@ def full_neighbor_embeddings(model, indptr, indices, node_ids=None, normalize=Tr
 
 
 def full_neighbor_outputs(model, indptr, indices, node_ids, normalize=True, minibatch=False, dropout=None,
-                          sampled=False, edge_weight=None):
+                          sampled=False, edge_weight=None, sample_weight=None):
     """full_neighbor_embeddings(indptr, indices, node_ids, normalize, minibatch, sampled) with an autograd graph over the
     aggregator weights and (identity_dim > 0) model.embeds.  Same values, bit for bit.  dropout = p > 0: the layers'
     sites of full_neighbor_site_plan, numbered from model.dropout_counter, which advances past them.  edge_weight: the
-    CSR's per-entry weights (oracle/weighted.py)."""
+    CSR's per-entry weights (oracle/weighted.py).  sample_weight (sampled): the weights the blocks draw by
+    (oracle/weighted_sampling.py)."""
     p = check_full_neighbor_dropout(dropout)
     layers, h = _layers(model, indptr, indices, node_ids, True, minibatch, dropout=p, sampled=sampled,
-                        edge_weight=edge_weight)
+                        edge_weight=edge_weight, sample_weight=sample_weight)
     if p:
         pool = isinstance(layers[0].agg, MaxPoolingAggregator)
         plan = full_neighbor_site_plan("maxpool" if pool else "mean", len(layers))

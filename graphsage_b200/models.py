@@ -278,7 +278,8 @@ class SampleAndAggregate(object):
         from .full_neighbor_training import full_neighbor_embeddings
         return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, edge_weight=edge_weight)
 
-    def sampled_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True, edge_weight=None):
+    def sampled_minibatch_embeddings(self, indptr, indices, node_ids, normalize=True, edge_weight=None,
+                                     sample_weight=None):
         """Embeddings of node_ids over SAMPLED receptive-field blocks (contract: oracle/sampled_blocks.py): block l keeps
         at most layer_infos[l].num_samples entries of each row of the full CSR, drawn without replacement (Floyd's
         algorithm, Philox keyed by layer_infos[0].neigh_sampler's seed at its counter, which advances by 1), and every
@@ -288,10 +289,14 @@ class SampleAndAggregate(object):
         captured in a CUDA graph.  Same refusals as full_neighbor_embeddings, except that a host-memory (HostFeatures) or
         int8 (Int8Features) table is taken: layer 0 then reads only V_0's rows, as fp32, and gives the bits of the device
         table (fp32 / bf16 twin, or the int8 table and its dequantize()).  edge_weight: as full_neighbor_embeddings, each
-        sampled entry carrying its raw CSR entry's weight (the draws stay uniform)."""
+        sampled entry carrying its raw CSR entry's weight (the draws stay uniform unless sample_weight is given).
+        sample_weight: None (uniform draws), or fp32, one weight per entry of indices (a CUDA tensor on the model's
+        device, or a numpy array, uploaded): block l then keeps at most num_samples of each row's entries with weight
+        > 0, drawn without replacement in proportion to weight (contract: oracle/weighted_sampling.py) - PinSAGE-style
+        importance sampling.  It may be the edge_weight tensor or another one; no gradient flows to it."""
         from .full_neighbor_training import full_neighbor_embeddings
         return full_neighbor_embeddings(self, indptr, indices, node_ids, normalize, minibatch=True, sampled=True,
-                                        edge_weight=edge_weight)
+                                        edge_weight=edge_weight, sample_weight=sample_weight)
 
     def _csr_input(self, t, dtype, name):
         """A CSR array on the model's device: numpy arrays are uploaded; tensors must already be there."""

@@ -854,7 +854,7 @@ def _sampled_csr_args(nnz):
         raise ValueError("sampled rows need fewer than 2^31 CSR entries (got %d)" % nnz)
 
 
-def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, entry_offsets=False):
+def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, entry_offsets=False, sample_weights=None):
     """The receptive field of `seeds` over n_layers layers of whole neighbourhoods (gs_csr_blocks_plan / _fill; contract
     in oracle/full_neighbor_blocks.py): a list, index l = layer l, of CsrBlock(src_ids int32 V_l, indptr int64 [|V_l|],
     indices int32, rows int32).  A block is a CSR over |V_l| - 1 local nodes whose last local row is the dummy, so
@@ -867,9 +867,15 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, e
     (seed, call) gives the same bytes.
     entry_offsets (with fanouts): return (blocks, offsets), offsets[l] int32 [entries of block l] aligned with block l's
     indices - each entry's offset in its node's raw CSR row, which training dropout masks it by
-    (gs_csr_sampled_blocks_fill_offsets; contract in oracle/sampled_blocks_dropout.py).  The blocks are the same bytes."""
+    (gs_csr_sampled_blocks_fill_offsets; contract in oracle/sampled_blocks_dropout.py).  The blocks are the same bytes.
+    sample_weights (with fanouts): fp32 CUDA [len(indices)], one weight per CSR entry.  Block l is then built over
+    S_l^w: at most fanouts[l] of each row's entries with weight > 0, drawn without replacement in proportion to weight
+    (the exponential race; gs_csr_weighted_blocks_plan / _fill / _fill_offsets; contract in
+    oracle/weighted_sampling.py), with the same layout, offsets and one size read."""
     if entry_offsets and fanouts is None:
         raise ValueError("entry_offsets needs fanouts (a whole-neighbourhood block entry is its raw row's entry)")
+    if sample_weights is not None and fanouts is None:
+        raise ValueError("sample_weights needs fanouts (a whole-neighbourhood block draws nothing)")
     require_cuda(indptr, indices, seeds)
     if indptr.dtype != torch.int64 or indptr.dim() != 1 or indptr.numel() < 1:
         raise TypeError("indptr must be a 1-D int64 tensor with >= 1 element")
@@ -882,6 +888,9 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, e
         fan = (_lib.c_i32 * L)(*check_fanouts(fanouts, L))
         _sampled_csr_args(nnz)
         draw = (fan, int(seed) & _U64, int(call) & _U64)
+    weighted = sample_weights is not None
+    if weighted:
+        sw = _csr_weights(sample_weights, nnz, "sample_weights")
     nbytes = lib().gs_csr_blocks_workspace_bytes(n_nodes, nnz, n, L)
     if nbytes < 0:
         check(-1)
@@ -890,8 +899,12 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, e
     counts = torch.empty((2 * L,), dtype=torch.int64, device=dev)
     ev = _probe("csr_blocks/%d" % n)
     head = (ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, ptr(seeds) if n else 0, n, L)
+    if weighted:
+        head = head[:2] + (ptr(sw),) + head[2:]
     if fanouts is None:
         check(lib().gs_csr_blocks_plan(*head, ptr(ws), nbytes, ptr(counts), stream_ptr()))
+    elif weighted:
+        check(lib().gs_csr_weighted_blocks_plan(*head, *draw, ptr(ws), nbytes, ptr(counts), stream_ptr()))
     else:
         check(lib().gs_csr_sampled_blocks_plan(*head, *draw, ptr(ws), nbytes, ptr(counts), stream_ptr()))
     sizes = [int(x) for x in counts.tolist()]                # the one device-to-host read
@@ -907,18 +920,23 @@ def csr_blocks(indptr, indices, seeds, n_layers, fanouts=None, seed=0, call=0, e
     elif entry_offsets:
         offsets = [torch.empty((sizes[2 * l + 1],), dtype=torch.int32, device=dev) for l in range(L)]
         off_arr = (_lib.c_vp * L)(*[ptr(o) if o.numel() else 0 for o in offsets])
-        check(lib().gs_csr_sampled_blocks_fill_offsets(*head, *draw, ptr(ws), nbytes, sz, *arrs, off_arr, stream_ptr()))
+        fill = lib().gs_csr_weighted_blocks_fill_offsets if weighted else lib().gs_csr_sampled_blocks_fill_offsets
+        check(fill(*head, *draw, ptr(ws), nbytes, sz, *arrs, off_arr, stream_ptr()))
     else:
-        check(lib().gs_csr_sampled_blocks_fill(*head, *draw, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
+        fill = lib().gs_csr_weighted_blocks_fill if weighted else lib().gs_csr_sampled_blocks_fill
+        check(fill(*head, *draw, ptr(ws), nbytes, sz, *arrs, stream_ptr()))
     _launched(6 * L + 4, ev)           # plan: mark, compact, size, degrees per level; fill: degrees, fill, rows (+ CUB)
     return (blocks, offsets) if entry_offsets else blocks
 
 
-def sample_csr_rows(indptr, indices, k, seed, call, layer):
+def sample_csr_rows(indptr, indices, k, seed, call, layer, weights=None):
     """S_layer over every node (gs_csr_sample_rows; contract in oracle/sampled_blocks.py): (indptr int64 [N + 1], indices
     int32), row v holding min(d, k) entries of v's row - all of them in CSR order when d <= k, else Floyd's k draws in
     ascending position order - with the entries' values as stored (not clamped).  The draws are the ones
-    csr_blocks(..., fanouts, seed, call) makes for its block `layer`.  Reads the entry count back once."""
+    csr_blocks(..., fanouts, seed, call) makes for its block `layer`.  Reads the entry count back once.
+    weights: None, or fp32 CUDA [len(indices)]: S_layer^w instead - min(d+, k) of the d+ entries with weight > 0, drawn
+    in proportion to weight, in ascending position order (gs_csr_sample_rows_weighted; contract in
+    oracle/weighted_sampling.py), the draws csr_blocks(..., sample_weights=weights) makes for its block `layer`."""
     indptr, indices = _csr_args(indptr, indices)
     k, layer = int(k), int(layer)
     if not 1 <= k <= _lib.MAX_FANOUT:
@@ -934,11 +952,16 @@ def sample_csr_rows(indptr, indices, k, seed, call, layer):
     out_indptr = torch.empty((n_nodes + 1,), dtype=torch.int64, device=indptr.device)
     args = (ptr(indptr), ptr(indices) if nnz else 0, n_nodes, nnz, k, int(seed) & _U64, int(call) & _U64, layer, ptr(ws),
             nbytes, ptr(out_indptr))
-    check(lib().gs_csr_sample_rows(*args, 0, stream_ptr()))
+    sample = lib().gs_csr_sample_rows
+    if weights is not None:
+        w = _csr_weights(weights, nnz)
+        args = args[:2] + (ptr(w),) + args[2:]
+        sample = lib().gs_csr_sample_rows_weighted
+    check(sample(*args, 0, stream_ptr()))
     total = int(out_indptr[-1].item())                       # the one device-to-host read
     out_indices = torch.empty((total,), dtype=torch.int32, device=indptr.device)
     if total:
-        check(lib().gs_csr_sample_rows(*args, ptr(out_indices), stream_ptr()))
+        check(sample(*args, ptr(out_indices), stream_ptr()))
     _launched(4 if total else 2)
     return out_indptr, out_indices
 

@@ -730,7 +730,7 @@ class SupervisedGraphsage(SampleAndAggregate):
         return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout,
                                                                     edge_weight=edge_weight))
 
-    def sampled_minibatch_outputs(self, indptr, indices, node_ids, dropout=None, edge_weight=None):
+    def sampled_minibatch_outputs(self, indptr, indices, node_ids, dropout=None, edge_weight=None, sample_weight=None):
         """outputs() over sampled receptive-field blocks (SampleAndAggregate.sampled_minibatch_embeddings; contract:
         oracle/sampled_blocks.py), with an autograd graph over the aggregator weights and (identity_dim > 0) the node
         embeddings.  One block set per call: the sampler's counter advances by 1.  dropout: None (no masks), or a
@@ -740,23 +740,28 @@ class SupervisedGraphsage(SampleAndAggregate):
         full_neighbor_outputs refuses but host-memory and int8 tables (taken here: see sampled_minibatch_embeddings),
         CUDA-graph capture, dropout=None on a model whose dropout_rate > 0, and dropout = p > 0 on an int8 table.
         edge_weight: as full_neighbor_outputs, each sampled entry carrying its raw CSR entry's weight; refused with
-        dropout p > 0."""
+        dropout p > 0.  sample_weight: as sampled_minibatch_embeddings, the blocks drawn in proportion to it; it
+        combines with edge_weight and with dropout."""
         from .full_neighbor_training import full_neighbor_outputs
         return full_neighbor_outputs(self, indptr, indices, node_ids, minibatch=True, sampled=True, dropout=dropout,
-                                     edge_weight=edge_weight)
+                                     edge_weight=edge_weight, sample_weight=sample_weight)
 
-    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
+    def sampled_minibatch_loss(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None,
+                               sample_weight=None):
         """loss() over sampled_minibatch_outputs: the same head, cross-entropy and weight decay.  dropout: as
-        sampled_minibatch_outputs; p > 0 also drops the head input (row r of node_ids at position r)."""
+        sampled_minibatch_outputs; p > 0 also drops the head input (row r of node_ids at position r).  sample_weight: as
+        sampled_minibatch_outputs."""
         check_full_neighbor_dropout(dropout)
-        out = self.sampled_minibatch_outputs(indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight)
+        out = self.sampled_minibatch_outputs(indptr, indices, node_ids, dropout=dropout, edge_weight=edge_weight,
+                                             sample_weight=sample_weight)
         return self._logits_loss(self._full_neighbor_logits(out, dropout), labels)
 
-    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None):
+    def sampled_minibatch_train_step(self, indptr, indices, node_ids, labels, dropout=None, edge_weight=None,
+                                     sample_weight=None):
         """One Adam step on sampled_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the detached
         loss."""
         return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, node_ids, labels, dropout=dropout,
-                                                              edge_weight=edge_weight))
+                                                              edge_weight=edge_weight, sample_weight=sample_weight))
 
     def full_neighbor_predict(self, indptr, indices, node_ids, edge_weight=None):
         """predict() over whole neighbourhoods: the head (supervised_models.py:88-92, 120-126) on

@@ -140,14 +140,16 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         return clipped_step(self, self.full_neighbor_minibatch_loss(indptr, indices, batch1, batch2, dropout=dropout,
                                                                     edge_weight=edge_weight))
 
-    def sampled_minibatch_loss(self, indptr, indices, batch1, batch2, dropout=None, edge_weight=None):
+    def sampled_minibatch_loss(self, indptr, indices, batch1, batch2, dropout=None, edge_weight=None,
+                               sample_weight=None):
         """loss() with every embedding computed over sampled receptive-field blocks (contract: oracle/sampled_blocks.py):
         the negatives are drawn first (one neg_sampler call), then ONE sampled block set over cat(batch1, batch2,
         negatives) - the sampler's counter advances by 1 - and its outputs split; then the same link-prediction loss and
         weight decay, divided by len(batch1), and the affinities for mrr().  dropout: None, or a rate p in [0, 1) masking
         that one block set (SupervisedGraphsage.sampled_minibatch_outputs; there is no head site).  Refusals as
         SupervisedGraphsage.sampled_minibatch_outputs, checked before the negatives are drawn.  edge_weight: as
-        full_neighbor_minibatch_loss."""
+        full_neighbor_minibatch_loss.  sample_weight: as SupervisedGraphsage.sampled_minibatch_outputs (the block set
+        is drawn in proportion to it; the negatives stay the unigram draws)."""
         from .full_neighbor_training import full_neighbor_outputs, refuse_sampled, refuse_weighted_dropout
         check_full_neighbor_dropout(dropout)
         refuse_sampled(self, training=True, dropout=dropout)                        # before drawing the negatives
@@ -155,14 +157,15 @@ class UnsupervisedGraphsage(SampleAndAggregate):
         neg = self.neg_sampler(self.neg_sample_size)
         b1, b2 = (torch.as_tensor(b).to(device=self.device, dtype=torch.int32).reshape(-1) for b in (batch1, batch2))
         out = full_neighbor_outputs(self, indptr, indices, torch.cat([b1, b2, neg]), minibatch=True, sampled=True,
-                                    dropout=dropout, edge_weight=edge_weight)
+                                    dropout=dropout, edge_weight=edge_weight, sample_weight=sample_weight)
         return self._pairs_loss(*torch.split(out, [b1.numel(), b2.numel(), neg.numel()]))
 
-    def sampled_minibatch_train_step(self, indptr, indices, batch1, batch2, dropout=None, edge_weight=None):
+    def sampled_minibatch_train_step(self, indptr, indices, batch1, batch2, dropout=None, edge_weight=None,
+                                     sample_weight=None):
         """One Adam step on sampled_minibatch_loss, gradients clipped to +-5 as in train_step.  Returns the detached
         loss."""
         return clipped_step(self, self.sampled_minibatch_loss(indptr, indices, batch1, batch2, dropout=dropout,
-                                                              edge_weight=edge_weight))
+                                                              edge_weight=edge_weight, sample_weight=sample_weight))
 
     def graphed_train_step(self, batch_size):
         """train_step for a fixed batch size captured in one CUDA graph: returns step(batch1, batch2) -> loss, a static 0-d

@@ -961,6 +961,44 @@ int32_t gs_csr_sample_rows(const int64_t* indptr, const int32_t* indices, int64_
                            uint64_t seed, uint64_t call, int32_t layer, void* workspace, int64_t workspace_bytes,
                            int64_t* out_indptr, int32_t* out_indices /* may be NULL */, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Weighted sampled blocks: the sampled blocks above with S_l^w(v), neighbours drawn in proportion to sample_weight
+ * (fp32, one per CSR entry, aligned with indices; NULL only when nnz = 0).  Contract: oracle/weighted_sampling.py.
+ * Eligible entries have w > 0 (NaN, zero and negative weights are never drawn), d+ of them: every eligible entry in CSR
+ * order when d+ <= k; else the k eligible entries with the smallest (key_j, j), key_j = E_j / w_j in fp64 (+inf weights
+ * give 0), E_j = -ln U_j by the oracle's fixed sequence of fp64 operations, U_j = (2m + 1) 2^-53 from words (0, 1) (j
+ * even) or (2, 3) (j odd) of Philox4x32-10(counter = (j >> 1, v, call mod 2^32, 0x80000000 | l), key = seed) - sorted
+ * ascending by position.  The order of the smallest keys is successive sampling in proportion to w.
+ * gs_csr_weighted_blocks_plan / _fill / _fill_offsets - gs_csr_sampled_blocks_plan / _fill / _fill_offsets over
+ *   S_l^w: the same workspace (gs_csr_blocks_workspace_bytes), layout, offsets and one read of counts_dev; block
+ *   entries: sum over V_{l+1} of min(d+, k_l).  The plan and the fill recompute the selection (nothing is stored between
+ *   them); a selection reads every weight of its row, a row of 4096 or more entries spread over a CTA.  No atomics: two
+ *   calls with the same (seed, call) give the same bytes.
+ * gs_csr_sample_rows_weighted - gs_csr_sample_rows over S_layer^w (out_indptr: exclusive scan of min(d+, k)); the same
+ *   workspace (gs_csr_sample_rows_workspace_bytes) and two-call protocol.
+ * --------------------------------------------------------------------------------------------- */
+int32_t gs_csr_weighted_blocks_plan(const int64_t* indptr, const int32_t* indices, const float* sample_weight,
+                                    int64_t n_nodes, int64_t nnz, const int32_t* seeds, int64_t n_seeds, int32_t n_layers,
+                                    const int32_t* fanouts, uint64_t seed, uint64_t call, void* workspace,
+                                    int64_t workspace_bytes, int64_t* counts_dev, void* stream);
+int32_t gs_csr_weighted_blocks_fill(const int64_t* indptr, const int32_t* indices, const float* sample_weight,
+                                    int64_t n_nodes, int64_t nnz, const int32_t* seeds, int64_t n_seeds, int32_t n_layers,
+                                    const int32_t* fanouts, uint64_t seed, uint64_t call, void* workspace,
+                                    int64_t workspace_bytes, const int64_t* counts, int32_t* const* src_ids,
+                                    int64_t* const* indptr_out, int32_t* const* indices_out, int32_t* const* rows_out,
+                                    void* stream);
+int32_t gs_csr_weighted_blocks_fill_offsets(const int64_t* indptr, const int32_t* indices, const float* sample_weight,
+                                            int64_t n_nodes, int64_t nnz, const int32_t* seeds, int64_t n_seeds,
+                                            int32_t n_layers, const int32_t* fanouts, uint64_t seed, uint64_t call,
+                                            void* workspace, int64_t workspace_bytes, const int64_t* counts,
+                                            int32_t* const* src_ids, int64_t* const* indptr_out,
+                                            int32_t* const* indices_out, int32_t* const* rows_out,
+                                            int32_t* const* offsets_out, void* stream);
+int32_t gs_csr_sample_rows_weighted(const int64_t* indptr, const int32_t* indices, const float* sample_weight,
+                                    int64_t n_nodes, int64_t nnz, int32_t k, uint64_t seed, uint64_t call, int32_t layer,
+                                    void* workspace, int64_t workspace_bytes, int64_t* out_indptr,
+                                    int32_t* out_indices /* may be NULL */, void* stream);
+
 /* tf.nn.l2_normalize(x, 1)   reference graphsage/models.py:368-370, supervised_models.py:85 */
 int32_t gs_l2_normalize_rows(float* x, int64_t n, int32_t C, int64_t ldx, void* stream);
 
