@@ -13,7 +13,7 @@ from .host_features import HostFeatures  # noqa: F401
 from .int8_features import Int8Features  # noqa: F401
 from .layers import Dense, Layer, identity, relu  # noqa: F401
 from .models import Node2VecModel, SAGEInfo, SampleAndAggregate  # noqa: F401
-from .neigh_samplers import CSRNeighborSampler, UniformNeighborSampler  # noqa: F401
+from .neigh_samplers import CSRNeighborSampler, UniformNeighborSampler, WeightedNeighborSampler  # noqa: F401
 from .prediction import BipartiteEdgePredLayer  # noqa: F401
 from .supervised_models import SupervisedGraphsage  # noqa: F401
 from .unsupervised_models import UnigramNegativeSampler, UnsupervisedGraphsage  # noqa: F401

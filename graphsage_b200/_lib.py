@@ -75,6 +75,10 @@ _SIGNATURES = {
     "gs_build_padded_adj": (c_i32, [c_vp, c_vp, c_i64, c_i32, c_vp, c_u64, c_u64, c_vp, c_vp, c_vp]),
     "gs_sample_unigram": (c_i32, [c_vp, c_i64, c_i32, c_u64, c_u64, c_vp, c_vp, c_vp]),
     "gs_sample_unigram_unique": (c_i32, [c_vp, c_i64, c_i32, c_u64, c_u64, c_vp, c_vp, c_vp, c_vp]),
+    "gs_csr_alias_build": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp]),
+    "gs_sample_alias": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_u64, c_u64, c_vp, c_vp, c_vp]),
+    "gs_sample_alias_khop": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, ctypes.POINTER(c_i32), c_i32, c_u64, c_u64, c_vp,
+                                     ctypes.POINTER(c_vp), c_vp]),
     "gs_sample_csr": (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_u64, c_u64, c_vp, c_i32, c_vp, c_vp]),
     "gs_perm_prefix_host": (c_i32, [c_u64, c_u64, c_i32, c_i32, ctypes.POINTER(c_i32)]),
     "gs_gather_rows": (c_i32, [c_vp, c_i32, c_i64, c_i32, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp]),

@@ -146,6 +146,8 @@ constexpr uint32_t kStreamWalkBiased = 0x60000000u;  // 2^28 words: ((w * 32 + m
 constexpr uint32_t kStreamSampledBlocks = 0x70000000u;  // GS_MAX_BLOCK_LAYERS words: | layer (counter (i, v, call, .))
 // weighted blocks: [0x80000000, 0x80000008), | layer (counter (j >> 1, v, call, .)); past every range above
 constexpr uint32_t kStreamWeightedBlocks = 0x80000000u;
+// alias draws: [0x90000000, 0x90000000 + GS_MAX_ALIAS_FANOUT / 2), + (j >> 1) (counter (c_lo, c_hi, t, .))
+constexpr uint32_t kStreamAlias = 0x90000000u;
 
 // ---- PTX wrappers (mbarrier / bulk copy) ---------------------------------------------------
 #ifdef __CUDACC__

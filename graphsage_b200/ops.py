@@ -94,6 +94,70 @@ def sample_padded_khop(adj, seeds, fanouts, seed, counter, counter_dev=None):
     return outs
 
 
+def csr_alias_table(indptr, indices, weights):
+    """The per-row alias tables of WeightedNeighborSampler (gs_csr_alias_build; contract in oracle/alias_sampling.py):
+    int32 [E, 4], one 16-byte record (thr, id, alias, 0) per entry of `indices`.  weights: float32 [E], one per entry
+    (TypeError for another dtype, ValueError for another length or device).  Set-up work, once per graph.  Records of
+    entries outside every row (before indptr[0] or from indptr[N] on) are zero."""
+    require_cuda(indptr, indices)
+    if indptr.dtype != torch.int64:
+        raise TypeError("indptr must be int64")
+    indices = _i32(indices, "indices")
+    E = indices.numel()
+    if isinstance(weights, torch.Tensor) and weights.dtype == torch.float32 and weights.device != indices.device:
+        raise ValueError("weights must be on %s (got %s)" % (indices.device, weights.device))
+    w = _csr_weights(weights, E)
+    table = torch.zeros((E, 4), dtype=torch.int32, device=indices.device)
+    check(lib().gs_csr_alias_build(ptr(indptr.contiguous()), ptr(indices), ptr(w), indptr.numel() - 1, E, ptr(table),
+                                   stream_ptr()))
+    _launched(1 if E and indptr.numel() > 1 else 0)
+    return table
+
+
+def _alias_args(indptr, table, ids, name):
+    require_cuda(indptr, table, ids)
+    if indptr.dtype != torch.int64:
+        raise TypeError("indptr must be int64")
+    if table.dtype != torch.int32 or table.dim() != 2 or table.shape[1] != 4:
+        raise TypeError("table must be the int32 [E, 4] tensor of csr_alias_table")
+    return indptr.contiguous(), table.contiguous(), _i32(ids.reshape(-1), name)
+
+
+def sample_alias(indptr, table, ids, k, seed, counter, counter_dev=None, out=None):
+    """WeightedNeighborSampler._call: int32 [n, k], draw j of ids[t] in proportion to the weights csr_alias_table was
+    built from, with replacement (gs_sample_alias; contract in oracle/alias_sampling.py).  k <= 1024 (GS_MAX_ALIAS_FANOUT)."""
+    indptr, table, ids = _alias_args(indptr, table, ids, "ids")
+    require_cuda(counter_dev)
+    n = ids.numel()
+    if out is None:
+        out = torch.empty((n, k), dtype=torch.int32, device=ids.device)
+    ev = _probe("sample_alias")
+    check(lib().gs_sample_alias(ptr(indptr), ptr(table), indptr.numel() - 1, ptr(ids), n, int(k), seed & _U64,
+                                counter & _U64, ptr(counter_dev), ptr(out), stream_ptr()))
+    _launched(1 if n * k else 0, ev)
+    return out
+
+
+def sample_alias_khop(indptr, table, seeds, fanouts, seed, counter, counter_dev=None):
+    """sample_alias over SampleAndAggregate.sample's whole frontier in one launch: fanouts in HOP order, returns
+    [hop1 ids, hop2 ids, ...] (flat int32), byte-identical to successive sample_alias calls with counters counter,
+    counter+1, ...  At most GS_MAX_HOPS (4) hops of fanout <= 64."""
+    indptr, table, seeds = _alias_args(indptr, table, seeds, "seeds")
+    require_cuda(counter_dev)
+    n = seeds.numel()
+    outs, cnt = [], n
+    for k in fanouts:
+        cnt *= int(k)
+        outs.append(torch.empty((cnt,), dtype=torch.int32, device=seeds.device))
+    fan = (_lib.c_i32 * len(fanouts))(*[int(k) for k in fanouts])
+    optr = (_lib.c_vp * len(fanouts))(*[ptr(o) for o in outs])
+    ev = _probe("sample_alias_khop")
+    check(lib().gs_sample_alias_khop(ptr(indptr), ptr(table), indptr.numel() - 1, ptr(seeds), n, fan, len(fanouts),
+                                     seed & _U64, counter & _U64, ptr(counter_dev), optr, stream_ptr()))
+    _launched(1 if n else 0, ev)
+    return outs
+
+
 def build_padded_adj(indptr, indices, max_degree, seed=123, counter=0, skip=None):
     """Padded adjacency [N+1, max_degree] (+ degree vector) from CSR on the device - the sampler's input contract,
     reference graphsage/minibatch.py:227-259.  skip: optional bool/uint8 [N] (val/test nodes keep all-N rows)."""

@@ -108,6 +108,30 @@ int32_t gs_sample_padded_khop(const int32_t* adj, int64_t n_rows, int32_t max_de
                               int32_t n_hops, uint64_t seed, uint64_t counter,
                               const uint64_t* counter_dev, int32_t* const* out_host, void* stream);
 
+/* WeightedNeighborSampler - fixed-fanout draws with replacement in proportion to a per-entry weight, from per-row
+ * alias tables (contract: oracle/alias_sampling.py, bit for bit).
+ * gs_csr_alias_build - the table: one 16-byte record (thr, id, alias, 0) per CSR entry, int32 table[n_entries * 4]
+ *   aligned with indices (row v's d buckets at indptr[v] ..).  weights: fp32, one per entry; finite w > 0 is eligible,
+ *   a row with +inf entries draws uniformly among them, a row with none eligible draws the dummy n_nodes.  Integer
+ *   masses summing to d 2^32 per row (every eligible entry >= 1) and an integer Vose sweep, both in a fixed order.
+ *   Rows of 2^31 entries or more: GS_ERR_UNSUPPORTED.  Set-up work; deterministic, no atomics, no allocation on the
+ *   device.
+ * gs_sample_alias - out[t * k + j] (k <= GS_MAX_ALIAS_FANOUT) = draw j of ids[t]: Philox4x32-10 block
+ *   (c_lo, c_hi, t, 0x90000000 + (j >> 1)) with c = counter + (counter_dev ? *counter_dev : 0), words (0, 1) for even j,
+ *   (2, 3) for odd j: bucket = mulhi32(a, d), id if b < thr else alias.  ids outside [0, n_nodes) and empty rows give
+ *   n_nodes.
+ * gs_sample_alias_khop - every hop of SampleAndAggregate.sample in one launch (n_hops <= GS_MAX_HOPS, fanout <= 64),
+ *   byte-identical to n_hops gs_sample_alias calls with counters counter, counter + 1, ... */
+#define GS_MAX_ALIAS_FANOUT 1024
+int32_t gs_csr_alias_build(const int64_t* indptr, const int32_t* indices, const float* weights, int64_t n_nodes,
+                           int64_t n_entries, int32_t* table, void* stream);
+int32_t gs_sample_alias(const int64_t* indptr, const int32_t* table, int64_t n_nodes, const int32_t* ids, int64_t n,
+                        int32_t k, uint64_t seed, uint64_t counter, const uint64_t* counter_dev, int32_t* out,
+                        void* stream);
+int32_t gs_sample_alias_khop(const int64_t* indptr, const int32_t* table, int64_t n_nodes, const int32_t* seeds,
+                             int64_t n_seeds, const int32_t* fanout_host, int32_t n_hops, uint64_t seed,
+                             uint64_t counter, const uint64_t* counter_dev, int32_t* const* out_host, void* stream);
+
 /* Per-node draws from a CSR adjacency (north_star's warp-per-node mode; no reference
  * counterpart).  Semantics: oracle/sampler.py:sample_csr.  k <= 32. */
 int32_t gs_sample_csr(const int64_t* indptr, const int32_t* indices, int64_t n_nodes,
